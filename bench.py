@@ -1,26 +1,27 @@
 #!/usr/bin/env python
-"""OSVOS hot-path benchmark (contract: the task statement; method: DESIGN.md section 6).
+"""OSVOS hot-path benchmark (contract: the task statement; method: DESIGN.md section 9).
 
     python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload infer480|train480|parent480]
 
-Default run (`--workload infer480`, what the driver launches), ONE JSON line on rank 0:
+Default run (`--workload infer480`), ONE JSON line on rank 0:
 
-  headline   BASELINE.json configs[1]: forward of one 480x854 frame per step and GPU, device-resident (`value`) and end to
-             end from pinned host memory (`e2e`).  One timed BLOCK = exactly K steps between barrier + synchronize pairs,
-             CUDA events on the launching stream, max over ranks.  K steps of a 0.7 ms frame are too short a window to
-             trust, so blocks are repeated until >= 1 s has been timed and the MEDIAN block is reported (`blocks`).
+  headline   BASELINE.json configs[1]: forward of one 480x854 frame per step and GPU, device-resident (`value`): exactly K
+             timed steps between barrier + synchronize pairs, CUDA events on the launching stream, max over ranks.  End to
+             end from pinned host memory (`e2e`): blocks of K steps repeated until >= 1 s has been timed, MEDIAN block.
   dp         BASELINE.json configs[3], the one multi-GPU path north_star names: parent training, batch 12 per GPU at
              480x854, 5-loss objective, FusedSGD, ONE NCCL allreduce(mean) of the 59.7 MB gradient bucket per step; run
              at every N including 1, with its own parity check (R ranks x 1 small frame against the oracle's
              nAveGrad = R accumulation, reference train_parent.py:163-172).
   parity     the CUDA forward against the CPU oracle on the benchmarked 480x854 frame: per-map max-rel logit error, mask
              flips (total / outside the |logit| < 1e-3 max band), IoU.
-  roofline   dominant kernel class = the tcgen05 3x3 convolutions; per-launch CUDA events behind a parked GPU.
-  gpu_reference   the UNMODIFIED reference modules (oracle/_ref) on the same B200 through cuDNN: TF32 default, strict
+  roofline   dominant kernel class = the wgmma 3x3 convolutions; per-launch CUDA events behind a parked GPU.
+  gpu_reference   the UNMODIFIED reference modules (oracle/_ref) on the same GPU through cuDNN: TF32 default, strict
              fp32, channels_last + bf16 autocast - "the real kernel to beat" (SURVEY.md 8d).
   cpu_baseline    the same reference modules on the host cores (bounded sample).
 
 `--impl reference` times the reference's own CPU path (oracle/_ref when present, else the oracle port).
+`--dump-outputs DIR` writes what the last timed step returned (infer480: the five logit maps; train480: the loss and a
+fixed, seeded sample of every parameter gradient of that step) as DIR/<name>.npy in float32; inputs and weights are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -65,7 +66,8 @@ def load_peaks():
         return {"hbm_gbs": p["hbm_gbs"], "tflops_burst": p["bf16_tflops"],
                 "tflops_sustained": p.get("bf16_tflops_sustained", p["bf16_tflops"]), "source": "measured"}
     except Exception:
-        return {"hbm_gbs": 6650.0, "tflops_burst": 1590.0, "tflops_sustained": 1400.0, "source": "fallback"}
+        # NVIDIA H100 SXM data sheet (700 W card), dense BF16: a ceiling, not a measured rate
+        return {"hbm_gbs": 3350.0, "tflops_burst": 989.0, "tflops_sustained": 989.0, "source": "H100 SXM data-sheet"}
 
 
 class ClockSampler:
@@ -493,19 +495,6 @@ def gpu_reference(dev):
     return out
 
 
-def conv_traffic(precision, calls):
-    """DRAM bytes per conv launch from the committed ncu capture matching this configuration, else None."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "conv_dram_traffic.json")) as f:
-            t = json.load(f)
-        e = t.get(f"{precision}_{H}x{W}")
-        if e and e.get("launches") == calls:
-            return e["dram_bytes_per_step"] / calls, e.get("source")
-    except Exception:
-        pass
-    return None, None
-
-
 # ----------------------------------------------------------------------------------------------------------------
 def run_parent_headline(args, rank, world, local, dev, timer):
     """--workload parent480: the dp object promoted to the headline line."""
@@ -524,6 +513,40 @@ def run_parent_headline(args, rank, world, local, dev, timer):
         dist.destroy_process_group()
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+GRAD_SAMPLE = 4096                     # gradient values written per parameter by --dump-outputs (train480)
+
+
+def gradient_sample(net):
+    """grad_<parameter>: the whole gradient of a small parameter, else GRAD_SAMPLE entries at fixed seeded positions."""
+    import torch
+    out = {}
+    for k, (name, p) in enumerate(net.named_parameters()):
+        if p.grad is None:
+            continue
+        g = p.grad.detach().reshape(-1)
+        if g.numel() > GRAD_SAMPLE:
+            gen = torch.Generator().manual_seed(1000 + k)
+            idx = torch.randperm(g.numel(), generator=gen)[:GRAD_SAMPLE].sort().values
+            g = g[idx.to(g.device)]
+        out["grad_" + name.replace(".", "_")] = g
+    return out
+
+
+def dump_outputs(out_dir, outs):
+    """Each output of the last timed step as out_dir/<name>.npy in float32 (64 MB in all at most)."""
+    import numpy as np
+    arrays = {k: v.detach().float().cpu().numpy() for k, v in outs.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        raise SystemExit(f"--dump-outputs: {total} bytes exceed the {DUMP_LIMIT_BYTES}-byte limit")
+    os.makedirs(out_dir, exist_ok=True)
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -538,6 +561,8 @@ def main():
     ap.add_argument("--skip", default="", help="comma list of legs to skip: dp,parity,gpu_reference,cpu_baseline,roofline,e2e_extra")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--eager-train", action="store_true", help="train480: eager launches instead of the step graph")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (infer480, train480)")
     args = ap.parse_args()
     skip = {s for s in args.skip.split(",") if s}
     if args.no_cpu_baseline:
@@ -564,6 +589,8 @@ def main():
     timer = Timer(dev, world)
     steps, warmup = max(1, args.steps), max(3, args.warmup)
     if args.workload == "parent480":
+        if args.dump_outputs:
+            raise SystemExit("--dump-outputs: supported for --workload infer480 and train480")
         return run_parent_headline(args, rank, world, local, dev, timer)
     train = args.workload == "train480"
 
@@ -578,6 +605,7 @@ def main():
     loss_host = torch.empty((), dtype=torch.float32).pin_memory()
 
     graphed = {"step": None}
+    last = {}                                         # what the most recent step returned to its caller
 
     def step(i, x=None):
         x = xs[i % n_in] if x is None else x
@@ -587,6 +615,7 @@ def main():
                 outs = net(x)
                 loss = class_balanced_cross_entropy_loss(outs[-1], gts[i % n_in], size_average=False)
                 loss.backward()
+                last["out"] = {"loss": loss.detach()}   # detached: a kept autograd graph would break a later graph capture
                 return loss
             # fwd + online loss + bwd of the micro-batch as one replayed CUDA graph (osvos_pytorch_b200.training)
             sample = {"image": x, "gt": gts[i % n_in]}
@@ -594,9 +623,14 @@ def main():
                 from osvos_pytorch_b200.training import GraphedTrainStep
                 graphed["step"] = GraphedTrainStep(
                     net, lambda outs, gt: class_balanced_cross_entropy_loss(outs[-1], gt, size_average=False), sample)
-            return graphed["step"](sample)          # gradients accumulate, as between the reference's optimizer steps
+            loss = graphed["step"](sample)          # gradients accumulate, as between the reference's optimizer steps
+            last["out"] = {"loss": loss.detach()}
+            return loss
         with torch.no_grad():
-            return net(x)[-1]
+            outs = net(x)
+        last["out"] = {f"logits_side{k + 1}": o for k, o in enumerate(outs[:-1])}
+        last["out"]["logits_fused"] = outs[-1]
+        return outs[-1]
 
     # kernels per step, counted on an eager pass (the timed inference steps replay a captured CUDA graph of
     # exactly these launches)
@@ -624,8 +658,20 @@ def main():
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
-    ms, blocks_info = timer.blocks(step, steps)
+    ms, blocks_info = timer.blocks(step, steps, min_ms=0.0, min_blocks=1)    # exactly K timed steps
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        outs = dict(last["out"])
+        if train:
+            # The caller of a training step receives the loss and the gradients it adds to p.grad.  Gradients
+            # accumulate over every step run so far (warm-up and settling included, a time-dependent count), so the last
+            # timed step is run once more on cleared gradients - same frame, same weights (no optimizer step here) - and
+            # a fixed, seeded sample of each parameter's gradient is written with its loss.
+            net.zero_grad(set_to_none=False)
+            outs = {"loss": step(steps - 1)}
+            torch.cuda.synchronize()
+            outs.update(gradient_sample(net))
+        dump_outputs(args.dump_outputs, outs)
 
     # ---- end to end: pinned host frame -> H2D -> OSVOS.forward -> D2H of the result ---
     def e2e_step(i):
@@ -669,8 +715,8 @@ def main():
                                             "d2h_bytes_per_step": H * W,
                                             "note": "sigmoid + imsave bytescale on the device (ops.logits_to_u8)"}}
 
-    # ---- roofline of the dominant kernel class (tcgen05 convs) ----------------------------------------------------
-    # In forward_inference every kernel between the first conv and the tail IS a tcgen05 conv (stage-1 kernel, trunk, side
+    # ---- roofline of the dominant kernel class (wgmma convs) ------------------------------------------------------
+    # In forward_inference every kernel between the first conv and the tail IS a wgmma conv (stage-1 kernel, trunk, side
     # convs; the fold / pack kernels only run on the first pass), so ONE event pair - recorded just before the first conv
     # launch and just before the tail launch - brackets exactly the conv kernels of a pass, back to back, without the
     # per-launch event pairs that used to cost the stream a few us each (their sum exceeded the whole graphed step).
@@ -781,10 +827,9 @@ def main():
         "config": {"workload": workload_label(args.workload), "precision": args.precision,
                    "parallelism": f"replicas x{world} for this headline (inference has no collective); the data-parallel "
                                   f"parent-training path is the `dp` object of this line",
-                   "l2": "per-step activation traffic (~0.9 GB exact) exceeds the 126 MB L2; inputs rotate over 4 frames; no explicit flush",
+                   "l2": "per-step activation traffic (~0.9 GB exact) exceeds the 50 MB L2; inputs rotate over 4 frames; no explicit flush",
                    "timing": "CUDA events on the launching stream, max over ranks; W warm-up steps + 0.5 s of untimed steps, "
-                             "then blocks of exactly K steps (barrier + synchronize on both sides) repeated until >= 1 s "
-                             "is timed; the MEDIAN block is reported",
+                             "then ONE block of exactly K timed steps (barrier + synchronize on both sides)",
                    "launch": ("captured CUDA graph of the step's kernels, replayed per step"
                               if ((graphs_on and not train) or (train and not args.eager_train)) else "eager launches")},
         "blocks": blocks_info,
@@ -817,13 +862,12 @@ def main():
         ach = conv_flops / (conv_ms * 1e-3) / 1e12
         # upper bound from the headline itself: all conv flops over the WHOLE graphed step (as if nothing else ran in it)
         ach_floor_step = conv_flops / (ms * 1e-3) / 1e12
-        traffic, tsrc = conv_traffic(args.precision, per)
         line["roofline"] = {
             "bound": "tensor",
-            "kernel": "the step's tcgen05 implicit-GEMM 3x3 convolutions: " + " + ".join(f"{k} x{v}" for k, v in kinds.items())
+            "kernel": "the step's wgmma implicit-GEMM 3x3 convolutions: " + " + ".join(f"{k} x{v}" for k, v in kinds.items())
                       + f" = {per} launches per step (every kernel of the step between the frame and the tail)",
             "achieved": ach, "peak": peaks["tflops_sustained"], "unit": "TFLOP/s", "frac": ach / peaks["tflops_sustained"],
-            "peak_source": f"{peaks['source']} bf16_tflops_sustained (kernels timed inside the step)",
+            "peak_source": f"{peaks['source']} dense BF16 (kernels timed inside the step)",
             "algorithmic_flops_per_step": conv_flops, "launches_per_step": per, "kernel_ms_per_step": conv_ms,
             "how": "ONE CUDA-event pair per pass spanning the conv launches (first conv launch -> tail launch), eager launches "
                    + ("queued behind a parked GPU (back-to-back kernel time)" if parked else "(host launch gaps included)"),
@@ -833,9 +877,7 @@ def main():
             "tensor_pipe_passes": passes,
             # exact mode emulates fp32 operands with three bf16 passes (hi*hi + hi*lo + lo*hi): the tensor pipe EXECUTES
             # passes x the algorithmic flops; this is that figure over the peak
-            "issued_mma_frac": ach * passes / peaks["tflops_sustained"],
-            "traffic": traffic, "traffic_unit": "dram bytes per launch (average over the step's conv launches)",
-            "traffic_source": tsrc}
+            "issued_mma_frac": ach * passes / peaks["tflops_sustained"]}
     if dp is not None:
         line["dp"] = dp
     if not train and "parity" not in skip:

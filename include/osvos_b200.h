@@ -1,4 +1,4 @@
-/* libosvos_b200 - C ABI of the B200-native OSVOS hot path.
+/* libosvos_b200 - C ABI of the H100-native OSVOS hot path.
  *
  * The reference (kmaninis/OSVOS-PyTorch) has no FFI of its own: its hot path is
  * Python calling torch.nn modules (SURVEY.md section 8b).  This header is the native
@@ -18,7 +18,7 @@
  *     16 for the side-branch gradient).  In OSVOS_FLAG_FAST mode only `hi`
  *     exists (lo pointers may be NULL) and a single tensor-core pass is issued;
  *     the default (exact) mode issues the three passes hi*hi + hi*lo + lo*hi
- *     with fp32 accumulation in TMEM.
+ *     with fp32 accumulation in registers.
  */
 #ifndef OSVOS_B200_H_
 #define OSVOS_B200_H_
@@ -88,7 +88,7 @@ OSVOS_API int osvos_act_to_nchw(const void* act_hi, const void* act_lo, float* y
 OSVOS_API int osvos_conv_first_fwd(const float* x_nchw, const float* w_oihw, const float* bias, void* y_hi, void* y_lo,
                          int n, int h, int w, int flags, osvos_stream_t stream);
 
-/* ---- 3x3 convolution, padding 1, stride 1, as a tcgen05 implicit GEMM -------
+/* ---- 3x3 convolution, padding 1, stride 1, as a wgmma implicit GEMM -------
  * Replaces every other nn.Conv2d(k=3, p=1) on the path: the 12 remaining trunk
  * convs (+ReLU, networks/vgg_osvos.py:142-143, run at :61,:66) and the four
  * side_prep convs (:41, run at :67, no ReLU); with transpose-flipped packed
@@ -120,7 +120,7 @@ typedef struct {
   int flags;
   /* 0 or 64: all input channels carry data.  16 / 32 / 48: only the first k_valid channels of every 64-channel
    * chunk can be non-zero (e.g. a 16-channel operand stored padded to 64): the remaining K steps
-   * are skipped - fewer tcgen05.mma, identical result. */
+   * are skipped - fewer wgmma, identical result. */
   int k_valid;
 } osvos_conv3x3_args;
 OSVOS_API int osvos_conv3x3(const osvos_conv3x3_args* args /* host */, osvos_stream_t stream);
@@ -225,7 +225,7 @@ OSVOS_API int osvos_cbce_bwd(const float* output, const float* label, const doub
 
 /* ======================= backward (training) entry points ======================= */
 
-/* ---- weight gradient of a 3x3 conv (tcgen05 GEMM over the pixel axis) -----------
+/* ---- weight gradient of a 3x3 conv (wgmma GEMM over the pixel axis) -----------
  * Replaces autograd's weight gradient of nn.Conv2d(k=3,p=1) (reference
  * networks/vgg_osvos.py:41,142; backward at train_online.py:141 / train_parent.py:164):
  *   dw[co][ci][r][s] = sum_px dz[px][co] * x[px + (r-1, s-1)][ci]

@@ -1,4 +1,4 @@
-"""Builds libosvos_b200.so (hand-written sm_100a CUDA, C ABI) in-tree with nvcc.
+"""Builds libosvos_b200.so (hand-written sm_90a CUDA, C ABI) in-tree with nvcc.
 
 The library has no torch / libcuda link-time dependency: cudart is linked
 statically and the one driver call (cuTensorMapEncodeTiled) is resolved at run
@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libosvos_b200.so")
 SOURCES = ["runtime.cu", "layout_kernels.cu", "conv3x3_halo.cu", "conv_stage1_fused.cu", "conv_first_tc.cu", "side_conv.cu", "tail.cu", "loss.cu", "wgrad_tc.cu", "bwd_kernels.cu", "side_bwd_folded.cu", "output_kernels.cu", "augment.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 
@@ -34,7 +34,7 @@ def _stale():
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_100a into lib/libosvos_b200.so."""
+    """Compile every CUDA source for sm_90a into lib/libosvos_b200.so."""
     if not force and not _stale():
         return LIB_PATH
     os.makedirs(LIB_DIR, exist_ok=True)
@@ -51,7 +51,7 @@ def build(force=False, verbose=False):
             raise RuntimeError(f"nvcc failed on {src}:\n{out}")
         if verbose:
             print(out)
-    cmd = [_nvcc(), "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [_nvcc(), "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}")

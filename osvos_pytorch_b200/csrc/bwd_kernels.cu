@@ -226,12 +226,11 @@ channel_sum_kernel(const __nv_bfloat16* __restrict__ hi, const __nv_bfloat16* __
 // -------------------------------------------------------------- conv1_1 bwd
 // dW[co][ci][r][s] = sum_px dz[px][co] * x[ci][px + (r-1, s-1)]: a [32 (27 used) x 64] output with the whole image
 // as reduction axis - 1.4 GFLOP at 480x854 against 105 MB of dz, i.e. HBM-bound once the arithmetic is cheap.  The
-// tile is too thin for tcgen05 (N = 27), so the products run on warp-level mma.sync.m16n8k16 (bf16 in, fp32 acc):
+// tile is too thin for wgmma (N = 27), so the products run on warp-level mma.sync.m16n8k16 (bf16 in, fp32 acc):
 //   C[k][co] += A[k][px] * B[px][co],  A = im2col rows of x (split into bf16 hi/lo here), B = dz (already hi/lo),
 // three passes hi*hi + hi*lo + lo*hi like every other product of the path.  A chunk is 64 consecutive pixels of one
 // image row: dz is copied 16 B at a time into padded rows (ldmatrix.trans reads them conflict-free), the 27 shifted
 // row segments of x are coalesced loads with no index division.  Each of the 8 warps owns 8 output channels.
-// (History: flat-pixel chunks + fp32 register tiles 146 us -> row chunks 103 us -> this kernel, see profiles/.)
 constexpr int kFwPix = 64;
 constexpr int kFwDzStride = 72;   // bf16 elements per smem row of a dz plane (64 + 8 pad -> 144 B, odd multiple of 16 B)
 constexpr int kFwXStride = 72;    // bf16 elements per smem row of an im2col plane

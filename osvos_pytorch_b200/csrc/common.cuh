@@ -45,7 +45,7 @@ int device_sm_count();
 bool pdl_enabled();
 
 // Launches `kern` on `stream`; with PDL enabled the launch carries the programmatic-stream-serialization attribute,
-// so the kernel's prologue (barrier init, TMEM allocation, descriptor prefetch) overlaps the previous kernel's tail.
+// so the kernel's prologue (barrier init, descriptor prefetch) overlaps the previous kernel's tail.
 // ONLY for kernels that execute pdl_wait() (ptx.cuh) before their first dependent global access.
 template <typename... KArgs, typename... Args>
 static inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,

@@ -1,23 +1,20 @@
-// 3x3 convolution as a tcgen05 implicit GEMM with HALO REUSE (sm_100a).
+// 3x3 convolution as a wgmma implicit GEMM with HALO REUSE (sm_90a).
 //
-// Same GEMM view, tile geometry, precision scheme, warp roles and epilogue as conv3x3_tc.cu, but the
-// activation operand is loaded ONCE per (tile, 64-channel chunk) as the 18-row x 10-px halo patch and the
-// nine taps are nine UMMA smem descriptors into it: tap (r, s) starts at smem row (r * PITCH + s); the 16
-// tile rows are the sixteen 8-row swizzle groups at stride SBO = PITCH * 128 B.  That divides the
-// activation traffic through L2 -> smem by ~6 relative to one shifted box per tap, which is what bounded
-// the per-tap kernel (DESIGN.md section 4).  The weight slabs stream through their own, deeper ring
-// (one stage per tap), and the next chunk's halo is prefetched while the current one is being consumed.
+// GEMM view: M = 128 pixels of an 8 x 16 output tile, N = output channels, K = 9 taps x input channels.  The
+// activation operand is loaded ONCE per (tile, 64-channel chunk) as the 18-row x 10-px halo patch (one TMA box,
+// SWIZZLE_128B) and the nine taps are nine wgmma descriptors into it: tap (r, s) starts at smem row (r * PITCH + s);
+// the 16 tile rows are sixteen 8-row swizzle groups at stride SBO = PITCH * 128 B.  That divides the activation
+// traffic through L2 -> smem by ~6 relative to one shifted box per tap.  The weight slabs stream through their own,
+// deeper ring (one stage per tap), and the next chunk's halo is prefetched while the current one is being consumed.
 //
-// PITCH is the smem row pitch in pixels: 10 packs the patch rows (1280 B) and relies on the UMMA swizzle being a
-// function of the absolute shared-memory address, validated on hardware together with the padded 16-pixel pitch and the
-// descriptor's base-offset field in round 1 (the base-offset field must stay 0).
+// PITCH is the smem row pitch in pixels: 10 packs the patch rows (1280 B); a tap descriptor then starts at any
+// 128-byte row, which relies on the hardware applying the 128-byte swizzle to the absolute shared-memory address
+// (the descriptor's base-offset field stays 0), as the TMA unit does when it writes the box.
 //
-// Producer and issuer loops: one elected thread each, taps unrolled, descriptors by addition - see the comments at
-// the two loops and DESIGN.md section 4 for the measurements behind that.
+// Precision: exact mode carries every operand as split bf16 (hi + lo) and sums A_hi.B_hi + A_hi.B_lo + A_lo.B_hi in
+// fp32; fast mode uses the hi planes only.
 #include <stdlib.h>
 #include <string.h>
-
-#include <type_traits>
 
 #include "conv_common.cuh"
 
@@ -25,7 +22,7 @@ namespace osvos {
 
 constexpr int kHaloRows = kTileH + 2;  // 18
 
-template <int BLOCK_N, int PLANES, int PITCH, bool SPLIT, bool LEAN = false>
+template <int BLOCK_N, int PLANES, int PITCH, bool SPLIT>
 struct HaloCfg {
   static constexpr int kABoxBytes = kHaloRows * PITCH * 128;                // one plane, one chunk
   static constexpr int kAPlaneBytes = (kABoxBytes + 1023) / 1024 * 1024;    // keep 1 KiB alignment
@@ -33,34 +30,30 @@ struct HaloCfg {
   static constexpr int kAStages = 2;
   static constexpr int kBPlaneBytes = BLOCK_N * 128;
   static constexpr int kBStageBytes = PLANES * kBPlaneBytes;
-  // LEAN: the forward-only epilogue (conv_common.cuh: conv_epilogue_lean) instead of the general one.
   static constexpr int kBudget = 225 * 1024 - kAStages * kAStageBytes;   // 227 KiB per CTA minus align/barriers
   static constexpr int kBStagesRaw = kBudget / kBStageBytes;
   static constexpr int kBStages = kBStagesRaw > 9 ? 9 : kBStagesRaw;
   // Exact mode with BLOCK_N <= 128: N-concatenated split-B.  The hi and lo weight planes are contiguous in the B
-  // stage, so ONE tcgen05.mma of N = 2 * BLOCK_N computes [A_hi.B_hi | A_hi.B_lo] into two column halves of the
-  // accumulator; with the N = BLOCK_N pass A_lo.B_hi that is 2 instructions per K step instead of 3 (the per-
-  // instruction floor of ~85 cycles makes instruction count, not flops, the cost).  The epilogue adds the halves.
+  // stage, so ONE wgmma of N = 2 * BLOCK_N computes [A_hi.B_hi | A_hi.B_lo] into two column halves of the
+  // accumulator; with the N = BLOCK_N pass A_lo.B_hi that is 2 instructions per K step instead of 3.  The epilogue
+  // adds the halves.
   static constexpr bool kSplitAcc = SPLIT;
   static_assert(!SPLIT || (PLANES == 2 && BLOCK_N <= 128), "split accumulators need two planes and 2 * BLOCK_N <= 256");
   static constexpr int kAccCols = kSplitAcc ? 2 * BLOCK_N : BLOCK_N;
-  static constexpr int kTmemCols = (2 * kAccCols) < 32 ? 32 : 2 * kAccCols;
+  static constexpr int kAcc = kAccCols / 2;                                 // accumulator registers per consumer thread
   static constexpr int kSmemBytes = kAStages * kAStageBytes + kBStages * kBStageBytes + 1024 + 512;
   static_assert(kBStages >= 2, "weight ring too shallow");
-  // The issuer forms descriptors by ADDING (bytes >> 4) to a base descriptor: every address it can reach - the end of
-  // the dynamic allocation plus the static shared variables' 1 KiB alignment slack - must stay inside the 14-bit
-  // start-address field (256 KiB), or the add would carry into the leading-dimension field.
-  static_assert(kSmemBytes <= 227 * 1024, "more than the per-CTA shared memory of sm_100");
+  static_assert(kSmemBytes <= 227 * 1024, "more than the per-CTA shared memory of sm_90");
   static_assert(kSmemBytes + 4096 < (1 << 18), "descriptor start-address field would overflow");
   static_assert(kBStageBytes % 1024 == 0, "B stage must keep 1024-byte alignment");
 };
 
 template <int BLOCK_N, int PLANES, int PITCH, bool SPLIT, bool LEAN>
-__global__ void __launch_bounds__(64 + EpiCfg<BLOCK_N>::kThreads, 1)
+__global__ void __launch_bounds__(kConvThreads, 1)
 conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__ CUtensorMap map_x_lo,
                     const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
                     const ConvParams p) {
-  using Cfg = HaloCfg<BLOCK_N, PLANES, PITCH, SPLIT, LEAN>;
+  using Cfg = HaloCfg<BLOCK_N, PLANES, PITCH, SPLIT>;
   constexpr int SA = Cfg::kAStages, SB = Cfg::kBStages;
 
   extern __shared__ uint8_t smem_raw[];
@@ -72,9 +65,6 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_c
   uint64_t* a_empty = bars + SA;
   uint64_t* b_full = bars + 2 * SA;
   uint64_t* b_empty = bars + 2 * SA + SB;
-  uint64_t* tfull_bar = bars + 2 * SA + 2 * SB;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -88,33 +78,24 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_c
     }
     for (int i = 0; i < SA; ++i) {
       mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 1);
+      mbar_init(&a_empty[i], 2);   // one arrival per consumer warpgroup
     }
     for (int i = 0; i < SB; ++i) {
       mbar_init(&b_full[i], 1);
-      mbar_init(&b_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], EpiCfg<BLOCK_N>::kThreads);
+      mbar_init(&b_empty[i], 2);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, Cfg::kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // PDL: everything above touched only shared memory, TMEM and the kernel parameters; the previous kernel's
-  // outputs (activations, masks, pooled planes, workspaces) are first accessed below.
+  // PDL: everything above touched only shared memory and the kernel parameters; the previous kernel's outputs
+  // (activations, masks, pooled planes, workspaces) are first accessed below.
   pdl_wait();
   pdl_launch_dependents();
 
   if (warp == 0) {
     // ------------------------------------------------------------ TMA producer (one elected thread)
-    // Same economy as the MMA issuer below: ONE elected thread runs the whole loop (no per-step ELECT / warp
-    // reconvergence), taps unrolled (the tap coordinate is an immediate), tile coordinates decoded once per tile
-    // (three integer divisions) instead of once per halo load.
+    // ONE elected thread runs the whole loop, taps unrolled (the tap coordinate is an immediate), tile coordinates
+    // decoded once per tile.
     if (elect_one()) {
       int a_stage = 0, b_stage = 0;
       uint32_t a_phase = 0, b_phase = 0;
@@ -172,116 +153,81 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_c
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // -------------------------------------------------------------- MMA issuer (one elected thread)
-    // The per-tap scalar work of this warp is what bounds the kernel, not the tensor pipe: timing ablations
-    // (scripts/ablate.py, profiles/r01f_ablation_480p.txt) showed that with every load, MMA and store removed the
-    // barrier skeleton alone still took 50-100 % of the full time, i.e. 600-900 cycles per (tap, 64-channel) step
-    // against 448 (N = 64) / 768 (N = 128) cycles of MMA time, while a bare issue loop sustains 48 / 64 cycles per
-    // MMA (scripts/microbench/operand_reuse_bench.cu).  So: the nine taps are unrolled (tap offsets are immediates),
-    // descriptors are formed by ADDING to one per-chunk base instead of being rebuilt, and nothing is recomputed
-    // per K step.  (A negative result from before, for the record: flattening the (tile, chunk, tap) nest to probe
-    // the next step's barrier between MMAs was 8 % slower - more index math on this warp.)
-    {
-      constexpr uint32_t idesc = make_idesc_f16(kBlockM, BLOCK_N, /*bf16=*/true);
-      constexpr uint32_t idesc2 = make_idesc_f16(kBlockM, Cfg::kSplitAcc ? 2 * BLOCK_N : BLOCK_N, /*bf16=*/true);
-      // descriptor templates without the start-address field (bits [0,14) = address >> 4): adding (bytes >> 4) to a
-      // descriptor moves its start address (shared-memory addresses stay below 2^18, no carry out of the field)
-      constexpr uint64_t kDescA = (static_cast<uint64_t>(16 >> 4) << 16) | (static_cast<uint64_t>((PITCH * 128) >> 4) << 32) |
-                                  (1ull << 46) | (static_cast<uint64_t>(kLayoutSW128) << 61);
-      constexpr uint64_t kDescB = (static_cast<uint64_t>(16 >> 4) << 16) | (static_cast<uint64_t>(1024 >> 4) << 32) |
-                                  (1ull << 46) | (static_cast<uint64_t>(kLayoutSW128) << 61);
-      constexpr uint32_t kLoPlaneA = Cfg::kAPlaneBytes >> 4, kLoPlaneB = Cfg::kBPlaneBytes >> 4;
-      const uint32_t smem_a_u32 = smem_u32(smem_a), smem_b_u32 = smem_u32(smem_b);
-      const int k_steps = (p.ablate & 4) ? 0 : p.k_steps;   // < 4 only for zero-padded input channels (k_valid)
-      // One tap = wait for its weight slab, FULLK ? 8 : up to 8 MMAs, release the slab.  FULLK (all four K steps of
-      // the 64-channel chunk) is the common case and has no per-K-step branches.
-      auto run = [&](auto fullk_tag) {
-        constexpr bool FULLK = decltype(fullk_tag)::value;
-        int a_stage = 0, b_stage = 0;
-        uint32_t a_phase = 0, b_phase = 0;
-        int it = 0;
-        for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-          const int as = it & 1;
-          const uint32_t aph = (it >> 1) & 1;
-          mbar_wait(&tempty_bar[as], aph ^ 1);
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + as * Cfg::kAccCols;
-          for (int kc = 0; kc < p.k_chunks; ++kc) {
-            mbar_wait(&a_full[a_stage], a_phase);
-            tc_fence_after();
-            const uint64_t da0 = kDescA | static_cast<uint64_t>((smem_a_u32 + a_stage * Cfg::kAStageBytes) >> 4);
-            const uint32_t not_first_chunk = kc != 0;
-            const bool last_chunk = kc == p.k_chunks - 1;
+  } else if (warp >= 4) {
+    // -------------------------------------------------- consumer warpgroups: wgmma + epilogue for 64 rows each
+    // The nine taps are nine descriptors into the halo patch: tap (r, s) starts at smem row (r * PITCH + s), the
+    // warpgroup's eight patch rows are eight 8-row swizzle groups at stride SBO = PITCH * 128 B.
+    const int wg = (warp - 4) >> 2, wl = warp & 3;
+    const bool leader = (threadIdx.x & 127) == 0;
+    constexpr uint64_t kDescA = desc_template(16, PITCH * 128, kDescSW128);
+    constexpr uint64_t kDescB = desc_template(16, 1024, kDescSW128);
+    constexpr uint32_t kLoPlaneA = Cfg::kAPlaneBytes >> 4, kLoPlaneB = Cfg::kBPlaneBytes >> 4;
+    const uint32_t smem_a_u32 = smem_u32(smem_a) + wg * 8 * PITCH * 128, smem_b_u32 = smem_u32(smem_b);
+    const int k_steps = (p.ablate & 4) ? 0 : p.k_steps;   // < 4 only for zero-padded input channels (k_valid)
+    float acc[Cfg::kAcc];
+    int a_stage = 0, b_stage = 0;
+    uint32_t a_phase = 0, b_phase = 0;
+    StageRelease pending;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
 #pragma unroll
-            for (int tap = 0; tap < 9; ++tap) {
-              constexpr int kRowBytes16 = 128 >> 4;
-              const uint32_t tap_off = static_cast<uint32_t>(((tap / 3) * PITCH + (tap % 3)) * kRowBytes16);
-              mbar_wait(&b_full[b_stage], b_phase);
-              tc_fence_after();
-              const uint64_t db_hi = kDescB | static_cast<uint64_t>((smem_b_u32 + b_stage * Cfg::kBStageBytes) >> 4);
-              {
-                const uint64_t da_hi = da0 + tap_off;
-                const uint64_t da_lo = da_hi + kLoPlaneA;
+      for (int i = 0; i < Cfg::kAcc; ++i) acc[i] = 0.f;
+      for (int kc = 0; kc < p.k_chunks; ++kc) {
+        mbar_wait(&a_full[a_stage], a_phase);
+        const uint64_t da0 = kDescA | static_cast<uint64_t>((smem_a_u32 + a_stage * Cfg::kAStageBytes) >> 4);
 #pragma unroll
-                for (int k = 0; k < kBlockK / 16; ++k) {
-                  if (FULLK || k < k_steps) {
-                    const uint32_t acc = (tap == 0 && k == 0) ? not_first_chunk : 1u;
-                    if (Cfg::kSplitAcc) {
-                      umma_f16(tmem_d, da_hi + 2 * k, db_hi + 2 * k, idesc2, acc);   // [A_hi.B_hi | A_hi.B_lo], N = 2 * BLOCK_N
-                      umma_f16(tmem_d, da_lo + 2 * k, db_hi + 2 * k, idesc, 1);      // + A_lo.B_hi into the first half
-                    } else if (PLANES == 2) {
-                      umma_f16(tmem_d, da_lo + 2 * k, db_hi + 2 * k, idesc, acc);
-                      umma_f16(tmem_d, da_hi + 2 * k, db_hi + kLoPlaneB + 2 * k, idesc, 1);
-                      umma_f16(tmem_d, da_hi + 2 * k, db_hi + 2 * k, idesc, 1);
-                    } else {
-                      umma_f16(tmem_d, da_hi + 2 * k, db_hi + 2 * k, idesc, acc);
-                    }
-                  }
-                }
-                umma_commit(&b_empty[b_stage]);
-                if (tap == 8) {
-                  umma_commit(&a_empty[a_stage]);
-                  if (last_chunk) umma_commit(&tfull_bar[as]);
-                }
-              }
-              if (++b_stage == SB) {
-                b_stage = 0;
-                b_phase ^= 1;
-              }
+        for (int tap = 0; tap < 9; ++tap) {
+          const uint32_t tap_off = static_cast<uint32_t>(((tap / 3) * PITCH + (tap % 3)) * (128 >> 4));
+          mbar_wait(&b_full[b_stage], b_phase);
+          const uint64_t db_hi = kDescB | static_cast<uint64_t>((smem_b_u32 + b_stage * Cfg::kBStageBytes) >> 4);
+          const uint64_t da_hi = da0 + tap_off;
+          const uint64_t da_lo = da_hi + kLoPlaneA;
+          wgmma_fence();
+          // all four K steps is the common case; fewer only for zero-padded input channels (k_valid)
+          auto k_step = [&](int k) {
+            if constexpr (Cfg::kSplitAcc) {
+              wgmma_bf16<2 * BLOCK_N>(acc, da_hi + 2 * k, db_hi + 2 * k, 1);   // [A_hi.B_hi | A_hi.B_lo]
+              wgmma_bf16<BLOCK_N>(acc, da_lo + 2 * k, db_hi + 2 * k, 1);       // + A_lo.B_hi into the first half
+            } else if constexpr (PLANES == 2) {
+              wgmma_bf16<BLOCK_N>(acc, da_lo + 2 * k, db_hi + 2 * k, 1);
+              wgmma_bf16<BLOCK_N>(acc, da_hi + 2 * k, db_hi + kLoPlaneB + 2 * k, 1);
+              wgmma_bf16<BLOCK_N>(acc, da_hi + 2 * k, db_hi + 2 * k, 1);
+            } else {
+              wgmma_bf16<BLOCK_N>(acc, da_hi + 2 * k, db_hi + 2 * k, 1);
             }
-            if (++a_stage == SA) {
-              a_stage = 0;
-              a_phase ^= 1;
-            }
+          };
+          if (k_steps == kBlockK / 16) {
+#pragma unroll
+            for (int k = 0; k < kBlockK / 16; ++k) k_step(k);
+          } else {
+            for (int k = 0; k < k_steps; ++k) k_step(k);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();               // the previous tap's group is done: its stages may be refilled
+          pending.release(leader);
+          pending.bar_b = &b_empty[b_stage];
+          if (tap == 8) pending.bar_a = &a_empty[a_stage];
+          if (++b_stage == SB) {
+            b_stage = 0;
+            b_phase ^= 1;
           }
         }
-      };
-      // ONE elected thread runs the whole issue loop (waits included): no per-tap ELECT / BSSY / BSYNC / warp
-      // reconvergence; the other 31 lanes go straight to the closing __syncthreads.
-      if (elect_one()) {
-        if (k_steps == kBlockK / 16) run(std::true_type{});
-        else run(std::false_type{});
+        if (++a_stage == SA) {
+          a_stage = 0;
+          a_phase ^= 1;
+        }
       }
-      __syncwarp();
+      wgmma_wait<0>();
+      wgmma_fence_operands(acc);
+      pending.release(leader);
+      conv_epilogue<BLOCK_N, Cfg::kSplitAcc, LEAN>(p, acc, tile, wg, wl, lane);
     }
-  } else {
-    if constexpr (LEAN) conv_epilogue_lean<BLOCK_N>(p, tmem_base, tfull_bar, tempty_bar, warp, lane);
-    else conv_epilogue_loop<BLOCK_N, Cfg::kSplitAcc>(p, tmem_base, tfull_bar, tempty_bar, warp, lane);
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
   }
 }
 
-// Environment switches of the dispatcher (A/B and diagnosis; defaults are the measured winners).  Read ONCE per process;
+// Environment switches of the dispatcher (A/B and diagnosis).  Read ONCE per process;
 // OSVOS_ENV_RELOAD=1 makes every dispatch re-read them (scripts/ab_env.py flips switches inside one process).
 struct HaloSwitches {
-  bool lean;        // OSVOS_HALO_LEAN      (default 1): lean epilogue for plain forward launches
+  bool lean;        // OSVOS_HALO_LEAN      (default 1): lean epilogue instantiation for plain forward launches
   bool n256;        // OSVOS_CONV_N256      (default 1): 256-wide tiles where they pay
   bool splitacc128; // OSVOS_SPLITACC128    (default 1): N-concatenated accumulator for 128-wide exact tiles
 };
@@ -303,7 +249,7 @@ static HaloSwitches halo_switches() {
 
 template <int BLOCK_N, int PLANES, int PITCH, bool SPLIT = (PLANES == 2 && BLOCK_N <= 128), bool LEAN = false>
 static int launch_halo(const osvos_conv3x3_args* a, cudaStream_t stream) {
-  using Cfg = HaloCfg<BLOCK_N, PLANES, PITCH, SPLIT, LEAN>;
+  using Cfg = HaloCfg<BLOCK_N, PLANES, PITCH, SPLIT>;
   ConvParams p;
   fill_conv_params(p, a, BLOCK_N);
   const int sms = device_sm_count();
@@ -326,7 +272,7 @@ static int launch_halo(const osvos_conv3x3_args* a, cudaStream_t stream) {
   static uint64_t attr_done = 0;   // per instantiation: bit d = device d has the shared-memory opt-in
   OSVOS_CHECK_CUDA(ensure_dynamic_smem(kern, Cfg::kSmemBytes, &attr_done));
   const int grid = p.total_tiles < sms ? p.total_tiles : sms;
-  OSVOS_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(64 + EpiCfg<BLOCK_N>::kThreads), Cfg::kSmemBytes, stream, mx_hi, mx_lo,
+  OSVOS_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kConvThreads), Cfg::kSmemBytes, stream, mx_hi, mx_lo,
                               mw_hi, mw_lo, p));
   return OSVOS_OK;
 }
@@ -338,9 +284,7 @@ static int dispatch_halo(const osvos_conv3x3_args* a, cudaStream_t stream) {
   if (a->cout == 16) return fast ? launch_halo<16, 1, PITCH>(a, stream) : launch_halo<16, 2, PITCH>(a, stream);
   // the lean epilogue serves launches that use nothing but bias / ReLU / split-bf16 act output / fused pool (exact mode)
   const bool lean = sw.lean && !fast && !(a->flags & OSVOS_FLAG_RELU_MASK) && a->colsum == nullptr && a->y_f32 == nullptr &&
-                    a->pq == nullptr && (a->y_hi != nullptr || a->pool_hi != nullptr) &&
-                    (a->y_hi == nullptr || a->y_lo != nullptr) && (a->pool_hi == nullptr || a->pool_lo != nullptr) &&
-                    a->k_valid == 0;
+                    a->pq == nullptr && a->k_valid == 0;
   if (a->cout == 64) {
     if (lean) return launch_halo<64, 2, PITCH, true, true>(a, stream);
     return fast ? launch_halo<64, 1, PITCH>(a, stream) : launch_halo<64, 2, PITCH>(a, stream);
@@ -351,32 +295,27 @@ static int dispatch_halo(const osvos_conv3x3_args* a, cudaStream_t stream) {
   const long waves128 = (tiles128 + sms - 1) / sms;
   const long waves256 = (static_cast<long>(m_tiles) * (a->cout / 256) + sms - 1) / sms;
   // few tiles (stage 5 at 480x854: 56 of 128 x 128): N = 64 tiles double the CTA count at ~0.8x the time per tile.
-  // (Stream-K - (tile, chunk) units in balanced contiguous ranges, tiles cut by a range boundary exchanging fp32 partial
-  // accumulators - was built, validated and measured in round 2: -18 % on 240x427 frames and -5 % at 480x854 when
-  // applied to every badly quantised layer, -1 % / +-0 / +2 % (240p / 480p / 720p) when restricted to layers with at
-  // least one whole tile per CTA.  The layers it would help are power-limited: the idle SMs of a ragged last wave are
-  // what lets the busy ones clock higher.  Removed again; profiles/r02c_ab_matrix.txt, r02d_ab_matrix_*.txt.)
   if (waves128 == 1 && tiles128 * 5 <= static_cast<long>(sms) * 3) {
     if (lean) return launch_halo<64, 2, PITCH, true, true>(a, stream);
     return fast ? launch_halo<64, 1, PITCH>(a, stream) : launch_halo<64, 2, PITCH>(a, stream);
   }
-  // N = 256 tiles (one tcgen05.mma of 128 cycles per pass) whenever that does not cost a wave; measured cycles per
-  // (tap, 64-channel) step: N = 128 ~ 1000 (2 + 1 instructions), N = 256 ~ 2200 exact
+  // N = 256 tiles whenever that does not cost a wave.  The cost model per (tap, 64-channel) step (N = 128 ~ 1000 cycles
+  // for 2 + 1 instructions, N = 256 ~ 2200 exact) is carried over from the first tensor-core generation this was tuned on;
+  // on an H100 the choice measured neutral at 480x854 (552-553 frames/s with and without OSVOS_CONV_N256=0).
   const bool prefer256 = fast ? waves256 * 1100 < waves128 * 700 : waves256 * 2200 < waves128 * 1000;
   if (a->cout % 256 == 0 && prefer256 && sw.n256)
     return fast ? launch_halo<256, 1, PITCH>(a, stream) : launch_halo<256, 2, PITCH>(a, stream);
   if (fast) return launch_halo<128, 1, PITCH>(a, stream);
   // Exact mode, N = 128: the N-concatenated split accumulator (2 MMAs per K step, 256 accumulator columns, the
-  // epilogue sums two halves) and the plain three-pass form (3 MMAs, 128 columns) cost the SAME tensor time
-  // (scripts/microbench/operand_reuse_bench.cu) and measured the same; OSVOS_SPLITACC128=0 selects the three-pass form.
+  // epilogue sums two halves) and the plain three-pass form (3 MMAs, 128 columns) do the same tensor work;
+  // OSVOS_SPLITACC128=0 selects the three-pass form.
   if (!sw.splitacc128) return launch_halo<128, 2, PITCH, false>(a, stream);
   if (lean) return launch_halo<128, 2, PITCH, true, true>(a, stream);
   return launch_halo<128, 2, PITCH>(a, stream);
 }
 
 int conv3x3_halo_dispatch(const osvos_conv3x3_args* a, cudaStream_t stream) {
-  // packed patch rows (pitch 10) are the only instantiation: the padded 16-pixel pitch and the descriptor base-offset
-  // field were validated equivalent on hardware in round 1 and dropped
+  // packed patch rows (pitch 10) are the only instantiation
   return dispatch_halo<10>(a, stream);
 }
 
@@ -398,11 +337,12 @@ static int check_conv_args(const osvos_conv3x3_args* a) {
   OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(a->x_hi) & 15) == 0);
   OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(a->w_packed) & 15) == 0);
   OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(a->bias) & 15) == 0);
-  if (a->cout >= 64) {   // 256-bit stores / loads in the epilogues
-    const uintptr_t any = reinterpret_cast<uintptr_t>(a->y_hi) | reinterpret_cast<uintptr_t>(a->y_lo) |
-                          reinterpret_cast<uintptr_t>(a->y_f32) | reinterpret_cast<uintptr_t>(a->pool_hi) |
-                          reinterpret_cast<uintptr_t>(a->pool_lo) | reinterpret_cast<uintptr_t>(a->mask_hi);
-    OSVOS_CHECK_ARG((any & 31) == 0);
+  if (a->cout >= 64) {   // the epilogue moves channel pairs: 4-byte bf16x2 words, 8-byte float2
+    const uintptr_t bf16_planes = reinterpret_cast<uintptr_t>(a->y_hi) | reinterpret_cast<uintptr_t>(a->y_lo) |
+                                  reinterpret_cast<uintptr_t>(a->pool_hi) | reinterpret_cast<uintptr_t>(a->pool_lo) |
+                                  reinterpret_cast<uintptr_t>(a->mask_hi);
+    OSVOS_CHECK_ARG((bf16_planes & 3) == 0);
+    OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(a->y_f32) & 7) == 0);
   }
   OSVOS_CHECK_ARG(a->k_valid >= 0 && a->k_valid <= 64 && a->k_valid % 16 == 0);
   return OSVOS_OK;

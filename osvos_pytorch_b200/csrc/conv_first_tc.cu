@@ -1,16 +1,13 @@
 // conv1_1 (3 -> 64 channels, 3x3, pad 1) + bias + ReLU on the tensor cores.
 //
 // K = 27 is too small for TMA-fed operands (and the frame is NCHW fp32), so the im2col A tile is BUILT in
-// shared memory by four producer warps straight from the caller's frame: row m = pixel, k = ci*9 + 3r + s,
+// shared memory by warpgroup 0 straight from the caller's frame: row m = pixel, k = ci*9 + 3r + s,
 // split into bf16 hi / lo, written in the canonical K-major SWIZZLE_128B layout (16-byte chunk j of row m
-// lands at chunk j ^ (m & 7)).  Only k < 32 is ever written or read: two UMMA K-steps x three passes = 6
-// tcgen05.mma per 128-pixel tile.  The 64 x 27 weight matrix is converted once per CTA into the same
-// layout (B operand, resident).  Epilogue = the shared conv epilogue (bias, ReLU, split-bf16 act store).
-// Generic-proxy smem writes are made visible to the tensor core with fence.proxy.async before the
-// mbarrier arrive.
-//
-// Measured alternatives (round 1): staging the 3 x 18 x 10 input patch in shared memory and gathering the taps from
-// it was slower (110 vs 74 us); direct 16-byte global stores instead of the TMA-store epilogue were slower (93 us).
+// lands at chunk j ^ (m & 7)).  Only k < 32 is ever written or read: two wgmma K-steps x three passes per
+// 64-row half of a 128-pixel tile.  The 64 x 27 weight matrix is converted once per CTA into the same
+// layout (B operand, resident).  Warpgroups 1 and 2 issue the wgmma for the two halves and run the shared
+// conv epilogue (bias, ReLU, split-bf16 act store).  Generic-proxy smem writes are made visible to the
+// tensor core with fence.proxy.async before the mbarrier arrive.
 //
 // Replaces stages[0][0..1] of the reference (networks/vgg_osvos.py:61,142-143).
 #include <string.h>
@@ -19,28 +16,20 @@
 
 namespace osvos {
 
-constexpr int kFirstTcThreads = 448;  // warp 0 idle, warp 1 MMA, warps 2-9 epilogue, warps 10-13 A builders
 constexpr int kFirstStages = 3;
 constexpr int kFirstStageBytes = 2 * kABytes;           // hi + lo planes of the A tile (128 rows x 128 B each)
 constexpr int kFirstBBytes = 2 * 64 * 128;              // hi + lo planes of the weights (64 rows x 128 B)
-constexpr int kFirstStagingBytes = 2 * kABytes;         // TMA-store staging (hi + lo slab of the output tile)
-constexpr int kFirstSmem = kFirstStages * kFirstStageBytes + kFirstBBytes + kFirstStagingBytes + 1024 + 256;
+constexpr int kFirstSmem = kFirstStages * kFirstStageBytes + kFirstBBytes + 1024 + 256;
 
 template <int PLANES>
-__global__ void __launch_bounds__(kFirstTcThreads, 1)
-conv_first_tc_kernel(const float* __restrict__ x, const float* __restrict__ wgt,
-                     const __grid_constant__ CUtensorMap map_y_hi, const __grid_constant__ CUtensorMap map_y_lo,
-                     const ConvParams p) {
+__global__ void __launch_bounds__(kConvThreads, 1)
+conv_first_tc_kernel(const float* __restrict__ x, const float* __restrict__ wgt, const ConvParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_b = smem + kFirstStages * kFirstStageBytes;
-  uint8_t* staging = smem_b + kFirstBBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + kFirstStagingBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + kFirstBBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kFirstStages;
-  uint64_t* tfull_bar = bars + 2 * kFirstStages;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -48,21 +37,16 @@ conv_first_tc_kernel(const float* __restrict__ x, const float* __restrict__ wgt,
   if (threadIdx.x == 0) {
     for (int i = 0; i < kFirstStages; ++i) {
       mbar_init(&full_bar[i], 128);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], EpiCfg<64>::kThreads);
+      mbar_init(&empty_bar[i], 2);   // one arrival per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 128);
   // PDL: the weights may have been rewritten by the previous kernel of the stream (the optimizer step), so even
-  // the resident B operand is built after the wait; only barrier init and the TMEM allocation overlap its tail.
+  // the resident B operand is built after the wait; only barrier init overlaps its tail.
   pdl_wait();
   pdl_launch_dependents();
   // resident B operand: rows = co, k = ci*9 + 3r + s (the OIHW flattening), chunks 0..3 (k < 32)
-  for (int i = threadIdx.x; i < 64 * 4; i += kFirstTcThreads) {
+  for (int i = threadIdx.x; i < 64 * 4; i += kConvThreads) {
     const int co = i >> 2, chunk = i & 3;
     uint32_t hi[4], lo[4];
 #pragma unroll
@@ -80,65 +64,51 @@ conv_first_tc_kernel(const float* __restrict__ x, const float* __restrict__ wgt,
     *reinterpret_cast<uint4*>(smem_b + 64 * 128 + sw128_offset(co, chunk)) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
   }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 1) {
-    // -------------------------------------------------------------- MMA issuer (one elected thread, see conv3x3_halo.cu)
-    if (elect_one()) {
-    constexpr uint32_t idesc = make_idesc_f16(kBlockM, 64, /*bf16=*/true);
+  if (warp >= 4) {
+    // -------------------------------------------------------------- consumer warpgroups: wgmma + epilogue
+    const int wg = (warp - 4) >> 2, wl = warp & 3;
+    const bool leader = (threadIdx.x & 127) == 0;
+    const uint64_t db_hi = make_smem_desc(smem_b, 16, 1024, kDescSW128);
+    const uint64_t db_lo = db_hi + ((64 * 128) >> 4);
     int stage = 0;
     uint32_t phase = 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
-      const uint32_t aph = (it >> 1) & 1;
-      mbar_wait(&tempty_bar[as], aph ^ 1);
+    float acc[32];
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       mbar_wait(&full_bar[stage], phase);
-      tc_fence_after();
-      {
-        const uint32_t tmem_d = tmem_base + as * 64;
-        const uint32_t a_hi = smem_u32(smem + stage * kFirstStageBytes);
-        const uint32_t b_hi = smem_u32(smem_b);
-        const uint64_t da_hi = make_smem_desc(a_hi, 16, 1024, kLayoutSW128);
-        const uint64_t da_lo = make_smem_desc(a_hi + kABytes, 16, 1024, kLayoutSW128);
-        const uint64_t db_hi = make_smem_desc(b_hi, 16, 1024, kLayoutSW128);
-        const uint64_t db_lo = make_smem_desc(b_hi + 64 * 128, 16, 1024, kLayoutSW128);
+      const uint64_t da_hi = make_smem_desc(smem + stage * kFirstStageBytes + wg * 64 * 128, 16, 1024, kDescSW128);
+      const uint64_t da_lo = da_hi + (kABytes >> 4);
 #pragma unroll
-        for (int k = 0; k < 2; ++k) {
-          const uint64_t adv = static_cast<uint64_t>(k * 2);
-          if (PLANES == 2) {
-            umma_f16(tmem_d, da_lo + adv, db_hi + adv, idesc, k != 0);
-            umma_f16(tmem_d, da_hi + adv, db_lo + adv, idesc, 1);
-            umma_f16(tmem_d, da_hi + adv, db_hi + adv, idesc, 1);
-          } else {
-            umma_f16(tmem_d, da_hi + adv, db_hi + adv, idesc, k != 0);
-          }
+      for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        if (PLANES == 2) {
+          wgmma_bf16<64>(acc, da_lo + 2 * k, db_hi + 2 * k, 1);
+          wgmma_bf16<64>(acc, da_hi + 2 * k, db_lo + 2 * k, 1);
         }
-        umma_commit(&empty_bar[stage]);
-        umma_commit(&tfull_bar[as]);
+        wgmma_bf16<64>(acc, da_hi + 2 * k, db_hi + 2 * k, 1);
       }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_operands(acc);
+      if (leader) mbar_arrive(&empty_bar[stage]);
       if (++stage == kFirstStages) {
         stage = 0;
         phase ^= 1;
       }
+      conv_epilogue<64, false>(p, acc, tile, wg, wl, lane);
     }
-    }
-    __syncwarp();
-  } else if (warp >= 2 && warp < 10) {
-    conv_epilogue_loop<64, false, true>(p, tmem_base, tfull_bar, tempty_bar, warp, lane, &map_y_hi, &map_y_lo, staging);
-  } else if (warp >= 10) {
-    // ------------------------------------------------------------- A builders
-    const int row = (warp - 10) * 32 + lane;  // GEMM row = pixel of the tile
+  } else {
+    // ------------------------------------------------------------- A builders (warpgroup 0: one pixel per thread)
+    const int row = threadIdx.x;  // GEMM row = pixel of the tile
     const int ly = row / kTileW, lx = row % kTileW;
     int stage = 0;
     uint32_t phase = 0;
     const size_t plane_sz = static_cast<size_t>(p.h) * p.w;
     // Register double buffering: the 27 taps of the NEXT tile are requested before the current tile is converted and
-    // written, so the global-load latency (the builders handle one tile at a time) overlaps the shared-memory work
-    // and the wait for a free stage instead of being paid once per tile.
+    // written, so the global-load latency overlaps the shared-memory work and the wait for a free stage.
     auto load_tile = [&](int tile, float (&v)[27]) {
       int nb, tx, ty, img;
       decode_tile(p, tile, nb, tx, ty, img);
@@ -192,13 +162,6 @@ conv_first_tc_kernel(const float* __restrict__ x, const float* __restrict__ wgt,
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 128);
-  }
 }
 
 int conv_first_tc_launch(const float* x, const float* w_oihw, const float* bias, void* y_hi, void* y_lo, int n, int h,
@@ -216,18 +179,13 @@ int conv_first_tc_launch(const float* x, const float* w_oihw, const float* bias,
   a.flags = flags;
   ConvParams p;
   fill_conv_params(p, &a, 64);
-  CUtensorMap my_hi, my_lo;
-  {
-    int rc = encode_output_maps(&my_hi, &my_lo, &a);
-    if (rc) return rc;
-  }
   const bool fast = (flags & OSVOS_FLAG_FAST) != 0;
   auto kern = fast ? conv_first_tc_kernel<1> : conv_first_tc_kernel<2>;
   static uint64_t attr_done[2] = {0, 0};   // per instantiation: bit d = device d has the shared-memory opt-in
   OSVOS_CHECK_CUDA(ensure_dynamic_smem(kern, kFirstSmem, &attr_done[fast ? 1 : 0]));
   const int sms = device_sm_count();
   const int grid = p.total_tiles < sms ? p.total_tiles : sms;
-  OSVOS_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kFirstTcThreads), kFirstSmem, stream, x, w_oihw, my_hi, my_lo, p));
+  OSVOS_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kConvThreads), kFirstSmem, stream, x, w_oihw, p));
   return OSVOS_OK;
 }
 

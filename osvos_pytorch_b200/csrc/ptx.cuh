@@ -1,11 +1,12 @@
-// Thin inline-PTX wrappers for the sm_100a features the OSVOS kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM alloc / ld / commit).
-// Hand-written; encodings follow the PTX ISA 8.7 tcgen05 chapter (smem matrix
-// descriptor, instruction descriptor) as summarised in DESIGN.md section 4.
+// Thin inline-PTX wrappers for the sm_90a features the OSVOS kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma descriptors (wgmma.cuh holds the MMA itself).
+// Hand-written; encodings follow the PTX ISA chapter on warpgroup-level matrix multiply.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "wgmma.cuh"
 
 namespace osvos {
 
@@ -38,22 +39,6 @@ __device__ __forceinline__ bool elect_one() {
 // every block of this grid has issued it (they then park in their own pdl_wait()).
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
-// 256-bit global store (sm_100: STG.E.ENL2.256): one full 32-byte sector per lane and instruction.  `p` must be
-// 32-byte aligned.
-__device__ __forceinline__ void st_global_256(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t e,
-                                              uint32_t f, uint32_t g, uint32_t h) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(a), "r"(b), "r"(c), "r"(d),
-               "r"(e), "r"(f), "r"(g), "r"(h)
-               : "memory");
-}
-
-// 256-bit read-only global load (LDG.E.ENL2.256.CONSTANT).  `p` must be 32-byte aligned.
-__device__ __forceinline__ void ld_global_nc_256(const void* p, uint32_t (&v)[8]) {
-  asm volatile("ld.global.nc.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "l"(p));
-}
 
 // ----------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -165,159 +150,40 @@ __device__ __forceinline__ void tma_store_wait_all() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// Whole warp. Writes the TMEM base address of `cols` columns to *dst (smem).
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst)), "r"(cols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; one thread issues.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrives once on `bar` when every tcgen05.mma issued so far by this thread has
-// completed (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives row
-// (lane_base + i), columns [col, col+32).  taddr = (lane << 16) | col.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
 // --------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor (64 bit):
+// wgmma shared-memory matrix descriptor (64 bit):
 //   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset>>4 [46,48) version = 1 on sm_100
-//   [49,52) base offset               [61,64) layout: 0 none, 2 SW128, 4 SW64, 6 SW32
-enum : uint64_t { kLayoutNone = 0, kLayoutSW128 = 2, kLayoutSW64 = 4, kLayoutSW32 = 6 };
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint64_t layout, uint32_t base_offset = 0) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= 1ull << 46;
-  d |= static_cast<uint64_t>(base_offset & 7) << 49;
-  d |= layout << 61;
-  return d;
+//   [32,46) stride-dim byte offset>>4 [49,52) base offset (0: the swizzle follows the absolute address)
+//   [62,64) layout: 0 none, 1 SW128, 2 SW64, 3 SW32
+// Descriptors are advanced by ADDING (bytes >> 4): shared-memory addresses stay below 2^18, so the add never carries out
+// of the start-address field.
+constexpr uint64_t kDescSW128 = 1ull << 62;
+constexpr uint64_t kDescSW64 = 2ull << 62;
+__host__ __device__ constexpr uint64_t desc_template(uint32_t lbo_bytes, uint32_t sbo_bytes, uint64_t layout) {
+  return (static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16) | (static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32) |
+         layout;
 }
-// Instruction descriptor for kind::f16 with fp32 accumulation:
-//   [4,6) D fmt (1 = f32)  [7,10) A fmt  [10,13) B fmt (0 = f16, 1 = bf16)
-//   [15] A major (0 = K)   [16] B major   [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_f16(int m, int n, bool bf16, bool a_mn_major = false,
-                                                      bool b_mn_major = false) {
-  return (1u << 4) | ((bf16 ? 1u : 0u) << 7) | ((bf16 ? 1u : 0u) << 10) | ((a_mn_major ? 1u : 0u) << 15) |
-         ((b_mn_major ? 1u : 0u) << 16) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
+__device__ __forceinline__ uint64_t make_smem_desc(const void* p, uint32_t lbo_bytes, uint32_t sbo_bytes, uint64_t layout) {
+  return desc_template(lbo_bytes, sbo_bytes, layout) | static_cast<uint64_t>((smem_u32(p) >> 4) & 0x3FFF);
 }
 
-}  // namespace osvos
+// Named barrier over `nthreads` threads (a multiple of 32) of the CTA; ids 1.. (0 is __syncthreads).
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
-// ===================== cluster / cta_group::2 (CTA pair) primitives =====================
-namespace osvos {
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the same smem offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t local_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx_cluster(uint32_t bar_cluster_addr, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.release.cluster.shared::cluster.b64 _, [%0], %1;" ::"r"(bar_cluster_addr),
-               "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster_addr) : "memory");
-}
-// TMA loads whose completion is signalled on a barrier that may live in the peer CTA of the pair
-__device__ __forceinline__ void tma_load_4d_2sm(const CUtensorMap* m, uint32_t bar_cluster_addr, void* dst, int c0,
-                                                int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2),
-      "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2sm(const CUtensorMap* m, uint32_t bar_cluster_addr, void* dst, int c0,
-                                                int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* dst, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst)), "r"(cols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t addr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
-}
-// D[tmem, 256 rows over the CTA pair] (+)= A * B; issued by one thread of the leader CTA.
-__device__ __forceinline__ void umma_f16_2cta(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (once all prior MMAs of this thread completed) on the barrier at this smem offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(mask)
-      : "memory");
-}
+// Stage bookkeeping of a consumer warpgroup: a shared-memory stage may be handed back to the producer only once the wgmma
+// groups reading it have completed.  With one group in flight (wgmma_wait<1>) that is the PREVIOUS group's stage.
+struct StageRelease {
+  uint64_t* bar_b = nullptr;
+  uint64_t* bar_a = nullptr;
+  __device__ __forceinline__ void release(bool leader) {
+    if (leader) {
+      if (bar_b) mbar_arrive(bar_b);
+      if (bar_a) mbar_arrive(bar_a);
+    }
+    bar_b = bar_a = nullptr;
+  }
+};
 
 }  // namespace osvos

@@ -73,18 +73,17 @@ int encode_tensor_map(CUtensorMap* map, CUtensorMapDataType dtype, int elem_byte
 int device_sm_count() {
   static int sms[64];
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (sms[dev] == 0) {
     int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
     sms[dev] = v;
   }
   return sms[dev];
 }
 
 // Programmatic dependent launch: process default from OSVOS_PDL (read once), overridden per call sequence by
-// osvos_set_pdl() - the engine switches it on around the inference pass (measured +1.4 % there, -1.7 % on the fwd+bwd
-// graph: profiles/r01f_pdl_ab.txt).  A captured graph keeps the attribute its launches were captured with.
+// osvos_set_pdl() - the engine switches it on around the inference pass.  A captured graph keeps the attribute its launches were captured with.
 static int g_pdl_override = -1;   // -1: environment default
 bool pdl_enabled() {
   if (g_pdl_override >= 0) return g_pdl_override == 1;

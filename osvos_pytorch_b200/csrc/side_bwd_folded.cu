@@ -35,9 +35,6 @@ constexpr int kSwSlab = 128;
 // 28 x 128-channel tile of each bf16 plane by ONE 2-D TMA box (the map is a [pixels, C] matrix), the 3 x 30 window of
 // dpq by 8-byte cp.async copies that arrive on the same barrier.  Compute warp w takes pixels 4w .. 4w+3 of the chunk: its lane holds four
 // channels x 18 accumulators; per pixel it reads 8 + 8 bytes of x and nine float2 of the window from shared memory.
-// (History, stage-2 map of 52 MB at 480p: per-warp row segments with register prefetch, a dpq column and one pixel
-// loaded per iteration: 54 us; window in shared memory + the next four pixels in flight: 44 us - 4,700 concurrent
-// 256-byte streams kept DRAM at 1.3 TB/s with 2.5 us of load latency (profiles/r02l_ncu_side_folded_wgrad_v2.txt).)
 constexpr int kSwChunk = 28;                       // pixels per chunk: four per compute warp
 constexpr int kSwStages = 4;
 constexpr int kSwTileBytes = kSwChunk * kSwSlab * 2;          // one plane: 8 KiB
@@ -57,7 +54,7 @@ static_assert(kSwDataBytes % 8 == 0 && ((2 * kSwComputeWarps + 2) * 4) % 8 == 0,
 
 // Up to four SCALES per launch (the backward runs the four side branches' G kernels as one): the grid is cut into one
 // block range per scale, sized by the scale's chunk count, so the fixed cost of a launch (first tile's latency, block
-// reduction, atomics: ~9 us of a 10 us launch on the 30 x 54 map) is paid once.
+// reduction, atomics: most of a launch on the small maps) is paid once.
 constexpr int kSwMaxScales = 4;
 struct SwScale {
   const float* dpq;
@@ -117,8 +114,8 @@ side_folded_wgrad_kernel(const __grid_constant__ SwMaps maps, const __grid_const
     // Per chunk and stage: the 3 x 30 window of dpq by 8-byte cp.async with zero fill outside the image (window entry
     // idx = r * 30 + k <-> dpq[(y + 1 - r, x0 - 1 + k)]; up to kSwWinPerLane entries per lane), each lane's copies arriving
     // on the stage's full barrier when they land, and the two x tiles by TMA - nothing here waits for memory, so all four
-    // stages are in flight.  (With the window prefetched ONE chunk ahead into registers the producer handed over one chunk
-    // per load latency: 34 us for the stage-2 map.)
+    // stages are in flight.  (With the window prefetched ONE chunk ahead into registers the producer would hand over one
+    // chunk per load latency.)
     int stage = 0;
     uint32_t phase = 0;
     for (int ci = blk; ci < chunks; ci += nblk) {

@@ -1,10 +1,10 @@
 // side_prep: 3x3 convolution C -> 16 (no ReLU) + the fused 1x1 projections, with the NINE TAPS CONCATENATED ALONG N.
 //
-// With N = 16 a tcgen05.mma still costs its ~85-cycle floor, and the generic kernel issues one per (tap, K step, pass):
-// the four side convolutions took 137 us of a 866 us frame at 9-14 % tensor activity.  Here the GEMM is turned around:
+// With N = 16 the generic kernel would issue one small MMA per (tap, K step, pass).  Here the GEMM is turned around:
 //   Y[p][tap*16 + co] = sum_ci X[p][ci] * W[tap][co][ci]        p = pixel of the UNSHIFTED halo patch
 // i.e. ONE MMA of N = 144 per K step and pass (A = the 12 x 10-pixel halo patch of a 10 x 8 output tile, 120 of the 128
-// GEMM rows; B = all nine 16 x 64 weight slabs of the chunk, one TMA box {64, 16, 9}), 9x fewer instructions.  The
+// GEMM rows, 64 per consumer warpgroup; B = all nine 16 x 64 weight slabs of the chunk, one TMA box {64, 16, 9}), 9x
+// fewer instructions.  The
 // spatial shift moves to the epilogue: out[y][x][co] = sum_{r,s} Y[(y + r) * 10 + (x + s)][(3r + s) * 16 + co], done
 // through a shared-memory exchange in three deterministic rounds (one tap row each).
 //
@@ -15,8 +15,7 @@
 // (score_dsn, this scale's slice of fuse) is ONE linear 3x3 convolution C -> 2 whose weights are
 // W'[o][ci][tap] = sum_co proj[o][co] * W_side[co][ci][tap] (osvos_fold_side_weights).  The same kernel then runs with
 // N = 32 (18 used) instead of 144: 1/8 of the accumulator columns to exchange, 1/4.5 of the weight bytes to stream,
-// a third less tensor time - the side branch was bound by exactly those (shared-memory bandwidth: the N = 144 MMA alone
-// reads 120 B/clk of operands).  The backward of the folded form needs no features either (side_bwd_folded.cu); NCO = 16 stays
+// a third less tensor time.  The backward of the folded form needs no features either (side_bwd_folded.cu); NCO = 16 stays
 // for osvos_conv3x3 calls with cout == 16 (the literal side_prep op).
 #include <string.h>
 
@@ -26,7 +25,7 @@ namespace osvos {
 
 constexpr int kSideTileW = 8, kSideTileH = 10;              // output tile
 constexpr int kSideHaloW = 10, kSideHaloH = 12;             // 120 halo pixels = GEMM rows
-constexpr int kSideThreads = 192;                           // warp 0 TMA, warp 1 MMA, warps 2-5 epilogue
+constexpr int kSideThreads = 384;                           // warp 0 TMA, warpgroups 1-2 wgmma + epilogue
 constexpr int kSideABox = kSideHaloW * kSideHaloH * 128;    // 15360 B
 constexpr int kSideAPlane = 128 * 128;                      // the MMA reads 128 rows
 
@@ -61,8 +60,8 @@ struct SideCfg {
   static constexpr int kBBox = 9 * NCO * 128;                 // bytes the weight box of one chunk and plane delivers
   static constexpr int kBPlane = kN * 128;                    // 18432 / 4096 B: what the MMA reads (1 KiB multiple)
   static constexpr int kBStages = NCO == 16 ? 3 : 6;
-  // activation ring: the folded kernel's step is ~600 cycles of MMA per 30 KiB chunk, far below the latency of the
-  // chunk's TMA load - it needs loads of several chunks in flight (measured with 2 stages: 21 us for a 52 MB input)
+  // activation ring: the folded kernel's MMA step per 30 KiB chunk is far shorter than the latency of the chunk's TMA
+  // load - it needs loads of several chunks in flight
   static constexpr int kAStages = NCO == 16 ? 2 : 4;
   static constexpr int kAStage = PLANES * kSideAPlane;
   static constexpr int kBStage = PLANES * kBPlane;
@@ -98,9 +97,6 @@ side_conv_kernel(const __grid_constant__ SideMaps maps, const __grid_constant__ 
   uint64_t* a_empty = bars + kSideAStages;
   uint64_t* b_full = a_empty + kSideAStages;
   uint64_t* b_empty = b_full + kSideBStages;
-  uint64_t* tfull_bar = b_empty + kSideBStages;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -112,23 +108,15 @@ side_conv_kernel(const __grid_constant__ SideMaps maps, const __grid_constant__ 
     }
     for (int i = 0; i < kSideAStages; ++i) {
       mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 1);
+      mbar_init(&a_empty[i], 2);   // one arrival per consumer warpgroup
     }
     for (int i = 0; i < kSideBStages; ++i) {
       mbar_init(&b_full[i], 1);
-      mbar_init(&b_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 128);
+      mbar_init(&b_empty[i], 2);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);  // 2 accumulator stages x 144 columns (256-column stride)
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();               // the previous kernel's activations are first read below (ptx.cuh)
   pdl_launch_dependents();
 
@@ -172,47 +160,46 @@ side_conv_kernel(const __grid_constant__ SideMaps maps, const __grid_constant__ 
     }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // MMA issuer: one elected thread for the whole loop
-    if (elect_one()) {
-    constexpr uint32_t idesc = make_idesc_f16(128, kSideN, /*bf16=*/true);
+  } else if (warp >= 4) {
+    // --------------------------------------------- consumer warpgroups: wgmma over 64 halo pixels each, then the shift-add
+    const int wg = (warp - 4) >> 2, wl = warp & 3;
+    const bool leader = (threadIdx.x & 127) == 0;
+    const int ct = threadIdx.x - 128;                          // consumer thread 0 .. 255 (output pixel if < 80)
+    const int oy = ct / kSideTileW, ox = ct % kSideTileW;
+    const int ra = wg * 64 + wl * 16 + (lane >> 2);            // halo pixels of this thread's accumulator rows: ra, ra + 8
+    float acc[kSideN / 2];
     int a_stage = 0, b_stage = 0;
     uint32_t a_phase = 0, b_phase = 0;
     int it = 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
-      const uint32_t aph = (it >> 1) & 1;
-      mbar_wait(&tempty_bar[as], aph ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + as * 256;
-      int sc, tx_, ty_, img_;
-      side_decode(p, tile, sc, tx_, ty_, img_);
-      const int k_chunks = p.sc[sc].k_chunks;
-      for (int kc = 0; kc < k_chunks; ++kc) {
+      int sc, tx, ty, img;
+      side_decode(p, tile, sc, tx, ty, img);
+      const SideScale& L = p.sc[sc];
+#pragma unroll
+      for (int i = 0; i < kSideN / 2; ++i) acc[i] = 0.f;
+      for (int kc = 0; kc < L.k_chunks; ++kc) {
         mbar_wait(&a_full[a_stage], a_phase);
         mbar_wait(&b_full[b_stage], b_phase);
-        tc_fence_after();
-        {
-          const uint32_t a_hi = smem_u32(smem_a + a_stage * Cfg::kAStage);
-          const uint32_t b_hi = smem_u32(smem_b + b_stage * Cfg::kBStage);
-          const uint64_t da_hi = make_smem_desc(a_hi, 16, 1024, kLayoutSW128);
-          const uint64_t da_lo = make_smem_desc(a_hi + kSideAPlane, 16, 1024, kLayoutSW128);
-          const uint64_t db_hi = make_smem_desc(b_hi, 16, 1024, kLayoutSW128);
-          const uint64_t db_lo = make_smem_desc(b_hi + kSideBPlane, 16, 1024, kLayoutSW128);
+        const uint64_t da_hi = make_smem_desc(smem_a + a_stage * Cfg::kAStage + wg * 64 * 128, 16, 1024, kDescSW128);
+        const uint64_t da_lo = da_hi + (kSideAPlane >> 4);
+        const uint64_t db_hi = make_smem_desc(smem_b + b_stage * Cfg::kBStage, 16, 1024, kDescSW128);
+        const uint64_t db_lo = db_hi + (kSideBPlane >> 4);
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t adv = static_cast<uint64_t>(k * 2);
-            if (PLANES == 2) {
-              umma_f16(tmem_d, da_lo + adv, db_hi + adv, idesc, (kc | k) != 0);
-              umma_f16(tmem_d, da_hi + adv, db_lo + adv, idesc, 1);
-              umma_f16(tmem_d, da_hi + adv, db_hi + adv, idesc, 1);
-            } else {
-              umma_f16(tmem_d, da_hi + adv, db_hi + adv, idesc, (kc | k) != 0);
-            }
+        for (int k = 0; k < 4; ++k) {
+          const uint64_t adv = static_cast<uint64_t>(k * 2);
+          if (PLANES == 2) {
+            wgmma_bf16<kSideN>(acc, da_lo + adv, db_hi + adv, 1);
+            wgmma_bf16<kSideN>(acc, da_hi + adv, db_lo + adv, 1);
           }
-          umma_commit(&a_empty[a_stage]);
-          umma_commit(&b_empty[b_stage]);
-          if (kc == k_chunks - 1) umma_commit(&tfull_bar[as]);
+          wgmma_bf16<kSideN>(acc, da_hi + adv, db_hi + adv, 1);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_operands(acc);
+        if (leader) {
+          mbar_arrive(&a_empty[a_stage]);
+          mbar_arrive(&b_empty[b_stage]);
         }
         if (++a_stage == kSideAStages) {
           a_stage = 0;
@@ -223,39 +210,23 @@ side_conv_kernel(const __grid_constant__ SideMaps maps, const __grid_constant__ 
           b_phase ^= 1;
         }
       }
-    }
-    }
-    __syncwarp();
-  } else {
-    // ---------------------------------------------------------------- epilogue: shift-add through shared memory
-    const int q = warp & 3;
-    const int row = q * 32 + lane;                 // halo pixel index (valid < 120) / output thread index (< 80)
-    const int oy = row / kSideTileW, ox = row % kSideTileW;   // as an OUTPUT pixel of the tile (row < 80)
-    int it = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-      int sc, tx, ty, img;
-      side_decode(p, tile, sc, tx, ty, img);
-      const SideScale& L = p.sc[sc];
-      const int as = it & 1;
-      const uint32_t aph = (it >> 1) & 1;
-      mbar_wait(&tfull_bar[as], aph);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + as * 256 + (static_cast<uint32_t>(q * 32) << 16);
+      const int y = ty * kSideTileH + oy, x = tx * kSideTileW + ox;
+      const bool out_ok = ct < kSideTileW * kSideTileH && y < L.h && x < L.w;
+      const size_t pix = (static_cast<size_t>(img) * L.h + y) * L.w + x;
       if constexpr (NCO == 2) {
-        // folded projections: column 2 * tap + o of halo pixel `row`.  One read, accumulator handed back at once, one
-        // exchange through the buffer of this tile's parity (a single barrier per tile), nine float2 gathers.
-        uint32_t v[32];
-        tmem_ld32(taddr, v);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(&tempty_bar[as]);
+        // folded projections: column 2 * tap + o of the halo pixel.  One exchange through the buffer of this tile's
+        // parity (a single barrier per tile: the buffer is next written two tiles later, after the next tile's barrier)
         float2* yb = reinterpret_cast<float2*>(ybuf) + (it & 1) * 9 * 128;
 #pragma unroll
-        for (int tap = 0; tap < 9; ++tap)
-          yb[tap * 128 + row] = make_float2(__uint_as_float(v[2 * tap]), __uint_as_float(v[2 * tap + 1]));
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        const int y = ty * kSideTileH + oy, x = tx * kSideTileW + ox;
-        if (row < kSideTileW * kSideTileH && y < L.h && x < L.w) {
+        for (int j = 0; j < kSideN / 8; ++j) {
+          const int tap = 4 * j + (lane & 3);                  // columns 8j + 2 (lane % 4) + {0, 1}
+          if (tap < 9) {
+            yb[tap * 128 + ra] = make_float2(acc[4 * j], acc[4 * j + 1]);
+            yb[tap * 128 + ra + 8] = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+          }
+        }
+        named_bar_sync(1, 256);
+        if (out_ok) {
           float sp = L.bias ? __ldg(L.bias) : 0.f, sq = L.bias ? __ldg(L.bias + 1) : 0.f;
 #pragma unroll
           for (int tap = 0; tap < 9; ++tap) {
@@ -263,69 +234,58 @@ side_conv_kernel(const __grid_constant__ SideMaps maps, const __grid_constant__ 
             sp += t.x;
             sq += t.y;
           }
-          const size_t pix = (static_cast<size_t>(img) * L.h + y) * L.w + x;
           *reinterpret_cast<float2*>(L.pq + pix * 2) = make_float2(sp, sq);
         }
         continue;
       }
-      float acc[16];
+      float o[16];
 #pragma unroll
-      for (int j = 0; j < 16; ++j) acc[j] = L.bias ? __ldg(L.bias + j) : 0.f;
-#pragma unroll 1
+      for (int j = 0; j < 16; ++j) o[j] = L.bias ? __ldg(L.bias + j) : 0.f;
+#pragma unroll
       for (int r = 0; r < 3; ++r) {
-        // (1) every halo-pixel thread publishes its three taps of row r: ybuf[s][co][pixel]
+        // (1) every halo-pixel row publishes its three taps of row r: ybuf[s][co][pixel]
 #pragma unroll
-        for (int s = 0; s < 3; ++s) {
-          uint32_t v[16];
-          tmem_ld16(taddr + (r * 3 + s) * 16, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int co = 0; co < 16; ++co) ybuf[(s * 16 + co) * 128 + row] = __uint_as_float(v[co]);
+        for (int j = 6 * r; j < 6 * r + 6; ++j) {
+          const int c = 8 * j + 2 * (lane & 3);
+          const int s = c / 16 - 3 * r, co = c % 16;
+          ybuf[(s * 16 + co) * 128 + ra] = acc[4 * j];
+          ybuf[(s * 16 + co + 1) * 128 + ra] = acc[4 * j + 1];
+          ybuf[(s * 16 + co) * 128 + ra + 8] = acc[4 * j + 2];
+          ybuf[(s * 16 + co + 1) * 128 + ra + 8] = acc[4 * j + 3];
         }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
+        named_bar_sync(1, 256);
         // (2) output-pixel threads gather: halo pixel (oy + r, ox + s)
-        if (row < kSideTileW * kSideTileH) {
+        if (ct < kSideTileW * kSideTileH) {
 #pragma unroll
           for (int s = 0; s < 3; ++s) {
             const int src = (oy + r) * kSideHaloW + ox + s;
 #pragma unroll
-            for (int co = 0; co < 16; ++co) acc[co] += ybuf[(s * 16 + co) * 128 + src];
+            for (int co = 0; co < 16; ++co) o[co] += ybuf[(s * 16 + co) * 128 + src];
           }
         }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
+        named_bar_sync(1, 256);
       }
-      tc_fence_before();
-      mbar_arrive(&tempty_bar[as]);
-      const int y = ty * kSideTileH + oy, x = tx * kSideTileW + ox;
-      if (row < kSideTileW * kSideTileH && y < L.h && x < L.w) {
-        const size_t pix = (static_cast<size_t>(img) * L.h + y) * L.w + x;
+      if (out_ok) {
         if (L.relu) {
 #pragma unroll
-          for (int j = 0; j < 16; ++j) acc[j] = fmaxf(acc[j], 0.f);
+          for (int j = 0; j < 16; ++j) o[j] = fmaxf(o[j], 0.f);
         }
         if (L.y_f32) {
           float4* dst = reinterpret_cast<float4*>(L.y_f32 + pix * 16);
 #pragma unroll
-          for (int j = 0; j < 4; ++j) dst[j] = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
+          for (int j = 0; j < 4; ++j) dst[j] = make_float4(o[4 * j], o[4 * j + 1], o[4 * j + 2], o[4 * j + 3]);
         }
         if (L.pq) {
           float sp = L.proj_b ? __ldg(L.proj_b) : 0.f, sq = 0.f;
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
-            sp = fmaf(acc[j], __ldg(L.proj_w + j), sp);
-            sq = fmaf(acc[j], __ldg(L.proj_w + 16 + j), sq);
+            sp = fmaf(o[j], __ldg(L.proj_w + j), sp);
+            sq = fmaf(o[j], __ldg(L.proj_w + 16 + j), sq);
           }
           *reinterpret_cast<float2*>(L.pq + pix * 2) = make_float2(sp, sq);
         }
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 

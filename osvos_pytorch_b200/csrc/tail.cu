@@ -48,8 +48,7 @@ __device__ __forceinline__ float softplus_f(float x) { return fmaxf(x, 0.f) + lo
 // are blended into shared memory, v_k[c] = wy0 * pq_k[ay - 1][c] + wy1 * pq_k[ay][c] (806 float2 for a 854-pixel row).
 // Phase 2: a thread takes four consecutive pixels (shifted so that the four are a 16-byte aligned group of the flat map
 // whatever the row length) and blends HORIZONTALLY from shared memory: two LDS.64 and four FMAs per scale and pixel.
-// (The first version did the full 2 x 2 gather with its index arithmetic per pixel and scale: ~850 instructions per
-// pixel group, 14 us for a 480 x 854 frame whose 9.3 MB would take 1.5 us at the HBM roof.)
+// (The full 2 x 2 gather with its index arithmetic per pixel and scale costs ~850 instructions per pixel group.)
 __global__ void __launch_bounds__(kTailThreads) tail_fwd_kernel(const TailParams p) {
   extern __shared__ float2 vbuf[];     // [scale 0 .. 3][wk_k] vertically blended (p, q)
   pdl_wait();               // side maps, biases and the accumulators all come from earlier kernels (ptx.cuh)
@@ -276,7 +275,7 @@ __global__ void __launch_bounds__(256) tail_bwd2_kernel(const __grid_constant__ 
       const bool xin = x >= 0 && x < p.w;
       float ap = 0.f, aq = 0.f;
       // four source rows per step with all their loads issued before the first use: the row loop is a chain of
-      // dependent global loads otherwise (16 round trips for s = 16: the first version took 37 us in LOSS mode)
+      // dependent global loads otherwise (16 round trips for s = 16)
       for (int t0 = r; t0 < fs; t0 += 4 * rgroups) {
         float fyv[4], lv[4], pv[4], qv[4];
 #pragma unroll

@@ -1,4 +1,4 @@
-// Weight gradient of the 3x3 convolutions as a tcgen05 GEMM whose reduction
+// Weight gradient of the 3x3 convolutions as a wgmma GEMM whose reduction
 // dimension is the PIXEL axis:
 //
 //   ws[tap][m][n] += sum_px P[px (+tap)][m] * Q[px (+tap)][n]
@@ -7,17 +7,17 @@
 // activation shifted by the tap (n = ci).  (side_prep's weight gradient is not a GEMM
 // of this shape any more: side_bwd_folded.cu.)  Both operands are
 // NHWC acts, i.e. the reduction index (pixel) is the strided one: they are
-// "MN-major" UMMA operands.  A K block is a patch of 8 x 8 pixels; its TMA box
+// "MN-major" (transposed) wgmma operands.  A K block is a patch of 8 x 8 pixels; its TMA box
 // {64 ch, 8 px, 8 rows, 1} lands as 64 rows x 128 B (SWIZZLE_128B), which is the
 // canonical MN-major SW128 atom layout (64 MN elements x 8 K rows per atom,
 // SBO = 1024 B between K groups, LBO = 8192 B between 64-wide MN atoms).
 // Out-of-image pixels are zero-filled by TMA: they are both the conv padding of
 // the shifted operand and the ragged-edge mask of the unshifted one.
 //
-// Work item = (m block of 128, n block, tap, pixel-range split); the fp32 TMEM
-// accumulator is flushed with vector atomics (red.global.add.v4.f32) into the
-// zero-initialised workspace, which a small kernel then transposes into the
-// OIHW gradient.  Same warp roles / mbarrier pipeline as conv3x3_tc.cu.
+// Work item = (m block of 128, n block, tap, pixel-range split); each of the two
+// consumer warpgroups accumulates 64 of the 128 m rows in registers and flushes
+// them with vector atomics (red.global.add.v2.f32) into the zero-initialised
+// workspace, which a small kernel then transposes into the OIHW gradient.
 //
 // Replaces autograd's weight gradient of nn.Conv2d(k=3, p=1)
 // (reference networks/vgg_osvos.py:41,142; backward triggered at train_online.py:141).
@@ -28,7 +28,7 @@
 
 namespace osvos {
 
-constexpr int kWgThreads = 224;   // warp 0: P producer, 1: MMA, 2-5: epilogue, 6: Q producer
+constexpr int kWgThreads = 384;   // warp 0: P producer, warp 1: Q producer, warpgroups 1-2: wgmma + flush
 constexpr int kWgPatchW = 8, kWgPatchH = 8;
 constexpr int kWgBlockK = 64;                  // pixels per K block
 constexpr int kWgBoxBytes = kWgBlockK * 128;   // 8 KiB: 64 pixels x 64 channels of bf16
@@ -53,11 +53,10 @@ struct WgCfg {
   static constexpr int kStagesRaw = (212 * 1024) / kStageBytes;
   static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
   // Exact mode: N-concatenated split-Q.  The hi and lo planes of the Q tile are contiguous (uniform LBO between
-  // the 64-wide MN atoms), so one tcgen05.mma of N = 2 * BLOCK_N yields [P_hi.Q_hi | P_hi.Q_lo]; with P_lo.Q_hi
+  // the 64-wide MN atoms), so one wgmma of N = 2 * BLOCK_N yields [P_hi.Q_hi | P_hi.Q_lo]; with P_lo.Q_hi
   // that is 2 instructions per K step instead of 3 (see conv3x3_halo.cu).  The epilogue adds the two halves.
   static constexpr bool kSplitAcc = (PLANES == 2) && (BLOCK_N <= 128);
   static constexpr int kAccCols = kSplitAcc ? 2 * BLOCK_N : BLOCK_N;
-  static constexpr int kTmemCols = 2 * kAccCols < 32 ? 32 : 2 * kAccCols;
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 256;
   // descriptors are formed by adding (bytes >> 4) to a base descriptor (see conv3x3_halo.cu): stay inside the field
   static_assert(kSmemBytes <= 227 * 1024 && kSmemBytes + 8192 < (1 << 18), "shared memory / descriptor address field");
@@ -84,9 +83,6 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_p_hi, const __grid_const
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kStages;
-  uint64_t* tfull_bar = bars + 2 * kStages;
-  uint64_t* tempty_bar = bars + 2 * kStages + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -96,26 +92,17 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_p_hi, const __grid_const
     tma_prefetch_desc(&map_q_hi);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 2);   // one arrive.expect_tx from each of the two producer warps
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 128);
+      mbar_init(&empty_bar[i], 2);  // one arrival per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, Cfg::kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();               // dz / x come from the previous kernels of the stream (ptx.cuh)
   pdl_launch_dependents();
 
-  if (warp == 0 || warp == 6) {
-    // two producer warps (P operand: warp 0, Q operand: warp 6) halve the per-K-block TMA issue time.  ONE elected
-    // thread per warp runs the whole loop (no per-step ELECT / reconvergence - see conv3x3_halo.cu); the patch
-    // coordinates advance incrementally instead of by two integer divisions per K block.
+  if (warp == 0 || warp == 1) {
+    // two producer warps (P operand: warp 0, Q operand: warp 1) halve the per-K-block TMA issue time.  ONE elected
+    // thread per warp runs the whole loop; the patch coordinates advance incrementally.
     if (elect_one()) {
       const bool load_p = (warp == 0);
       int stage = 0;
@@ -185,120 +172,92 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_p_hi, const __grid_const
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // MMA issuer: one elected thread, descriptors formed by adding the stage offset to a constant template
-    if (elect_one()) {
-      constexpr uint32_t idesc = make_idesc_f16(128, BLOCK_N, true, /*a_mn=*/true, /*b_mn=*/true);
-      constexpr uint32_t idesc2 = make_idesc_f16(128, Cfg::kAccCols, true, /*a_mn=*/true, /*b_mn=*/true);
-      // MN-major SW128: LBO = bytes between 64-wide MN atoms, SBO = bytes between 8-row K groups
-      constexpr uint64_t kDesc = (static_cast<uint64_t>(kWgBoxBytes >> 4) << 16) | (static_cast<uint64_t>(1024 >> 4) << 32) |
-                                 (1ull << 46) | (static_cast<uint64_t>(kLayoutSW128) << 61);
-      constexpr uint32_t kQOff = (PLANES * Cfg::kPBytes) >> 4, kPLo = Cfg::kPBytes >> 4, kQLo = Cfg::kQBytes >> 4;
-      const uint32_t smem_base = smem_u32(smem);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int item = blockIdx.x; item < p.total_items; item += gridDim.x, ++it) {
-        int mb, nb, tap, split;
-        wg_decode_item(p, item, mb, nb, tap, split);
-        const int pb = split * p.patches_per_split;
-        int pe = pb + p.patches_per_split;
-        if (pe > p.patches_total) pe = p.patches_total;
-        const int as = it & 1;
-        const uint32_t aph = (it >> 1) & 1;
-        mbar_wait(&tempty_bar[as], aph ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * Cfg::kAccCols;
-        for (int patch = pb; patch < pe; ++patch) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t dp_hi = kDesc | static_cast<uint64_t>((smem_base + stage * Cfg::kStageBytes) >> 4);
-          const uint64_t dq_hi = dp_hi + kQOff;
-          const uint64_t dp_lo = dp_hi + kPLo;
-          const uint64_t dq_lo = dq_hi + kQLo;
-#pragma unroll
-          for (int k = 0; k < kWgBlockK / 16; ++k) {
-            const uint32_t adv = static_cast<uint32_t>(k * (2048 >> 4));  // 16 pixel rows x 128 B
-            const uint32_t acc = (k != 0) ? 1u : (patch != pb ? 1u : 0u);
-            if (Cfg::kSplitAcc) {
-              umma_f16(tmem_d, dp_hi + adv, dq_hi + adv, idesc2, acc);   // [P_hi.Q_hi | P_hi.Q_lo]
-              umma_f16(tmem_d, dp_lo + adv, dq_hi + adv, idesc, 1);      // + P_lo.Q_hi into the first half
-            } else if (PLANES == 2) {
-              umma_f16(tmem_d, dp_lo + adv, dq_hi + adv, idesc, acc);
-              umma_f16(tmem_d, dp_hi + adv, dq_lo + adv, idesc, 1);
-              umma_f16(tmem_d, dp_hi + adv, dq_hi + adv, idesc, 1);
-            } else {
-              umma_f16(tmem_d, dp_hi + adv, dq_hi + adv, idesc, acc);
-            }
-          }
-          umma_commit(&empty_bar[stage]);
-          if (patch == pe - 1) umma_commit(&tfull_bar[as]);
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp >= 2 && warp < 6) {
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    int it = 0;
-    for (int item = blockIdx.x; item < p.total_items; item += gridDim.x, ++it) {
+  } else if (warp >= 4) {
+    // ------------------------------------------------ consumer warpgroups: M atom wg (64 rows of P) x all BLOCK_N columns
+    const int wg = (warp - 4) >> 2, wl = warp & 3;
+    const bool leader = (threadIdx.x & 127) == 0;
+    // MN-major SW128: LBO = bytes between 64-wide MN atoms, SBO = bytes between 8-row K groups
+    constexpr uint64_t kDesc = desc_template(kWgBoxBytes, 1024, kDescSW128);
+    constexpr uint32_t kQOff = (PLANES * Cfg::kPBytes) >> 4, kPLo = Cfg::kPBytes >> 4, kQLo = Cfg::kQBytes >> 4;
+    const uint32_t smem_base = smem_u32(smem);
+    float acc[Cfg::kAccCols / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    StageRelease pending;
+    for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
       int mb, nb, tap, split;
       wg_decode_item(p, item, mb, nb, tap, split);
-      const int as = it & 1;
-      const uint32_t aph = (it >> 1) & 1;
-      const int m = mb * 128 + row;
-      mbar_wait(&tfull_bar[as], aph);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + as * Cfg::kAccCols + (static_cast<uint32_t>(q * 32) << 16);
-#pragma unroll 1
-      for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
-        // destination of this 32-column chunk: channel block nb, or (tap_pairs) tap 2g + c0/64 of the 64 channels, or
-        // (tap_rows) the tap = shift of the N atom minus shift of the M atom: (M0,N0) -> s = 1, (M0,N1) -> s = 2,
-        // (M1,N0) -> s = 0, (M1,N1) -> s = 1 again (discarded)
-        int tap_c = p.tap_pairs ? 2 * tap + (c0 >> 6) : tap;
-        bool chunk_ok = tap_c < 9;
-        int m_out = m;
-        if (p.tap_rows) {
-          const int pj = row >> 6, qj = c0 >> 6;
-          chunk_ok = !(pj && qj);
-          tap_c = 3 * tap + (pj ? 0 : 1 + qj);
-          m_out = row & 63;
-        }
-        float* dst = p.ws + (static_cast<size_t>(chunk_ok ? tap_c : 0) * p.m_total + m_out) * p.n_total +
-                     ((p.tap_pairs || p.tap_rows) ? -(c0 & ~63) : nb * BLOCK_N);
-        uint32_t v[32], v2[32];
-        tmem_ld32(taddr + c0, v);
-        if (Cfg::kSplitAcc) tmem_ld32(taddr + BLOCK_N + c0, v2);
-        tmem_ld_wait();
-        if ((m < p.m_valid || p.tap_rows) && chunk_ok) {
+      const int pb = split * p.patches_per_split;
+      int pe = pb + p.patches_per_split;
+      if (pe > p.patches_total) pe = p.patches_total;
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4 val = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
-                                     __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
+      for (int i = 0; i < Cfg::kAccCols / 2; ++i) acc[i] = 0.f;
+      for (int patch = pb; patch < pe; ++patch) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint64_t dq_hi = kDesc | static_cast<uint64_t>((smem_base + stage * Cfg::kStageBytes) >> 4) + kQOff;
+        const uint64_t dp_hi = kDesc | static_cast<uint64_t>((smem_base + stage * Cfg::kStageBytes + wg * kWgBoxBytes) >> 4);
+        const uint64_t dp_lo = dp_hi + kPLo;
+        const uint64_t dq_lo = dq_hi + kQLo;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kWgBlockK / 16; ++k) {
+          const uint32_t adv = static_cast<uint32_t>(k * (2048 >> 4));  // 16 pixel rows x 128 B
+          if constexpr (Cfg::kSplitAcc) {
+            wgmma_bf16<Cfg::kAccCols, 1, 1>(acc, dp_hi + adv, dq_hi + adv, 1);   // [P_hi.Q_hi | P_hi.Q_lo]
+            wgmma_bf16<BLOCK_N, 1, 1>(acc, dp_lo + adv, dq_hi + adv, 1);         // + P_lo.Q_hi into the first half
+          } else if constexpr (PLANES == 2) {
+            wgmma_bf16<BLOCK_N, 1, 1>(acc, dp_lo + adv, dq_hi + adv, 1);
+            wgmma_bf16<BLOCK_N, 1, 1>(acc, dp_hi + adv, dq_lo + adv, 1);
+            wgmma_bf16<BLOCK_N, 1, 1>(acc, dp_hi + adv, dq_hi + adv, 1);
+          } else {
+            wgmma_bf16<BLOCK_N, 1, 1>(acc, dp_hi + adv, dq_hi + adv, 1);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                 // the previous patch's group is done: its stage may be refilled
+        pending.release(leader);
+        pending.bar_b = &empty_bar[stage];
+        if (++stage == kStages) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_operands(acc);
+      pending.release(leader);
+      // flush: thread holds rows ra, ra + 8 (of this warpgroup's 64) and the column pairs 8j + 2 (lane % 4)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = wg * 64 + wl * 16 + (lane >> 2) + 8 * h;   // 0 .. 127 within the item
+        const int m = mb * 128 + row;
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          const int c = 8 * j + 2 * (lane & 3);
+          // destination column c: channel block nb, or (tap_pairs) tap 2g + c/64 of the 64 channels, or (tap_rows) the
+          // tap = shift of the N atom minus shift of the M atom: (M0,N0) -> s = 1, (M0,N1) -> s = 2, (M1,N0) -> s = 0,
+          // (M1,N1) -> s = 1 again (discarded)
+          int tap_c = p.tap_pairs ? 2 * tap + (c >> 6) : tap;
+          bool chunk_ok = tap_c < 9;
+          int m_out = m;
+          if (p.tap_rows) {
+            const int pj = row >> 6, qj = c >> 6;
+            chunk_ok = !(pj && qj);
+            tap_c = 3 * tap + (pj ? 0 : 1 + qj);
+            m_out = row & 63;
+          }
+          if ((m < p.m_valid || p.tap_rows) && chunk_ok) {
+            float* dst = p.ws + (static_cast<size_t>(tap_c) * p.m_total + m_out) * p.n_total +
+                         ((p.tap_pairs || p.tap_rows) ? -(c & ~63) : nb * BLOCK_N) + c;
+            float2 val = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
             if (Cfg::kSplitAcc) {
-              val.x += __uint_as_float(v2[4 * j]);
-              val.y += __uint_as_float(v2[4 * j + 1]);
-              val.z += __uint_as_float(v2[4 * j + 2]);
-              val.w += __uint_as_float(v2[4 * j + 3]);
+              val.x += acc[BLOCK_N / 2 + 4 * j + 2 * h];
+              val.y += acc[BLOCK_N / 2 + 4 * j + 2 * h + 1];
             }
-            atomicAdd(reinterpret_cast<float4*>(dst + c0 + 4 * j), val);
+            atomicAdd(reinterpret_cast<float2*>(dst), val);
           }
         }
       }
-      tc_fence_before();
-      mbar_arrive(&tempty_bar[as]);
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
   }
 }
 
@@ -403,10 +362,10 @@ static int launch_wgrad(const osvos_wgrad_args* a, cudaStream_t stream) {
   p.n_total = cq;
   p.m_blocks = (cp + 127) / 128;
   // Cin = 64 trunk layers (conv1_2, conv2_1): the 128-wide item holds two TAPS of the single 64-channel block, which
-  // halves the number of tcgen05.mma (the ~85-cycle instruction floor makes N = 64 items twice as expensive per flop)
+  // halves the number of MMA instructions
   // Cin = Cout = 64 (conv1_2): an item is a tap ROW r.  M = [dz | dz shifted by (0,+1)], N = [x shifted by (r-1, 0) |
   // x shifted by (r-1, +1)]: the four 64 x 64 quadrants are the taps s = 1, 2, 0 and 1 again - three of four useful
-  // instead of the two of four of tap pairs under a half-empty M (a tcgen05.mma costs max(M, 128) rows either way).
+  // instead of the two of four of tap pairs under a half-empty M.
   // Exact at the borders: the terms dz[u] x[u + (., -1)] the shifted M atom cannot reach (u.x = 0) multiply the zero
   // padding of x, and everything out of the image is zero-filled by TMA on both operands.
   static int rows_on = -1;   // OSVOS_WGRAD_ROWS=0: tap pairs instead (A/B; read once)
@@ -426,8 +385,7 @@ static int launch_wgrad(const osvos_wgrad_args* a, cudaStream_t stream) {
   // Pixel-range splits: items are dealt round-robin to the persistent CTAs, so the kernel lasts as long as the CTA with
   // the most items - ROUNDS x K blocks per item.  Pick the split count that minimises that (plus ~2 K-block times per
   // item for the accumulator flush that is not hidden behind the next item's MMAs).  The first rule, ceil(2 SMs /
-  // tiles), landed just ABOVE two full rounds for most layers (297 items on 148 CTAs: a third round for one item,
-  // 67 % of the tensor time) - profiles/r02l_*.
+  // tiles), can land just above a whole number of rounds (one extra round for a single item).
   const int max_splits = (p.patches_total + 3) / 4;
   static int split_rule = -1;   // OSVOS_WGRAD_SPLITS=legacy: the first rule (A/B; read once)
   if (split_rule < 0) {

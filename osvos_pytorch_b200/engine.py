@@ -149,7 +149,7 @@ class OSVOSEngine:
                 if tuple(w.shape[2:]) != (2 ** (i + 2),) * 2 or not torch.equal(w.detach().float(), ref):
                     raise NotImplementedError(
                         f"{name}.{i}.weight is not the fixed bilinear interpolation kernel written by interp_surgery; "
-                        "the B200 path only implements that (reference layers/osvos_layers.py:72-85)")
+                        "the native path only implements that (reference layers/osvos_layers.py:72-85)")
                 self._deconv_checked[key] = ver
 
     # ----------------------------------------------------------------- forward
@@ -157,7 +157,7 @@ class OSVOSEngine:
         if not isinstance(x, torch.Tensor) or x.dim() != 4 or x.size(1) != 3:
             raise ValueError("OSVOS.forward expects a [N, 3, H, W] tensor")
         if not x.is_cuda:
-            raise RuntimeError("osvos_pytorch_b200.OSVOS runs on CUDA (sm_100a) only: move the module and the input "
+            raise RuntimeError("osvos_pytorch_b200.OSVOS runs on CUDA (sm_90a) only: move the module and the input "
                                "to the GPU.  There is no CPU fallback for the hot path.")
         needs_grad = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.m.parameters()))
         if x.device != torch.device("cuda", torch.cuda.current_device()):
@@ -175,7 +175,7 @@ class OSVOSEngine:
         if not isinstance(x, torch.Tensor) or x.dim() != 4 or x.size(1) != 3:
             raise ValueError("OSVOS.forward_objective expects a [N, 3, H, W] tensor")
         if not x.is_cuda:
-            raise RuntimeError("osvos_pytorch_b200.OSVOS runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("osvos_pytorch_b200.OSVOS runs on CUDA (sm_90a) only; there is no CPU fallback")
         if len(loss_weights) != 5:
             raise ValueError("loss_weights: one weight per output map (5)")
         if size_average:
@@ -273,8 +273,10 @@ class OSVOSEngine:
         n, _, h, w = (int(v) for v in x.shape)
         inter = {}
         convs0 = [c for c in m.stages[0] if isinstance(c, nn.Conv2d)]
-        if not fast and not simt and os.environ.get("OSVOS_FUSE_STAGE1", "1") != "0":
-            # stage 1 as one kernel: conv1_1 is computed inside conv1_2's kernel on its halo patch (no 105 MB round trip)
+        if not fast and not simt and os.environ.get("OSVOS_FUSE_STAGE1", "0") == "1":
+            # stage 1 as one kernel (opt-in): conv1_1 is computed inside conv1_2's kernel on its halo patch (no 105 MB round
+            # trip).  Its fp32 conv1_1 builder warps take about as long as the tile's tensor work, and on an H100 it measured
+            # slower than the two kernels below (553 vs 584 frames/s at 480x854, 700 W card), so it is not the default.
             full, a = ops.stage1_fused(x, convs0[0].weight.detach().contiguous().float(), convs0[0].bias.detach(),
                                        self._packed(convs0[1], "s0c1"), convs0[1].bias.detach(), pool=True,
                                        out_act=return_intermediates)

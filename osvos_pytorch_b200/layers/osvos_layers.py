@@ -64,7 +64,7 @@ class _ClassBalancedBCE(torch.autograd.Function):
     @staticmethod
     def forward(ctx, output, label, divisor):
         if not output.is_cuda:
-            raise RuntimeError("class_balanced_cross_entropy_loss: CUDA tensors required; the B200 package has no "
+            raise RuntimeError("class_balanced_cross_entropy_loss: CUDA tensors required; the H100 package has no "
                                "CPU fallback (oracle/ holds the CPU restatement used by the tests)")
         lib = nat.load()
         x = output.detach().contiguous().float()

@@ -1,4 +1,4 @@
-"""OSVOS network with the reference's module surface and a native B200 forward.
+"""OSVOS network with the reference's module surface and a native H100 forward.
 
 Mirrors networks/vgg_osvos.py of the reference: same constructor
 (``OSVOS(pretrained=0|1|2)``, :17), same parameter containers ``stages``,

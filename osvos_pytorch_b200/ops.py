@@ -193,7 +193,7 @@ def side_folded_multi(xs, folded, fast=False):
 
 def conv3x3(x, w_packed, bias, cout, relu=False, fast=False, out_act=True, out_f32=False, mask=None,
             proj_w=None, proj_b=None, simt=False, pool=False, colsum=None, k_valid=0):
-    """3x3 / pad 1 conv of an Act through the tcgen05 kernel.  Returns (Act|None, f32|None, pq|None), or
+    """3x3 / pad 1 conv of an Act through the wgmma kernel.  Returns (Act|None, f32|None, pq|None), or
     (Act, pooled Act) when pool=True (fused MaxPool2d(2,2,ceil_mode)).  `colsum` ([cout] fp32, pre-zeroed)
     receives the per-channel sum of the output (fused bias gradient)."""
     lib = nat.load()

@@ -1,5 +1,5 @@
 """Data-parallel parent training: one process per GPU, frames sharded across ranks, ONE exchange step
-per optimizer step - an allreduce(mean) of the flat fp32 gradient bucket over NCCL (NVLink 5 / NVSwitch).
+per optimizer step - an allreduce(mean) of the flat fp32 gradient bucket over NCCL (NVLink / NVSwitch).
 
 The reference has no parallelism at all (single gpu_id, train_parent.py:25); its only batch-enlarging
 mechanism is gradient accumulation (``loss /= nAveGrad; loss.backward()``, train_parent.py:163-172).

@@ -1,10 +1,10 @@
-"""Timing ablations of the tcgen05 conv kernel (OSVOS_ABLATE bit mask, csrc/conv_common.cuh) - development aid.
+"""Timing ablations of the wgmma conv kernel (OSVOS_ABLATE bit mask, csrc/conv_common.cuh) - development aid.
 
     python scripts/ablate.py [H W] [masks...]
 
 For each mask a fresh process (the library reads the variable once) times every conv3x3 launch of one forward with
 CUDA events (best of 7 eager passes).  Results under an ablation are garbage; only the durations mean something:
-1 = no weight TMA loads, 2 = no activation TMA loads, 4 = no tcgen05.mma, 8 = no epilogue stores.
+1 = no weight TMA loads, 2 = no activation TMA loads, 4 = no wgmma, 8 = no epilogue stores.
 """
 import json
 import os

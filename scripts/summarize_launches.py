@@ -1,5 +1,5 @@
 """Condense an `ncu --metrics gpu__time_duration.sum,... --csv` launch list into a per-step kernel table
-(development aid; the raw list stays next to the summary under profiles/)."""
+(development aid; the raw list stays next to the summary)."""
 import csv
 import sys
 

@@ -7,7 +7,7 @@ import sys
 from summarize_launches import load
 
 prefix = sys.argv[1]
-peaks = {"hbm": 6569.3}
+peaks = {"hbm": 3350.0}   # GB/s, H100 SXM data sheet (HBM3)
 for path in sorted(glob.glob(prefix + "*.csv"), key=lambda p: int(p.split("_")[-1].split("x")[0])):
     res = path.split("_")[-1].replace(".csv", "")
     recs = load(path)

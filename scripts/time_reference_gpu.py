@@ -1,4 +1,4 @@
-"""Times the UNMODIFIED reference modules (oracle/_ref) on the B200 itself - the "real kernel to beat" of SURVEY 8(d):
+"""Times the UNMODIFIED reference modules (oracle/_ref) on the GPU itself - the "real kernel to beat" of SURVEY 8(d):
 stock cuDNN with TF32 (torch default for convs), strict fp32 (allow_tf32=False), and channels_last + bf16 autocast.
 
     python scripts/time_reference_gpu.py [H W] [--train]

@@ -1,5 +1,5 @@
 """Per-kernel parity tests of the CUDA path (through the C ABI) against CPU fp64 restatements.
-Run on the B200 box:  pytest -m gpu."""
+Run on the GPU:  pytest -m gpu."""
 import math
 
 import numpy as np
@@ -86,6 +86,33 @@ def test_conv3x3_tensor_core(dev, n, h, w, cin, cout, relu, fast):
     # CUDA-core cross-check on identical operands
     _, ys, _ = ops.conv3x3(a, wp, b.to(dev), cout, relu=relu, fast=fast, out_act=False, out_f32=True, simt=True)
     assert maxrel(got_f32, ys.permute(0, 3, 1, 2).cpu()) < 2e-5
+
+
+def test_conv3x3_outputs_need_only_element_pair_alignment(dev):
+    """The epilogue stores channel pairs (4-byte bf16x2 words, 8-byte float2), so output planes that start 4 / 8 bytes past
+    a 32-byte boundary are valid and must give the same result as the allocator-aligned call."""
+    from ctypes import byref
+    from osvos_pytorch_b200 import _native as nat, ops
+    n, h, w, cin, cout = 1, 20, 13, 64, 128
+    g = torch.Generator().manual_seed(7)
+    x = torch.randn(n, cin, h, w, generator=g)
+    wt = torch.randn(cout, cin, 3, 3, generator=g) * math.sqrt(2.0 / (9 * cin))
+    b = (torch.randn(cout, generator=g) * 0.1).to(dev)
+    a = ops.nchw_to_act(x.to(dev))
+    wp = ops.pack_conv3x3_weights(wt.to(dev))
+    y, yf, _ = ops.conv3x3(a, wp, b, cout, relu=True, out_act=True, out_f32=True)
+    numel = n * h * w * cout
+    hi = torch.zeros(numel + 2, dtype=torch.bfloat16, device=dev)      # planes at +4 bytes
+    lo = torch.zeros(numel + 2, dtype=torch.bfloat16, device=dev)
+    f32 = torch.zeros(numel + 2, dtype=torch.float32, device=dev)      # plane at +8 bytes
+    args = nat.Conv3x3Args()
+    args.x_hi, args.x_lo, args.w_packed, args.bias = a.hi.data_ptr(), a.lo.data_ptr(), wp.data_ptr(), b.data_ptr()
+    args.y_hi, args.y_lo, args.y_f32 = hi[2:].data_ptr(), lo[2:].data_ptr(), f32[2:].data_ptr()
+    args.n, args.h, args.w, args.cin, args.cout, args.flags = n, h, w, cin, cout, nat.FLAG_RELU
+    nat.check(nat.load().osvos_conv3x3(byref(args), torch.cuda.current_stream().cuda_stream), "osvos_conv3x3")
+    torch.cuda.synchronize()
+    assert torch.equal(f32[2:].view(n, h, w, cout), yf)
+    assert torch.equal(hi[2:].view(n, h, w, cout), y.hi) and torch.equal(lo[2:].view(n, h, w, cout), y.lo)
 
 
 @pytest.mark.parametrize("n,h,w", [(1, 16, 8), (1, 33, 45), (2, 40, 56), (1, 5, 3), (1, 480, 854), (3, 97, 131)])

@@ -2,7 +2,7 @@
 osvos_fold_side_weights_multi) against torch CPU fp64 autograd of the LITERAL branch the reference runs
 (networks/vgg_osvos.py:67,69,72: side_prep 3x3 C -> 16 without ReLU, score_dsn 1x1, this scale's slice of fuse).  The whole
 network's gradients through this route are held to the reference's golden gradients and to the oracle by
-tests/test_gpu_backward.py; the A/B against the literal 16-feature route this replaced is profiles/r02l_ab_train480.txt."""
+tests/test_gpu_backward.py."""
 import pytest
 import torch
 import torch.nn.functional as F
