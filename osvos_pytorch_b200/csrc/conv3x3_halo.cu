@@ -48,13 +48,24 @@ struct HaloCfg {
   static_assert(kBStageBytes % 1024 == 0, "B stage must keep 1024-byte alignment");
 };
 
-template <int BLOCK_N, int PLANES, int PITCH, bool SPLIT, bool LEAN>
+// Two schedules for the consumer warpgroups 1 and 2:
+//  - cooperative (PINGPONG = false): both take every tile, rows 0 .. 63 and 64 .. 127, and reach the epilogue together,
+//    so the tensor pipe idles while they run it.
+//  - ping-pong: the CTA's k-th tile goes to warpgroup k % 2, which computes all 128 rows as two m64 halves; one
+//    warpgroup's epilogue runs while the other issues the next tile's MMAs.  Both read the ONE ring the producer fills in
+//    tile order, each skipping the other's stages, and each stage is released by the one warpgroup that read it.  Named
+//    barriers 1 and 2 hand the ring over in tile order: warpgroup k % 2 starts waiting on tile k's full barriers only
+//    after tile k - 1's owner has passed its last full wait.  Without that, a warpgroup a whole ring round ahead of the
+//    producer would pass a parity wait on a phase that has not happened yet.
+template <int BLOCK_N, int PLANES, int PITCH, bool SPLIT, bool LEAN, bool PINGPONG>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__ CUtensorMap map_x_lo,
                     const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
                     const ConvParams p) {
   using Cfg = HaloCfg<BLOCK_N, PLANES, PITCH, SPLIT>;
   constexpr int SA = Cfg::kAStages, SB = Cfg::kBStages;
+  constexpr int kHalves = PINGPONG ? 2 : 1;   // m64 halves of the tile per consumer warpgroup
+  static_assert(!PINGPONG || kHalves * Cfg::kAcc <= 128, "a ping-pong warpgroup holds the whole tile's accumulator");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -76,13 +87,14 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_c
       tma_prefetch_desc(&map_x_lo);
       tma_prefetch_desc(&map_w_lo);
     }
+    constexpr uint32_t kReaders = PINGPONG ? 1 : 2;   // consumer warpgroups that read (and release) each stage
     for (int i = 0; i < SA; ++i) {
       mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 2);   // one arrival per consumer warpgroup
+      mbar_init(&a_empty[i], kReaders);
     }
     for (int i = 0; i < SB; ++i) {
       mbar_init(&b_full[i], 1);
-      mbar_init(&b_empty[i], 2);
+      mbar_init(&b_empty[i], kReaders);
     }
     fence_barrier_init();
   }
@@ -92,7 +104,11 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_c
   pdl_wait();
   pdl_launch_dependents();
 
-  if (warp == 0) {
+  // Ping-pong: the producer warpgroup (warps 0 - 3, all of which must execute the dec) hands registers to the two
+  // consumers, whose warpgroups each hold a whole tile's accumulator: 40 * 128 + 232 * 256 <= 64 K.
+  if (warp < 4) {
+    if (PINGPONG) setmaxnreg_dec<40>();
+    if (warp != 0) return;
     // ------------------------------------------------------------ TMA producer (one elected thread)
     // ONE elected thread runs the whole loop, taps unrolled (the tap coordinate is an immediate), tile coordinates
     // decoded once per tile.
@@ -153,24 +169,35 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_c
       }
     }
     __syncwarp();
-  } else if (warp >= 4) {
-    // -------------------------------------------------- consumer warpgroups: wgmma + epilogue for 64 rows each
-    // The nine taps are nine descriptors into the halo patch: tap (r, s) starts at smem row (r * PITCH + s), the
-    // warpgroup's eight patch rows are eight 8-row swizzle groups at stride SBO = PITCH * 128 B.
+  } else {
+    if (PINGPONG) setmaxnreg_inc<232>();
+    // ----------------------------------- consumer warpgroups: wgmma + epilogue, 64 rows (cooperative) or 128 (ping-pong)
+    // The nine taps are nine descriptors into the halo patch: tap (r, s) starts at smem row (r * PITCH + s), the eight
+    // patch rows of an m64 half are eight 8-row swizzle groups at stride SBO = PITCH * 128 B.
     const int wg = (warp - 4) >> 2, wl = warp & 3;
     const bool leader = (threadIdx.x & 127) == 0;
     constexpr uint64_t kDescA = desc_template(16, PITCH * 128, kDescSW128);
     constexpr uint64_t kDescB = desc_template(16, 1024, kDescSW128);
     constexpr uint32_t kLoPlaneA = Cfg::kAPlaneBytes >> 4, kLoPlaneB = Cfg::kBPlaneBytes >> 4;
-    const uint32_t smem_a_u32 = smem_u32(smem_a) + wg * 8 * PITCH * 128, smem_b_u32 = smem_u32(smem_b);
+    constexpr uint32_t kHalfA = (8 * PITCH * 128) >> 4;   // rows 64 .. 127 of the tile start 8 patch rows down
+    const uint32_t smem_a_u32 = smem_u32(smem_a) + (PINGPONG ? 0 : wg * 8 * PITCH * 128), smem_b_u32 = smem_u32(smem_b);
     const int k_steps = (p.ablate & 4) ? 0 : p.k_steps;   // < 4 only for zero-padded input channels (k_valid)
-    float acc[Cfg::kAcc];
-    int a_stage = 0, b_stage = 0;
-    uint32_t a_phase = 0, b_phase = 0;
+    float acc[kHalves][Cfg::kAcc];
     StageRelease pending;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    // k: the tile's place in the CTA's sequence, which is also the order the producer fills the rings in
+    constexpr int kOwners = PINGPONG ? 2 : 1;   // warpgroups the CTA's tiles are dealt to in turn
+    for (int k = PINGPONG ? wg : 0;; k += kOwners) {
+      const int tile = static_cast<int>(blockIdx.x) + k * static_cast<int>(gridDim.x);
+      if (tile >= p.total_tiles) break;
+      const bool has_next = tile + static_cast<int>(gridDim.x) < p.total_tiles;
+      const int a_seq = k * p.k_chunks, b_seq = 9 * a_seq;   // ring slots filled for the CTA's earlier tiles
+      int a_stage = a_seq % SA, b_stage = b_seq % SB;
+      uint32_t a_phase = (a_seq / SA) & 1, b_phase = (b_seq / SB) & 1;
+      if (PINGPONG && k > 0) named_bar_sync(1 + wg, 256);    // tile k - 1 has passed its last full wait
 #pragma unroll
-      for (int i = 0; i < Cfg::kAcc; ++i) acc[i] = 0.f;
+      for (int h = 0; h < kHalves; ++h)
+#pragma unroll
+        for (int i = 0; i < Cfg::kAcc; ++i) acc[h][i] = 0.f;
       for (int kc = 0; kc < p.k_chunks; ++kc) {
         mbar_wait(&a_full[a_stage], a_phase);
         const uint64_t da0 = kDescA | static_cast<uint64_t>((smem_a_u32 + a_stage * Cfg::kAStageBytes) >> 4);
@@ -178,28 +205,32 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_c
         for (int tap = 0; tap < 9; ++tap) {
           const uint32_t tap_off = static_cast<uint32_t>(((tap / 3) * PITCH + (tap % 3)) * (128 >> 4));
           mbar_wait(&b_full[b_stage], b_phase);
+          if (PINGPONG && tap == 8 && kc == p.k_chunks - 1 && has_next) named_bar_arrive(1 + (wg ^ 1), 256);
           const uint64_t db_hi = kDescB | static_cast<uint64_t>((smem_b_u32 + b_stage * Cfg::kBStageBytes) >> 4);
-          const uint64_t da_hi = da0 + tap_off;
-          const uint64_t da_lo = da_hi + kLoPlaneA;
           wgmma_fence();
-          // all four K steps is the common case; fewer only for zero-padded input channels (k_valid)
-          auto k_step = [&](int k) {
-            if constexpr (Cfg::kSplitAcc) {
-              wgmma_bf16<2 * BLOCK_N>(acc, da_hi + 2 * k, db_hi + 2 * k, 1);   // [A_hi.B_hi | A_hi.B_lo]
-              wgmma_bf16<BLOCK_N>(acc, da_lo + 2 * k, db_hi + 2 * k, 1);       // + A_lo.B_hi into the first half
-            } else if constexpr (PLANES == 2) {
-              wgmma_bf16<BLOCK_N>(acc, da_lo + 2 * k, db_hi + 2 * k, 1);
-              wgmma_bf16<BLOCK_N>(acc, da_hi + 2 * k, db_hi + kLoPlaneB + 2 * k, 1);
-              wgmma_bf16<BLOCK_N>(acc, da_hi + 2 * k, db_hi + 2 * k, 1);
-            } else {
-              wgmma_bf16<BLOCK_N>(acc, da_hi + 2 * k, db_hi + 2 * k, 1);
-            }
-          };
-          if (k_steps == kBlockK / 16) {
 #pragma unroll
-            for (int k = 0; k < kBlockK / 16; ++k) k_step(k);
-          } else {
-            for (int k = 0; k < k_steps; ++k) k_step(k);
+          for (int h = 0; h < kHalves; ++h) {
+            const uint64_t da_hi = da0 + h * kHalfA + tap_off;
+            const uint64_t da_lo = da_hi + kLoPlaneA;
+            // all four K steps is the common case; fewer only for zero-padded input channels (k_valid)
+            auto k_step = [&](int ks) {
+              if constexpr (Cfg::kSplitAcc) {
+                wgmma_bf16<2 * BLOCK_N>(acc[h], da_hi + 2 * ks, db_hi + 2 * ks, 1);   // [A_hi.B_hi | A_hi.B_lo]
+                wgmma_bf16<BLOCK_N>(acc[h], da_lo + 2 * ks, db_hi + 2 * ks, 1);       // + A_lo.B_hi into the first half
+              } else if constexpr (PLANES == 2) {
+                wgmma_bf16<BLOCK_N>(acc[h], da_lo + 2 * ks, db_hi + 2 * ks, 1);
+                wgmma_bf16<BLOCK_N>(acc[h], da_hi + 2 * ks, db_hi + kLoPlaneB + 2 * ks, 1);
+                wgmma_bf16<BLOCK_N>(acc[h], da_hi + 2 * ks, db_hi + 2 * ks, 1);
+              } else {
+                wgmma_bf16<BLOCK_N>(acc[h], da_hi + 2 * ks, db_hi + 2 * ks, 1);
+              }
+            };
+            if (k_steps == kBlockK / 16) {
+#pragma unroll
+              for (int ks = 0; ks < kBlockK / 16; ++ks) k_step(ks);
+            } else {
+              for (int ks = 0; ks < k_steps; ++ks) k_step(ks);
+            }
           }
           wgmma_commit();
           wgmma_wait<1>();               // the previous tap's group is done: its stages may be refilled
@@ -217,9 +248,12 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_c
         }
       }
       wgmma_wait<0>();
-      wgmma_fence_operands(acc);
+#pragma unroll
+      for (int h = 0; h < kHalves; ++h) wgmma_fence_operands(acc[h]);
       pending.release(leader);
-      conv_epilogue<BLOCK_N, Cfg::kSplitAcc, LEAN>(p, acc, tile, wg, wl, lane);
+#pragma unroll
+      for (int h = 0; h < kHalves; ++h)
+        conv_epilogue<BLOCK_N, Cfg::kSplitAcc, LEAN>(p, acc[h], tile, PINGPONG ? h : wg, wl, lane);
     }
   }
 }
@@ -229,7 +263,8 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_c
 struct HaloSwitches {
   bool lean;        // OSVOS_HALO_LEAN      (default 1): lean epilogue instantiation for plain forward launches
   bool n256;        // OSVOS_CONV_N256      (default 1): 256-wide tiles where they pay
-  bool splitacc128; // OSVOS_SPLITACC128    (default 1): N-concatenated accumulator for 128-wide exact tiles
+  bool splitacc128; // OSVOS_SPLITACC128    (default 1): N-concatenated accumulator for 128-wide exact tiles of
+                    //                      cooperative launches (ping-pong ones always take three passes)
 };
 static bool env_flag(const char* name, bool dflt) {
   const char* e = getenv(name);
@@ -268,10 +303,17 @@ static int launch_halo(const osvos_conv3x3_args* a, cudaStream_t stream) {
   }
   int rc = encode_weight_maps(&mw_hi, &mw_lo, a, BLOCK_N);
   if (rc) return rc;
-  auto kern = conv3x3_halo_kernel<BLOCK_N, PLANES, PITCH, SPLIT, LEAN>;
-  static uint64_t attr_done = 0;   // per instantiation: bit d = device d has the shared-memory opt-in
-  OSVOS_CHECK_CUDA(ensure_dynamic_smem(kern, Cfg::kSmemBytes, &attr_done));
   const int grid = p.total_tiles < sms ? p.total_tiles : sms;
+  // Ping-pong for the tile widths whose whole-tile accumulator fits one warpgroup: 128 columns, so N = 128 takes the
+  // three-pass form there (the split pair would need 256).  A CTA with T tiles then hides T - 1 epilogues, but its last
+  // one is a whole tile's run by one warpgroup, twice the cooperative schedule's share per warpgroup: against T
+  // half-tile epilogues that gains from T = 3 on.  So ping-pong wherever some CTA gets three tiles or more.
+  constexpr bool kCanPingPong = BLOCK_N == 64 || BLOCK_N == 128;
+  const bool pingpong = kCanPingPong && p.total_tiles > 2 * sms;
+  auto kern = pingpong ? conv3x3_halo_kernel<BLOCK_N, PLANES, PITCH, SPLIT && BLOCK_N == 64, LEAN, kCanPingPong>
+                       : conv3x3_halo_kernel<BLOCK_N, PLANES, PITCH, SPLIT, LEAN, false>;
+  static uint64_t attr_done[2] = {0, 0};   // per kernel: bit d = device d has the shared-memory opt-in
+  OSVOS_CHECK_CUDA(ensure_dynamic_smem(kern, Cfg::kSmemBytes, &attr_done[pingpong]));
   OSVOS_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kConvThreads), Cfg::kSmemBytes, stream, mx_hi, mx_lo,
                               mw_hi, mw_lo, p));
   return OSVOS_OK;
@@ -308,7 +350,8 @@ static int dispatch_halo(const osvos_conv3x3_args* a, cudaStream_t stream) {
   if (fast) return launch_halo<128, 1, PITCH>(a, stream);
   // Exact mode, N = 128: the N-concatenated split accumulator (2 MMAs per K step, 256 accumulator columns, the
   // epilogue sums two halves) and the plain three-pass form (3 MMAs, 128 columns) do the same tensor work;
-  // OSVOS_SPLITACC128=0 selects the three-pass form.
+  // OSVOS_SPLITACC128=0 selects the three-pass form.  Launches with two tiles or more per CTA run the ping-pong schedule,
+  // which always takes the three-pass form (launch_halo).
   if (!sw.splitacc128) return launch_halo<128, 2, PITCH, false>(a, stream);
   if (lean) return launch_halo<128, 2, PITCH, true, true>(a, stream);
   return launch_halo<128, 2, PITCH>(a, stream);

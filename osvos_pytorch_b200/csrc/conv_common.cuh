@@ -14,7 +14,8 @@ constexpr int kTileH = 16;    // patch rows
 constexpr int kBlockM = 128;  // kTileW * kTileH
 constexpr int kBlockK = 64;   // channels per K block (128 B of bf16)
 // Warp roles of the conv kernels: warpgroup 0 feeds shared memory (TMA producer warp, or the threads that build an
-// operand), warpgroups 1 and 2 issue the wgmma for GEMM rows 0 .. 63 / 64 .. 127 of a tile and run its epilogue.
+// operand), warpgroups 1 and 2 issue the wgmma for GEMM rows 0 .. 63 / 64 .. 127 of a tile and run its epilogue (or, in
+// the halo kernel's ping-pong schedule, each takes every other tile whole).
 constexpr int kConvThreads = 384;
 constexpr int kABytes = kBlockM * kBlockK * 2;  // 16 KiB per plane
 
@@ -35,7 +36,8 @@ struct ConvParams {
   int k_steps;               // wgmma K steps (of 16 channels) issued per 64-channel chunk: 4, or fewer (k_valid)
   int flags;
   // Timing ablations (OSVOS_ABLATE bit mask, diagnosis only - results are garbage): 1 = no weight TMA loads,
-  // 2 = no activation TMA loads, 4 = no wgmma, 8 = no global stores in the epilogue.  0 in production.
+  // 2 = no activation TMA loads, 4 = no wgmma, 8 = no global stores in the epilogue, 16 = no epilogue at all.
+  // 0 in production.
   int ablate;
 };
 
@@ -58,8 +60,8 @@ __device__ __forceinline__ void split_pack2(float a, float b, uint32_t& hi, uint
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(rb), "f"(ra));
 }
 
-// Consumer warpgroup `wg` (0, 1) of a conv kernel owns GEMM rows 64 wg .. 64 wg + 63 of the 128-pixel tile, i.e. patch
-// rows 8 wg .. 8 wg + 7.  Its wgmma accumulator fragment (wgmma.cuh) gives thread (warp wl of the warpgroup, lane) the
+// The m64 half `wg` (0, 1) of a tile is GEMM rows 64 wg .. 64 wg + 63 of the 128-pixel tile, i.e. patch rows
+// 8 wg .. 8 wg + 7; `acc` is a consumer warpgroup's accumulator for that half.  Its wgmma accumulator fragment (wgmma.cuh) gives thread (warp wl of the warpgroup, lane) the
 // pixels (lx = lane / 4, ly = 8 wg + 2 wl) and (lx, ly + 1) - the two rows of a 2 x 2 pooling window - and the channel
 // pairs 8j + 2 (lane % 4) + {0, 1}: the x partner of the window is lane ^ 4.
 //
@@ -72,6 +74,7 @@ __device__ __forceinline__ void split_pack2(float a, float b, uint32_t& hi, uint
 // Both forms compute every value with the same operations in the same order: their outputs are bit-identical.
 template <int BLOCK_N, bool SPLIT_ACC, bool LEAN = false>
 __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float* acc, int tile, int wg, int wl, int lane) {
+  if (p.ablate & 16) return;
   int nb, tx, ty, img;
   decode_tile(p, tile, nb, tx, ty, img);
   const int lx = lane >> 2;

@@ -171,6 +171,17 @@ __device__ __forceinline__ uint64_t make_smem_desc(const void* p, uint32_t lbo_b
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// Counts the calling warp toward named barrier `id` without waiting for it; the threads that bar.sync it wait.
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+// Per-thread register budget of the calling warpgroup (all four warps execute it): dec hands registers back to the SM's
+// pool, inc waits until it can take them.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // Stage bookkeeping of a consumer warpgroup: a shared-memory stage may be handed back to the producer only once the wgmma
 // groups reading it have completed.  With one group in flight (wgmma_wait<1>) that is the PREVIOUS group's stage.

@@ -4,7 +4,7 @@
 
 For each mask a fresh process (the library reads the variable once) times every conv3x3 launch of one forward with
 CUDA events (best of 7 eager passes).  Results under an ablation are garbage; only the durations mean something:
-1 = no weight TMA loads, 2 = no activation TMA loads, 4 = no wgmma, 8 = no epilogue stores.
+1 = no weight TMA loads, 2 = no activation TMA loads, 4 = no wgmma, 8 = no epilogue stores, 16 = no epilogue at all.
 """
 import json
 import os
@@ -62,7 +62,7 @@ def worker(h, w):
 def main():
     args = sys.argv[1:]
     h, w = (int(args[0]), int(args[1])) if len(args) >= 2 else (480, 854)
-    masks = [int(v) for v in args[2:]] or [0, 1, 2, 3, 4, 8, 12, 7, 15]
+    masks = [int(v) for v in args[2:]] or [0, 1, 2, 3, 4, 8, 12, 7, 15, 16]
     table = {}
     for m in masks:
         env = dict(os.environ, OSVOS_ABLATE=str(m))
@@ -75,7 +75,7 @@ def main():
         table[m] = json.loads(line[0][7:])
     names = [d for d, _ in table[masks[0]]]
     print(f"# {h}x{w} exact, per-launch CUDA-event us (best of 7); columns = OSVOS_ABLATE mask "
-          "(1 no weight loads, 2 no activation loads, 4 no MMAs, 8 no epilogue stores)")
+          "(1 no weight loads, 2 no activation loads, 4 no MMAs, 8 no epilogue stores, 16 no epilogue)")
     print(f"{'launch':34s}" + "".join(f"{m:>9d}" for m in table))
     for i, d in enumerate(names):
         print(f"{d:34s}" + "".join(f"{table[m][i][1]:9.1f}" for m in table))
