@@ -83,8 +83,8 @@ OSVOS_API int osvos_act_to_nchw(const void* act_hi, const void* act_lo, float* y
 
 /* ---- conv1_1: nn.Conv2d(3, 64, 3, padding=1) + ReLU ------------------------
  * Replaces stages[0][0..1] (networks/vgg_osvos.py:61,142-143).  Reads the
- * caller's NCHW fp32 frame directly (no layout pass), fp32 CUDA-core math
- * (K = 27 is bandwidth bound), writes an act [N,H,W,64].                       */
+ * caller's NCHW fp32 frame directly (no layout pass), wgmma over split-bf16
+ * operands (conv_first_tc.cu), writes an act [N,H,W,64].                       */
 OSVOS_API int osvos_conv_first_fwd(const float* x_nchw, const float* w_oihw, const float* bias, void* y_hi, void* y_lo,
                          int n, int h, int w, int flags, osvos_stream_t stream);
 
@@ -99,11 +99,12 @@ typedef struct {
   const void* x_lo;      /* NULL in FAST mode                                   */
   const void* w_packed;  /* osvos_pack_conv3x3_weights output, rows = cout      */
   const float* bias;     /* [cout] or NULL                                      */
-  void* y_hi;            /* act [n,h,w,cout] or NULL                            */
+  void* y_hi;            /* act [n,h,w,cout] or NULL (cout >= 64 only)          */
   void* y_lo;            /* NULL in FAST mode / when y_hi is NULL               */
   float* y_f32;          /* optional fp32 NHWC copy of the output [n,h,w,cout]  */
-  const void* mask_hi;   /* RELU_MASK: act hi plane [n,h,w,cout] of the fwd output this gradient flows into */
-  /* side_prep only (cout == 16): fused 1x1 projections of the 16 features
+  const void* mask_hi;   /* RELU_MASK (cout >= 64 only): act hi plane [n,h,w,cout] of the fwd output this gradient
+                            flows into */
+  /* side_prep only (cout == 16, whose outputs are y_f32 and / or pq): fused 1x1 projections of the 16 features
    *   pq[px][0] = <y, proj_w[0:16]>  + proj_b[0]   score_dsn (networks/vgg_osvos.py:44,69)
    *   pq[px][1] = <y, proj_w[16:32]>               this scale's slice of fuse (:54,72)  */
   const float* proj_w;   /* [32] or NULL */
@@ -118,10 +119,6 @@ typedef struct {
   float* colsum;
   int n, h, w, cin, cout;
   int flags;
-  /* 0 or 64: all input channels carry data.  16 / 32 / 48: only the first k_valid channels of every 64-channel
-   * chunk can be non-zero (e.g. a 16-channel operand stored padded to 64): the remaining K steps
-   * are skipped - fewer wgmma, identical result. */
-  int k_valid;
 } osvos_conv3x3_args;
 OSVOS_API int osvos_conv3x3(const osvos_conv3x3_args* args /* host */, osvos_stream_t stream);
 

@@ -29,8 +29,7 @@ class Conv3x3Args(Structure):
                 ("y_hi", c_void_p), ("y_lo", c_void_p), ("y_f32", c_void_p), ("mask_hi", c_void_p),
                 ("proj_w", c_void_p), ("proj_b", c_void_p), ("pq", c_void_p),
                 ("pool_hi", c_void_p), ("pool_lo", c_void_p), ("colsum", c_void_p),
-                ("n", c_int), ("h", c_int), ("w", c_int), ("cin", c_int), ("cout", c_int), ("flags", c_int),
-                ("k_valid", c_int)]
+                ("n", c_int), ("h", c_int), ("w", c_int), ("cin", c_int), ("cout", c_int), ("flags", c_int)]
 
 
 class Stage1Args(Structure):

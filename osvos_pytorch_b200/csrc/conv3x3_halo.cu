@@ -2,29 +2,27 @@
 //
 // GEMM view: M = 128 pixels of an 8 x 16 output tile, N = output channels, K = 9 taps x input channels.  The
 // activation operand is loaded ONCE per (tile, 64-channel chunk) as the 18-row x 10-px halo patch (one TMA box,
-// SWIZZLE_128B) and the nine taps are nine wgmma descriptors into it: tap (r, s) starts at smem row (r * PITCH + s);
-// the 16 tile rows are sixteen 8-row swizzle groups at stride SBO = PITCH * 128 B.  That divides the activation
+// SWIZZLE_128B) and the nine taps are nine wgmma descriptors into it: tap (r, s) starts at smem row (r * kPitch + s);
+// the 16 tile rows are sixteen 8-row swizzle groups at stride SBO = kPitch * 128 B.  That divides the activation
 // traffic through L2 -> smem by ~6 relative to one shifted box per tap.  The weight slabs stream through their own,
 // deeper ring (one stage per tap), and the next chunk's halo is prefetched while the current one is being consumed.
 //
-// PITCH is the smem row pitch in pixels: 10 packs the patch rows (1280 B); a tap descriptor then starts at any
+// kPitch is the smem row pitch in pixels: 10 packs the patch rows (1280 B); a tap descriptor then starts at any
 // 128-byte row, which relies on the hardware applying the 128-byte swizzle to the absolute shared-memory address
 // (the descriptor's base-offset field stays 0), as the TMA unit does when it writes the box.
 //
 // Precision: exact mode carries every operand as split bf16 (hi + lo) and sums A_hi.B_hi + A_hi.B_lo + A_lo.B_hi in
 // fp32; fast mode uses the hi planes only.
-#include <stdlib.h>
-#include <string.h>
-
 #include "conv_common.cuh"
 
 namespace osvos {
 
 constexpr int kHaloRows = kTileH + 2;  // 18
+constexpr int kPitch = kTileW + 2;     // 10: the halo patch's rows, packed
 
-template <int BLOCK_N, int PLANES, int PITCH, bool SPLIT>
+template <int BLOCK_N, int PLANES, bool SPLIT>
 struct HaloCfg {
-  static constexpr int kABoxBytes = kHaloRows * PITCH * 128;                // one plane, one chunk
+  static constexpr int kABoxBytes = kHaloRows * kPitch * 128;               // one plane, one chunk
   static constexpr int kAPlaneBytes = (kABoxBytes + 1023) / 1024 * 1024;    // keep 1 KiB alignment
   static constexpr int kAStageBytes = PLANES * kAPlaneBytes;
   static constexpr int kAStages = 2;
@@ -57,12 +55,12 @@ struct HaloCfg {
 //    barriers 1 and 2 hand the ring over in tile order: warpgroup k % 2 starts waiting on tile k's full barriers only
 //    after tile k - 1's owner has passed its last full wait.  Without that, a warpgroup a whole ring round ahead of the
 //    producer would pass a parity wait on a phase that has not happened yet.
-template <int BLOCK_N, int PLANES, int PITCH, bool SPLIT, bool LEAN, bool PINGPONG>
+template <int BLOCK_N, int PLANES, bool SPLIT, bool LEAN, bool PINGPONG>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__ CUtensorMap map_x_lo,
                     const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
                     const ConvParams p) {
-  using Cfg = HaloCfg<BLOCK_N, PLANES, PITCH, SPLIT>;
+  using Cfg = HaloCfg<BLOCK_N, PLANES, SPLIT>;
   constexpr int SA = Cfg::kAStages, SB = Cfg::kBStages;
   constexpr int kHalves = PINGPONG ? 2 : 1;   // m64 halves of the tile per consumer warpgroup
   static_assert(!PINGPONG || kHalves * Cfg::kAcc <= 128, "a ping-pong warpgroup holds the whole tile's accumulator");
@@ -172,16 +170,16 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_c
   } else {
     if (PINGPONG) setmaxnreg_inc<232>();
     // ----------------------------------- consumer warpgroups: wgmma + epilogue, 64 rows (cooperative) or 128 (ping-pong)
-    // The nine taps are nine descriptors into the halo patch: tap (r, s) starts at smem row (r * PITCH + s), the eight
-    // patch rows of an m64 half are eight 8-row swizzle groups at stride SBO = PITCH * 128 B.
+    // The nine taps are nine descriptors into the halo patch: tap (r, s) starts at smem row (r * kPitch + s), the eight
+    // patch rows of an m64 half are eight 8-row swizzle groups at stride SBO = kPitch * 128 B.
     const int wg = (warp - 4) >> 2, wl = warp & 3;
     const bool leader = (threadIdx.x & 127) == 0;
-    constexpr uint64_t kDescA = desc_template(16, PITCH * 128, kDescSW128);
+    constexpr uint64_t kDescA = desc_template(16, kPitch * 128, kDescSW128);
     constexpr uint64_t kDescB = desc_template(16, 1024, kDescSW128);
     constexpr uint32_t kLoPlaneA = Cfg::kAPlaneBytes >> 4, kLoPlaneB = Cfg::kBPlaneBytes >> 4;
-    constexpr uint32_t kHalfA = (8 * PITCH * 128) >> 4;   // rows 64 .. 127 of the tile start 8 patch rows down
-    const uint32_t smem_a_u32 = smem_u32(smem_a) + (PINGPONG ? 0 : wg * 8 * PITCH * 128), smem_b_u32 = smem_u32(smem_b);
-    const int k_steps = (p.ablate & 4) ? 0 : p.k_steps;   // < 4 only for zero-padded input channels (k_valid)
+    constexpr uint32_t kHalfA = (8 * kPitch * 128) >> 4;   // rows 64 .. 127 of the tile start 8 patch rows down
+    const uint32_t smem_a_u32 = smem_u32(smem_a) + (PINGPONG ? 0 : wg * 8 * kPitch * 128), smem_b_u32 = smem_u32(smem_b);
+    const bool skip_mma = (p.ablate & 4) != 0;
     float acc[kHalves][Cfg::kAcc];
     StageRelease pending;
     // k: the tile's place in the CTA's sequence, which is also the order the producer fills the rings in
@@ -203,7 +201,7 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_c
         const uint64_t da0 = kDescA | static_cast<uint64_t>((smem_a_u32 + a_stage * Cfg::kAStageBytes) >> 4);
 #pragma unroll
         for (int tap = 0; tap < 9; ++tap) {
-          const uint32_t tap_off = static_cast<uint32_t>(((tap / 3) * PITCH + (tap % 3)) * (128 >> 4));
+          const uint32_t tap_off = static_cast<uint32_t>(((tap / 3) * kPitch + (tap % 3)) * (128 >> 4));
           mbar_wait(&b_full[b_stage], b_phase);
           if (PINGPONG && tap == 8 && kc == p.k_chunks - 1 && has_next) named_bar_arrive(1 + (wg ^ 1), 256);
           const uint64_t db_hi = kDescB | static_cast<uint64_t>((smem_b_u32 + b_stage * Cfg::kBStageBytes) >> 4);
@@ -212,8 +210,9 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_c
           for (int h = 0; h < kHalves; ++h) {
             const uint64_t da_hi = da0 + h * kHalfA + tap_off;
             const uint64_t da_lo = da_hi + kLoPlaneA;
-            // all four K steps is the common case; fewer only for zero-padded input channels (k_valid)
-            auto k_step = [&](int ks) {
+            if (skip_mma) continue;   // ablation bit 4
+#pragma unroll
+            for (int ks = 0; ks < kBlockK / 16; ++ks) {
               if constexpr (Cfg::kSplitAcc) {
                 wgmma_bf16<2 * BLOCK_N>(acc[h], da_hi + 2 * ks, db_hi + 2 * ks, 1);   // [A_hi.B_hi | A_hi.B_lo]
                 wgmma_bf16<BLOCK_N>(acc[h], da_lo + 2 * ks, db_hi + 2 * ks, 1);       // + A_lo.B_hi into the first half
@@ -224,12 +223,6 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_c
               } else {
                 wgmma_bf16<BLOCK_N>(acc[h], da_hi + 2 * ks, db_hi + 2 * ks, 1);
               }
-            };
-            if (k_steps == kBlockK / 16) {
-#pragma unroll
-              for (int ks = 0; ks < kBlockK / 16; ++ks) k_step(ks);
-            } else {
-              for (int ks = 0; ks < k_steps; ++ks) k_step(ks);
             }
           }
           wgmma_commit();
@@ -258,33 +251,12 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_c
   }
 }
 
-// Environment switches of the dispatcher (A/B and diagnosis).  Read ONCE per process;
-// OSVOS_ENV_RELOAD=1 makes every dispatch re-read them (scripts/ab_env.py flips switches inside one process).
-struct HaloSwitches {
-  bool lean;        // OSVOS_HALO_LEAN      (default 1): lean epilogue instantiation for plain forward launches
-  bool n256;        // OSVOS_CONV_N256      (default 1): 256-wide tiles where they pay
-  bool splitacc128; // OSVOS_SPLITACC128    (default 1): N-concatenated accumulator for 128-wide exact tiles of
-                    //                      cooperative launches (ping-pong ones always take three passes)
-};
-static bool env_flag(const char* name, bool dflt) {
-  const char* e = getenv(name);
-  return e == nullptr ? dflt : atoi(e) != 0;
-}
-static HaloSwitches halo_switches() {
-  static HaloSwitches sw;
-  static int state = 0;          // 0: unread, 1: cached, 2: re-read on every call
-  if (state != 1) {
-    sw.lean = env_flag("OSVOS_HALO_LEAN", true);
-    sw.n256 = env_flag("OSVOS_CONV_N256", true);
-    sw.splitacc128 = env_flag("OSVOS_SPLITACC128", true);
-    state = env_flag("OSVOS_ENV_RELOAD", false) ? 2 : 1;
-  }
-  return sw;
-}
-
-template <int BLOCK_N, int PLANES, int PITCH, bool SPLIT = (PLANES == 2 && BLOCK_N <= 128), bool LEAN = false>
+// Exact mode with BLOCK_N <= 128 takes the N-concatenated split accumulator (HaloCfg), except under ping-pong for
+// BLOCK_N = 128 (below).
+template <int BLOCK_N, int PLANES, bool LEAN = false>
 static int launch_halo(const osvos_conv3x3_args* a, cudaStream_t stream) {
-  using Cfg = HaloCfg<BLOCK_N, PLANES, PITCH, SPLIT>;
+  constexpr bool kSplit = PLANES == 2 && BLOCK_N <= 128;
+  using Cfg = HaloCfg<BLOCK_N, PLANES, kSplit>;
   ConvParams p;
   fill_conv_params(p, a, BLOCK_N);
   const int sms = device_sm_count();
@@ -293,7 +265,7 @@ static int launch_halo(const osvos_conv3x3_args* a, cudaStream_t stream) {
     const uint64_t dims[4] = {(uint64_t)a->cin, (uint64_t)a->w, (uint64_t)a->h, (uint64_t)a->n};
     const uint64_t strides[3] = {(uint64_t)a->cin * 2, (uint64_t)a->w * a->cin * 2,
                                  (uint64_t)a->h * a->w * a->cin * 2};
-    const uint32_t box[4] = {kBlockK, PITCH, kHaloRows, 1};
+    const uint32_t box[4] = {kBlockK, kPitch, kHaloRows, 1};
     int rc = encode_tensor_map(&mx_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, 4, a->x_hi, dims, strides, box,
                                CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
@@ -310,8 +282,8 @@ static int launch_halo(const osvos_conv3x3_args* a, cudaStream_t stream) {
   // half-tile epilogues that gains from T = 3 on.  So ping-pong wherever some CTA gets three tiles or more.
   constexpr bool kCanPingPong = BLOCK_N == 64 || BLOCK_N == 128;
   const bool pingpong = kCanPingPong && p.total_tiles > 2 * sms;
-  auto kern = pingpong ? conv3x3_halo_kernel<BLOCK_N, PLANES, PITCH, SPLIT && BLOCK_N == 64, LEAN, kCanPingPong>
-                       : conv3x3_halo_kernel<BLOCK_N, PLANES, PITCH, SPLIT, LEAN, false>;
+  auto kern = pingpong ? conv3x3_halo_kernel<BLOCK_N, PLANES, kSplit && BLOCK_N == 64, LEAN, kCanPingPong>
+                       : conv3x3_halo_kernel<BLOCK_N, PLANES, kSplit, LEAN, false>;
   static uint64_t attr_done[2] = {0, 0};   // per kernel: bit d = device d has the shared-memory opt-in
   OSVOS_CHECK_CUDA(ensure_dynamic_smem(kern, Cfg::kSmemBytes, &attr_done[pingpong]));
   OSVOS_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kConvThreads), Cfg::kSmemBytes, stream, mx_hi, mx_lo,
@@ -319,47 +291,30 @@ static int launch_halo(const osvos_conv3x3_args* a, cudaStream_t stream) {
   return OSVOS_OK;
 }
 
-template <int PITCH>
-static int dispatch_halo(const osvos_conv3x3_args* a, cudaStream_t stream) {
+// cout 64 or a multiple of 128 (cout 2 and 16 go to side_conv.cu)
+static int conv3x3_halo_dispatch(const osvos_conv3x3_args* a, cudaStream_t stream) {
   const bool fast = (a->flags & OSVOS_FLAG_FAST) != 0;
-  const HaloSwitches sw = halo_switches();
-  if (a->cout == 16) return fast ? launch_halo<16, 1, PITCH>(a, stream) : launch_halo<16, 2, PITCH>(a, stream);
   // the lean epilogue serves launches that use nothing but bias / ReLU / split-bf16 act output / fused pool (exact mode)
-  const bool lean = sw.lean && !fast && !(a->flags & OSVOS_FLAG_RELU_MASK) && a->colsum == nullptr && a->y_f32 == nullptr &&
-                    a->pq == nullptr && a->k_valid == 0;
-  if (a->cout == 64) {
-    if (lean) return launch_halo<64, 2, PITCH, true, true>(a, stream);
-    return fast ? launch_halo<64, 1, PITCH>(a, stream) : launch_halo<64, 2, PITCH>(a, stream);
-  }
+  const bool lean = !fast && !(a->flags & OSVOS_FLAG_RELU_MASK) && a->colsum == nullptr && a->y_f32 == nullptr;
   const int m_tiles = ((a->w + kTileW - 1) / kTileW) * ((a->h + kTileH - 1) / kTileH) * a->n;
   const int sms = device_sm_count();
   const long tiles128 = static_cast<long>(m_tiles) * (a->cout / 128);
   const long waves128 = (tiles128 + sms - 1) / sms;
   const long waves256 = (static_cast<long>(m_tiles) * (a->cout / 256) + sms - 1) / sms;
   // few tiles (stage 5 at 480x854: 56 of 128 x 128): N = 64 tiles double the CTA count at ~0.8x the time per tile.
-  if (waves128 == 1 && tiles128 * 5 <= static_cast<long>(sms) * 3) {
-    if (lean) return launch_halo<64, 2, PITCH, true, true>(a, stream);
-    return fast ? launch_halo<64, 1, PITCH>(a, stream) : launch_halo<64, 2, PITCH>(a, stream);
+  if (a->cout == 64 || (waves128 == 1 && tiles128 * 5 <= static_cast<long>(sms) * 3)) {
+    if (lean) return launch_halo<64, 2, true>(a, stream);
+    return fast ? launch_halo<64, 1>(a, stream) : launch_halo<64, 2>(a, stream);
   }
   // N = 256 tiles whenever that does not cost a wave.  The cost model per (tap, 64-channel) step (N = 128 ~ 1000 cycles
   // for 2 + 1 instructions, N = 256 ~ 2200 exact) is carried over from the first tensor-core generation this was tuned on;
-  // on an H100 the choice measured neutral at 480x854 (552-553 frames/s with and without OSVOS_CONV_N256=0).
+  // on an H100 the choice measured neutral at 480x854 (552-553 frames/s with 256-wide tiles and with 128-wide ones only).
   const bool prefer256 = fast ? waves256 * 1100 < waves128 * 700 : waves256 * 2200 < waves128 * 1000;
-  if (a->cout % 256 == 0 && prefer256 && sw.n256)
-    return fast ? launch_halo<256, 1, PITCH>(a, stream) : launch_halo<256, 2, PITCH>(a, stream);
-  if (fast) return launch_halo<128, 1, PITCH>(a, stream);
-  // Exact mode, N = 128: the N-concatenated split accumulator (2 MMAs per K step, 256 accumulator columns, the
-  // epilogue sums two halves) and the plain three-pass form (3 MMAs, 128 columns) do the same tensor work;
-  // OSVOS_SPLITACC128=0 selects the three-pass form.  Launches with two tiles or more per CTA run the ping-pong schedule,
-  // which always takes the three-pass form (launch_halo).
-  if (!sw.splitacc128) return launch_halo<128, 2, PITCH, false>(a, stream);
-  if (lean) return launch_halo<128, 2, PITCH, true, true>(a, stream);
-  return launch_halo<128, 2, PITCH>(a, stream);
-}
-
-int conv3x3_halo_dispatch(const osvos_conv3x3_args* a, cudaStream_t stream) {
-  // packed patch rows (pitch 10) are the only instantiation
-  return dispatch_halo<10>(a, stream);
+  if (a->cout % 256 == 0 && prefer256)
+    return fast ? launch_halo<256, 1>(a, stream) : launch_halo<256, 2>(a, stream);
+  if (fast) return launch_halo<128, 1>(a, stream);
+  if (lean) return launch_halo<128, 2, true>(a, stream);
+  return launch_halo<128, 2>(a, stream);
 }
 
 static int check_conv_args(const osvos_conv3x3_args* a) {
@@ -369,8 +324,9 @@ static int check_conv_args(const osvos_conv3x3_args* a) {
   OSVOS_CHECK_ARG(a->cout == 2 || a->cout == 16 || a->cout == 64 || (a->cout > 0 && a->cout % 128 == 0));
   // cout == 2: the folded side branch (osvos_fold_side_weights) - pq is the only output, bias = the 2 folded biases
   OSVOS_CHECK_ARG(a->cout != 2 || (a->pq != nullptr && a->y_hi == nullptr && a->y_f32 == nullptr && a->pool_hi == nullptr &&
-                                   a->colsum == nullptr && !(a->flags & (OSVOS_FLAG_RELU | OSVOS_FLAG_RELU_MASK)) &&
-                                   a->k_valid == 0));
+                                   a->colsum == nullptr && !(a->flags & (OSVOS_FLAG_RELU | OSVOS_FLAG_RELU_MASK))));
+  // cout == 16: side_prep - fp32 features and / or projections only (no pool or colsum either, below)
+  OSVOS_CHECK_ARG(a->cout != 16 || (a->y_hi == nullptr && a->y_lo == nullptr && !(a->flags & OSVOS_FLAG_RELU_MASK)));
   OSVOS_CHECK_ARG(a->x_hi != nullptr && a->w_packed != nullptr);
   OSVOS_CHECK_ARG((a->flags & OSVOS_FLAG_FAST) || a->x_lo != nullptr);
   OSVOS_CHECK_ARG(a->y_hi != nullptr || a->y_f32 != nullptr || a->pq != nullptr || a->pool_hi != nullptr);
@@ -387,7 +343,6 @@ static int check_conv_args(const osvos_conv3x3_args* a) {
     OSVOS_CHECK_ARG((bf16_planes & 3) == 0);
     OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(a->y_f32) & 7) == 0);
   }
-  OSVOS_CHECK_ARG(a->k_valid >= 0 && a->k_valid <= 64 && a->k_valid % 16 == 0);
   return OSVOS_OK;
 }
 
@@ -419,16 +374,7 @@ extern "C" int osvos_conv3x3(const osvos_conv3x3_args* a, osvos_stream_t stream_
   int rc = check_conv_args(a);
   if (rc) return rc;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  // side_prep shape (16 outputs, fp32 features / projections only): nine-taps-along-N kernel (side_conv.cu);
-  // OSVOS_SIDE_IMPL=generic sends it through the halo kernel's N = 16 instantiation instead (cross-check)
-  if (a->cout == 2) return side_conv_dispatch(a, stream);
-  if (a->cout == 16 && a->y_hi == nullptr && !(a->flags & OSVOS_FLAG_RELU_MASK) && a->colsum == nullptr) {
-    static int generic = -1;
-    if (generic < 0) {
-      const char* side = getenv("OSVOS_SIDE_IMPL");
-      generic = (side != nullptr && strcmp(side, "generic") == 0) ? 1 : 0;
-    }
-    if (!generic) return side_conv_dispatch(a, stream);
-  }
+  // the folded side branch (cout == 2) and side_prep (cout == 16): nine-taps-along-N kernel (side_conv.cu)
+  if (a->cout == 2 || a->cout == 16) return side_conv_dispatch(a, stream);
   return conv3x3_halo_dispatch(a, stream);
 }

@@ -1,6 +1,6 @@
 // Shared pieces of the wgmma implicit-GEMM convolution kernels (conv3x3_halo.cu, conv_first_tc.cu,
 // conv_stage1_fused.cu): tile geometry, parameters, tile decode and the epilogue (accumulator registers ->
-// bias / ReLU / mask / split-bf16 / pool / projections -> global).
+// bias / ReLU / mask / split-bf16 / pool / column sums -> global).
 #pragma once
 #include <stdlib.h>
 
@@ -25,15 +25,11 @@ struct ConvParams {
   __nv_bfloat16* y_lo;
   float* y_f32;
   const __nv_bfloat16* mask_hi;
-  const float* proj_w;
-  const float* proj_b;
-  float* pq;
   __nv_bfloat16* pool_hi;  // optional fused 2x2 ceil-mode max pool of the output
   __nv_bfloat16* pool_lo;
   float* colsum;           // optional fused per-channel sum of the output (bias gradient), atomically accumulated
   int n, h, w, cin, cout;
   int tiles_x, tiles_y, n_blocks, total_tiles, k_chunks;
-  int k_steps;               // wgmma K steps (of 16 channels) issued per 64-channel chunk: 4, or fewer (k_valid)
   int flags;
   // Timing ablations (OSVOS_ABLATE bit mask, diagnosis only - results are garbage): 1 = no weight TMA loads,
   // 2 = no activation TMA loads, 4 = no wgmma, 8 = no global stores in the epilogue, 16 = no epilogue at all.
@@ -66,11 +62,11 @@ __device__ __forceinline__ void split_pack2(float a, float b, uint32_t& hi, uint
 // pairs 8j + 2 (lane % 4) + {0, 1}: the x partner of the window is lane ^ 4.
 //
 // The epilogue runs straight from those registers: bias, ReLU, ReLU mask of a later layer, fp32 / split-bf16 act output,
-// fused 2 x 2 ceil-mode max pool, fused per-channel column sums (bias gradient) and, for N = 16, the two 1x1 projections.
+// fused 2 x 2 ceil-mode max pool and fused per-channel column sums (bias gradient).
 // SPLIT_ACC: the accumulator holds 2 * BLOCK_N columns - [A_hi.B_hi | A_hi.B_lo] (+ A_lo.B_hi in the first half) from one
 // N-concatenated wgmma - and the result is the sum of the two halves.
-// LEAN: the plain-forward feature set only (bias, ReLU, split-bf16 act output and / or fused pool); the mask, fp32 output,
-// column-sum and projection code is not compiled in, which takes it out of the consumer warpgroups' instruction stream.
+// LEAN: the plain-forward feature set only (bias, ReLU, split-bf16 act output and / or fused pool); the mask, fp32 output
+// and column-sum code is not compiled in, which takes it out of the consumer warpgroups' instruction stream.
 // Both forms compute every value with the same operations in the same order: their outputs are bit-identical.
 template <int BLOCK_N, bool SPLIT_ACC, bool LEAN = false>
 __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float* acc, int tile, int wg, int wl, int lane) {
@@ -89,7 +85,6 @@ __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float* 
   const int oh = (p.h + 1) >> 1, ow = (p.w + 1) >> 1;
   const bool pool_writer = va && !(lx & 1) && store_ok;
   const size_t opix = (static_cast<size_t>(img) * oh + (y0 >> 1)) * ow + (x >> 1);
-  float sp[2] = {0.f, 0.f}, sq[2] = {0.f, 0.f};
 #pragma unroll
   for (int j = 0; j < BLOCK_N / 8; ++j) {
     const int c = 8 * j + 2 * (lane & 3);
@@ -122,10 +117,6 @@ __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float* 
           if (p.y_lo) *reinterpret_cast<uint32_t*>(p.y_lo + pix[h] * p.cout + ch) = lo;
         }
       }
-      if (!LEAN && BLOCK_N == 16 && p.pq) {
-        sp[h] = fmaf(f[h][0], __ldg(p.proj_w + c), fmaf(f[h][1], __ldg(p.proj_w + c + 1), sp[h]));
-        sq[h] = fmaf(f[h][0], __ldg(p.proj_w + 16 + c), fmaf(f[h][1], __ldg(p.proj_w + 16 + c + 1), sq[h]));
-      }
     }
     if (!LEAN && p.colsum) {   // per-channel sum over the tile's valid pixels: the 8 x-lanes of a channel pair are lanes ^ 4, 8, 16
       float s0 = (va ? f[0][0] : 0.f) + (vb ? f[1][0] : 0.f);
@@ -153,17 +144,6 @@ __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float* 
       }
     }
   }
-  if (!LEAN && BLOCK_N == 16 && p.pq) {   // the four lanes of a pixel hold its channel pairs
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      sp[h] += __shfl_xor_sync(0xffffffffu, sp[h], 1);
-      sp[h] += __shfl_xor_sync(0xffffffffu, sp[h], 2);
-      sq[h] += __shfl_xor_sync(0xffffffffu, sq[h], 1);
-      sq[h] += __shfl_xor_sync(0xffffffffu, sq[h], 2);
-      if ((lane & 3) == 0 && valid[h] && store_ok)
-        *reinterpret_cast<float2*>(p.pq + pix[h] * 2) = make_float2(sp[h] + (p.proj_b ? __ldg(p.proj_b) : 0.f), sq[h]);
-    }
-  }
 }
 
 
@@ -174,9 +154,6 @@ static inline void fill_conv_params(ConvParams& p, const osvos_conv3x3_args* a, 
   p.y_lo = static_cast<__nv_bfloat16*>(a->y_lo);
   p.y_f32 = a->y_f32;
   p.mask_hi = static_cast<const __nv_bfloat16*>(a->mask_hi);
-  p.proj_w = a->proj_w;
-  p.proj_b = a->proj_b;
-  p.pq = a->pq;
   p.pool_hi = static_cast<__nv_bfloat16*>(a->pool_hi);
   p.pool_lo = static_cast<__nv_bfloat16*>(a->pool_lo);
   p.colsum = a->colsum;
@@ -190,7 +167,6 @@ static inline void fill_conv_params(ConvParams& p, const osvos_conv3x3_args* a, 
   p.n_blocks = a->cout / block_n;
   p.total_tiles = p.tiles_x * p.tiles_y * a->n * p.n_blocks;
   p.k_chunks = a->cin / kBlockK;
-  p.k_steps = (a->k_valid > 0 && a->k_valid < kBlockK) ? (a->k_valid + 15) / 16 : kBlockK / 16;
   p.flags = a->flags;
   {
     static int ablate = -1;
@@ -220,6 +196,5 @@ int conv_first_tc_launch(const float* x, const float* w_oihw, const float* bias,
                          int w, int flags, cudaStream_t stream);
 int side_conv_dispatch(const osvos_conv3x3_args* a, cudaStream_t stream);
 int side_conv_multi_dispatch(const osvos_conv3x3_args* const* args, int count, cudaStream_t stream);
-int conv3x3_halo_dispatch(const osvos_conv3x3_args* a, cudaStream_t stream);
 
 }  // namespace osvos

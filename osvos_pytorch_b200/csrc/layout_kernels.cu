@@ -1,10 +1,7 @@
 // Bandwidth-bound helper kernels around the tensor-core convolutions:
-// weight packing, NCHW<->act conversion, conv1_1 (Cin = 3), 2x2 ceil-mode max
-// pooling, a CUDA-core reference conv (debug cross-check) and the standalone
-// side-feature projection.
-#include <stdlib.h>
-#include <string.h>
-
+// weight packing, NCHW<->act conversion, 2x2 ceil-mode max pooling, a CUDA-core
+// reference conv (debug cross-check) and the standalone side-feature projection;
+// also the entry point of conv1_1, whose kernel is in conv_first_tc.cu.
 #include "common.cuh"
 
 namespace osvos {
@@ -146,83 +143,6 @@ __global__ void act_to_nchw_kernel(const __nv_bfloat16* __restrict__ hi, const _
     const int nn = static_cast<int>(r / c);
     const size_t src = ((static_cast<size_t>(nn) * h + yy) * w + xx) * c + ch;
     y[i] = __bfloat162float(hi[src]) + (lo ? __bfloat162float(lo[src]) : 0.f);
-  }
-}
-
-// ---------------------------------------------------- conv1_1 (3 -> 64) + ReLU
-// One thread per output pixel, 64 fp32 accumulators, weights broadcast from
-// shared memory as [k = ci*9 + tap][co].  Input read straight from the caller's
-// NCHW fp32 frame (coalesced along x).
-constexpr int kFirstThreads = 128;
-__global__ void __launch_bounds__(kFirstThreads)
-conv_first_kernel(const float* __restrict__ x, const float* __restrict__ wgt, const float* __restrict__ bias,
-                  __nv_bfloat16* __restrict__ y_hi, __nv_bfloat16* __restrict__ y_lo, int n, int h, int w, int relu) {
-  __shared__ __align__(16) float ws[27 * 64];
-  __shared__ float bs[64];
-  for (int i = threadIdx.x; i < 27 * 64; i += kFirstThreads) {
-    const int co = i & 63, k = i >> 6;  // ws[k][co] = w[co][ci][r][s], k = ci*9 + 3r + s
-    ws[i] = wgt[co * 27 + k];
-  }
-  if (threadIdx.x < 64) bs[threadIdx.x] = bias ? bias[threadIdx.x] : 0.f;
-  __syncthreads();
-  const int xx = blockIdx.x * kFirstThreads + threadIdx.x;
-  const int yy = blockIdx.y;
-  const int nn = blockIdx.z;
-  if (xx >= w) return;
-  float in[27];
-#pragma unroll
-  for (int ci = 0; ci < 3; ++ci) {
-    const float* plane = x + (static_cast<size_t>(nn) * 3 + ci) * h * w;
-#pragma unroll
-    for (int r = 0; r < 3; ++r) {
-      const int iy = yy + r - 1;
-#pragma unroll
-      for (int s = 0; s < 3; ++s) {
-        const int ix = xx + s - 1;
-        in[ci * 9 + r * 3 + s] = (iy >= 0 && iy < h && ix >= 0 && ix < w) ? __ldg(plane + static_cast<size_t>(iy) * w + ix) : 0.f;
-      }
-    }
-  }
-  const size_t pix = (static_cast<size_t>(nn) * h + yy) * w + xx;
-#pragma unroll 1
-  for (int c0 = 0; c0 < 64; c0 += 16) {
-    float acc[16];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) acc[j] = bs[c0 + j];
-#pragma unroll
-    for (int k = 0; k < 27; ++k) {
-      const float4* wr = reinterpret_cast<const float4*>(ws + k * 64 + c0);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float4 wv = wr[j];
-        acc[4 * j + 0] = fmaf(in[k], wv.x, acc[4 * j + 0]);
-        acc[4 * j + 1] = fmaf(in[k], wv.y, acc[4 * j + 1]);
-        acc[4 * j + 2] = fmaf(in[k], wv.z, acc[4 * j + 2]);
-        acc[4 * j + 3] = fmaf(in[k], wv.w, acc[4 * j + 3]);
-      }
-    }
-    uint32_t hi[8], lo[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float a = acc[2 * j], b = acc[2 * j + 1];
-      if (relu) {
-        a = fmaxf(a, 0.f);
-        b = fmaxf(b, 0.f);
-      }
-      __nv_bfloat16 h0, l0, h1, l1;
-      split_bf16(a, h0, l0);
-      split_bf16(b, h1, l1);
-      hi[j] = pack_bf16x2(h0, h1);
-      lo[j] = pack_bf16x2(l0, l1);
-    }
-    uint4* dh = reinterpret_cast<uint4*>(y_hi + pix * 64 + c0);
-    dh[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-    dh[1] = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-    if (y_lo) {
-      uint4* dl = reinterpret_cast<uint4*>(y_lo + pix * 64 + c0);
-      dl[0] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-      dl[1] = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-    }
   }
 }
 
@@ -441,18 +361,7 @@ extern "C" int osvos_conv_first_fwd(const float* x, const float* w_oihw, const f
                                     int n, int h, int w, int flags, osvos_stream_t stream) {
   OSVOS_CHECK_ARG(x != nullptr && w_oihw != nullptr && y_hi != nullptr && n > 0 && h > 0 && w > 0);
   OSVOS_CHECK_ARG(h <= 65535 && n <= 65535);
-  {  // default: tensor-core kernel (conv_first_tc.cu); OSVOS_FIRST_IMPL=simt keeps the CUDA-core one as a cross-check
-    const char* impl = getenv("OSVOS_FIRST_IMPL");
-    if (impl == nullptr || strcmp(impl, "simt") != 0)
-      return conv_first_tc_launch(x, w_oihw, bias, y_hi, y_lo, n, h, w, flags, static_cast<cudaStream_t>(stream));
-  }
-  dim3 grid((w + kFirstThreads - 1) / kFirstThreads, h, n);
-  conv_first_kernel<<<grid, kFirstThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-      x, w_oihw, bias, static_cast<__nv_bfloat16*>(y_hi),
-      (flags & OSVOS_FLAG_FAST) ? nullptr : static_cast<__nv_bfloat16*>(y_lo), n, h, w,
-      (flags & OSVOS_FLAG_RELU) ? 1 : 0);
-  OSVOS_CHECK_CUDA(cudaGetLastError());
-  return OSVOS_OK;
+  return conv_first_tc_launch(x, w_oihw, bias, y_hi, y_lo, n, h, w, flags, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int osvos_maxpool2x2_fwd(const void* x_hi, const void* x_lo, void* y_hi, void* y_lo, int n, int h, int w,

@@ -19,7 +19,6 @@ namespace osvos {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
-__device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
 
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
@@ -68,18 +67,6 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// gpu-scope acquire load / release reduction on a global counter (split-K handshake between CTAs)
-__device__ __forceinline__ uint32_t ld_acquire_gpu_u32(const unsigned int* p) {
-  uint32_t v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void red_release_gpu_add_u32(unsigned int* p, uint32_t v) {
-  asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ void st_relaxed_gpu_u32(unsigned int* p, uint32_t v) {
-  asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
 
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
@@ -112,15 +99,6 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* m, uint64_t* bar,
       "r"(c3)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_5d(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, int c2,
-                                            int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2),
-      "r"(c3), "r"(c4)
-      : "memory");
-}
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
@@ -135,20 +113,6 @@ __device__ __forceinline__ void tma_load_3d(const CUtensorMap* m, uint64_t* bar,
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-template <int N>
-__device__ __forceinline__ void tma_store_wait_all() {
-  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
-}
 
 // --------------------------------------------------------------- descriptors
 // wgmma shared-memory matrix descriptor (64 bit):
@@ -158,7 +122,6 @@ __device__ __forceinline__ void tma_store_wait_all() {
 // Descriptors are advanced by ADDING (bytes >> 4): shared-memory addresses stay below 2^18, so the add never carries out
 // of the start-address field.
 constexpr uint64_t kDescSW128 = 1ull << 62;
-constexpr uint64_t kDescSW64 = 2ull << 62;
 __host__ __device__ constexpr uint64_t desc_template(uint32_t lbo_bytes, uint32_t sbo_bytes, uint64_t layout) {
   return (static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16) | (static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32) |
          layout;

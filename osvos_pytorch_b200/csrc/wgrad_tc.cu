@@ -21,8 +21,6 @@
 //
 // Replaces autograd's weight gradient of nn.Conv2d(k=3, p=1)
 // (reference networks/vgg_osvos.py:41,142; backward triggered at train_online.py:141).
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -368,12 +366,7 @@ static int launch_wgrad(const osvos_wgrad_args* a, cudaStream_t stream) {
   // instead of the two of four of tap pairs under a half-empty M.
   // Exact at the borders: the terms dz[u] x[u + (., -1)] the shifted M atom cannot reach (u.x = 0) multiply the zero
   // padding of x, and everything out of the image is zero-filled by TMA on both operands.
-  static int rows_on = -1;   // OSVOS_WGRAD_ROWS=0: tap pairs instead (A/B; read once)
-  if (rows_on < 0) {
-    const char* e = getenv("OSVOS_WGRAD_ROWS");
-    rows_on = (e == nullptr || atoi(e) != 0) ? 1 : 0;
-  }
-  p.tap_rows = (rows_on && cq == 64 && cp == 64 && BLOCK_N == 128) ? 1 : 0;
+  p.tap_rows = (cq == 64 && cp == 64 && BLOCK_N == 128) ? 1 : 0;
   p.tap_pairs = (cq == 64 && BLOCK_N == 128 && !p.tap_rows) ? 1 : 0;
   p.tap_items = p.tap_rows ? 3 : p.tap_pairs ? 5 : 9;
   p.n_blocks = (p.tap_pairs || p.tap_rows) ? 1 : cq / BLOCK_N;
@@ -384,33 +377,22 @@ static int launch_wgrad(const osvos_wgrad_args* a, cudaStream_t stream) {
   const int sms = device_sm_count();
   // Pixel-range splits: items are dealt round-robin to the persistent CTAs, so the kernel lasts as long as the CTA with
   // the most items - ROUNDS x K blocks per item.  Pick the split count that minimises that (plus ~2 K-block times per
-  // item for the accumulator flush that is not hidden behind the next item's MMAs).  The first rule, ceil(2 SMs /
-  // tiles), can land just above a whole number of rounds (one extra round for a single item).
+  // item for the accumulator flush that is not hidden behind the next item's MMAs).  A fixed rule such as ceil(2 SMs /
+  // tiles) can land just above a whole number of rounds (one extra round for a single item).
   const int max_splits = (p.patches_total + 3) / 4;
-  static int split_rule = -1;   // OSVOS_WGRAD_SPLITS=legacy: the first rule (A/B; read once)
-  if (split_rule < 0) {
-    const char* e = getenv("OSVOS_WGRAD_SPLITS");
-    split_rule = (e != nullptr && strcmp(e, "legacy") == 0) ? 1 : 0;
-  }
   int splits = 1;
-  if (split_rule == 1) {
-    splits = (2 * sms + tiles - 1) / tiles;
-  } else {
-    long best = -1;
-    const int s_hi = 4 * sms / tiles + 1;
-    for (int s = 1; s <= s_hi && s <= max_splits; ++s) {
-      const long pps = (p.patches_total + s - 1) / s;
-      const long se = (p.patches_total + pps - 1) / pps;
-      const long rounds = (static_cast<long>(tiles) * se + sms - 1) / sms;
-      const long cost = rounds * (pps + 2) + 4;
-      if (best < 0 || cost < best) {
-        best = cost;
-        splits = s;
-      }
+  long best = -1;
+  const int s_hi = 4 * sms / tiles + 1;
+  for (int s = 1; s <= s_hi && s <= max_splits; ++s) {
+    const long pps = (p.patches_total + s - 1) / s;
+    const long se = (p.patches_total + pps - 1) / pps;
+    const long rounds = (static_cast<long>(tiles) * se + sms - 1) / sms;
+    const long cost = rounds * (pps + 2) + 4;
+    if (best < 0 || cost < best) {
+      best = cost;
+      splits = s;
     }
   }
-  if (splits > max_splits) splits = max_splits;
-  if (splits < 1) splits = 1;
   p.patches_per_split = (p.patches_total + splits - 1) / splits;
   p.splits = (p.patches_total + p.patches_per_split - 1) / p.patches_per_split;
   p.total_items = tiles * p.splits;

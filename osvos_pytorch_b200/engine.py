@@ -34,9 +34,6 @@ class OSVOSEngine:
         # training loops of this package set this: backward adds weight / trunk-bias gradients straight into an
         # existing p.grad (and hands autograd None for them) instead of returning tensors for AccumulateGrad
         self.accumulate_param_grads_in_place = False
-        # inference: fold side_prep with its two 1x1 projections into one 3x3 conv C -> 2 (training always does; OSVOS_FOLD_SIDE=0, read per
-        # eager pass, switches it off for A/B runs)
-        self.fold_side_branch = True
 
     def direct_grad_accumulation(self):
         """Context manager enabling in-place gradient accumulation for the backward passes run inside it."""
@@ -117,10 +114,6 @@ class OSVOSEngine:
         return self._cached(("proj", i), [sd.weight, fu.weight],
                             lambda: torch.cat([sd.weight.detach().reshape(16),
                                                fu.weight.detach().reshape(64)[16 * i:16 * i + 16]]).float().contiguous())
-
-    def _folded_side(self, i):
-        """(packed [2,C,3,3] operand, bias2) of side_prep[i] folded with score_dsn[i] and fuse's slice."""
-        return self._folded_side_all()[i][:2]
 
     def _folded_side_all(self):
         """[(packed operand, bias2, fp32 W' [9,2,C])] of the four side scales, folded by ONE launch and cached on the
@@ -254,16 +247,14 @@ class OSVOSEngine:
     @torch.no_grad()
     def forward_inference(self, x, simt=False, return_intermediates=False):
         """The inference pass (eager, or while a CUDA graph captures it).  Programmatic dependent launch is switched on
-        for its kernels (every one of them waits before touching its predecessor's data, so only prologues overlap);
-        OSVOS_PDL_INFER=0 keeps plain stream order."""
+        for its kernels (every one of them waits before touching its predecessor's data, so only prologues overlap)."""
         from . import _native as nat
         lib = nat.load()
-        prev = lib.osvos_set_pdl(1) if os.environ.get("OSVOS_PDL_INFER", "1") != "0" else None
+        prev = lib.osvos_set_pdl(1)
         try:
             return self._forward_inference(x, simt, return_intermediates)
         finally:
-            if prev is not None:
-                lib.osvos_set_pdl(prev)
+            lib.osvos_set_pdl(prev)
 
     def _forward_inference(self, x, simt=False, return_intermediates=False):
         m = self.m
@@ -288,11 +279,9 @@ class OSVOSEngine:
         if return_intermediates:
             inter["stage0"] = full
         pqs = []
-        fold = not simt and not return_intermediates and self.fold_side_branch and \
-            os.environ.get("OSVOS_FOLD_SIDE", "1") != "0"
-        # folded side branches of the four scales in ONE launch after the last trunk conv (OSVOS_SIDE_MULTI=0: one launch
-        # per scale, right after its stage)
-        multi = fold and os.environ.get("OSVOS_SIDE_MULTI", "1") != "0"
+        # side_prep o (score_dsn, fuse slice) folded into one 3x3 conv C -> 2 (include/osvos_b200.h), the four scales in
+        # ONE launch after the last trunk conv; the side features themselves are only computed on request
+        fold = not simt and not return_intermediates
         stage_outs = []
         for i in range(1, 5):
             convs = [c for c in m.stages[i] if isinstance(c, nn.Conv2d)]
@@ -313,13 +302,9 @@ class OSVOSEngine:
                 _, feat, _ = ops.conv3x3(full, self._packed(sp, f"sp{i}"), sp.bias.detach(), 16, relu=False, fast=fast,
                                          out_act=False, out_f32=True, simt=True)
                 pq = ops.side_project(feat, self._proj(i - 1), m.score_dsn[i - 1].bias.detach())
-            elif multi:
+            elif fold:
                 stage_outs.append(full)
                 continue
-            elif fold:
-                # inference: side_prep o (score_dsn, fuse slice) folded into one 3x3 conv C -> 2 (include/osvos_b200.h)
-                feat = None
-                pq = ops.side_folded(full, *self._folded_side(i - 1), fast=fast)
             else:
                 _, feat, pq = ops.conv3x3(full, self._packed(sp, f"sp{i}"), sp.bias.detach(), 16, relu=False, fast=fast,
                                           out_act=False, out_f32=return_intermediates, proj_w=self._proj(i - 1),
@@ -328,7 +313,7 @@ class OSVOSEngine:
                 inter[f"side{i}"] = feat
                 inter[f"pq{i}"] = pq
             pqs.append(pq)
-        if multi:
+        if fold:
             pqs = ops.side_folded_multi(stage_outs, self._folded_side_all(), fast=fast)
         out, _ = ops.tail_fwd(pqs, m.fuse.bias.detach(), n, h, w)
         outs = [out[k] for k in range(5)]

@@ -192,7 +192,7 @@ def side_folded_multi(xs, folded, fast=False):
 
 
 def conv3x3(x, w_packed, bias, cout, relu=False, fast=False, out_act=True, out_f32=False, mask=None,
-            proj_w=None, proj_b=None, simt=False, pool=False, colsum=None, k_valid=0):
+            proj_w=None, proj_b=None, simt=False, pool=False, colsum=None):
     """3x3 / pad 1 conv of an Act through the wgmma kernel.  Returns (Act|None, f32|None, pq|None), or
     (Act, pooled Act) when pool=True (fused MaxPool2d(2,2,ceil_mode)).  `colsum` ([cout] fp32, pre-zeroed)
     receives the per-channel sum of the output (fused bias gradient)."""
@@ -214,7 +214,6 @@ def conv3x3(x, w_packed, bias, cout, relu=False, fast=False, out_act=True, out_f
     a.pool_hi = nat.ptr(yp.hi) if pool else None
     a.pool_lo = nat.ptr(yp.lo) if pool else None
     a.colsum = nat.ptr(colsum)
-    a.k_valid = k_valid
     a.n, a.h, a.w, a.cin, a.cout = n, h, w, cin, cout
     a.flags = (nat.FLAG_RELU if relu else 0) | (nat.FLAG_FAST if fast else 0) | \
               (nat.FLAG_RELU_MASK if mask is not None else 0)

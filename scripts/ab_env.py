@@ -1,6 +1,6 @@
-"""A/B of a per-launch environment switch of the library inside ONE process - development aid.
+"""A/B of an environment switch the engine reads on every pass, inside ONE process - development aid.
 
-    python scripts/ab_env.py OSVOS_SPLITACC128 1 0 [H W] [--train]
+    python scripts/ab_env.py OSVOS_FUSE_STAGE1 0 1 [H W] [--train]
 
 For each value: the engine's CUDA graphs are dropped and re-captured, 480x854 inference is replayed 200 times over
 four rotating frames (CUDA events), and the five output maps are compared with the first value's.

@@ -1,6 +1,6 @@
 """A/B of programmatic dependent launch (OSVOS_PDL=0 vs 1) on the two graphed hot loops - development aid.
-(Since round 2 the engine switches PDL ON for the inference pass whatever OSVOS_PDL says - osvos_set_pdl, OSVOS_PDL_INFER=0
-to disable; for the inference arm use `scripts/ab_env.py OSVOS_PDL_INFER 1 0`.  OSVOS_PDL still decides the training graph.)
+(The engine switches PDL on for the inference pass whatever OSVOS_PDL says (osvos_set_pdl), so the inference arms should
+match; OSVOS_PDL decides the training graph.)
 
     python scripts/pdl_ab.py [out_dir]
 

@@ -46,6 +46,39 @@ def test_ctypes_table_matches_header(lib_path):
     assert b"invalid argument" in lib.osvos_last_error()
 
 
+@pytest.mark.parametrize("field,rejected_by", [("none", "a->bias"), ("y_hi", "a->cout != 16"), ("y_lo", "a->cout != 16"),
+                                               ("relu_mask", "a->cout != 16"), ("colsum", "a->colsum == nullptr")])
+def test_conv3x3_16_channel_outputs_are_fp32_features_or_projections(lib_path, field, rejected_by):
+    """cout == 16 (side_prep) writes fp32 features and / or projections only; act outputs, ReLU masks and column sums are
+    refused.  Validation runs before any CUDA call.  The bias pointer is misaligned in every case, so a call that passes
+    the cout == 16 checks (the control, "none") stops at the alignment check and never reaches a kernel."""
+    from osvos_pytorch_b200 import _native as nat
+    lib = nat.load()
+    addr = 1 << 20                                   # placeholder device address, never dereferenced
+    a = nat.Conv3x3Args()
+    a.x_hi = a.x_lo = a.w_packed = a.y_f32 = addr
+    a.bias = addr + 4
+    a.n, a.h, a.w, a.cin, a.cout = 1, 8, 8, 64, 16
+    if field == "relu_mask":
+        a.mask_hi, a.flags = addr, nat.FLAG_RELU_MASK
+    elif field != "none":
+        setattr(a, field, addr)
+    assert lib.osvos_conv3x3(ctypes.byref(a), None) == 1
+    msg = lib.osvos_last_error()
+    assert b"invalid argument" in msg and rejected_by.encode() in msg, msg
+
+
+def test_library_reads_only_the_pdl_and_ablation_switches():
+    calls, names = 0, set()
+    for dirpath, _, files in os.walk(os.path.join(ROOT, "osvos_pytorch_b200", "csrc")):
+        for f in files:
+            txt = open(os.path.join(dirpath, f)).read()
+            calls += len(re.findall(r"\bgetenv\s*\(", txt))
+            names |= set(re.findall(r"\bgetenv\s*\(\s*\"(\w+)\"\s*\)", txt))
+    assert names == {"OSVOS_PDL", "OSVOS_ABLATE"}
+    assert calls == 2                                # every getenv call names its variable literally
+
+
 def test_product_package_never_imports_the_oracle():
     pkg = os.path.join(ROOT, "osvos_pytorch_b200")
     for dirpath, _, files in os.walk(pkg):

@@ -57,13 +57,12 @@ CONV_CASES = [
     (1, 33, 45, 64, 128, True),     # several tiles, n_block = 1 of 128
     (1, 9, 11, 256, 256, True),     # two N blocks, four K chunks
     (1, 3, 5, 512, 512, True),      # image smaller than the TMA box
-    (1, 30, 27, 128, 16, False),    # side_prep shape (N = 16)
 ]
 
 
-@pytest.mark.parametrize("n,h,w,cin,cout,relu", CONV_CASES)
-@pytest.mark.parametrize("fast", [False, True])
-def test_conv3x3_tensor_core(dev, n, h, w, cin, cout, relu, fast):
+def _conv_f32_case(dev, n, h, w, cin, cout, relu, fast, out_act):
+    """Seeded conv problem through osvos_conv3x3 with an fp32 output, checked against fp64 and against the CUDA-core
+    kernel on identical operands.  Returns (operands, act output or None, fp32 output as NCHW)."""
     from osvos_pytorch_b200 import ops
     g = torch.Generator().manual_seed(100 + h * w + cin)
     x = torch.randn(n, cin, h, w, generator=g) * 3.0
@@ -74,18 +73,37 @@ def test_conv3x3_tensor_core(dev, n, h, w, cin, cout, relu, fast):
         ref = ref.relu()
     a = ops.nchw_to_act(x.to(dev), fast)
     wp = ops.pack_conv3x3_weights(wt.to(dev))
-    y, yf, _ = ops.conv3x3(a, wp, b.to(dev), cout, relu=relu, fast=fast, out_act=True, out_f32=True)
+    y, yf, _ = ops.conv3x3(a, wp, b.to(dev), cout, relu=relu, fast=fast, out_act=out_act, out_f32=True)
     torch.cuda.synchronize()
     got_f32 = yf.permute(0, 3, 1, 2).cpu()
-    got_act = ops.act_to_nchw(y).cpu()
     tol = FAST_TOL if fast else EXACT_TOL
     assert maxrel(got_f32, ref) < tol, (maxrel(got_f32, ref), rmsrel(got_f32, ref))
-    # the act output is the split rounding of the fp32 result
-    want_act = split_round(got_f32) if not fast else got_f32.to(torch.bfloat16).float()
-    assert torch.equal(got_act, want_act)
-    # CUDA-core cross-check on identical operands
     _, ys, _ = ops.conv3x3(a, wp, b.to(dev), cout, relu=relu, fast=fast, out_act=False, out_f32=True, simt=True)
     assert maxrel(got_f32, ys.permute(0, 3, 1, 2).cpu()) < 2e-5
+    return (a, wp, b.to(dev)), y, got_f32
+
+
+@pytest.mark.parametrize("n,h,w,cin,cout,relu", CONV_CASES)
+@pytest.mark.parametrize("fast", [False, True])
+def test_conv3x3_tensor_core(dev, n, h, w, cin, cout, relu, fast):
+    from osvos_pytorch_b200 import ops
+    (a, wp, b), y, got_f32 = _conv_f32_case(dev, n, h, w, cin, cout, relu, fast, out_act=True)
+    # the act output is the split rounding of the fp32 result
+    want_act = split_round(got_f32) if not fast else got_f32.to(torch.bfloat16).float()
+    assert torch.equal(ops.act_to_nchw(y).cpu(), want_act)
+    # act output only: the lean epilogue of plain forward launches, bit-identical to the general one
+    y_lean, _, _ = ops.conv3x3(a, wp, b, cout, relu=relu, fast=fast, out_act=True)
+    assert torch.equal(y_lean.hi, y.hi)
+    assert y.lo is None or torch.equal(y_lean.lo, y.lo)
+
+
+@pytest.mark.parametrize("fast", [False, True])
+def test_conv3x3_side_prep_fp32_output(dev, fast):
+    """side_prep shape (16 outputs, no ReLU, side-branch kernel): fp32 features only; an act output is refused."""
+    from osvos_pytorch_b200 import _native as nat, ops
+    (a, wp, b), _, _ = _conv_f32_case(dev, 1, 30, 27, 128, 16, False, fast, out_act=False)
+    with pytest.raises(nat.NativeLibraryError, match="invalid argument"):
+        ops.conv3x3(a, wp, b, 16, fast=fast, out_act=True, out_f32=True)
 
 
 def test_conv3x3_outputs_need_only_element_pair_alignment(dev):

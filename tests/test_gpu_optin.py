@@ -1,10 +1,8 @@
-"""The library's alternative code paths against the default path (and through it the oracle): the general epilogue instead
-of the lean one (OSVOS_HALO_LEAN=0), the three-pass accumulator (OSVOS_SPLITACC128=0), no 256-wide tiles (OSVOS_CONV_N256=0), the unfolded side branch (OSVOS_FOLD_SIDE=0), separate conv1_1 and
-conv1_2 kernels (OSVOS_FUSE_STAGE1=0, the default) and the fused stage-1 kernel (OSVOS_FUSE_STAGE1=1).
+"""The engine's opt-in stage-1 path against the default path (and through it the oracle): separate conv1_1 and conv1_2
+kernels (OSVOS_FUSE_STAGE1=0, the default) and the fused stage-1 kernel (OSVOS_FUSE_STAGE1=1).
 
-Every switch is re-read per launch under OSVOS_ENV_RELOAD=1 (tests/conftest.py), so one process can flip it; CUDA graphs
-are off for the comparison.  Variants that only change which code is compiled into the epilogue must reproduce the default
-bit for bit; variants that change the fp32 summation order within float reassociation noise.
+The engine reads the switch on every eager pass, so one process can flip it; CUDA graphs are off for the comparison.  The
+fused kernel sums conv1_1 in another fp32 order, so the outputs agree within float reassociation noise.
 """
 import os
 
@@ -16,7 +14,7 @@ from gpu_util import maxrel
 
 pytestmark = [pytest.mark.gpu]
 
-VARIANTS = [("OSVOS_HALO_LEAN", "0", 0.0), ("OSVOS_SPLITACC128", "0", 1e-4), ("OSVOS_CONV_N256", "0", 1e-4), ("OSVOS_FOLD_SIDE", "0", 1e-4), ("OSVOS_FUSE_STAGE1", "0", 1e-4), ("OSVOS_FUSE_STAGE1", "1", 1e-4)]
+VARIANTS = [("OSVOS_FUSE_STAGE1", "0", 1e-4), ("OSVOS_FUSE_STAGE1", "1", 1e-4)]
 
 
 @pytest.fixture(scope="module")
