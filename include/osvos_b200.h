@@ -412,6 +412,35 @@ enum { OSVOS_WARP_CUBIC = 0, OSVOS_WARP_NEAREST = 1 };
 OSVOS_API int osvos_affine_warp(const float* src, float* dst, const double* inv_matrices_host, const int* flips_host,
                                 int n, int c, int h, int w, int mode, osvos_stream_t stream);
 
+/* ---- ingest of decoded frames (dataloaders/davis_2016.py:88-108 make_img_gt_pair, custom_transforms.py:103-122
+ * ToTensor) ------------------------------------------------------------------------------------------------------
+ * The host decodes with cv2.imread and copies the uint8 bytes; everything after the decode runs here, bit-identical
+ * to the reference's float arithmetic.  Any h, w and source alignment; n < 65536.
+ *   osvos_image_from_bgr8: src [n][h][w][3] uint8 (BGR, as cv2.imread returns it) -> dst [n][3][h][w] fp32,
+ *                          dst = float(v) - mean[c] with one fp32 rounding (np.subtract of two float32 arrays).
+ *   osvos_label_stats_u8:  src [n][h][w] uint8 mask -> stats [n][2] = {max byte, binary flag}; the flag is 1 when every
+ *                          byte is 0 or the max, i.e. the normalised mask is all 0 / 1.  Zeroes stats itself; run it
+ *                          before the two calls below that read stats.
+ *   osvos_label_from_u8:   dst [n][1][h][w] fp32 = float(v) / max(float(max), 1e-8f) (gt / np.max([gt.max(), 1e-8]),
+ *                          rounded to fp32).
+ *   osvos_affine_warp_u8:  RandomHorizontalFlip + ScaleNRotate of the ingested tensors read straight from the bytes,
+ *                          same matrices and arithmetic as osvos_affine_warp.  Image (image_src -> image_dst
+ *                          [n][3][h][w]): cubic over mean-subtracted taps, so the border is 0 of the mean-subtracted
+ *                          image; bit-identical to osvos_image_from_bgr8 + osvos_affine_warp(CUBIC).  Mask (label_src,
+ *                          label_stats -> label_dst [n][1][h][w]): nearest where the sample's binary flag is set, cubic
+ *                          otherwise (custom_transforms.py:46-49), chosen on the device; bit-identical to
+ *                          osvos_label_from_u8 + osvos_affine_warp in that mode.  Either tensor may be NULL (all three
+ *                          label pointers together).                                                               */
+OSVOS_API int osvos_image_from_bgr8(const uint8_t* src, float* dst, int n, int h, int w, float mean_b, float mean_g,
+                                    float mean_r, osvos_stream_t stream);
+OSVOS_API int osvos_label_stats_u8(const uint8_t* src, uint32_t* stats, int n, int h, int w, osvos_stream_t stream);
+OSVOS_API int osvos_label_from_u8(const uint8_t* src, const uint32_t* stats, float* dst, int n, int h, int w,
+                                  osvos_stream_t stream);
+OSVOS_API int osvos_affine_warp_u8(const uint8_t* image_src, const uint8_t* label_src, const uint32_t* label_stats,
+                                   float* image_dst, float* label_dst, const double* inv_matrices_host,
+                                   const int* flips_host, int n, int h, int w, float mean_b, float mean_g, float mean_r,
+                                   osvos_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

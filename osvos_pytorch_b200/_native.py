@@ -143,6 +143,11 @@ SIGNATURES = {
     "osvos_sgd_step": (c_int, [c_void_p, c_int, c_uint32, c_int, c_void_p]),
     "osvos_affine_warp": (c_int, [c_void_p, c_void_p, POINTER(c_double), POINTER(c_int), c_int, c_int, c_int, c_int,
                                   c_int, c_void_p]),
+    "osvos_image_from_bgr8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_float, c_float, c_void_p]),
+    "osvos_label_stats_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "osvos_label_from_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "osvos_affine_warp_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_double), POINTER(c_int),
+                                     c_int, c_int, c_int, c_float, c_float, c_float, c_void_p]),
 }
 
 _lib = None

@@ -48,12 +48,8 @@ def draw_params(n, rots=(-30, 30), scales=(.75, 1.25), rng=random):
     return out
 
 
-def affine_warp(x, params, mode):
-    """x [n,c,h,w] fp32 CUDA -> warped copy.  params: list of n (flip, rot_degrees, scale); mode 'cubic'|'nearest'."""
-    lib = nat.load()
-    ops._require_cuda(x, "x")
-    x = x.contiguous().float()
-    n, c, h, w = (int(v) for v in x.shape)
+def _warp_tables(params, n, h, w):
+    """Host tables of osvos_affine_warp*: n inverted 2x3 matrices and n flip flags."""
     if len(params) != n:
         raise ValueError("one (flip, rot, scale) triple per sample")
     mats = (ctypes.c_double * (6 * n))()
@@ -62,6 +58,16 @@ def affine_warp(x, params, mode):
         inv = invert_affine(rotation_matrix((w / 2, h / 2), rot, sc))
         mats[6 * i:6 * i + 6] = inv
         flips[i] = int(bool(flip))
+    return mats, flips
+
+
+def affine_warp(x, params, mode):
+    """x [n,c,h,w] fp32 CUDA -> warped copy.  params: list of n (flip, rot_degrees, scale); mode 'cubic'|'nearest'."""
+    lib = nat.load()
+    ops._require_cuda(x, "x")
+    x = x.contiguous().float()
+    n, c, h, w = (int(v) for v in x.shape)
+    mats, flips = _warp_tables(params, n, h, w)
     out = torch.empty_like(x)
     ops._count((n + 31) // 32)
     with torch.cuda.device(x.device):
@@ -77,3 +83,27 @@ def augment_batch(sample, rots=(-30, 30), scales=(.75, 1.25), rng=random, params
     n = int(sample["image"].shape[0])
     params = draw_params(n, rots, scales, rng) if params is None else params
     return {"image": affine_warp(sample["image"], params, "cubic"), "gt": affine_warp(sample["gt"], params, "nearest")}
+
+
+def affine_warp_u8(image_u8, gt_u8, params, stats=None, meanval=ops.MEANVAL):
+    """RandomHorizontalFlip + ScaleNRotate straight from decoded bytes: image_u8 uint8 [n,h,w,3] BGR and gt_u8 uint8
+    [n,h,w] on the GPU -> {'image': f32 [n,3,h,w], 'gt': f32 [n,1,h,w]}, bit-identical to ingesting them
+    (ops.image_from_bgr8 / ops.label_from_u8) and then warping with affine_warp.  The image is warped bicubic; each mask
+    nearest if it is binary and bicubic otherwise, the reference's per-sample rule (custom_transforms.py:46-49), decided
+    on the device from ``stats`` (ops.label_stats_u8, computed here when None)."""
+    lib = nat.load()
+    img = ops._require_u8(image_u8, "image_u8", 4)
+    gt = ops._require_u8(gt_u8, "gt_u8", 3)
+    n, h, w, c = (int(v) for v in img.shape)
+    if c != 3 or tuple(gt.shape) != (n, h, w):
+        raise ValueError("image_u8 must be [n,h,w,3] and gt_u8 [n,h,w]")
+    mats, flips = _warp_tables(params, n, h, w)
+    stats = ops.label_stats_u8(gt) if stats is None else stats
+    out_i = torch.empty((n, 3, h, w), dtype=torch.float32, device=img.device)
+    out_g = torch.empty((n, 1, h, w), dtype=torch.float32, device=img.device)
+    ops._count(2 * ((n + 31) // 32))
+    with torch.cuda.device(img.device):
+        nat.check(lib.osvos_affine_warp_u8(img.data_ptr(), gt.data_ptr(), stats.data_ptr(), out_i.data_ptr(),
+                                           out_g.data_ptr(), mats, flips, n, h, w, *(float(m) for m in meanval),
+                                           torch.cuda.current_stream().cuda_stream), "osvos_affine_warp_u8")
+    return {"image": out_i, "gt": out_g}

@@ -1,74 +1,7 @@
-// Device-side ScaleNRotate + RandomHorizontalFlip (reference dataloaders/custom_transforms.py:7-54, :87-100):
-// one gather kernel per tensor, a restatement of OpenCV's warpAffine (fixed-point coordinates, 1/32-pixel bicubic
-// table with A = -0.75, BORDER_CONSTANT 0).  HBM-bound: every destination pixel reads a 4x4 (cubic) or 1x1
+// Device-side ScaleNRotate + RandomHorizontalFlip (reference dataloaders/custom_transforms.py:7-54, :87-100) on fp32
+// tensors: one gather kernel per tensor (warp.cuh).  HBM-bound: every destination pixel reads a 4x4 (cubic) or 1x1
 // (nearest) source window through L1/L2; stores are coalesced along x.
-#include "common.cuh"
-
-namespace osvos {
-
-constexpr int kWarpMaxSamples = 32;
-struct WarpTable {
-  double m[kWarpMaxSamples][6];
-  int flip[kWarpMaxSamples];
-};
-
-__device__ __forceinline__ void cubic_coeffs(float x, float* c) {
-  const float A = -0.75f;
-  c[0] = ((A * (x + 1.f) - 5.f * A) * (x + 1.f) + 8.f * A) * (x + 1.f) - 4.f * A;
-  c[1] = ((A + 2.f) * x - (A + 3.f)) * x * x + 1.f;
-  c[2] = ((A + 2.f) * (1.f - x) - (A + 3.f)) * (1.f - x) * (1.f - x) + 1.f;
-  c[3] = 1.f - c[0] - c[1] - c[2];
-}
-
-__global__ void __launch_bounds__(256)
-affine_warp_kernel(const float* __restrict__ src, float* __restrict__ dst, const __grid_constant__ WarpTable t,
-                   int sample0, int c, int h, int w, int mode) {
-  const int s = blockIdx.z;
-  const int y = blockIdx.y;
-  const int x = blockIdx.x * blockDim.x + threadIdx.x;
-  if (x >= w) return;
-  const double* m = t.m[s];
-  const int flip = t.flip[s];
-  const int round_delta = mode == OSVOS_WARP_NEAREST ? 512 : 16;
-  const int X0 = __double2int_rn((m[1] * y + m[2]) * 1024.0) + round_delta;
-  const int Y0 = __double2int_rn((m[4] * y + m[5]) * 1024.0) + round_delta;
-  const int Xf = X0 + __double2int_rn(m[0] * x * 1024.0);
-  const int Yf = Y0 + __double2int_rn(m[3] * x * 1024.0);
-  const size_t plane = static_cast<size_t>(h) * w;
-  const float* sbase = src + static_cast<size_t>(sample0 + s) * c * plane;
-  float* dbase = dst + static_cast<size_t>(sample0 + s) * c * plane + static_cast<size_t>(y) * w + x;
-  if (mode == OSVOS_WARP_NEAREST) {
-    const int sx = Xf >> 10, sy = Yf >> 10;
-    const bool in = sx >= 0 && sx < w && sy >= 0 && sy < h;
-    const int ux = flip ? w - 1 - sx : sx;
-    for (int ch = 0; ch < c; ++ch) dbase[ch * plane] = in ? __ldg(sbase + ch * plane + static_cast<size_t>(sy) * w + ux) : 0.f;
-    return;
-  }
-  const int X = Xf >> 5, Y = Yf >> 5;
-  const int sx = (X >> 5) - 1, sy = (Y >> 5) - 1;
-  float cx[4], cy[4];
-  cubic_coeffs(static_cast<float>(X & 31) * (1.f / 32.f), cx);
-  cubic_coeffs(static_cast<float>(Y & 31) * (1.f / 32.f), cy);
-  for (int ch = 0; ch < c; ++ch) {
-    const float* sp = sbase + ch * plane;
-    float sum = 0.f;
-#pragma unroll
-    for (int ky = 0; ky < 4; ++ky) {
-      const int yy = sy + ky;
-      if (yy < 0 || yy >= h) continue;
-#pragma unroll
-      for (int kx = 0; kx < 4; ++kx) {
-        const int xx = sx + kx;
-        if (xx < 0 || xx >= w) continue;
-        const int ux = flip ? w - 1 - xx : xx;
-        sum += __ldg(sp + static_cast<size_t>(yy) * w + ux) * (cy[ky] * cx[kx]);
-      }
-    }
-    dbase[ch * plane] = sum;
-  }
-}
-
-}  // namespace osvos
+#include "warp.cuh"
 
 using namespace osvos;
 
@@ -77,17 +10,6 @@ extern "C" int osvos_affine_warp(const float* src, float* dst, const double* inv
   OSVOS_CHECK_ARG(src != nullptr && dst != nullptr && src != dst && inv_matrices_host != nullptr);
   OSVOS_CHECK_ARG(n > 0 && c > 0 && h > 0 && w > 0 && h < 32768 && w < 32768);
   OSVOS_CHECK_ARG(mode == OSVOS_WARP_CUBIC || mode == OSVOS_WARP_NEAREST);
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  for (int s0 = 0; s0 < n; s0 += kWarpMaxSamples) {
-    const int cnt = n - s0 < kWarpMaxSamples ? n - s0 : kWarpMaxSamples;
-    WarpTable t;
-    for (int i = 0; i < cnt; ++i) {
-      for (int k = 0; k < 6; ++k) t.m[i][k] = inv_matrices_host[static_cast<size_t>(s0 + i) * 6 + k];
-      t.flip[i] = flips_host ? flips_host[s0 + i] : 0;
-    }
-    const dim3 grid((w + 255) / 256, h, cnt);
-    affine_warp_kernel<<<grid, 256, 0, stream>>>(src, dst, t, s0, c, h, w, mode);
-    OSVOS_CHECK_CUDA(cudaGetLastError());
-  }
-  return OSVOS_OK;
+  return launch_affine_warp(WarpSrcF32{src, c, h, w}, dst, inv_matrices_host, flips_host, n, c, h, w, mode,
+                            static_cast<cudaStream_t>(stream_));
 }

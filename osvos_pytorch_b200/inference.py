@@ -16,38 +16,53 @@ from . import ops
 class SequenceSegmenter:
     """``for result in SequenceSegmenter(net)(frames): ...`` - ``frames`` yields host tensors [N,3,H,W] fp32 (pinned
     for real overlap); ``result`` is a pinned host tensor [N,1,H,W] (fp32 logits or uint8) that stays valid until
-    ``depth`` further frames have been consumed.  All frames of one call must share a shape."""
+    ``depth`` further frames have been consumed.  All frames of one call must share a shape.
 
-    def __init__(self, net, output="logits", depth=3):
+    ``frames="bgr8"``: the frames are decoded uint8 [N,H,W,3] BGR (what cv2.imread returns) instead; only those bytes
+    cross PCIe, and ops.image_from_bgr8 (float conversion and ``meanval`` subtraction, bit-identical to the reference's
+    dataset) fills the same fp32 ring slot on the compute stream before the forward."""
+
+    def __init__(self, net, output="logits", depth=3, frames="nchw_f32", meanval=ops.MEANVAL):
         if output not in ("logits", "bytescale", "prob", "mask"):
             raise ValueError("output must be one of logits / bytescale / prob / mask")
+        if frames not in ("nchw_f32", "bgr8"):
+            raise ValueError("frames must be nchw_f32 or bgr8")
         self.net, self.output, self.depth = net, output, max(2, int(depth))
+        self.frames, self.meanval = frames, tuple(meanval)
         self._shape = None
 
     def _allocate(self, shape, device):
-        n, _, h, w = shape
+        if self.frames == "bgr8":
+            n, h, w, _ = shape
+            self._dev_raw = [torch.empty(shape, dtype=torch.uint8, device=device) for _ in range(self.depth)]
+        else:
+            n, _, h, w = shape
         out_dtype = torch.float32 if self.output == "logits" else torch.uint8
-        self._dev_in = [torch.empty(shape, dtype=torch.float32, device=device) for _ in range(self.depth)]
+        self._dev_in = [torch.empty((n, 3, h, w), dtype=torch.float32, device=device) for _ in range(self.depth)]
         self._dev_out = [torch.empty((n, 1, h, w), dtype=out_dtype, device=device) for _ in range(self.depth)]
         self._host_out = [torch.empty((n, 1, h, w), dtype=out_dtype).pin_memory() for _ in range(self.depth)]
         self._s_in, self._s_out = torch.cuda.Stream(device), torch.cuda.Stream(device)
         mk = lambda: [torch.cuda.Event() for _ in range(self.depth)]
         self._ev_loaded, self._ev_consumed, self._ev_done, self._ev_host = mk(), mk(), mk(), mk()
         self._shape = tuple(shape)
-        self.h2d_bytes_per_frame = n * 3 * h * w * 4
+        self.h2d_bytes_per_frame = n * 3 * h * w * (1 if self.frames == "bgr8" else 4)
         self.d2h_bytes_per_frame = n * h * w * (4 if self.output == "logits" else 1)
 
     def _submit(self, i, frame, device):
         k = i % self.depth
         cur = torch.cuda.current_stream(device)
+        bgr8 = self.frames == "bgr8"
         with torch.cuda.stream(self._s_in):
             if i >= self.depth:
                 self._s_in.wait_event(self._ev_consumed[k])     # the network has read the previous tenant
-            self._dev_in[k].copy_(frame, non_blocking=True)
+            (self._dev_raw[k] if bgr8 else self._dev_in[k]).copy_(frame, non_blocking=True)
             self._ev_loaded[k].record(self._s_in)
         cur.wait_event(self._ev_loaded[k])
         if i >= self.depth:
             cur.wait_event(self._ev_host[k])                    # previous result of this slot is on the host
+        if bgr8:
+            # same slot address every time this slot comes round, so the engine's direct graph replay still applies
+            ops.image_from_bgr8(self._dev_raw[k], self.meanval, out=self._dev_in[k])
         with torch.no_grad():
             eng = getattr(self.net, "_engine", None)
             if eng is not None:
@@ -77,6 +92,8 @@ class SequenceSegmenter:
             for frame in frames:
                 if frame.dim() == 3:
                     frame = frame.unsqueeze(0)
+                if self.frames == "bgr8" and (frame.dtype != torch.uint8 or frame.shape[-1] != 3):
+                    raise ValueError("frames='bgr8' takes uint8 [N,H,W,3] frames")
                 if self._shape != tuple(frame.shape):
                     if submitted:
                         raise ValueError("all frames of one sequence must share a shape")

@@ -8,6 +8,8 @@ import torch
 from . import _native as nat
 
 
+MEANVAL = (104.00699, 116.66877, 122.67892)      # dataloaders/davis_2016.py:19 of the reference (BGR)
+
 # number of native kernels enqueued since import (bench.py reports the per-step delta)
 KERNEL_LAUNCHES = [0]
 
@@ -498,4 +500,53 @@ def logits_to_u8(logits, mode="bytescale", out=None):
     _count(3 if mode == "bytescale" else 1)
     nat.check(lib.osvos_logits_to_u8(x.data_ptr(), out.data_ptr(), nat.ptr(ws), frames, per, _U8_MODES[mode], _stream()),
               "osvos_logits_to_u8")
+    return out
+
+
+def _require_u8(t, name, dims):
+    _require_cuda(t, name)
+    if t.dtype != torch.uint8 or t.dim() != dims:
+        raise ValueError(f"{name} must be a uint8 tensor with {dims} dimensions, got {t.dtype} {tuple(t.shape)}")
+    return t.contiguous()
+
+
+def image_from_bgr8(frames, meanval=MEANVAL, out=None):
+    """Decoded frames uint8 [N,H,W,3] (BGR, as cv2.imread returns them) -> fp32 [N,3,H,W] = float(v) - meanval[c], the
+    reference's make_img_gt_pair + ToTensor (dataloaders/davis_2016.py:101-102), bit for bit."""
+    lib = nat.load()
+    x = _require_u8(frames, "frames", 4)
+    n, h, w, c = (int(v) for v in x.shape)
+    if c != 3:
+        raise ValueError("frames must be [N,H,W,3]")
+    if out is None:
+        out = torch.empty((n, 3, h, w), dtype=torch.float32, device=x.device)
+    _count()
+    nat.check(lib.osvos_image_from_bgr8(x.data_ptr(), out.data_ptr(), n, h, w, *(float(m) for m in meanval), _stream()),
+              "osvos_image_from_bgr8")
+    return out
+
+
+def label_stats_u8(masks):
+    """uint8 masks [N,H,W] -> int32 [N,2] on the device: {max byte, 1 if every byte is 0 or the max}."""
+    lib = nat.load()
+    x = _require_u8(masks, "masks", 3)
+    n, h, w = (int(v) for v in x.shape)
+    stats = torch.empty((n, 2), dtype=torch.int32, device=x.device)
+    _count(3)
+    nat.check(lib.osvos_label_stats_u8(x.data_ptr(), stats.data_ptr(), n, h, w, _stream()), "osvos_label_stats_u8")
+    return stats
+
+
+def label_from_u8(masks, stats=None, out=None):
+    """uint8 masks [N,H,W] -> fp32 [N,1,H,W] = v / max(frame max, 1e-8), the reference's gt normalisation
+    (dataloaders/davis_2016.py:104-106) rounded to fp32, bit for bit.  ``stats``: label_stats_u8 of the same masks."""
+    lib = nat.load()
+    x = _require_u8(masks, "masks", 3)
+    n, h, w = (int(v) for v in x.shape)
+    stats = label_stats_u8(x) if stats is None else stats
+    if out is None:
+        out = torch.empty((n, 1, h, w), dtype=torch.float32, device=x.device)
+    _count()
+    nat.check(lib.osvos_label_from_u8(x.data_ptr(), stats.data_ptr(), out.data_ptr(), n, h, w, _stream()),
+              "osvos_label_from_u8")
     return out

@@ -5,8 +5,7 @@ data-parallel exchange step (train_parent.py:129-176 + parallel.py)."""
 import torch
 
 from .layers.osvos_layers import class_balanced_cross_entropy_loss
-
-MEANVAL = (104.00699, 116.66877, 122.67892)      # dataloaders/davis_2016.py:19 of the reference
+from .ops import MEANVAL  # noqa: F401  (dataloaders/davis_2016.py:19 of the reference)
 ONLINE_WEIGHTS = (0.0, 0.0, 0.0, 0.0, 1.0)       # train_online.py:127: only the fused map is supervised
 
 

@@ -3,7 +3,8 @@
 train_online.py: load the parent model, run nAveGrad x 2000 forward/backward passes on the annotated
 first frame with SGD(lr 1e-8, momentum .9), save the weights, then segment the sequence.
 
-    SEQ_NAME=blackswan python train_online.py                 # DAVIS on disk (needs cv2 + the dataset)
+    SEQ_NAME=blackswan python train_online.py --loader native # DAVIS on disk (needs cv2 + the dataset)
+    SEQ_NAME=blackswan python train_online.py                 # the same through the reference's dataloaders package
     python train_online.py --synthetic --iters 200            # synthetic 480x854 frame, no dataset
 
 Single GPU by design (BASELINE.json: online fine-tune stays single-GPU; run one sequence per GPU)."""
@@ -19,7 +20,7 @@ from mypath import Path
 from osvos_pytorch_b200 import training
 
 
-def parse():
+def parse(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--seq-name", default=os.environ.get("SEQ_NAME", "blackswan"))
     ap.add_argument("--n-ave-grad", type=int, default=5)
@@ -40,11 +41,15 @@ def parse():
     ap.add_argument("--gpu-augment", action="store_true",
                     help="RandomHorizontalFlip + ScaleNRotate on the device (osvos_pytorch_b200.augment) on the "
                          "GPU-resident annotated frame instead of cv2 in a DataLoader worker")
-    return ap.parse_args()
+    ap.add_argument("--loader", default="reference", choices=["reference", "native"],
+                    help="real data: the reference's dataloaders package (reference), or osvos_pytorch_b200.davis "
+                         "(native: cv2 decodes, the device ingests and augments; the augmentation is always on the "
+                         "device)")
+    return ap.parse_args(argv)
 
 
-def main():
-    a = parse()
+def main(argv=None):
+    a = parse(argv)
     iters = a.iters if a.iters is not None else 2000 * a.n_ave_grad
     if a.lr is None:
         a.lr = 1e-10 if a.synthetic else 1e-8
@@ -79,6 +84,23 @@ def main():
             def sample_fn(it):
                 return fixed
         test_frames = [fixed]
+    elif a.loader == "native":
+        # the annotated frame is decoded once and stays on the device as bytes; every iteration draws a flip, rotation
+        # and scale (the reference's order) and the fused warp ingests and augments it in one pass
+        import random
+        from torch.utils.data import DataLoader
+        from osvos_pytorch_b200 import augment, davis
+        first = davis.DAVIS2016Frames(train=True, db_root_dir=Path.db_root_dir(), seq_name=a.seq_name)
+        img_u8, gt_u8, stats = davis.upload(davis.collate([first[0]]), device)
+        rng = random.Random(a.seed)
+
+        def sample_fn(it):
+            return augment.affine_warp_u8(img_u8, gt_u8, augment.draw_params(1, rng=rng), stats)
+        db_test = davis.DAVIS2016Frames(train=False, db_root_dir=Path.db_root_dir(), seq_name=a.seq_name)
+        # pinned here, between forwards, not by a loader thread that could allocate during a graph capture
+        test_frames = ({"image": davis.views(davis.pinned(b["data"]), *(int(v) for v in b["size"]))[0],
+                        "fname": b["fname"]}
+                       for b in DataLoader(db_test, batch_size=1, shuffle=False, num_workers=1, collate_fn=davis.collate))
     else:
         from dataloaders import davis_2016 as db
         from dataloaders import custom_transforms as tr
@@ -138,7 +160,8 @@ def main():
             n = int(s["image"].shape[0])
             names.append([os.path.basename(s["fname"][jj]) if "fname" in s else f"{ii:05d}_{jj}" for jj in range(n)])
             yield s["image"]
-    for pred in SequenceSegmenter(net, output="bytescale")(frames()):
+    native = a.loader == "native" and not a.synthetic
+    for pred in SequenceSegmenter(net, output="bytescale", frames="bgr8" if native else "nchw_f32")(frames()):
         arr = pred.numpy()
         for jj, name in enumerate(names.popleft()):
             try:

@@ -20,7 +20,20 @@ from mypath import Path
 from osvos_pytorch_b200 import parallel, training
 
 
-def parse():
+class _Mapped:
+    """A re-iterable view of a DataLoader with ``fn`` applied to every batch (keeps ``len``)."""
+
+    def __init__(self, loader, fn):
+        self.loader, self.fn = loader, fn
+
+    def __len__(self):
+        return len(self.loader)
+
+    def __iter__(self):
+        return (self.fn(b) for b in self.loader)
+
+
+def parse(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--epochs", type=int, default=240)
     ap.add_argument("--resume-epoch", type=int, default=0)
@@ -38,11 +51,15 @@ def parse():
     ap.add_argument("--height", type=int, default=480)
     ap.add_argument("--width", type=int, default=854)
     ap.add_argument("--model-name", default="parent")
-    return ap.parse_args()
+    ap.add_argument("--loader", default="reference", choices=["reference", "native"],
+                    help="real data: the reference's dataloaders package (reference), or osvos_pytorch_b200.davis "
+                         "(native: workers only decode; ingest and augmentation run on the device)")
+    ap.add_argument("--workers", type=int, default=2, help="DataLoader decode workers per rank")
+    return ap.parse_args(argv)
 
 
-def main():
-    a = parse()
+def main(argv=None):
+    a = parse(argv)
     rank, world, local = parallel.init_distributed()
     device = torch.device("cuda", local)
     torch.cuda.set_device(device)
@@ -73,6 +90,26 @@ def main():
             for i in range(rank * per, (rank + 1) * per):
                 yield training.synthetic_batch(a.batch, a.height, a.width, 7919 * epoch + i, device)
         val_batches = None
+    elif a.loader == "native":
+        import random
+        from torch.utils.data import DataLoader
+        from torch.utils.data.distributed import DistributedSampler
+        from osvos_pytorch_b200 import davis
+        db_train = davis.DAVIS2016Frames(train=True, db_root_dir=Path.db_root_dir())
+        sampler = DistributedSampler(db_train, world, rank, shuffle=True, drop_last=True) if world > 1 else None
+        loader = DataLoader(db_train, batch_size=a.batch, shuffle=sampler is None, sampler=sampler, num_workers=a.workers,
+                            drop_last=world > 1, collate_fn=davis.collate,
+                            persistent_workers=a.workers > 0)
+        db_test = davis.DAVIS2016Frames(train=False, db_root_dir=Path.db_root_dir())
+        # no pin_memory=True: to_device pins in this thread (davis.pinned says why)
+        val_loader = DataLoader(db_test, batch_size=1, shuffle=False, num_workers=a.workers, collate_fn=davis.collate)
+        val_batches = _Mapped(val_loader, lambda b: davis.to_device(b, device))
+
+        def epoch_batches(epoch):
+            if sampler is not None:
+                sampler.set_epoch(epoch)
+            for b in loader:      # flip / rotation / scale drawn from Python's random, as the reference's transforms do
+                yield davis.to_device(b, device, augment=random)
     else:
         from dataloaders import davis_2016 as db
         from dataloaders import custom_transforms as tr
