@@ -441,6 +441,24 @@ OSVOS_API int osvos_affine_warp_u8(const uint8_t* image_src, const uint8_t* labe
                                    const int* flips_host, int n, int h, int w, float mean_b, float mean_g, float mean_r,
                                    osvos_stream_t stream);
 
+/* ---- DAVIS-2016 region and boundary measures (J and F; DESIGN.md §14) -------------------------------------------
+ * Per frame, P = logit > 0 (±0.0 is background, as osvos_logits_to_u8 mode MASK) and G = byte != 0.  The boundary map
+ * of a mask is b = seg^E | seg^S | seg^SE (E, S, SE: the right, lower and lower-right neighbour, zeros past the frame),
+ * with the last row = seg^E, the last column = seg^S and the last pixel 0.  Each boundary map is dilated by the disk
+ * dx² + dy² <= r² (pixels outside the frame are background) and ANDed with the other one.
+ *   osvos_davis_measures: logits [n][h][w] fp32 (4-byte aligned), masks [n][h][w] uint8 (any alignment) ->
+ *                         counts [n][6] int32 = {|P∧G|, |P∨G|, |B(P)|, |B(G)|, |B(P) ∧ dilate(B(G))|,
+ *                         |B(G) ∧ dilate(B(P))|}.  1 <= r <= OSVOS_DAVIS_MAX_RADIUS (31 covers frames up to a 3875-pixel
+ *                         diagonal at the benchmark's 0.008 tolerance; 1080p needs 18); n < 65536, h, w < 32768.
+ *                         `workspace`: osvos_davis_measures_workspace_bytes(n, h, w) bytes, 4-byte aligned, owned by the
+ *                         caller; nothing is allocated.  Zeroes counts itself.  Integer counts: the result does not
+ *                         depend on the launch configuration.
+ *   osvos_davis_measures_workspace_bytes: host query; 0 for a non-positive dimension.                               */
+#define OSVOS_DAVIS_MAX_RADIUS 31
+OSVOS_API size_t osvos_davis_measures_workspace_bytes(int n, int h, int w);
+OSVOS_API int osvos_davis_measures(const float* logits, const uint8_t* masks, int* counts, void* workspace, int n, int h,
+                                   int w, int r, osvos_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

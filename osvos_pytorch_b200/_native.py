@@ -148,7 +148,11 @@ SIGNATURES = {
     "osvos_label_from_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "osvos_affine_warp_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_double), POINTER(c_int),
                                      c_int, c_int, c_int, c_float, c_float, c_float, c_void_p]),
+    "osvos_davis_measures_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "osvos_davis_measures": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
 }
+
+DAVIS_MAX_RADIUS = 31
 
 _lib = None
 

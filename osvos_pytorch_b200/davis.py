@@ -42,9 +42,13 @@ class DAVIS2016Frames(Dataset):
     annotation.  With ``seq_name``: the frames of that sequence, only the first one annotated (``train=True`` keeps
     just that first frame).  Items: ``image`` uint8 [H,W,3] BGR, ``gt`` uint8 [H,W] (zeros for a frame without an
     annotation), ``has_gt``, and ``fname`` = ``seq/%05d`` of the index in sequence mode (the reference's rule), else
-    ``seq/<file stem>``."""
+    ``seq/<file stem>``.
 
-    def __init__(self, train=True, db_root_dir=None, seq_name=None, meanval=MEANVAL, inputRes=None):
+    ``all_annotations=True`` (sequence mode): every frame carries its own annotation, as scoring the sequence needs; a
+    sequence whose frame and annotation counts differ raises."""
+
+    def __init__(self, train=True, db_root_dir=None, seq_name=None, meanval=MEANVAL, inputRes=None,
+                 all_annotations=False):
         if inputRes is not None:
             raise NotImplementedError("inputRes: the reference resizes with scipy.misc.imresize, which SciPy no longer "
                                       "has, and neither entry point uses it; frames are read at their stored size")
@@ -65,7 +69,13 @@ class DAVIS2016Frames(Dataset):
             names_img = np.sort(os.listdir(os.path.join(root, "JPEGImages/480p/", str(seq_name))))
             img_list = [os.path.join("JPEGImages/480p/", str(seq_name), x) for x in names_img]
             name_label = np.sort(os.listdir(os.path.join(root, "Annotations/480p/", str(seq_name))))
-            labels = [os.path.join("Annotations/480p/", str(seq_name), name_label[0])] + [None] * (len(names_img) - 1)
+            if all_annotations:
+                if len(name_label) != len(names_img):
+                    raise ValueError(f"{root}: sequence {seq_name} has {len(names_img)} frames but {len(name_label)} "
+                                     "annotations; scoring needs one per frame")
+                labels = [os.path.join("Annotations/480p/", str(seq_name), x) for x in name_label]
+            else:
+                labels = [os.path.join("Annotations/480p/", str(seq_name), name_label[0])] + [None] * (len(names_img) - 1)
             if train:
                 img_list, labels = [img_list[0]], [labels[0]]
         if len(labels) != len(img_list):

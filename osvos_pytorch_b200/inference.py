@@ -20,16 +20,23 @@ class SequenceSegmenter:
 
     ``frames="bgr8"``: the frames are decoded uint8 [N,H,W,3] BGR (what cv2.imread returns) instead; only those bytes
     cross PCIe, and ops.image_from_bgr8 (float conversion and ``meanval`` subtraction, bit-identical to the reference's
-    dataset) fills the same fp32 ring slot on the compute stream before the forward."""
+    dataset) fills the same fp32 ring slot on the compute stream before the forward.
 
-    def __init__(self, net, output="logits", depth=3, frames="nchw_f32", meanval=ops.MEANVAL):
+    ``score=True``: ``frames`` yields ``(frame, gt_u8)`` pairs, ``gt_u8`` the host uint8 annotations [N,H,W] (pinned
+    for real overlap).  The mask crosses on the input stream into a ring slot beside the frame, and ops.davis_measures
+    scores the fused map on the compute stream right after the forward; the counts stay on the device until
+    ``frame_counts()``.  The results are the same bytes as without scoring."""
+
+    def __init__(self, net, output="logits", depth=3, frames="nchw_f32", meanval=ops.MEANVAL, score=False):
         if output not in ("logits", "bytescale", "prob", "mask"):
             raise ValueError("output must be one of logits / bytescale / prob / mask")
         if frames not in ("nchw_f32", "bgr8"):
             raise ValueError("frames must be nchw_f32 or bgr8")
         self.net, self.output, self.depth = net, output, max(2, int(depth))
         self.frames, self.meanval = frames, tuple(meanval)
+        self.score = bool(score)
         self._shape = None
+        self._counts = []
 
     def _allocate(self, shape, device):
         if self.frames == "bgr8":
@@ -41,14 +48,16 @@ class SequenceSegmenter:
         self._dev_in = [torch.empty((n, 3, h, w), dtype=torch.float32, device=device) for _ in range(self.depth)]
         self._dev_out = [torch.empty((n, 1, h, w), dtype=out_dtype, device=device) for _ in range(self.depth)]
         self._host_out = [torch.empty((n, 1, h, w), dtype=out_dtype).pin_memory() for _ in range(self.depth)]
+        if self.score:
+            self._dev_gt = [torch.empty((n, h, w), dtype=torch.uint8, device=device) for _ in range(self.depth)]
         self._s_in, self._s_out = torch.cuda.Stream(device), torch.cuda.Stream(device)
         mk = lambda: [torch.cuda.Event() for _ in range(self.depth)]
         self._ev_loaded, self._ev_consumed, self._ev_done, self._ev_host = mk(), mk(), mk(), mk()
         self._shape = tuple(shape)
-        self.h2d_bytes_per_frame = n * 3 * h * w * (1 if self.frames == "bgr8" else 4)
+        self.h2d_bytes_per_frame = n * 3 * h * w * (1 if self.frames == "bgr8" else 4) + (n * h * w if self.score else 0)
         self.d2h_bytes_per_frame = n * h * w * (4 if self.output == "logits" else 1)
 
-    def _submit(self, i, frame, device):
+    def _submit(self, i, frame, gt, device):
         k = i % self.depth
         cur = torch.cuda.current_stream(device)
         bgr8 = self.frames == "bgr8"
@@ -56,6 +65,8 @@ class SequenceSegmenter:
             if i >= self.depth:
                 self._s_in.wait_event(self._ev_consumed[k])     # the network has read the previous tenant
             (self._dev_raw[k] if bgr8 else self._dev_in[k]).copy_(frame, non_blocking=True)
+            if self.score:
+                self._dev_gt[k].copy_(gt, non_blocking=True)
             self._ev_loaded[k].record(self._s_in)
         cur.wait_event(self._ev_loaded[k])
         if i >= self.depth:
@@ -72,7 +83,9 @@ class SequenceSegmenter:
                 fused = eng.forward(self._dev_in[k], fresh_outputs=False)[-1]
             else:
                 fused = self.net(self._dev_in[k])[-1]
-            self._ev_consumed[k].record(cur)
+            if self.score:
+                self._counts.append(ops.davis_measures(fused, self._dev_gt[k]))
+            self._ev_consumed[k].record(cur)                    # after the last read of this slot's frame and mask
             if self.output == "logits":
                 self._dev_out[k].copy_(fused)
             else:
@@ -88,17 +101,26 @@ class SequenceSegmenter:
         if device.type != "cuda":
             raise RuntimeError("SequenceSegmenter runs on CUDA only; there is no CPU fallback for the OSVOS hot path")
         submitted = 0
+        self._counts = []
         with torch.cuda.device(device):
-            for frame in frames:
+            for item in frames:
+                frame, gt = item if self.score else (item, None)
                 if frame.dim() == 3:
                     frame = frame.unsqueeze(0)
+                if self.score:
+                    gt = gt.unsqueeze(0) if gt.dim() == 2 else gt
+                    n = frame.shape[0]
+                    hw = tuple(frame.shape[1:3]) if self.frames == "bgr8" else tuple(frame.shape[2:4])
+                    if gt.dtype != torch.uint8 or tuple(gt.shape) != (n,) + hw:
+                        raise ValueError(f"score=True takes uint8 [N,H,W] annotations matching the frames, got "
+                                         f"{gt.dtype} {tuple(gt.shape)}")
                 if self.frames == "bgr8" and (frame.dtype != torch.uint8 or frame.shape[-1] != 3):
                     raise ValueError("frames='bgr8' takes uint8 [N,H,W,3] frames")
                 if self._shape != tuple(frame.shape):
                     if submitted:
                         raise ValueError("all frames of one sequence must share a shape")
                     self._allocate(tuple(frame.shape), device)
-                self._submit(submitted, frame, device)
+                self._submit(submitted, frame, gt, device)
                 submitted += 1
                 ready = submitted - self.depth + 1              # keep depth-1 frames in flight
                 if ready >= 1:
@@ -109,6 +131,15 @@ class SequenceSegmenter:
                 k = j % self.depth
                 self._ev_host[k].synchronize()
                 yield self._host_out[k]
+
+    def frame_counts(self):
+        """int32 [frames*N, 6] host tensor of the last run's ops.davis_measures counts, frame order (score=True);
+        one synchronisation."""
+        if not self.score:
+            raise RuntimeError("frame_counts() needs SequenceSegmenter(..., score=True)")
+        if not self._counts:
+            return torch.zeros((0, 6), dtype=torch.int32)
+        return torch.cat(self._counts).cpu()
 
     def join_current_stream(self):
         """Make the current stream wait for every copy issued so far (lets CUDA events on the current stream bracket

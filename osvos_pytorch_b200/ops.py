@@ -550,3 +550,27 @@ def label_from_u8(masks, stats=None, out=None):
     nat.check(lib.osvos_label_from_u8(x.data_ptr(), stats.data_ptr(), out.data_ptr(), n, h, w, _stream()),
               "osvos_label_from_u8")
     return out
+
+
+def davis_measures(logits, gt_u8, r=None, out=None):
+    """DAVIS-2016 J and F counts on the device (csrc/measures.cu, DESIGN.md §14): fused logits fp32 [N,1,H,W] or
+    [N,H,W] and annotations uint8 [N,H,W] -> int32 [N,6] = {|P∧G|, |P∨G|, |B(P)|, |B(G)|, fg_match, gt_match} with
+    P = logit > 0 and G = byte != 0.  ``r``: boundary tolerance in pixels, default evaluation.bound_pix(H, W).
+    evaluation.j_and_f turns the counts into J and F.  No host synchronisation."""
+    from .evaluation import bound_pix
+    lib = nat.load()
+    _require_cuda(logits, "logits")
+    g = _require_u8(gt_u8, "gt_u8", 3)
+    n, h, w = (int(v) for v in g.shape)
+    if logits.dtype != torch.float32 or logits.numel() != n * h * w or tuple(logits.shape[-2:]) != (h, w):
+        raise ValueError(f"logits must be fp32 [N,1,H,W] or [N,H,W] matching gt_u8 {tuple(g.shape)}, got "
+                         f"{logits.dtype} {tuple(logits.shape)}")
+    x = logits.detach().contiguous()
+    r = bound_pix(h, w) if r is None else int(r)
+    if out is None:
+        out = torch.empty((n, 6), dtype=torch.int32, device=g.device)
+    ws = torch.empty(lib.osvos_davis_measures_workspace_bytes(n, h, w), dtype=torch.uint8, device=g.device)
+    _count(4)
+    nat.check(lib.osvos_davis_measures(x.data_ptr(), g.data_ptr(), out.data_ptr(), ws.data_ptr(), n, h, w, r, _stream()),
+              "osvos_davis_measures")
+    return out

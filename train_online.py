@@ -4,6 +4,7 @@ train_online.py: load the parent model, run nAveGrad x 2000 forward/backward pas
 first frame with SGD(lr 1e-8, momentum .9), save the weights, then segment the sequence.
 
     SEQ_NAME=blackswan python train_online.py --loader native # DAVIS on disk (needs cv2 + the dataset)
+    SEQ_NAME=blackswan python train_online.py --loader native --evaluate   # ... and score the masks (J and F)
     SEQ_NAME=blackswan python train_online.py                 # the same through the reference's dataloaders package
     python train_online.py --synthetic --iters 200            # synthetic 480x854 frame, no dataset
 
@@ -45,7 +46,15 @@ def parse(argv=None):
                     help="real data: the reference's dataloaders package (reference), or osvos_pytorch_b200.davis "
                          "(native: cv2 decodes, the device ingests and augments; the augmentation is always on the "
                          "device)")
-    return ap.parse_args(argv)
+    ap.add_argument("--evaluate", action="store_true",
+                    help="score the segmentation against every frame's annotation on the device (DAVIS-2016 J and F, "
+                         "osvos_pytorch_b200.evaluation); prints them and writes Results/<seq>_scores.json. "
+                         "Needs --loader native")
+    a = ap.parse_args(argv)
+    if a.evaluate and (a.synthetic or a.loader != "native"):
+        ap.error("--evaluate scores against the DAVIS annotations read by --loader native; it cannot be combined with "
+                 + ("--synthetic" if a.synthetic else "--loader reference"))
+    return a
 
 
 def main(argv=None):
@@ -96,10 +105,12 @@ def main(argv=None):
 
         def sample_fn(it):
             return augment.affine_warp_u8(img_u8, gt_u8, augment.draw_params(1, rng=rng), stats)
-        db_test = davis.DAVIS2016Frames(train=False, db_root_dir=Path.db_root_dir(), seq_name=a.seq_name)
-        # pinned here, between forwards, not by a loader thread that could allocate during a graph capture
-        test_frames = ({"image": davis.views(davis.pinned(b["data"]), *(int(v) for v in b["size"]))[0],
-                        "fname": b["fname"]}
+        db_test = davis.DAVIS2016Frames(train=False, db_root_dir=Path.db_root_dir(), seq_name=a.seq_name,
+                                        all_annotations=a.evaluate)
+        # pinned here, between forwards, not by a loader thread that could allocate during a graph capture; the image
+        # and the mask are two views of the one pinned buffer
+        test_frames = (dict(zip(("image", "gt"), davis.views(davis.pinned(b["data"]), *(int(v) for v in b["size"]))),
+                            fname=b["fname"])
                        for b in DataLoader(db_test, batch_size=1, shuffle=False, num_workers=1, collate_fn=davis.collate))
     else:
         from dataloaders import davis_2016 as db
@@ -159,9 +170,10 @@ def main(argv=None):
         for ii, s in enumerate(test_frames):
             n = int(s["image"].shape[0])
             names.append([os.path.basename(s["fname"][jj]) if "fname" in s else f"{ii:05d}_{jj}" for jj in range(n)])
-            yield s["image"]
+            yield (s["image"], s["gt"]) if a.evaluate else s["image"]
     native = a.loader == "native" and not a.synthetic
-    for pred in SequenceSegmenter(net, output="bytescale", frames="bgr8" if native else "nchw_f32")(frames()):
+    seg = SequenceSegmenter(net, output="bytescale", frames="bgr8" if native else "nchw_f32", score=a.evaluate)
+    for pred in seg(frames()):
         arr = pred.numpy()
         for jj, name in enumerate(names.popleft()):
             try:
@@ -169,6 +181,17 @@ def main(argv=None):
                 Image.fromarray(arr[jj, 0], mode="L").save(os.path.join(out_dir, name + ".png"))
             except ImportError:
                 np.save(os.path.join(out_dir, name + ".npy"), arr[jj, 0])
+    if a.evaluate:
+        import json
+        from osvos_pytorch_b200.evaluation import SequenceScores
+        scores = SequenceScores()
+        scores.add(seg.frame_counts())
+        res = scores.result()
+        st = res["statistics"]
+        print("Scores of " + a.seq_name + " (frames 1 .. n-2): "
+              + "  ".join(f"{m} M/O/D: {st[m]['M']:.4f} / {st[m]['O']:.4f} / {st[m]['D']:.4f}" for m in ("J", "F")))
+        with open(os.path.join(save_dir, "Results", a.seq_name + "_scores.json"), "w") as f:
+            json.dump(dict(sequence=a.seq_name, **res), f, indent=1)
     return history
 
 

@@ -17,7 +17,7 @@ import torch.distributed as dist
 
 import networks.vgg_osvos as vo
 from mypath import Path
-from osvos_pytorch_b200 import parallel, training
+from osvos_pytorch_b200 import evaluation, ops, parallel, training
 
 
 class _Mapped:
@@ -55,7 +55,22 @@ def parse(argv=None):
                     help="real data: the reference's dataloaders package (reference), or osvos_pytorch_b200.davis "
                          "(native: workers only decode; ingest and augmentation run on the device)")
     ap.add_argument("--workers", type=int, default=2, help="DataLoader decode workers per rank")
-    return ap.parse_args(argv)
+    ap.add_argument("--val-measures", action="store_true",
+                    help="also score every validation frame on the device (DAVIS-2016 J and F, mean over sequences); "
+                         "needs --loader native")
+    a = ap.parse_args(argv)
+    if a.val_measures and (a.synthetic or a.loader != "native"):
+        ap.error("--val-measures scores against the DAVIS annotations read by --loader native; it cannot be combined "
+                 "with " + ("--synthetic" if a.synthetic else "--loader reference"))
+    return a
+
+
+def _val_scores(per_seq):
+    """{sequence: SequenceScores} -> the dataset means over sequences of the J and F statistics."""
+    import numpy as np
+    stats = [sc.result()["statistics"] for sc in per_seq.values()]
+    return {m: {k: float(np.mean([st[m][k] for st in stats])) if stats else float("nan") for k in "MOD"}
+            for m in ("J", "F")}
 
 
 def main(argv=None):
@@ -103,7 +118,15 @@ def main(argv=None):
         db_test = davis.DAVIS2016Frames(train=False, db_root_dir=Path.db_root_dir())
         # no pin_memory=True: to_device pins in this thread (davis.pinned says why)
         val_loader = DataLoader(db_test, batch_size=1, shuffle=False, num_workers=a.workers, collate_fn=davis.collate)
-        val_batches = _Mapped(val_loader, lambda b: davis.to_device(b, device))
+        if a.val_measures:
+            def val_item(b):                         # davis.to_device without augmentation, keeping the mask bytes
+                with torch.cuda.device(device):
+                    img, gt, stats = davis.upload(b, device)
+                    return {"image": ops.image_from_bgr8(img), "gt": ops.label_from_u8(gt, stats), "gt_u8": gt,
+                            "fname": b["fname"]}
+            val_batches = _Mapped(val_loader, val_item)
+        else:
+            val_batches = _Mapped(val_loader, lambda b: davis.to_device(b, device))
 
         def epoch_batches(epoch):
             if sampler is not None:
@@ -147,12 +170,21 @@ def main(argv=None):
         if val_batches is not None and rank == 0 and epoch % a.test_interval == a.test_interval - 1:
             net.eval()
             tot = torch.zeros(5, device=device)
+            per_seq = {}
             with torch.no_grad():
                 for s in val_batches:
                     outs = net.forward(s["image"].to(device))
                     tot += torch.stack([training.class_balanced_cross_entropy_loss(o, s["gt"].to(device),
                                                                                    size_average=False) for o in outs])
+                    if a.val_measures:
+                        counts = ops.davis_measures(outs[-1], s["gt_u8"])
+                        for i, fname in enumerate(s["fname"]):
+                            per_seq.setdefault(fname.split("/")[0], evaluation.SequenceScores()).add(counts[i:i + 1])
             print("***Testing *** " + " ".join(f"Loss {k}: {v:.4f}" for k, v in enumerate((tot / len(val_batches)).tolist())))
+            if a.val_measures:
+                sc = _val_scores(per_seq)
+                print("***Testing *** " + "  ".join(f"{m} M/O/D: {sc[m]['M']:.4f} / {sc[m]['O']:.4f} / {sc[m]['D']:.4f}"
+                                                    for m in ("J", "F")) + f"  ({len(per_seq)} sequences)")
     if world > 1:
         dist.destroy_process_group()
 
