@@ -430,7 +430,15 @@ OSVOS_API int osvos_affine_warp(const float* src, float* dst, const double* inv_
  *                          label_stats -> label_dst [n][1][h][w]): nearest where the sample's binary flag is set, cubic
  *                          otherwise (custom_transforms.py:46-49), chosen on the device; bit-identical to
  *                          osvos_label_from_u8 + osvos_affine_warp in that mode.  Either tensor may be NULL (all three
- *                          label pointers together).                                                               */
+ *                          label pointers together).
+ *   osvos_affine_warp_u8_indexed: the same warp over a batch gathered from frame stores that stay on the device
+ *                          (image_store [n_store][h][w][3], label_store [n_store][h][w], label_stats [n_store][2]):
+ *                          output sample i (image_dst [n][3][h][w], label_dst [n][1][h][w]) is store frame
+ *                          index_host[i], bit-identical to osvos_affine_warp_u8 on the gathered contiguous batch.
+ *                          index_host[n] is host memory and travels with the matrices as a kernel parameter;
+ *                          indices may repeat, and each must lie in [0, n_store).  NULL rules as osvos_affine_warp_u8.
+ *                          (custom_transforms.py:7-54, :87-100 applied to frames decoded once per run instead of once
+ *                          per epoch.)                                                                             */
 OSVOS_API int osvos_image_from_bgr8(const uint8_t* src, float* dst, int n, int h, int w, float mean_b, float mean_g,
                                     float mean_r, osvos_stream_t stream);
 OSVOS_API int osvos_label_stats_u8(const uint8_t* src, uint32_t* stats, int n, int h, int w, osvos_stream_t stream);
@@ -440,6 +448,11 @@ OSVOS_API int osvos_affine_warp_u8(const uint8_t* image_src, const uint8_t* labe
                                    float* image_dst, float* label_dst, const double* inv_matrices_host,
                                    const int* flips_host, int n, int h, int w, float mean_b, float mean_g, float mean_r,
                                    osvos_stream_t stream);
+OSVOS_API int osvos_affine_warp_u8_indexed(const uint8_t* image_store, const uint8_t* label_store,
+                                           const uint32_t* label_stats, float* image_dst, float* label_dst,
+                                           const int* index_host, const double* inv_matrices_host,
+                                           const int* flips_host, int n, int n_store, int h, int w, float mean_b,
+                                           float mean_g, float mean_r, osvos_stream_t stream);
 
 /* ---- DAVIS-2016 region and boundary measures (J and F; DESIGN.md §14) -------------------------------------------
  * Per frame, P = logit > 0 (±0.0 is background, as osvos_logits_to_u8 mode MASK) and G = byte != 0.  The boundary map

@@ -85,25 +85,49 @@ def augment_batch(sample, rots=(-30, 30), scales=(.75, 1.25), rng=random, params
     return {"image": affine_warp(sample["image"], params, "cubic"), "gt": affine_warp(sample["gt"], params, "nearest")}
 
 
-def affine_warp_u8(image_u8, gt_u8, params, stats=None, meanval=ops.MEANVAL):
+def affine_warp_u8(image_u8, gt_u8, params, stats=None, meanval=ops.MEANVAL, index=None):
     """RandomHorizontalFlip + ScaleNRotate straight from decoded bytes: image_u8 uint8 [n,h,w,3] BGR and gt_u8 uint8
     [n,h,w] on the GPU -> {'image': f32 [n,3,h,w], 'gt': f32 [n,1,h,w]}, bit-identical to ingesting them
     (ops.image_from_bgr8 / ops.label_from_u8) and then warping with affine_warp.  The image is warped bicubic; each mask
     nearest if it is binary and bicubic otherwise, the reference's per-sample rule (custom_transforms.py:46-49), decided
-    on the device from ``stats`` (ops.label_stats_u8, computed here when None)."""
+    on the device from ``stats`` (ops.label_stats_u8, computed here when None).
+
+    ``index``: a sequence of frame indices.  Then image_u8, gt_u8 and stats are stores of any number of frames, and the
+    output has len(index) samples, sample i warped from frame index[i] (repeats allowed): the same result as gathering
+    those frames into a contiguous batch first, without the copy.  ``stats`` is required in this mode (computing it over
+    a whole store per batch would cost more than the warp); an index outside the store raises IndexError."""
     lib = nat.load()
     img = ops._require_u8(image_u8, "image_u8", 4)
     gt = ops._require_u8(gt_u8, "gt_u8", 3)
     n, h, w, c = (int(v) for v in img.shape)
     if c != 3 or tuple(gt.shape) != (n, h, w):
         raise ValueError("image_u8 must be [n,h,w,3] and gt_u8 [n,h,w]")
-    mats, flips = _warp_tables(params, n, h, w)
-    stats = ops.label_stats_u8(gt) if stats is None else stats
-    out_i = torch.empty((n, 3, h, w), dtype=torch.float32, device=img.device)
-    out_g = torch.empty((n, 1, h, w), dtype=torch.float32, device=img.device)
-    ops._count(2 * ((n + 31) // 32))
+    m = n if index is None else len(index)
+    mats, flips = _warp_tables(params, m, h, w)
+    if index is None:
+        stats = ops.label_stats_u8(gt) if stats is None else stats
+    else:
+        if stats is None:
+            raise ValueError("affine_warp_u8(index=...) needs the store's label stats (ops.label_stats_u8)")
+        if tuple(stats.shape) != (n, 2):
+            raise ValueError(f"stats must be [{n},2] for a store of {n} frames, got {tuple(stats.shape)}")
+        idx = [int(i) for i in index]
+        bad = [i for i in idx if not 0 <= i < n]
+        if bad:
+            raise IndexError(f"frame indices {bad[:8]} outside a store of {n} frames")
+        idx = (ctypes.c_int * m)(*idx)
+    out_i = torch.empty((m, 3, h, w), dtype=torch.float32, device=img.device)
+    out_g = torch.empty((m, 1, h, w), dtype=torch.float32, device=img.device)
+    ops._count(2 * ((m + 31) // 32))
     with torch.cuda.device(img.device):
-        nat.check(lib.osvos_affine_warp_u8(img.data_ptr(), gt.data_ptr(), stats.data_ptr(), out_i.data_ptr(),
-                                           out_g.data_ptr(), mats, flips, n, h, w, *(float(m) for m in meanval),
-                                           torch.cuda.current_stream().cuda_stream), "osvos_affine_warp_u8")
+        if index is None:
+            nat.check(lib.osvos_affine_warp_u8(img.data_ptr(), gt.data_ptr(), stats.data_ptr(), out_i.data_ptr(),
+                                               out_g.data_ptr(), mats, flips, n, h, w, *(float(v) for v in meanval),
+                                               torch.cuda.current_stream().cuda_stream), "osvos_affine_warp_u8")
+        else:
+            nat.check(lib.osvos_affine_warp_u8_indexed(img.data_ptr(), gt.data_ptr(), stats.data_ptr(),
+                                                       out_i.data_ptr(), out_g.data_ptr(), idx, mats, flips, m, n, h, w,
+                                                       *(float(v) for v in meanval),
+                                                       torch.cuda.current_stream().cuda_stream),
+                      "osvos_affine_warp_u8_indexed")
     return {"image": out_i, "gt": out_g}

@@ -180,3 +180,31 @@ extern "C" int osvos_affine_warp_u8(const uint8_t* image_src, const uint8_t* lab
   }
   return OSVOS_OK;
 }
+
+// osvos_affine_warp_u8 over a batch gathered from a device-resident store: output sample i is store frame
+// index_host[i].  The indices travel in the kernel's parameter table, so the gather costs no copy.
+extern "C" int osvos_affine_warp_u8_indexed(const uint8_t* image_store, const uint8_t* label_store,
+                                            const uint32_t* label_stats, float* image_dst, float* label_dst,
+                                            const int* index_host, const double* inv_matrices_host,
+                                            const int* flips_host, int n, int n_store, int h, int w, float mean_b,
+                                            float mean_g, float mean_r, osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(index_host != nullptr && inv_matrices_host != nullptr);
+  OSVOS_CHECK_ARG(image_store != nullptr || label_store != nullptr);
+  OSVOS_CHECK_ARG((image_store == nullptr) == (image_dst == nullptr));
+  OSVOS_CHECK_ARG((label_store == nullptr) == (label_dst == nullptr) &&
+                  (label_store == nullptr) == (label_stats == nullptr));
+  OSVOS_CHECK_FRAME_DIMS(n, h, w);
+  OSVOS_CHECK_ARG(n_store > 0);
+  for (int i = 0; i < n; ++i) OSVOS_CHECK_ARG(index_host[i] >= 0 && index_host[i] < n_store);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (image_store != nullptr) {
+    const int st = launch_affine_warp(WarpSrcBgr8{image_store, h, w, mean_b, mean_g, mean_r}, image_dst,
+                                      inv_matrices_host, flips_host, n, 3, h, w, OSVOS_WARP_CUBIC, stream, index_host);
+    if (st != OSVOS_OK) return st;
+  }
+  if (label_store != nullptr) {
+    return launch_affine_warp(WarpSrcLabel8{label_store, label_stats, h, w}, label_dst, inv_matrices_host, flips_host,
+                              n, 1, h, w, OSVOS_WARP_CUBIC, stream, index_host);
+  }
+  return OSVOS_OK;
+}

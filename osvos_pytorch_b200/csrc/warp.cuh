@@ -9,10 +9,14 @@
 namespace osvos {
 
 constexpr int kWarpMaxSamples = 32;
+// Per-launch host data, passed by value as a __grid_constant__ parameter (1,792 bytes): no device table, no copy.
+// src[s] is the source sample that destination slot sample0 + s reads (and whose mask mode it uses).
 struct WarpTable {
   double m[kWarpMaxSamples][6];
   int flip[kWarpMaxSamples];
+  int src[kWarpMaxSamples];
 };
+static_assert(sizeof(WarpTable) == 1792, "WarpTable is a kernel parameter; keep it well inside the 4 KB limit");
 
 __device__ __forceinline__ void cubic_coeffs(float x, float* c) {
   const float A = -0.75f;
@@ -95,14 +99,15 @@ affine_warp_kernel(const Src src, float* __restrict__ dst, const __grid_constant
   if (x >= w) return;
   const double* m = t.m[s];
   const int flip = t.flip[s];
-  mode = src.mode(sample0 + s, mode);
+  const int si = t.src[s];
+  mode = src.mode(si, mode);
   const int round_delta = mode == OSVOS_WARP_NEAREST ? 512 : 16;
   const int X0 = __double2int_rn((m[1] * y + m[2]) * 1024.0) + round_delta;
   const int Y0 = __double2int_rn((m[4] * y + m[5]) * 1024.0) + round_delta;
   const int Xf = X0 + __double2int_rn(m[0] * x * 1024.0);
   const int Yf = Y0 + __double2int_rn(m[3] * x * 1024.0);
   const size_t plane = static_cast<size_t>(h) * w;
-  const typename Src::Sample sp = src.sample(sample0 + s);
+  const typename Src::Sample sp = src.sample(si);
   float* dbase = dst + static_cast<size_t>(sample0 + s) * c * plane + static_cast<size_t>(y) * w + x;
   if (mode == OSVOS_WARP_NEAREST) {
     const int sx = Xf >> 10, sy = Yf >> 10;
@@ -134,16 +139,18 @@ affine_warp_kernel(const Src src, float* __restrict__ dst, const __grid_constant
   }
 }
 
-// Enqueues the warp of n samples in chunks of kWarpMaxSamples (the matrices travel as a kernel parameter).
+// Enqueues the warp of n samples in chunks of kWarpMaxSamples (the matrices travel as a kernel parameter).  Output
+// sample i reads source sample index_host[i], or sample i when index_host is NULL.
 template <class Src>
 int launch_affine_warp(const Src& src, float* dst, const double* inv_matrices_host, const int* flips_host, int n, int c,
-                       int h, int w, int mode, cudaStream_t stream) {
+                       int h, int w, int mode, cudaStream_t stream, const int* index_host = nullptr) {
   for (int s0 = 0; s0 < n; s0 += kWarpMaxSamples) {
     const int cnt = n - s0 < kWarpMaxSamples ? n - s0 : kWarpMaxSamples;
     WarpTable t;
     for (int i = 0; i < cnt; ++i) {
       for (int k = 0; k < 6; ++k) t.m[i][k] = inv_matrices_host[static_cast<size_t>(s0 + i) * 6 + k];
       t.flip[i] = flips_host ? flips_host[s0 + i] : 0;
+      t.src[i] = index_host ? index_host[s0 + i] : s0 + i;
     }
     const dim3 grid((w + 255) / 256, h, cnt);
     affine_warp_kernel<Src><<<grid, 256, 0, stream>>>(src, dst, t, s0, c, h, w, mode);

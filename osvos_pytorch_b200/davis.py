@@ -8,10 +8,15 @@ buffer, so a ``DataLoader(..., collate_fn=collate)`` moves 4 bytes per pixel and
 host-to-device copy of it.  There the ingest kernels (csrc/frames.cu) produce exactly the reference's float
 tensors, or the fused warp produces the augmented ones (augment.affine_warp_u8).
 
+``DeviceFrames`` decodes a whole split once and keeps the bytes on the device, so parent training decodes once per
+run instead of once per epoch; each batch is then one indexed warp from the store (DESIGN.md §15).
+
 ``inputRes`` is not supported: the reference resizes with ``scipy.misc.imresize``, which no longer exists in SciPy, and
 neither entry point sets it.
 """
 import os
+import random
+import time
 
 import numpy as np
 import torch
@@ -154,3 +159,133 @@ def to_device(batch, device, augment=None, meanval=MEANVAL):
             return {"image": ops.image_from_bgr8(img, meanval), "gt": ops.label_from_u8(gt, stats)}
         params = augment if isinstance(augment, (list, tuple)) else _augment.draw_params(int(img.shape[0]), rng=augment)
         return _augment.affine_warp_u8(img, gt, params, stats, meanval)
+
+
+_MAX_STATS_FRAMES = 65535                                # osvos_label_stats_u8 takes n < 65536
+
+
+def shard(n, world, rank):
+    """The dataset indices rank ``rank`` of ``world`` decodes for a DeviceFrames store: every world-th one, so each
+    size group splits nearly evenly over the ranks and little padding is gathered."""
+    return range(rank, n, world)
+
+
+def shard_plan(sizes, world):
+    """The store layout ``world`` ranks gather.  ``sizes``: (h, w) of every dataset index.  Returns one entry per size,
+    in order of first appearance: ((h, w), pad, members), members[r] = the dataset indices of that size in rank r's
+    shard, in decode order.  pad = the largest len(members[r]); rank r's share is sent as pad frames, so the gathered
+    store has world * pad slots and member j of rank r sits in slot r * pad + j (the rest is padding)."""
+    groups = {}
+    for r in range(world):
+        for i in shard(len(sizes), world, r):
+            groups.setdefault(tuple(sizes[i]), [[] for _ in range(world)])[r].append(i)
+    order = sorted(groups, key=lambda size: min(i for m in groups[size] for i in m))
+    return [(size, max(len(m) for m in groups[size]), groups[size]) for size in order]
+
+
+class DeviceFrames:
+    """Every item of a DAVIS2016Frames, decoded once and kept on ``device`` as uint8 bytes.
+
+    Frames are grouped by size; group g holds ``img`` uint8 [n_g,H,W,3], ``gt`` uint8 [n_g,H,W] and ``stats``
+    (ops.label_stats_u8 of gt).  ``where[i]`` is dataset index i's (group, slot); ``has_gt`` and ``fname`` are the
+    items' own.  A 480x854 frame takes 1.64 MB, so DAVIS-2016's train split (2,079 frames) takes 3.4 GB.
+
+    The host decodes through a DataLoader(num_workers=workers, collate_fn=collate) in dataset order and holds its
+    share until the device memory needed is known; the bytes are pinned in this thread (``pinned`` says why).  If
+    they do not fit in torch.cuda.mem_get_info()'s free memory, ValueError is raised before anything is allocated.
+
+    ``group``: a torch.distributed process group of R ranks.  Each rank then decodes a 1/R share (``shard``), the
+    frame sizes are exchanged with all_gather_object, and the shares are gathered with NCCL all_gather_into_tensor,
+    one call per size group and tensor, so every rank holds the whole store (layout: ``shard_plan``)."""
+
+    def __init__(self, dataset, device, workers=0, group=None):
+        import torch.distributed as dist
+        from torch.utils.data import DataLoader, Subset
+        t0 = time.perf_counter()
+        self.device = torch.device(device)
+        world = 1 if group is None else dist.get_world_size(group)
+        rank = 0 if group is None else dist.get_rank(group)
+        n = len(dataset)
+        mine = list(shard(n, world, rank))
+        # a private generator: the loader's seed draw must not move the global RNG that training's samplers use
+        loader = DataLoader(Subset(dataset, mine), batch_size=1, shuffle=False, num_workers=workers,
+                            collate_fn=collate, generator=torch.Generator())
+        decoded = dict(zip(mine, list(loader)))         # drained: the workers stop here, not in a finaliser
+        meta = [(i, tuple(int(v) for v in b["size"][1:]), bool(b["has_gt"][0]), b["fname"][0])
+                for i, b in decoded.items()]
+        if group is not None:
+            metas = [None] * world
+            dist.all_gather_object(metas, meta, group=group)
+            meta = sorted(m for ms in metas for m in ms)
+        sizes = [m[1] for m in meta]
+        self.has_gt = [m[2] for m in meta]
+        self.fname = [m[3] for m in meta]
+        plan = shard_plan(sizes, world)
+        need = sum(world * pad * (h * w * 4 + 8) for (h, w), pad, _ in plan)
+        free, _ = torch.cuda.mem_get_info(self.device)
+        if need > free:
+            raise ValueError(f"DeviceFrames: the {n} decoded frames need {need} bytes on {self.device} but only {free} "
+                             "are free")
+        self.groups, self.where = [], [None] * n
+        with torch.cuda.device(self.device):
+            for g, ((h, w), pad, members) in enumerate(plan):
+                img = torch.zeros((world * pad, h, w, 3), dtype=torch.uint8, device=self.device)
+                gt = torch.zeros((world * pad, h, w), dtype=torch.uint8, device=self.device)
+                for j, i in enumerate(members[rank]):
+                    data = pinned(decoded.pop(i)["data"])
+                    src_img, src_gt = views(data, 1, h, w)
+                    img[rank * pad + j].copy_(src_img[0], non_blocking=True)
+                    gt[rank * pad + j].copy_(src_gt[0], non_blocking=True)
+                if group is not None:              # in place: this rank's share is already in its slots
+                    share = slice(rank * pad, (rank + 1) * pad)
+                    dist.all_gather_into_tensor(img, img[share], group=group)
+                    dist.all_gather_into_tensor(gt, gt[share], group=group)
+                stats = torch.empty((world * pad, 2), dtype=torch.int32, device=self.device)
+                for c0 in range(0, world * pad, _MAX_STATS_FRAMES):
+                    stats[c0:c0 + _MAX_STATS_FRAMES] = ops.label_stats_u8(gt[c0:c0 + _MAX_STATS_FRAMES])
+                self.groups.append({"size": (h, w), "img": img, "gt": gt, "stats": stats})
+                for r, m in enumerate(members):
+                    for j, i in enumerate(m):
+                        self.where[i] = (g, r * pad + j)
+        torch.cuda.synchronize(self.device)
+        self.nbytes = sum(t.numel() * t.element_size() for grp in self.groups for t in (grp["img"], grp["gt"], grp["stats"]))
+        self.build_s = time.perf_counter() - t0
+
+    def __len__(self):
+        return len(self.where)
+
+    def _slot(self, i):
+        if not 0 <= i < len(self.where):
+            raise IndexError(f"frame {i} outside a store of {len(self.where)} frames")
+        return self.where[i]
+
+    def augmented(self, indices, params):
+        """The frames ``indices`` (dataset indices, one size), flipped and warped by ``params`` (one (flip, rot, scale)
+        per frame) -> {'image': f32 [N,3,H,W], 'gt': f32 [N,1,H,W]}, bit-identical to
+        to_device(collate(items), device, augment=params).  One indexed warp per 32 frames
+        (augment.affine_warp_u8(index=...)); nothing is copied."""
+        where = [self._slot(int(i)) for i in indices]
+        g = where[0][0]
+        if any(gi != g for gi, _ in where):
+            raise ValueError("all frames of a batch must share a size")
+        grp = self.groups[g]
+        with torch.cuda.device(self.device):
+            return _augment.affine_warp_u8(grp["img"], grp["gt"], params, grp["stats"], index=[s for _, s in where])
+
+    def batches(self, index_batches, rng=random):
+        """Augmented batches for an iterable of index batches (e.g. a DataLoader over dataset indices), the (flip, rot,
+        scale) triples drawn from ``rng`` per batch as to_device(..., augment=rng) draws them."""
+        for idx in index_batches:
+            idx = [int(i) for i in idx]
+            yield self.augmented(idx, _augment.draw_params(len(idx), rng=rng))
+
+    def ingest(self, i):
+        """Frame i without augmentation -> {'image': f32 [1,3,H,W], 'gt': f32 [1,1,H,W], 'gt_u8': uint8 [1,H,W] (a view
+        of the store), 'fname': [name]}; image and gt are bit-identical to to_device(collate([item]), device)."""
+        i = int(i)
+        g, s = self._slot(i)
+        grp = self.groups[g]
+        gt = grp["gt"][s:s + 1]
+        with torch.cuda.device(self.device):
+            return {"image": ops.image_from_bgr8(grp["img"][s:s + 1]), "gt": ops.label_from_u8(gt, grp["stats"][s:s + 1]),
+                    "gt_u8": gt, "fname": [self.fname[i]]}

@@ -9,7 +9,11 @@ Builds a synthetic DAVIS tree of 480x854 JPEG frames and PNG masks in a temporar
      thread as davis.to_device does) at 1, 2 and 4 workers;
   3. the same for a host restatement of the reference's pipeline (cv2 decode, float32 conversion, mean subtraction,
      mask normalisation, flip, warpAffine, ToTensor), at the same worker counts;
-  4. train_parent.py frames/s with --loader native on that tree next to --synthetic (second epoch, batch 1).
+  4. train_parent.py frames/s with --loader native on that tree next to --synthetic (second epoch, batch 1);
+  5. the device frame store (davis.DeviceFrames): its build time at 1, 2 and 4 workers; the indexed warp of a batch of
+     12 against collate + upload + affine_warp_u8 of the same frames; and frames/s of resident parent epochs at batch 12
+     (training.parent_epoch fed by DeviceFrames.batches) alternated with training.timed_parent_steps on
+     device-resident synthetic batches, with the host time per step that is not spent waiting for the device.
 Writes <out>/time_data.json; the GPU's name, power limit and SM clock limit go with the numbers.
 """
 import argparse
@@ -162,6 +166,84 @@ def parent_fps(extra, env, frames):
     return round(frames / times[-1], 1), times
 
 
+def time_store(frames, workers, steps, epochs=4, batch=12):
+    """Leg 5: build time of the store per worker count, the indexed warp against the streaming path's
+    collate + upload + affine_warp_u8, and resident parent epochs against timed_parent_steps on resident batches."""
+    from torch.utils.data import DataLoader
+    from osvos_pytorch_b200 import augment, davis, parallel, training
+    from osvos_pytorch_b200.networks.vgg_osvos import OSVOS, he_init_
+    dev = torch.device("cuda")
+    res = {"build_s": {}}
+    for nw in workers:
+        store = davis.DeviceFrames(frames, dev, workers=nw)
+        res["build_s"][nw] = round(store.build_s, 2)
+        print(f"DeviceFrames build, {nw} worker(s): {store.build_s:.2f} s for {len(store)} frames "
+              f"({store.nbytes / 1e9:.2f} GB)")
+        del store
+    torch.cuda.empty_cache()
+    store = davis.DeviceFrames(frames, dev, workers=max(workers))
+    res["frames"], res["store_GB"] = len(store), round(store.nbytes / 1e9, 3)
+
+    idx = list(range(0, batch * 5, 5))[:batch]
+    params = augment.draw_params(batch, rng=random.Random(0))
+    items = [frames[i] for i in idx]
+
+    def streamed():
+        return davis.to_device(davis.collate(items), dev, augment=params)
+
+    for name, fn in (("indexed_warp", lambda: store.augmented(idx, params)),
+                     ("collate_upload_affine_warp_u8", streamed)):
+        for _ in range(10):
+            fn()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        t0 = time.perf_counter()
+        e0.record()
+        for _ in range(steps):
+            fn()
+        e1.record()
+        torch.cuda.synchronize()
+        wall = (time.perf_counter() - t0) * 1e3 / steps
+        res[name] = {"device_ms_per_batch": round(e0.elapsed_time(e1) / steps, 3), "wall_ms_per_batch": round(wall, 3)}
+        print(f"{name:32s} batch {batch}: {res[name]['device_ms_per_batch']:.3f} ms device, {wall:.3f} ms wall")
+
+    net = he_init_(OSVOS(pretrained=0, verbose=False), seed=0)
+    with torch.no_grad():                   # keep the synthetic logits O(10), as bench.py's dp leg does
+        for mod in list(net.side_prep) + [net.fuse]:
+            mod.weight.mul_(0.1)
+    net = net.to(dev)
+    opt = training.make_optimizer(net, "parent", lr=1e-10, fused=True)
+    bucket = parallel.GradientBucket(parallel.trainable_parameters(net), dev)
+    index_loader = DataLoader(range(len(store)), batch_size=batch, shuffle=True, num_workers=0, drop_last=True)
+    steps_per_epoch = len(index_loader)
+    synth = [training.synthetic_batch(batch, H, W, i, dev) for i in range(2)]
+    rng = random.Random(0)
+    resident, synthetic, host_ms = [], [], []
+    for epoch in range(epochs + 1):         # epoch 0 warms up both paths
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        training.parent_epoch(net, opt, bucket, store.batches(index_loader, rng=rng), epoch, 240, 1)
+        host = time.perf_counter() - t0     # enqueue finished; the device may still be working
+        torch.cuda.synchronize()
+        dt = time.perf_counter() - t0
+        ms = training.timed_parent_steps(net, opt, bucket, lambda i: synth[i % 2], steps_per_epoch, 2 if epoch == 0 else 0)
+        if epoch:
+            resident.append(round(steps_per_epoch * batch / dt, 1))
+            synthetic.append(round(batch * 1e3 / ms, 1))
+            host_ms.append(round(host * 1e3 / steps_per_epoch, 2))
+    res["parent_batch12"] = {"resident_epoch_frames_per_s": resident, "timed_parent_steps_frames_per_s": synthetic,
+                             "resident_host_enqueue_ms_per_step": host_ms, "steps_per_epoch": steps_per_epoch}
+    print(f"parent epoch at batch {batch} from the store: {resident} frames/s; timed_parent_steps on resident "
+          f"synthetic batches: {synthetic} frames/s; host enqueue per step {host_ms} ms")
+    # share of a 240-epoch run over DAVIS-2016's 2,079 train frames, at the measured per-frame rates
+    per_frame_build = res["build_s"][max(workers)] / len(store)
+    run_s = 240 * 2079 / float(np.median(resident))
+    res["build_share_of_240_epochs"] = round(per_frame_build * 2079 / (per_frame_build * 2079 + run_s), 5)
+    print(f"store build ({max(workers)} workers) scaled to 2,079 frames: {per_frame_build * 2079:.1f} s, "
+          f"{100 * res['build_share_of_240_epochs']:.3f} % of a 240-epoch run")
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=os.environ.get("OSVOS_RESULTS", os.path.join(ROOT, "results")))
@@ -198,6 +280,7 @@ def main():
         fps, times = parent_fps(["--synthetic", "--iters-per-epoch", str(len(frames))], env, len(frames))
         res["train_parent"]["synthetic"] = {"frames_per_s": fps, "epoch_s": times}
         print(f"train_parent.py --synthetic: {fps} frames/s (epoch times {times})")
+        res["device_store"] = time_store(frames, workers, a.steps)
     os.makedirs(a.out, exist_ok=True)
     path = os.path.join(a.out, "time_data.json")
     with open(path, "w") as f:

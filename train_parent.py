@@ -58,9 +58,16 @@ def parse(argv=None):
     ap.add_argument("--val-measures", action="store_true",
                     help="also score every validation frame on the device (DAVIS-2016 J and F, mean over sequences); "
                          "needs --loader native")
+    ap.add_argument("--cache", default="none", choices=["none", "device"],
+                    help="device: decode the train split once and keep its bytes on every GPU (about 3.4 GB per rank, "
+                         "plus 2.3 GB of val frames on rank 0), then augment each batch from there instead of "
+                         "decoding every frame in every epoch; needs --loader native")
     a = ap.parse_args(argv)
     if a.val_measures and (a.synthetic or a.loader != "native"):
         ap.error("--val-measures scores against the DAVIS annotations read by --loader native; it cannot be combined "
+                 "with " + ("--synthetic" if a.synthetic else "--loader reference"))
+    if a.cache == "device" and (a.synthetic or a.loader != "native"):
+        ap.error("--cache device keeps the frames decoded by --loader native on the device; it cannot be combined "
                  "with " + ("--synthetic" if a.synthetic else "--loader reference"))
     return a
 
@@ -112,27 +119,50 @@ def main(argv=None):
         from osvos_pytorch_b200 import davis
         db_train = davis.DAVIS2016Frames(train=True, db_root_dir=Path.db_root_dir())
         sampler = DistributedSampler(db_train, world, rank, shuffle=True, drop_last=True) if world > 1 else None
-        loader = DataLoader(db_train, batch_size=a.batch, shuffle=sampler is None, sampler=sampler, num_workers=a.workers,
-                            drop_last=world > 1, collate_fn=davis.collate,
-                            persistent_workers=a.workers > 0)
         db_test = davis.DAVIS2016Frames(train=False, db_root_dir=Path.db_root_dir())
-        # no pin_memory=True: to_device pins in this thread (davis.pinned says why)
-        val_loader = DataLoader(db_test, batch_size=1, shuffle=False, num_workers=a.workers, collate_fn=davis.collate)
-        if a.val_measures:
-            def val_item(b):                         # davis.to_device without augmentation, keeping the mask bytes
-                with torch.cuda.device(device):
-                    img, gt, stats = davis.upload(b, device)
-                    return {"image": ops.image_from_bgr8(img), "gt": ops.label_from_u8(gt, stats), "gt_u8": gt,
-                            "fname": b["fname"]}
-            val_batches = _Mapped(val_loader, val_item)
-        else:
-            val_batches = _Mapped(val_loader, lambda b: davis.to_device(b, device))
+        if a.cache == "device":
+            # The stores replace the decoding loaders.  Index loaders with the streaming loaders' batching and sampling
+            # and no workers draw from the global RNG as 0-worker streaming loaders do (one base seed per pass, then
+            # the sampler's own draw), so a seeded run sees the same batches and the same augmentation draws.
+            train_store = davis.DeviceFrames(db_train, device, workers=a.workers,
+                                             group=dist.group.WORLD if world > 1 else None)
+            loader = DataLoader(range(len(db_train)), batch_size=a.batch, shuffle=sampler is None, sampler=sampler,
+                                num_workers=0, drop_last=world > 1)
+            val_batches = None
+            if rank == 0:                            # only rank 0 validates
+                val_store = davis.DeviceFrames(db_test, device, workers=a.workers)
+                val_batches = _Mapped(DataLoader(range(len(db_test)), batch_size=1, shuffle=False, num_workers=0),
+                                      lambda b: val_store.ingest(int(b[0])))
+                for name, st in (("train", train_store), ("val", val_store)):
+                    print(f"Device frame store ({name}): {len(st)} frames, {st.nbytes / 1e9:.2f} GB, built in "
+                          f"{st.build_s:.1f} s")
 
-        def epoch_batches(epoch):
-            if sampler is not None:
-                sampler.set_epoch(epoch)
-            for b in loader:      # flip / rotation / scale drawn from Python's random, as the reference's transforms do
-                yield davis.to_device(b, device, augment=random)
+            def epoch_batches(epoch):
+                if sampler is not None:
+                    sampler.set_epoch(epoch)
+                yield from train_store.batches(loader, rng=random)
+        else:
+            loader = DataLoader(db_train, batch_size=a.batch, shuffle=sampler is None, sampler=sampler,
+                                num_workers=a.workers, drop_last=world > 1, collate_fn=davis.collate,
+                                persistent_workers=a.workers > 0)
+            # no pin_memory=True: to_device pins in this thread (davis.pinned says why)
+            val_loader = DataLoader(db_test, batch_size=1, shuffle=False, num_workers=a.workers,
+                                    collate_fn=davis.collate)
+            if a.val_measures:
+                def val_item(b):                     # davis.to_device without augmentation, keeping the mask bytes
+                    with torch.cuda.device(device):
+                        img, gt, stats = davis.upload(b, device)
+                        return {"image": ops.image_from_bgr8(img), "gt": ops.label_from_u8(gt, stats), "gt_u8": gt,
+                                "fname": b["fname"]}
+                val_batches = _Mapped(val_loader, val_item)
+            else:
+                val_batches = _Mapped(val_loader, lambda b: davis.to_device(b, device))
+
+            def epoch_batches(epoch):
+                if sampler is not None:
+                    sampler.set_epoch(epoch)
+                for b in loader:      # flip / rotation / scale drawn from Python's random, as the reference's transforms do
+                    yield davis.to_device(b, device, augment=random)
     else:
         from dataloaders import davis_2016 as db
         from dataloaders import custom_transforms as tr
