@@ -146,6 +146,71 @@ __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float* 
   }
 }
 
+// ---- staged epilogue: registers -> shared memory -> TMA store (conv1_1) -------------------------------------------
+// Per consumer warpgroup, one staging box: one plane of 64 channels of its m64 half (8 x 8 pixels, 64 rows of 128 B),
+// SWIZZLE_128B like the tensor maps that store it.  A multiple of 1024 B, so consecutive boxes keep the swizzle phase.
+constexpr int kStageBoxBytes = 64 * 64 * 2;
+
+// Output tensor maps of the staged epilogue: {cout, w, h, n} with box {64, 8, 8, 1}.  The lo map of a hi-only output is
+// left zeroed and never used.
+struct OutMaps {
+  CUtensorMap y_hi, y_lo;
+};
+
+// The plain forward epilogue of a 64-channel tile (bias, ReLU, split-bf16 act output) with the same operations in the
+// same order as conv_epilogue<64, false>, so the outputs are bit-identical; only the route to global memory differs.  For
+// each output plane the warpgroup writes its values into `box` (the 8 pixel rows of a warp store land in 8 different
+// 16-byte swizzle slots: no bank conflicts), fences them to the async proxy, and one thread issues the TMA store, which
+// drains while the next plane is computed or the next tile's MMAs run, instead of 4-byte stores that each cover a
+// partial sector of 8 lines.  The box is rewritten only after the previous store has read it (wait_group.read), so the
+// hi and lo planes take two rounds and the values are recomputed for the second: that costs a few ALU instructions and
+// keeps the lo words out of the register file.  Edge tiles rely on TMA clipping the stores at the tensor bounds.  The
+// caller waits for the stores (bulk_wait_group<0>) on `leader` before the kernel exits.
+__device__ __forceinline__ void conv_epilogue_staged(const ConvParams& p, const OutMaps& maps, const float* acc, int tile,
+                                                     int half, int wl, int lane, uint8_t* box, int bar_id, bool leader) {
+  if (p.ablate & 16) return;
+  int nb, tx, ty, img;
+  decode_tile(p, tile, nb, tx, ty, img);
+  const int lx = lane >> 2;
+  const bool relu = (p.flags & OSVOS_FLAG_RELU) != 0;
+  const bool store_ok = !(p.ablate & 8);
+  const int planes = p.y_lo ? 2 : 1;
+  const uint32_t act_row = smem_u32(box) + (wl * 2 * 8 + lx) * 128;   // pixel (lx, 2 wl); the row below is 8 rows on
+  const uint32_t col = 4 * (lane & 3);
+#pragma unroll 1
+  for (int plane = 0; plane < planes; ++plane) {
+    if (leader) bulk_wait_group_read<0>();
+    named_bar_sync(bar_id, 128);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int ch = nb * 64 + 8 * j + 2 * (lane & 3);
+      const float2 b = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + ch)) : make_float2(0.f, 0.f);
+      float f[2][2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float v = e ? b.y : b.x;
+          v += acc[4 * j + 2 * h + e];
+          f[h][e] = relu ? fmaxf(v, 0.f) : v;
+        }
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        uint32_t hi, lo;
+        split_pack2(f[h][0], f[h][1], hi, lo);
+        st_shared_u32(act_row + h * 8 * 128 + ((j ^ lx) << 4) + col, plane ? lo : hi);
+      }
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(bar_id, 128);
+    if (leader && store_ok) {
+      tma_store_4d(plane ? &maps.y_lo : &maps.y_hi, box, nb * 64, tx * kTileW, ty * kTileH + half * 8, img);
+      bulk_commit_group();
+    }
+  }
+}
+
 
 // ---- host helpers shared by the launchers ------------------------------------------------
 static inline void fill_conv_params(ConvParams& p, const osvos_conv3x3_args* a, int block_n) {
@@ -190,6 +255,26 @@ static inline int encode_weight_maps(CUtensorMap* hi, CUtensorMap* lo, const osv
   if (rc) return rc;
   return encode_tensor_map(lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, 3, wp + plane, dims, strides, box,
                            CU_TENSOR_MAP_SWIZZLE_128B);
+}
+
+// TMA stores need 16-byte aligned bases (the row strides, multiples of cout * 2 B, are); the ABI promises only the
+// 4-byte alignment of a channel pair, so launches with other outputs keep the direct-store epilogue.
+static inline bool outputs_tma_aligned(const osvos_conv3x3_args* a) {
+  return ((reinterpret_cast<uintptr_t>(a->y_hi) | reinterpret_cast<uintptr_t>(a->y_lo)) & 15) == 0;
+}
+
+static inline int encode_output_maps(OutMaps* m, const osvos_conv3x3_args* a) {
+  memset(m, 0, sizeof(*m));
+  const uint64_t c = a->cout;
+  const uint64_t dims[4] = {c, (uint64_t)a->w, (uint64_t)a->h, (uint64_t)a->n};
+  const uint64_t strides[3] = {c * 2, c * 2 * a->w, c * 2 * a->w * a->h};
+  const uint32_t box[4] = {64, kTileW, kTileH / 2, 1};
+  int rc = encode_tensor_map(&m->y_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, 4, a->y_hi, dims, strides, box,
+                             CU_TENSOR_MAP_SWIZZLE_128B);
+  if (rc == OSVOS_OK && a->y_lo)
+    rc = encode_tensor_map(&m->y_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, 4, a->y_lo, dims, strides, box,
+                           CU_TENSOR_MAP_SWIZZLE_128B);
+  return rc;
 }
 
 int conv_first_tc_launch(const float* x, const float* w_oihw, const float* bias, void* y_hi, void* y_lo, int n, int h,

@@ -6,7 +6,8 @@
 // lands at chunk j ^ (m & 7)).  Only k < 32 is ever written or read: two wgmma K-steps x three passes per
 // 64-row half of a 128-pixel tile.  The 64 x 27 weight matrix is converted once per CTA into the same
 // layout (B operand, resident).  Warpgroups 1 and 2 issue the wgmma for the two halves and run the shared
-// conv epilogue (bias, ReLU, split-bf16 act store).  Generic-proxy smem writes are made visible to the
+// conv epilogue (bias, ReLU, split-bf16 act store; staged through shared memory and stored with TMA when the output
+// planes allow it).  Generic-proxy smem writes are made visible to the
 // tensor core with fence.proxy.async before the mbarrier arrive.
 //
 // Replaces stages[0][0..1] of the reference (networks/vgg_osvos.py:61,142-143).
@@ -19,15 +20,18 @@ namespace osvos {
 constexpr int kFirstStages = 3;
 constexpr int kFirstStageBytes = 2 * kABytes;           // hi + lo planes of the A tile (128 rows x 128 B each)
 constexpr int kFirstBBytes = 2 * 64 * 128;              // hi + lo planes of the weights (64 rows x 128 B)
-constexpr int kFirstSmem = kFirstStages * kFirstStageBytes + kFirstBBytes + 1024 + 256;
+template <bool STAGED>
+constexpr int kFirstSmem = kFirstStages * kFirstStageBytes + kFirstBBytes + (STAGED ? 2 * kStageBoxBytes : 0) + 1024 + 256;
 
-template <int PLANES>
+template <int PLANES, bool STAGED>
 __global__ void __launch_bounds__(kConvThreads, 1)
-conv_first_tc_kernel(const float* __restrict__ x, const float* __restrict__ wgt, const ConvParams p) {
+conv_first_tc_kernel(const float* __restrict__ x, const float* __restrict__ wgt, const __grid_constant__ OutMaps out,
+                     const ConvParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_b = smem + kFirstStages * kFirstStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + kFirstBBytes);
+  uint8_t* smem_stage = smem_b + kFirstBBytes;   // STAGED: one staging box per consumer warpgroup
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_stage + (STAGED ? 2 * kStageBoxBytes : 0));
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kFirstStages;
 
@@ -98,8 +102,12 @@ conv_first_tc_kernel(const float* __restrict__ x, const float* __restrict__ wgt,
         stage = 0;
         phase ^= 1;
       }
-      conv_epilogue<64, false>(p, acc, tile, wg, wl, lane);
+      if constexpr (STAGED)
+        conv_epilogue_staged(p, out, acc, tile, wg, wl, lane, smem_stage + wg * kStageBoxBytes, 1 + wg, leader);
+      else
+        conv_epilogue<64, false>(p, acc, tile, wg, wl, lane);
     }
+    if (STAGED && leader) bulk_wait_group<0>();
   } else {
     // ------------------------------------------------------------- A builders (warpgroup 0: one pixel per thread)
     const int row = threadIdx.x;  // GEMM row = pixel of the tile
@@ -180,12 +188,22 @@ int conv_first_tc_launch(const float* x, const float* w_oihw, const float* bias,
   ConvParams p;
   fill_conv_params(p, &a, 64);
   const bool fast = (flags & OSVOS_FLAG_FAST) != 0;
-  auto kern = fast ? conv_first_tc_kernel<1> : conv_first_tc_kernel<2>;
-  static uint64_t attr_done[2] = {0, 0};   // per instantiation: bit d = device d has the shared-memory opt-in
-  OSVOS_CHECK_CUDA(ensure_dynamic_smem(kern, kFirstSmem, &attr_done[fast ? 1 : 0]));
+  const bool staged = outputs_tma_aligned(&a);
+  OutMaps out;
+  if (staged) {
+    const int rc = encode_output_maps(&out, &a);
+    if (rc) return rc;
+  } else {
+    memset(&out, 0, sizeof(out));
+  }
+  auto kern = staged ? (fast ? conv_first_tc_kernel<1, true> : conv_first_tc_kernel<2, true>)
+                     : (fast ? conv_first_tc_kernel<1, false> : conv_first_tc_kernel<2, false>);
+  const int smem = staged ? kFirstSmem<true> : kFirstSmem<false>;
+  static uint64_t attr_done[4] = {0, 0, 0, 0};   // per instantiation: bit d = device d has the shared-memory opt-in
+  OSVOS_CHECK_CUDA(ensure_dynamic_smem(kern, smem, &attr_done[(staged ? 2 : 0) + (fast ? 1 : 0)]));
   const int sms = device_sm_count();
   const int grid = p.total_tiles < sms ? p.total_tiles : sms;
-  OSVOS_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kConvThreads), kFirstSmem, stream, x, w_oihw, p));
+  OSVOS_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kConvThreads), smem, stream, x, w_oihw, out, p));
   return OSVOS_OK;
 }
 

@@ -113,6 +113,25 @@ __device__ __forceinline__ void tma_load_3d(const CUtensorMap* m, uint64_t* bar,
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+// Shared -> global tensor store; elements outside the tensor's bounds are skipped.  The source must have been written
+// before a fence.proxy.async (fence_proxy_async_smem) by every thread that wrote it.
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* src, int c0, int c1, int c2, int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+      ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
+// Closes the calling thread's bulk group of the stores issued since the last commit.
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// Waits until at most N of the calling thread's bulk groups are pending: .read only until their shared-memory sources
+// have been read (the source may then be rewritten), the plain form until their writes are complete.
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 
 // --------------------------------------------------------------- descriptors
 // wgmma shared-memory matrix descriptor (64 bit):
