@@ -50,8 +50,11 @@ enum {
   OSVOS_FLAG_FAST = 2,       /* single-pass bf16 operands (hi planes only)               */
   OSVOS_FLAG_RELU_MASK = 4,  /* dgrad: dx *= (mask_hi > 0)    (autograd of :143)          */
   OSVOS_FLAG_ACCUMULATE = 8, /* add into the existing output instead of overwriting it    */
-  OSVOS_FLAG_DEFER_FINISH = 16 /* osvos_conv3x3_wgrad: accumulate into a caller-zeroed workspace only; the
+  OSVOS_FLAG_DEFER_FINISH = 16, /* osvos_conv3x3_wgrad: accumulate into a caller-zeroed workspace only; the
                                   workspace -> OIHW step is done later by osvos_wgrad_finish for many layers */
+  OSVOS_FLAG_DETERMINISTIC = 32 /* reduce floats in an order that does not depend on scheduling: partial results go to
+                                   per-block / per-tile slots written with plain stores, which are added in a fixed order
+                                   (see "Deterministic forms" below).  Without it the kernels add with atomics. */
 };
 
 typedef void* osvos_stream_t; /* cudaStream_t */
@@ -115,7 +118,9 @@ typedef struct {
   void* pool_hi;
   void* pool_lo;
   /* fused per-channel sum of the (masked) output over all pixels = bias gradient of the layer this
-   * gradient belongs to; [cout] fp32, ACCUMULATED with atomics (caller zeroes); cout >= 64 only */
+   * gradient belongs to; [cout] fp32, ACCUMULATED with atomics (caller zeroes); cout >= 64 only.
+   * With OSVOS_FLAG_DETERMINISTIC: partial rows [osvos_conv3x3_colsum_rows(n, h, w)][cout] instead, each written once
+   * (no zeroing needed); osvos_reduce_rows adds them in order. */
   float* colsum;
   int n, h, w, cin, cout;
   int flags;
@@ -202,6 +207,9 @@ typedef struct {
   float loss_weights[5];   /* weights of the five losses in losses[5]                 */
   float divisor;           /* batch size (batch_average), numel (size_average) or 1   */
   int n, h, w;
+  int flags;               /* 0 or OSVOS_FLAG_DETERMINISTIC: then `sums` holds osvos_tail_fwd_deterministic_sums(n, h, w)
+                              doubles - the 15 above, then one row of block partials per block, added in a fixed order.
+                              Added after the other members: zero-initialise the struct (other bits are refused). */
 } osvos_tail_fwd_args;
 OSVOS_API int osvos_tail_fwd(const osvos_tail_fwd_args* args /* host */, osvos_stream_t stream);
 
@@ -237,7 +245,8 @@ typedef struct {
   float* dw;          /* [cout][cin][3][3] fp32, overwritten */
   float* workspace;
   int n, h, w, cin, cout, dz_channels;
-  int flags;          /* OSVOS_FLAG_FAST | OSVOS_FLAG_DEFER_FINISH (then dw may be NULL) */
+  int flags;          /* OSVOS_FLAG_FAST | OSVOS_FLAG_DEFER_FINISH (then dw may be NULL) | OSVOS_FLAG_DETERMINISTIC (then
+                         the workspace is osvos_wgrad_deterministic_workspace_bytes and needs no zeroing) */
 } osvos_wgrad_args;
 OSVOS_API size_t osvos_wgrad_workspace_bytes(int dz_channels, int cin);
 OSVOS_API int osvos_conv3x3_wgrad(const osvos_wgrad_args* args /* host */, osvos_stream_t stream);
@@ -263,6 +272,7 @@ typedef struct {
   const float* grad_out[5]; /* each [n,1,h,w] or NULL */
   float* dpq[4];            /* [n,h_k,w_k,2] */
   int n, h, w;
+  int flags;                /* 0 or OSVOS_FLAG_DETERMINISTIC; zero-initialise the struct (other bits are refused) */
 } osvos_tail_bwd_args;
 OSVOS_API int osvos_tail_bwd(const osvos_tail_bwd_args* args /* host */, osvos_stream_t stream);
 
@@ -282,6 +292,7 @@ typedef struct {
   float* dpq[4];            /* [n,h_k,w_k,2] */
   float* fuse_bias_grad;    /* [1] or NULL */
   int n, h, w;
+  int flags;                /* 0 or OSVOS_FLAG_DETERMINISTIC; zero-initialise the struct (other bits are refused) */
 } osvos_tail_loss_bwd_args;
 OSVOS_API int osvos_tail_loss_bwd(const osvos_tail_loss_bwd_args* args /* host */, osvos_stream_t stream);
 
@@ -353,6 +364,62 @@ OSVOS_API size_t osvos_conv_first_bwd_workspace_bytes(void);
 OSVOS_API int osvos_conv_first_bwd(const float* x_nchw, const void* dz_hi, const void* dz_lo, const float* w_oihw,
                                    float* dw, float* dx_nchw /* or NULL */, void* workspace, int n, int h, int w,
                                    osvos_stream_t stream);
+
+/* ---- Deterministic forms (OSVOS_FLAG_DETERMINISTIC; torch.use_deterministic_algorithms in the package) ----------
+ * Every float reduction of the training path has a form whose summation order depends on the shapes (and, where a
+ * grid is sized by it, the device's SM count) only, so two runs on one device give bit-identical results:
+ *   osvos_reduce_rows:      out[c] = (accumulate ? out[c] : 0) + sum_r rows[r][c], rows [nrows][ncols] fp32, in a fixed
+ *                           order (up to 64 row segments, each summed by 8 interleaved row lanes); scratch:
+ *                           osvos_reduce_rows_scratch_floats(nrows, ncols) floats.
+ *   osvos_conv3x3_colsum_rows: rows of the colsum partials of osvos_conv3x3 with OSVOS_FLAG_DETERMINISTIC (8 per
+ *                           128-pixel tile).
+ *   osvos_conv3x3_wgrad with the flag: one workspace slice per pixel-range split, written with plain stores; the split
+ *                           count comes from a nominal 132-SM device (osvos_wgrad_deterministic_splits), so it does not
+ *                           depend on the H100 variant.  osvos_wgrad_finish_deterministic sums the splits[i] slices of
+ *                           item i in order before it scales and accumulates.
+ *   osvos_unpool_mask_deterministic: osvos_unpool_side_mask (dpq, wfold set) or osvos_unpool_add_mask without dside (dpq,
+ *                           wfold NULL) whose column sums go to partial rows [osvos_unpool_colsum_rows(n, h, w, c, pool,
+ *                           side)][c], one per block (pool = dpool_hi != NULL, side = dpq != NULL), or nowhere (NULL).
+ *   osvos_side_folded_wgrad_multi_deterministic: G += the blocks' partial rows in order; workspace
+ *                           osvos_side_folded_wgrad_deterministic_workspace_bytes(items, count) bytes, 16-byte aligned.
+ *   osvos_conv_first_bwd_deterministic: one partial slot per block, added by the ordered row reduction; workspace
+ *                           osvos_conv_first_bwd_deterministic_workspace_bytes(n, h, w) bytes.
+ *   osvos_cbce_fwd_deterministic: osvos_cbce_fwd with one row of block sums per block behind sums[0..4], added in a
+ *                           fixed order by the last block; `sums` holds osvos_cbce_fwd_deterministic_sums(numel) doubles
+ *                           (osvos_cbce_bwd reads sums[0..4] as before).
+ *   osvos_sum_f32_deterministic: osvos_sum_f32 over a fixed grid of 256 contiguous ranges, their totals added in order
+ *                           by the last block; scratch: osvos_sum_f32_deterministic_scratch_bytes() bytes.
+ *   osvos_tail_fwd / osvos_tail_bwd / osvos_tail_loss_bwd: the `flags` member of their argument blocks (appended:
+ *                           callers zero-initialise the blocks).
+ * The queries return 0 for shapes the entry points refuse.                                                        */
+OSVOS_API size_t osvos_reduce_rows_scratch_floats(int nrows, int ncols);
+OSVOS_API int osvos_reduce_rows(const float* rows, int nrows, int ncols, float* scratch, float* out, int accumulate,
+                                osvos_stream_t stream);
+OSVOS_API size_t osvos_conv3x3_colsum_rows(int n, int h, int w);
+OSVOS_API int osvos_wgrad_deterministic_splits(int n, int h, int w, int cin, int dz_channels);
+OSVOS_API size_t osvos_wgrad_deterministic_workspace_bytes(int n, int h, int w, int cin, int dz_channels);
+OSVOS_API int osvos_wgrad_finish_deterministic(const osvos_wgrad_finish_item* items /* host */,
+                                               const int* splits /* host, [count] */, int count, osvos_stream_t stream);
+OSVOS_API size_t osvos_unpool_colsum_rows(int n, int h, int w, int c, int pool, int side);
+OSVOS_API int osvos_unpool_mask_deterministic(const void* dpool_hi /* or NULL */, const void* dpool_lo, const void* x_hi,
+                                              const void* x_lo, const float* dpq /* or NULL */,
+                                              const float* wfold /* or NULL */, void* dz_hi, void* dz_lo,
+                                              float* colsum_rows /* or NULL */, int n, int h, int w, int c,
+                                              osvos_stream_t stream);
+OSVOS_API size_t osvos_side_folded_wgrad_deterministic_workspace_bytes(const osvos_side_wgrad_item* items /* host */,
+                                                                       int count);
+OSVOS_API int osvos_side_folded_wgrad_multi_deterministic(const osvos_side_wgrad_item* items /* host */, int count,
+                                                          void* workspace, osvos_stream_t stream);
+OSVOS_API size_t osvos_conv_first_bwd_deterministic_workspace_bytes(int n, int h, int w);
+OSVOS_API int osvos_conv_first_bwd_deterministic(const float* x_nchw, const void* dz_hi, const void* dz_lo,
+                                                 const float* w_oihw, float* dw, float* dx_nchw /* or NULL */,
+                                                 void* workspace, int n, int h, int w, osvos_stream_t stream);
+OSVOS_API size_t osvos_tail_fwd_deterministic_sums(int n, int h, int w);
+OSVOS_API size_t osvos_cbce_fwd_deterministic_sums(size_t numel);
+OSVOS_API int osvos_cbce_fwd_deterministic(const float* output, const float* label, size_t numel, double divisor,
+                                           double* sums, float* loss, osvos_stream_t stream);
+OSVOS_API size_t osvos_sum_f32_deterministic_scratch_bytes(void);
+OSVOS_API int osvos_sum_f32_deterministic(const float* x, size_t n, void* scratch, float* out, osvos_stream_t stream);
 
 /* ===================== SURVEY.md 8(f) "next" rows: callers either side ===================== */
 

@@ -17,6 +17,7 @@ FLAG_FAST = 2
 FLAG_RELU_MASK = 4
 FLAG_ACCUMULATE = 8
 FLAG_DEFER_FINISH = 16
+FLAG_DETERMINISTIC = 32
 WGRAD_FINISH_MAX = 24
 
 
@@ -41,7 +42,7 @@ class Stage1Args(Structure):
 class TailFwdArgs(Structure):
     _fields_ = [("pq", c_void_p * 4), ("fuse_bias", c_void_p), ("out", c_void_p * 5), ("label", c_void_p),
                 ("sums", c_void_p), ("losses", c_void_p), ("loss_weights", c_float * 5), ("divisor", c_float),
-                ("n", c_int), ("h", c_int), ("w", c_int)]
+                ("n", c_int), ("h", c_int), ("w", c_int), ("flags", c_int)]
 
 
 TAIL_SUMS = 15
@@ -50,7 +51,7 @@ TAIL_SUMS = 15
 class TailLossBwdArgs(Structure):
     _fields_ = [("logits", c_void_p * 5), ("label", c_void_p), ("sums", c_void_p), ("upstream", c_void_p),
                 ("loss_weights", c_float * 5), ("divisor", c_float), ("dpq", c_void_p * 4), ("fuse_bias_grad", c_void_p),
-                ("n", c_int), ("h", c_int), ("w", c_int)]
+                ("n", c_int), ("h", c_int), ("w", c_int), ("flags", c_int)]
 
 
 class WgradArgs(Structure):
@@ -84,7 +85,8 @@ class SideGradsItem(Structure):
 
 
 class TailBwdArgs(Structure):
-    _fields_ = [("grad_out", c_void_p * 5), ("dpq", c_void_p * 4), ("n", c_int), ("h", c_int), ("w", c_int)]
+    _fields_ = [("grad_out", c_void_p * 5), ("dpq", c_void_p * 4), ("n", c_int), ("h", c_int), ("w", c_int),
+                ("flags", c_int)]
 
 
 class SgdSegment(Structure):
@@ -153,6 +155,25 @@ SIGNATURES = {
                                              c_float, c_float, c_void_p]),
     "osvos_davis_measures_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "osvos_davis_measures": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "osvos_reduce_rows_scratch_floats": (c_size_t, [c_int, c_int]),
+    "osvos_reduce_rows": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
+    "osvos_conv3x3_colsum_rows": (c_size_t, [c_int, c_int, c_int]),
+    "osvos_wgrad_deterministic_splits": (c_int, [c_int, c_int, c_int, c_int, c_int]),
+    "osvos_wgrad_deterministic_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
+    "osvos_wgrad_finish_deterministic": (c_int, [POINTER(WgradFinishItem), POINTER(c_int), c_int, c_void_p]),
+    "osvos_unpool_colsum_rows": (c_size_t, [c_int, c_int, c_int, c_int, c_int, c_int]),
+    "osvos_unpool_mask_deterministic": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "osvos_side_folded_wgrad_deterministic_workspace_bytes": (c_size_t, [POINTER(SideWgradItem), c_int]),
+    "osvos_side_folded_wgrad_multi_deterministic": (c_int, [POINTER(SideWgradItem), c_int, c_void_p, c_void_p]),
+    "osvos_conv_first_bwd_deterministic_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "osvos_conv_first_bwd_deterministic": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                   c_int, c_int, c_int, c_void_p]),
+    "osvos_tail_fwd_deterministic_sums": (c_size_t, [c_int, c_int, c_int]),
+    "osvos_cbce_fwd_deterministic_sums": (c_size_t, [c_size_t]),
+    "osvos_cbce_fwd_deterministic": (c_int, [c_void_p, c_void_p, c_size_t, c_double, c_void_p, c_void_p, c_void_p]),
+    "osvos_sum_f32_deterministic_scratch_bytes": (c_size_t, []),
+    "osvos_sum_f32_deterministic": (c_int, [c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
 }
 
 DAVIS_MAX_RADIUS = 31

@@ -6,6 +6,10 @@ train_online.py:124 / train_parent.py:140 and walked at :141 / :164.
 Gradient bookkeeping mirrors the reference: parameters that do not influence the objective get
 ``None`` (e.g. score_dsn.* under the fuse-only online loss, SURVEY.md 8c item 9); the fixed
 bilinear deconvolution weights (lr = 0 in both scripts) receive no gradient.
+
+Determinism: the forward reads ``torch.are_deterministic_algorithms_enabled()`` once and keeps it on ``ctx``; the loss
+sums of the fused objective and every float reduction of the backward then take their fixed-order forms
+(OSVOS_FLAG_DETERMINISTIC, DESIGN.md §16), so two runs on one device give bit-identical losses and gradients.
 """
 import torch
 import torch.nn as nn
@@ -20,6 +24,16 @@ def _trunk_convs(m):
 class _OSVOSFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, engine, x, objective, *params):
+        with ops.no_uninitialized_fill():             # every buffer below is written in full by a kernel
+            return _OSVOSFunction._forward(ctx, engine, x, objective, *params)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        with ops.no_uninitialized_fill():
+            return _OSVOSFunction._backward(ctx, *grads)
+
+    @staticmethod
+    def _forward(ctx, engine, x, objective, *params):
         """objective: None (plain forward: the five maps, each differentiable) or (label, loss_weights[5], divisor):
         the package's own objective fused into the tail - outputs are then (5 maps, total, losses[5]) with only
         `total = sum_k w_k * class_balanced_cross_entropy_loss(map_k, label)` differentiable."""
@@ -27,6 +41,8 @@ class _OSVOSFunction(torch.autograd.Function):
         fast = m.precision == "fast"
         engine._check_deconvs()
         ctx.set_materialize_grads(False)
+        det = torch.are_deterministic_algorithms_enabled()      # the backward uses the mode this forward saw
+        ctx.det = det
         xin = x.detach().contiguous().float()
         n, _, h, w = (int(v) for v in xin.shape)
         convs = _trunk_convs(m)
@@ -70,7 +86,7 @@ class _OSVOSFunction(torch.autograd.Function):
             raise ValueError("objective label must be [N,1,H,W] like the output maps")
         weights = tuple(float(v) for v in weights)
         out, sums, losses = ops.tail_fwd(pqs, m.fuse.bias.detach(), n, h, w, label=label, loss_weights=weights,
-                                         divisor=divisor)
+                                         divisor=divisor, deterministic=det)
         ctx.objective = (out, label, sums, weights, float(divisor))
         ctx.saved = (xin, acts, pooled)
         maps = tuple(out[k] for k in range(5))
@@ -80,10 +96,11 @@ class _OSVOSFunction(torch.autograd.Function):
         return maps + (total, per_map)
 
     @staticmethod
-    def backward(ctx, *grads):
+    def _backward(ctx, *grads):
         engine = ctx.engine
         m = engine.m
         fast = ctx.fast
+        det = ctx.det
         xin, acts, pooled = ctx.saved
         n, h, w = ctx.dims
         convs = _trunk_convs(m)
@@ -108,10 +125,23 @@ class _OSVOSFunction(torch.autograd.Function):
                 return g
             return None
         wconvs = [c for stage in convs for c in stage][1:]
-        ws_sizes = [ops.wgrad_workspace_floats(c.out_channels, c.in_channels) for c in wconvs]
+        in_shape = {}                                  # conv -> (n, h, w) of its input
+        for i, stage in enumerate(convs):
+            hs, ws_ = h, w
+            for _ in range(i):
+                hs, ws_ = (hs + 1) // 2, (ws_ + 1) // 2
+            for c in stage:
+                in_shape[c] = (n, hs, ws_)
+        ws_sizes = [(ops.wgrad_workspace_floats(c.out_channels, c.in_channels, in_shape[c], det) + 3) // 4 * 4
+                    for c in wconvs]
         # side branch: G [18 C + 2] per scale (rounded up to 16 bytes) behind the wgrad workspaces
         g_sizes = [(ops.side_folded_wgrad_floats(sp.in_channels) + 3) // 4 * 4 for sp in m.side_prep]
-        arena = torch.zeros(sum(ws_sizes) + sum(g_sizes), dtype=torch.float32, device=xin.device)
+        if det:
+            # the per-split slices are written in full: only G needs zeroing
+            arena = torch.empty(sum(ws_sizes) + sum(g_sizes), dtype=torch.float32, device=xin.device)
+            arena[sum(ws_sizes):].zero_()
+        else:
+            arena = torch.zeros(sum(ws_sizes) + sum(g_sizes), dtype=torch.float32, device=xin.device)
         ws_of, off = {}, 0
         for c, sz in zip(wconvs, ws_sizes):
             ws_of[c] = arena[off:off + sz]
@@ -126,7 +156,7 @@ class _OSVOSFunction(torch.autograd.Function):
 
         def wgrad(conv, inp, dz_act):
             nonlocal off
-            it = ops.conv3x3_wgrad(inp, dz_act, conv.out_channels, fast=fast, deferred_ws=ws_of[conv])
+            it = ops.conv3x3_wgrad(inp, dz_act, conv.out_channels, fast=fast, deferred_ws=ws_of[conv], deterministic=det)
             tgt = grad_target(conv.weight)
             if tgt is not None:
                 it["dw"], it["accumulate"] = tgt, True
@@ -143,13 +173,13 @@ class _OSVOSFunction(torch.autograd.Function):
             # the forward's sums
             out, label, sums, weights, divisor = obj
             dpq, fb = ops.tail_loss_bwd(out, label, sums, weights, divisor, g_total.detach().contiguous().float(),
-                                        n, h, w, want_fuse_bias=grads[4] is not None)
+                                        n, h, w, want_fuse_bias=grads[4] is not None, deterministic=det)
             if fb is not None:
                 pg[m.fuse.bias] = fb.reshape(m.fuse.bias.shape)
         else:
-            dpq = ops.tail_bwd(list(grads), n, h, w)
+            dpq = ops.tail_bwd(list(grads), n, h, w, deterministic=det)
             if grads[4] is not None:
-                pg[m.fuse.bias] = ops.sum_f32(grads[4]).reshape(m.fuse.bias.shape)
+                pg[m.fuse.bias] = ops.sum_f32(grads[4], deterministic=det).reshape(m.fuse.bias.shape)
         # one zeroed buffer for all 13 trunk bias gradients; the dgrad / unpool epilogues accumulate into its slices
         flat_convs = [c for stage in convs for c in stage]
         bias_buf = torch.zeros(sum(c.out_channels for c in flat_convs), dtype=torch.float32, device=xin.device)
@@ -176,7 +206,7 @@ class _OSVOSFunction(torch.autograd.Function):
             fresh_small = torch.zeros(4 * 34 + 64, dtype=torch.float32, device=xin.device)
             fresh_side = torch.empty(sum(sp.weight.numel() for sp in m.side_prep), dtype=torch.float32,
                                      device=xin.device)
-        ops.side_folded_wgrad_multi([acts[i + 1][-1] for i in range(4)], dpq, g_of)      # G of the four scales, one launch
+        ops.side_folded_wgrad_multi([acts[i + 1][-1] for i in range(4)], dpq, g_of, deterministic=det)   # G, one launch
         entries, off_side = [], 0
         for i in range(4):
             sp, sd = m.side_prep[i], m.score_dsn[i]
@@ -214,7 +244,7 @@ class _OSVOSFunction(torch.autograd.Function):
             last_bias = bias_slices[convs[i][-1]]
             # ReLU'(x) * (unpool(dpool) + side gradient), the latter formed on the fly from dpq and the fp32 folded weights
             # (18 FMAs per element); deepest stage: dpool None, the side branch is the only consumer
-            dz = ops.unpool_side_mask(dpool, s_out, dpq[i - 1], fold[i - 1][2], colsum=last_bias)
+            dz = ops.unpool_side_mask(dpool, s_out, dpq[i - 1], fold[i - 1][2], colsum=last_bias, deterministic=det)
             for j in range(len(convs[i]) - 1, -1, -1):
                 conv = convs[i][j]
                 inp = acts[i][j - 1] if j > 0 else pooled[i]
@@ -223,17 +253,17 @@ class _OSVOSFunction(torch.autograd.Function):
                 wt = engine._packed(conv, f"s{i}c{j}", transpose_flip=True)
                 if j > 0:
                     dz, _, _ = ops.conv3x3(dz, wt, None, conv.in_channels, fast=fast, mask=inp.hi,
-                                           colsum=bias_slices[convs[i][j - 1]])
+                                           colsum=bias_slices[convs[i][j - 1]], deterministic=det)
                 else:
                     dpool, _, _ = ops.conv3x3(dz, wt, None, conv.in_channels, fast=fast)
         # stage 1 (no side branch)
         c12, c11 = convs[0][1], convs[0][0]
-        dz = ops.unpool_add_mask(dpool, acts[0][1], None, colsum=bias_slices[c12])
+        dz = ops.unpool_add_mask(dpool, acts[0][1], None, colsum=bias_slices[c12], deterministic=det)
         wgrad(c12, acts[0][0], dz)
         pg[c12.bias] = bias_grad(c12)
         dz, _, _ = ops.conv3x3(dz, engine._packed(c12, "s0c1", transpose_flip=True), None, 64, fast=fast,
-                               mask=acts[0][0].hi, colsum=bias_slices[c11])
-        dw0, dx = ops.conv_first_bwd(xin, dz, c11.weight.detach(), ctx.needs_input_grad[1])
+                               mask=acts[0][0].hi, colsum=bias_slices[c11], deterministic=det)
+        dw0, dx = ops.conv_first_bwd(xin, dz, c11.weight.detach(), ctx.needs_input_grad[1], deterministic=det)
         pg[c11.weight] = dw0
         pg[c11.bias] = bias_grad(c11)
         ops.wgrad_finish(finish_items)

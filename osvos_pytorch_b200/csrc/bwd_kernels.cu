@@ -10,6 +10,77 @@ namespace osvos {
 
 // (the adjoint of the bilinear tail lives in tail.cu, next to its forward)
 
+// ------------------------------------------------------- ordered row reduction
+// out[c] = (accumulate ? out[c] : 0) + sum_r rows[r][c] with an order that depends on (nrows, ncols) only: segment s of
+// kRedSegs holds rows [s * seg, (s + 1) * seg); inside a segment eight row lanes stride the rows and are added lane 0
+// first; the segment totals are added in segment order.  The deterministic forms of the backward reduce their
+// per-block / per-tile partial rows with it instead of adding them with atomics.
+constexpr int kRedSegs = 64;
+__global__ void __launch_bounds__(256)
+reduce_rows_segments_kernel(const float* __restrict__ rows, int nrows, int ncols, int ld, int seg,
+                            float* __restrict__ scratch) {
+  __shared__ float red[8][33];
+  pdl_wait();
+  const int lane = threadIdx.x & 31, sub = threadIdx.x >> 5;
+  const int col = blockIdx.x * 32 + lane;
+  const int r0 = blockIdx.y * seg, r1 = min(r0 + seg, nrows);
+  float acc = 0.f;
+  if (col < ncols)
+    for (int r = r0 + sub; r < r1; r += 8) acc += __ldcg(rows + static_cast<size_t>(r) * ld + col);
+  red[sub][lane] = acc;
+  __syncthreads();
+  if (sub == 0 && col < ncols) {
+    float t = red[0][lane];
+#pragma unroll
+    for (int i = 1; i < 8; ++i) t += red[i][lane];
+    scratch[static_cast<size_t>(blockIdx.y) * ncols + col] = t;
+  }
+}
+__global__ void __launch_bounds__(256)
+reduce_rows_final_kernel(const float* __restrict__ scratch, int segs, int ncols, float* __restrict__ out, int accumulate) {
+  const int col = blockIdx.x * 256 + threadIdx.x;
+  if (col >= ncols) return;
+  float t = __ldcg(scratch + col);
+  for (int s = 1; s < segs; ++s) t += __ldcg(scratch + static_cast<size_t>(s) * ncols + col);
+  out[col] = accumulate ? out[col] + t : t;
+}
+
+// rows: [nrows] rows of `ld` floats, the first ncols of each summed
+// ---------------------------------------------------- ordered sum of one vector
+// out[0] = sum x[0..n) for the deterministic form of osvos_sum_f32: a fixed grid of kSumBlocks blocks, block b sums the
+// contiguous range [b * seg, (b + 1) * seg) (thread strides, then a shuffle tree and the warps in order), the last block
+// adds the block partials in block order.  The order depends on n only.
+constexpr int kSumBlocks = 256;
+__global__ void __launch_bounds__(256) sum_f32_det_kernel(const float* __restrict__ x, size_t n, size_t seg,
+                                                          float* __restrict__ part, float* __restrict__ result) {
+  __shared__ float red[256];
+  const size_t b0 = blockIdx.x * seg, b1 = min(b0 + seg, n);
+  float acc = 0.f;
+  for (size_t i = b0 + threadIdx.x; i < b1; i += 256) acc += __ldg(x + i);
+  red[threadIdx.x] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+    for (int i = 0; i < 256; ++i) s += red[i];
+    part[blockIdx.x] = s;
+  }
+  if (last_block_arrives(reinterpret_cast<unsigned int*>(part + kSumBlocks))) {
+    const float s = block_ordered_sum(part, kSumBlocks, 1, red);
+    if (threadIdx.x == 0) result[0] = s;
+  }
+}
+
+int reduce_rows_launch(const float* rows, int nrows, int ncols, int ld, float* scratch, float* out, int accumulate,
+                       cudaStream_t stream) {
+  const int seg = (nrows + kRedSegs - 1) / kRedSegs;
+  const int segs = (nrows + seg - 1) / seg;
+  reduce_rows_segments_kernel<<<dim3((ncols + 31) / 32, segs), 256, 0, stream>>>(rows, nrows, ncols, ld, seg, scratch);
+  OSVOS_CHECK_CUDA(cudaGetLastError());
+  reduce_rows_final_kernel<<<(ncols + 255) / 256, 256, 0, stream>>>(scratch, segs, ncols, out, accumulate);
+  OSVOS_CHECK_CUDA(cudaGetLastError());
+  return OSVOS_OK;
+}
+
 // ---------------------------------------------------------------- generic sum
 __global__ void __launch_bounds__(256) sum_f32_kernel(const float* __restrict__ x, size_t n, double* __restrict__ out,
                                                       float* __restrict__ result) {
@@ -54,7 +125,8 @@ __device__ __forceinline__ void load_pair8(const __nv_bfloat16* hi, const __nv_b
 //   ONCE and applied to all four pixels (64 FMAs per 4 vector loads).  `wsrc` is the table in shared memory when a block
 //   has enough tiles to amortise copying it (18 c floats), else the table in global memory through L1.
 // POOL = false: the deepest stage, whose output has no pooling consumer (dz = ReLU' * side gradient only).
-template <bool POOL, bool SIDE>
+// DET: `colsum` is a partial row per block, [gridDim.x][c], from a fixed-order block reduction (no atomics).
+template <bool POOL, bool SIDE, bool DET = false>
 __global__ void __launch_bounds__(256, SIDE ? 2 : 4)
 unpool_add_mask_kernel(const __nv_bfloat16* __restrict__ dp_hi, const __nv_bfloat16* __restrict__ dp_lo,
                        const __nv_bfloat16* __restrict__ x_hi, const __nv_bfloat16* __restrict__ x_lo,
@@ -181,10 +253,23 @@ unpool_add_mask_kernel(const __nv_bfloat16* __restrict__ dp_hi, const __nv_bfloa
     }
   }
   if (colsum) {
+    if constexpr (DET) {
+      float* red = cs + c * ((SIDE && wf_in_smem) ? 19 : 1);   // [256][8]
 #pragma unroll
-    for (int j = 0; j < 8; ++j) atomicAdd(&cs[g * 8 + j], csum[j]);
-    __syncthreads();
-    for (int i = threadIdx.x; i < c; i += blockDim.x) atomicAdd(colsum + i, cs[i]);
+      for (int j = 0; j < 8; ++j) red[threadIdx.x * 8 + j] = csum[j];
+      __syncthreads();
+      for (int ch = threadIdx.x; ch < c; ch += blockDim.x) {
+        const int gg = ch / 8, j = ch % 8;
+        float t = 0.f;
+        for (int r = 0; r < ppb; ++r) t += red[(r * groups + gg) * 8 + j];
+        colsum[static_cast<size_t>(blockIdx.x) * c + ch] = t;
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) atomicAdd(&cs[g * 8 + j], csum[j]);
+      __syncthreads();
+      for (int i = threadIdx.x; i < c; i += blockDim.x) atomicAdd(colsum + i, cs[i]);
+    }
   }
 }
 
@@ -258,6 +343,9 @@ __device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
+// DET: one slot of partial results per block (instead of kFwCopies shared ones) written with plain stores, added by
+// osvos_reduce_rows' ordered reduction afterwards (no last-block pass).
+template <bool DET = false>
 __global__ void __launch_bounds__(256)
 conv_first_wgrad_kernel(const float* __restrict__ x, const __nv_bfloat16* __restrict__ dz_hi,
                         const __nv_bfloat16* __restrict__ dz_lo, float* __restrict__ dw, float* __restrict__ partial,
@@ -371,14 +459,21 @@ conv_first_wgrad_kernel(const float* __restrict__ x, const __nv_bfloat16* __rest
       const int k = mt * 16 + g + (j >> 1) * 8;
       const int co = 8 * warp + 2 * t + (j & 1);
       // kFwCopies replicas of the 64 x 27 result spread the same-address atomic traffic of the blocks
-      if (k < 27) atomicAdd(partial + (blockIdx.x % kFwCopies) * (64 * 27) + co * 27 + k, acc[mt][j]);
+      if (k < 27) {
+        if constexpr (DET)
+          partial[static_cast<size_t>(blockIdx.x) * (64 * 27) + co * 27 + k] = acc[mt][j];
+        else
+          atomicAdd(partial + (blockIdx.x % kFwCopies) * (64 * 27) + co * 27 + k, acc[mt][j]);
+      }
     }
-  if (last_block_arrives(reinterpret_cast<unsigned int*>(partial + kFwCopies * 64 * 27))) {
-    for (int i = threadIdx.x; i < 64 * 27; i += 256) {
-      float t = 0.f;
+  if constexpr (!DET) {
+    if (last_block_arrives(reinterpret_cast<unsigned int*>(partial + kFwCopies * 64 * 27))) {
+      for (int i = threadIdx.x; i < 64 * 27; i += 256) {
+        float t = 0.f;
 #pragma unroll
-      for (int c = 0; c < kFwCopies; ++c) t += __ldcg(partial + c * (64 * 27) + i);
-      dw[i] = t;
+        for (int c = 0; c < kFwCopies; ++c) t += __ldcg(partial + c * (64 * 27) + i);
+        dw[i] = t;
+      }
     }
   }
 }
@@ -451,21 +546,27 @@ extern "C" int osvos_sum_f32(const float* x, size_t n, double* scratch, float* o
   return OSVOS_OK;
 }
 
-template <bool POOL, bool SIDE>
+static size_t unpool_tiles(int n, int h, int w, int c, bool pool) {
+  const int oh = pool ? (h + 1) / 2 : h, ow = pool ? (w + 1) / 2 : w;
+  const int ppb = 256 / (c / 8);
+  return static_cast<size_t>(n) * oh * ((ow + ppb - 1) / ppb);
+}
+
+template <bool POOL, bool SIDE, bool DET = false>
 static int launch_unpool(const void* dpool_hi, const void* dpool_lo, const void* x_hi, const void* x_lo, const float* dside,
                          const float* dpq, const float* wfold, void* dz_hi, void* dz_lo, float* colsum, int n, int h, int w,
                          int c, cudaStream_t stream) {
   const int oh = POOL ? (h + 1) / 2 : h, ow = POOL ? (w + 1) / 2 : w;
-  const int ppb = 256 / (c / 8);
-  const size_t tiles = static_cast<size_t>(n) * oh * ((ow + ppb - 1) / ppb);
+  const size_t tiles = unpool_tiles(n, h, w, c, POOL);
   OSVOS_CHECK_ARG(tiles < (static_cast<size_t>(1) << 31));
   const int grid = grid_cap(tiles, SIDE ? 2 : 4);
   // the folded weights go to shared memory when every block has tiles enough to amortise the copy
   const int wf_in_smem = (SIDE && tiles >= static_cast<size_t>(grid) * 4) ? 1 : 0;
-  const size_t smem = static_cast<size_t>(c) * sizeof(float) * (wf_in_smem ? 19 : 1);
-  auto kern = unpool_add_mask_kernel<POOL, SIDE>;
+  const size_t smem = static_cast<size_t>(c) * sizeof(float) * (wf_in_smem ? 19 : 1) + (DET ? 256 * 8 * sizeof(float) : 0);
+  auto kern = unpool_add_mask_kernel<POOL, SIDE, DET>;
   static uint64_t attr_done = 0;
-  if (smem > 48 * 1024) OSVOS_CHECK_CUDA(ensure_dynamic_smem(kern, 19 * 2048 * sizeof(float), &attr_done));
+  if (smem > 48 * 1024)
+    OSVOS_CHECK_CUDA(ensure_dynamic_smem(kern, (19 * 2048 + (DET ? 256 * 8 : 0)) * sizeof(float), &attr_done));
   OSVOS_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(256), smem, stream,
                               static_cast<const __nv_bfloat16*>(dpool_hi), static_cast<const __nv_bfloat16*>(dpool_lo),
                               static_cast<const __nv_bfloat16*>(x_hi), static_cast<const __nv_bfloat16*>(x_lo), dside, dpq,
@@ -497,6 +598,56 @@ extern "C" int osvos_unpool_side_mask(const void* dpool_hi, const void* dpool_lo
   return launch_unpool<false, true>(nullptr, nullptr, x_hi, x_lo, nullptr, dpq, wfold, dz_hi, dz_lo, colsum, n, h, w, c, stream);
 }
 
+extern "C" size_t osvos_sum_f32_deterministic_scratch_bytes(void) { return (kSumBlocks + 1) * sizeof(float); }
+
+extern "C" int osvos_sum_f32_deterministic(const float* x, size_t n, void* scratch, float* out, osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(x != nullptr && scratch != nullptr && out != nullptr && n > 0);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  float* part = static_cast<float*>(scratch);
+  // the block partials are written in full: only the arrival counter behind them is zeroed
+  OSVOS_CHECK_CUDA(cudaMemsetAsync(part + kSumBlocks, 0, sizeof(float), stream));
+  sum_f32_det_kernel<<<kSumBlocks, 256, 0, stream>>>(x, n, (n + kSumBlocks - 1) / kSumBlocks, part, out);
+  OSVOS_CHECK_CUDA(cudaGetLastError());
+  return OSVOS_OK;
+}
+
+extern "C" size_t osvos_reduce_rows_scratch_floats(int nrows, int ncols) {
+  if (nrows <= 0 || ncols <= 0) return 0;
+  return static_cast<size_t>(kRedSegs < nrows ? kRedSegs : nrows) * ncols;
+}
+
+extern "C" int osvos_reduce_rows(const float* rows, int nrows, int ncols, float* scratch, float* out, int accumulate,
+                                 osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(rows != nullptr && scratch != nullptr && out != nullptr && nrows > 0 && ncols > 0);
+  return reduce_rows_launch(rows, nrows, ncols, ncols, scratch, out, accumulate, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" size_t osvos_unpool_colsum_rows(int n, int h, int w, int c, int pool, int side) {
+  if (n <= 0 || h <= 0 || w <= 0 || c < 8 || c % 8 != 0 || c > 2048 || 256 % (c / 8) != 0) return 0;
+  return static_cast<size_t>(grid_cap(unpool_tiles(n, h, w, c, pool != 0), side ? 2 : 4));
+}
+
+extern "C" int osvos_unpool_mask_deterministic(const void* dpool_hi, const void* dpool_lo, const void* x_hi,
+                                               const void* x_lo, const float* dpq, const float* wfold, void* dz_hi,
+                                               void* dz_lo, float* colsum_rows, int n, int h, int w, int c,
+                                               osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(x_hi != nullptr && dz_hi != nullptr && n > 0 && h > 0 && w > 0 && c % 8 == 0);
+  OSVOS_CHECK_ARG(c <= 2048 && 256 % (c / 8) == 0);
+  OSVOS_CHECK_ARG((dpq == nullptr) == (wfold == nullptr));
+  OSVOS_CHECK_ARG(dpq != nullptr || dpool_hi != nullptr);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (dpq == nullptr)
+    return launch_unpool<true, false, true>(dpool_hi, dpool_lo, x_hi, x_lo, nullptr, nullptr, nullptr, dz_hi, dz_lo,
+                                            colsum_rows, n, h, w, c, stream);
+  OSVOS_CHECK_ARG(static_cast<long>(h) * w < (1l << 30));
+  OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(wfold) & 15) == 0);
+  if (dpool_hi != nullptr)
+    return launch_unpool<true, true, true>(dpool_hi, dpool_lo, x_hi, x_lo, nullptr, dpq, wfold, dz_hi, dz_lo, colsum_rows,
+                                           n, h, w, c, stream);
+  return launch_unpool<false, true, true>(nullptr, nullptr, x_hi, x_lo, nullptr, dpq, wfold, dz_hi, dz_lo, colsum_rows, n,
+                                          h, w, c, stream);
+}
+
 extern "C" int osvos_channel_sum(const void* act_hi, const void* act_lo, float* out, size_t npix, int c,
                                  osvos_stream_t stream_) {
   OSVOS_CHECK_ARG(act_hi != nullptr && out != nullptr && npix > 0 && c % 8 == 0 && c >= 8 && c <= 2048 &&
@@ -522,7 +673,7 @@ extern "C" int osvos_conv_first_bwd(const float* x_nchw, const void* dz_hi, cons
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   OSVOS_CHECK_CUDA(cudaMemsetAsync(workspace, 0, osvos_conv_first_bwd_workspace_bytes(), stream));
   const size_t tiles = static_cast<size_t>(n) * h * ((w + kFwPix - 1) / kFwPix);
-  conv_first_wgrad_kernel<<<grid_cap(tiles, 4), 256, 0, stream>>>(
+  conv_first_wgrad_kernel<false><<<grid_cap(tiles, 4), 256, 0, stream>>>(
       x_nchw, static_cast<const __nv_bfloat16*>(dz_hi), static_cast<const __nv_bfloat16*>(dz_lo), dw,
       static_cast<float*>(workspace), n, h, w);
   if (dx_nchw) {
@@ -530,6 +681,41 @@ extern "C" int osvos_conv_first_bwd(const float* x_nchw, const void* dz_hi, cons
     conv_first_dgrad_kernel<<<grid, 128, 0, stream>>>(static_cast<const __nv_bfloat16*>(dz_hi),
                                                        static_cast<const __nv_bfloat16*>(dz_lo), w_oihw, dx_nchw, n, h,
                                                        w);
+  }
+  OSVOS_CHECK_CUDA(cudaGetLastError());
+  return OSVOS_OK;
+}
+
+static size_t conv_first_tiles(int n, int h, int w) {
+  return static_cast<size_t>(n) * h * ((w + kFwPix - 1) / kFwPix);
+}
+
+extern "C" size_t osvos_conv_first_bwd_deterministic_workspace_bytes(int n, int h, int w) {
+  if (n <= 0 || h <= 0 || w <= 0) return 0;
+  const int grid = grid_cap(conv_first_tiles(n, h, w), 4);
+  // the blocks' slots, then the ordered reduction's scratch
+  return (static_cast<size_t>(grid) * 64 * 27 + osvos_reduce_rows_scratch_floats(grid, 64 * 27)) * sizeof(float);
+}
+
+extern "C" int osvos_conv_first_bwd_deterministic(const float* x_nchw, const void* dz_hi, const void* dz_lo,
+                                                  const float* w_oihw, float* dw, float* dx_nchw, void* workspace, int n,
+                                                  int h, int w, osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(x_nchw != nullptr && dz_hi != nullptr && dw != nullptr && workspace != nullptr && n > 0 && h > 0 &&
+                  w > 0);
+  OSVOS_CHECK_ARG(dx_nchw == nullptr || w_oihw != nullptr);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const int grid = grid_cap(conv_first_tiles(n, h, w), 4);
+  float* slots = static_cast<float*>(workspace);
+  // every slot is written in full by its block (no zeroing); the slots are then added in block order
+  conv_first_wgrad_kernel<true><<<grid, 256, 0, stream>>>(
+      x_nchw, static_cast<const __nv_bfloat16*>(dz_hi), static_cast<const __nv_bfloat16*>(dz_lo), dw, slots, n, h, w);
+  OSVOS_CHECK_CUDA(cudaGetLastError());
+  int rc = reduce_rows_launch(slots, grid, 64 * 27, 64 * 27, slots + static_cast<size_t>(grid) * 64 * 27, dw, 0, stream);
+  if (rc) return rc;
+  if (dx_nchw) {
+    dim3 dgrid((w + 127) / 128, h, n);
+    conv_first_dgrad_kernel<<<dgrid, 128, 0, stream>>>(static_cast<const __nv_bfloat16*>(dz_hi),
+                                                        static_cast<const __nv_bfloat16*>(dz_lo), w_oihw, dx_nchw, n, h, w);
   }
   OSVOS_CHECK_CUDA(cudaGetLastError());
   return OSVOS_OK;

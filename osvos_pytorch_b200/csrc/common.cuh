@@ -97,6 +97,22 @@ __device__ __forceinline__ bool last_block_arrives(unsigned int* counter) {
   return is_last;
 }
 
+// Fixed-order sum of rows[0..nrows)[col] * stride by one whole block (blockDim.x a multiple of 32, <= 1024): thread t
+// adds rows t, t + blockDim.x, ... in order, the block's partials are then added in thread order by thread 0.  The order
+// depends on nrows and blockDim.x only.  Every thread must call it; the result is valid in thread 0.
+template <typename T>
+__device__ __forceinline__ T block_ordered_sum(const T* rows, int nrows, size_t stride, T* red /* [blockDim.x] shared */) {
+  T t = T(0);
+  for (int r = threadIdx.x; r < nrows; r += blockDim.x) t += __ldcg(rows + static_cast<size_t>(r) * stride);
+  __syncthreads();   // `red` may still be read by a previous call
+  red[threadIdx.x] = t;
+  __syncthreads();
+  T s = T(0);
+  if (threadIdx.x == 0)
+    for (int i = 0; i < static_cast<int>(blockDim.x); ++i) s += red[i];
+  return s;
+}
+
 __device__ __forceinline__ float bf16_lo_to_float(uint32_t packed) { return __uint_as_float(packed << 16); }
 __device__ __forceinline__ float bf16_hi_to_float(uint32_t packed) { return __uint_as_float(packed & 0xFFFF0000u); }
 

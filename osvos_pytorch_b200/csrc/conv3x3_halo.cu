@@ -55,7 +55,7 @@ struct HaloCfg {
 //    barriers 1 and 2 hand the ring over in tile order: warpgroup k % 2 starts waiting on tile k's full barriers only
 //    after tile k - 1's owner has passed its last full wait.  Without that, a warpgroup a whole ring round ahead of the
 //    producer would pass a parity wait on a phase that has not happened yet.
-template <int BLOCK_N, int PLANES, bool SPLIT, bool LEAN, bool PINGPONG>
+template <int BLOCK_N, int PLANES, bool SPLIT, bool LEAN, bool PINGPONG, bool DET = false>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__ CUtensorMap map_x_lo,
                     const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
@@ -246,14 +246,15 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_c
       pending.release(leader);
 #pragma unroll
       for (int h = 0; h < kHalves; ++h)
-        conv_epilogue<BLOCK_N, Cfg::kSplitAcc, LEAN>(p, acc[h], tile, PINGPONG ? h : wg, wl, lane);
+        conv_epilogue<BLOCK_N, Cfg::kSplitAcc, LEAN, DET>(p, acc[h], tile, PINGPONG ? h : wg, wl, lane);
     }
   }
 }
 
 // Exact mode with BLOCK_N <= 128 takes the N-concatenated split accumulator (HaloCfg), except under ping-pong for
 // BLOCK_N = 128 (below).
-template <int BLOCK_N, int PLANES, bool LEAN = false>
+// DET: OSVOS_FLAG_DETERMINISTIC with column sums (partial rows instead of atomics).
+template <int BLOCK_N, int PLANES, bool LEAN = false, bool DET = false>
 static int launch_halo(const osvos_conv3x3_args* a, cudaStream_t stream) {
   constexpr bool kSplit = PLANES == 2 && BLOCK_N <= 128;
   using Cfg = HaloCfg<BLOCK_N, PLANES, kSplit>;
@@ -282,8 +283,8 @@ static int launch_halo(const osvos_conv3x3_args* a, cudaStream_t stream) {
   // half-tile epilogues that gains from T = 3 on.  So ping-pong wherever some CTA gets three tiles or more.
   constexpr bool kCanPingPong = BLOCK_N == 64 || BLOCK_N == 128;
   const bool pingpong = kCanPingPong && p.total_tiles > 2 * sms;
-  auto kern = pingpong ? conv3x3_halo_kernel<BLOCK_N, PLANES, kSplit && BLOCK_N == 64, LEAN, kCanPingPong>
-                       : conv3x3_halo_kernel<BLOCK_N, PLANES, kSplit, LEAN, false>;
+  auto kern = pingpong ? conv3x3_halo_kernel<BLOCK_N, PLANES, kSplit && BLOCK_N == 64, LEAN, kCanPingPong, DET>
+                       : conv3x3_halo_kernel<BLOCK_N, PLANES, kSplit, LEAN, false, DET>;
   static uint64_t attr_done[2] = {0, 0};   // per kernel: bit d = device d has the shared-memory opt-in
   OSVOS_CHECK_CUDA(ensure_dynamic_smem(kern, Cfg::kSmemBytes, &attr_done[pingpong]));
   OSVOS_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kConvThreads), Cfg::kSmemBytes, stream, mx_hi, mx_lo,
@@ -292,6 +293,7 @@ static int launch_halo(const osvos_conv3x3_args* a, cudaStream_t stream) {
 }
 
 // cout 64 or a multiple of 128 (cout 2 and 16 go to side_conv.cu)
+template <bool DET>
 static int conv3x3_halo_dispatch(const osvos_conv3x3_args* a, cudaStream_t stream) {
   const bool fast = (a->flags & OSVOS_FLAG_FAST) != 0;
   // the lean epilogue serves launches that use nothing but bias / ReLU / split-bf16 act output / fused pool (exact mode)
@@ -304,17 +306,17 @@ static int conv3x3_halo_dispatch(const osvos_conv3x3_args* a, cudaStream_t strea
   // few tiles (stage 5 at 480x854: 56 of 128 x 128): N = 64 tiles double the CTA count at ~0.8x the time per tile.
   if (a->cout == 64 || (waves128 == 1 && tiles128 * 5 <= static_cast<long>(sms) * 3)) {
     if (lean) return launch_halo<64, 2, true>(a, stream);
-    return fast ? launch_halo<64, 1>(a, stream) : launch_halo<64, 2>(a, stream);
+    return fast ? launch_halo<64, 1, false, DET>(a, stream) : launch_halo<64, 2, false, DET>(a, stream);
   }
   // N = 256 tiles whenever that does not cost a wave.  The cost model per (tap, 64-channel) step (N = 128 ~ 1000 cycles
   // for 2 + 1 instructions, N = 256 ~ 2200 exact) is carried over from the first tensor-core generation this was tuned on;
   // on an H100 the choice measured neutral at 480x854 (552-553 frames/s with 256-wide tiles and with 128-wide ones only).
   const bool prefer256 = fast ? waves256 * 1100 < waves128 * 700 : waves256 * 2200 < waves128 * 1000;
   if (a->cout % 256 == 0 && prefer256)
-    return fast ? launch_halo<256, 1>(a, stream) : launch_halo<256, 2>(a, stream);
-  if (fast) return launch_halo<128, 1>(a, stream);
+    return fast ? launch_halo<256, 1, false, DET>(a, stream) : launch_halo<256, 2, false, DET>(a, stream);
+  if (fast) return launch_halo<128, 1, false, DET>(a, stream);
   if (lean) return launch_halo<128, 2, true>(a, stream);
-  return launch_halo<128, 2>(a, stream);
+  return launch_halo<128, 2, false, DET>(a, stream);
 }
 
 static int check_conv_args(const osvos_conv3x3_args* a) {
@@ -336,6 +338,7 @@ static int check_conv_args(const osvos_conv3x3_args* a) {
   OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(a->x_hi) & 15) == 0);
   OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(a->w_packed) & 15) == 0);
   OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(a->bias) & 15) == 0);
+  OSVOS_CHECK_ARG(!(a->flags & OSVOS_FLAG_DETERMINISTIC) || (reinterpret_cast<uintptr_t>(a->colsum) & 7) == 0);
   if (a->cout >= 64) {   // the epilogue moves channel pairs: 4-byte bf16x2 words, 8-byte float2
     const uintptr_t bf16_planes = reinterpret_cast<uintptr_t>(a->y_hi) | reinterpret_cast<uintptr_t>(a->y_lo) |
                                   reinterpret_cast<uintptr_t>(a->pool_hi) | reinterpret_cast<uintptr_t>(a->pool_lo) |
@@ -376,5 +379,13 @@ extern "C" int osvos_conv3x3(const osvos_conv3x3_args* a, osvos_stream_t stream_
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   // the folded side branch (cout == 2) and side_prep (cout == 16): nine-taps-along-N kernel (side_conv.cu)
   if (a->cout == 2 || a->cout == 16) return side_conv_dispatch(a, stream);
-  return conv3x3_halo_dispatch(a, stream);
+  // deterministic column sums: partial rows instead of atomics (the other outputs are the same either way)
+  if ((a->flags & OSVOS_FLAG_DETERMINISTIC) && a->colsum != nullptr) return conv3x3_halo_dispatch<true>(a, stream);
+  return conv3x3_halo_dispatch<false>(a, stream);
+}
+
+extern "C" size_t osvos_conv3x3_colsum_rows(int n, int h, int w) {
+  if (n <= 0 || h <= 0 || w <= 0) return 0;
+  // 8 partial rows (2 m64 halves x 4 warps) per 128-pixel tile; see conv_epilogue
+  return static_cast<size_t>(n) * ((h + kTileH - 1) / kTileH) * ((w + kTileW - 1) / kTileW) * 8;
 }

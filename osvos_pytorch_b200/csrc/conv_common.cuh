@@ -27,7 +27,8 @@ struct ConvParams {
   const __nv_bfloat16* mask_hi;
   __nv_bfloat16* pool_hi;  // optional fused 2x2 ceil-mode max pool of the output
   __nv_bfloat16* pool_lo;
-  float* colsum;           // optional fused per-channel sum of the output (bias gradient), atomically accumulated
+  float* colsum;           // optional fused per-channel sum of the output (bias gradient), atomically accumulated; with
+                           // OSVOS_FLAG_DETERMINISTIC partial rows [pixel tile][half][warp][cout] written with plain stores
   int n, h, w, cin, cout;
   int tiles_x, tiles_y, n_blocks, total_tiles, k_chunks;
   int flags;
@@ -68,7 +69,8 @@ __device__ __forceinline__ void split_pack2(float a, float b, uint32_t& hi, uint
 // LEAN: the plain-forward feature set only (bias, ReLU, split-bf16 act output and / or fused pool); the mask, fp32 output
 // and column-sum code is not compiled in, which takes it out of the consumer warpgroups' instruction stream.
 // Both forms compute every value with the same operations in the same order: their outputs are bit-identical.
-template <int BLOCK_N, bool SPLIT_ACC, bool LEAN = false>
+// DET: the column sums go to partial rows (OSVOS_FLAG_DETERMINISTIC) instead of atomics.
+template <int BLOCK_N, bool SPLIT_ACC, bool LEAN = false, bool DET = false>
 __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float* acc, int tile, int wg, int wl, int lane) {
   if (p.ablate & 16) return;
   int nb, tx, ty, img;
@@ -127,8 +129,13 @@ __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float* 
         s1 += __shfl_xor_sync(0xffffffffu, s1, o);
       }
       if (lane < 4) {
-        atomicAdd(p.colsum + ch, s0);
-        atomicAdd(p.colsum + ch + 1, s1);
+        if constexpr (DET) {   // one partial row per (pixel tile, m64 half, warp), reduced in order later
+          const size_t prow = (static_cast<size_t>(tile / p.n_blocks) * 2 + wg) * 4 + wl;
+          *reinterpret_cast<float2*>(p.colsum + prow * p.cout + ch) = make_float2(s0, s1);
+        } else {
+          atomicAdd(p.colsum + ch, s0);
+          atomicAdd(p.colsum + ch + 1, s1);
+        }
       }
     }
     if (p.pool_hi) {  // MaxPool2d(2, 2, ceil_mode=True); out-of-image members of the window are excluded

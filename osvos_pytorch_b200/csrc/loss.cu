@@ -12,6 +12,9 @@ constexpr int kLossThreads = 256;
 
 __device__ __forceinline__ float softplus_l(float x) { return fmaxf(x, 0.f) + log1pf(__expf(-fabsf(x))); }
 
+// DET: each block stores its three sums in its own row behind sums[5] (plain stores), and the last block adds the rows
+// in block order instead of the fp64 atomics.
+template <bool DET = false>
 __global__ void __launch_bounds__(kLossThreads)
 cbce_fwd_kernel(const float* __restrict__ x, const float* __restrict__ label, size_t total, double* __restrict__ sums,
                 double divisor, float* __restrict__ loss) {
@@ -61,10 +64,23 @@ cbce_fwd_kernel(const float* __restrict__ x, const float* __restrict__ label, si
   if (threadIdx.x < 3) {
     double acc = 0.0;
     for (int w = 0; w < kLossThreads / 32; ++w) acc += static_cast<double>(red[w][threadIdx.x]);
-    atomicAdd(sums + threadIdx.x, acc);
+    if constexpr (DET)
+      sums[5 + 3 * static_cast<size_t>(blockIdx.x) + threadIdx.x] = acc;
+    else
+      atomicAdd(sums + threadIdx.x, acc);
   }
   // last block to arrive (counter in sums[4]): loss[0] = (Nn/N * S_pos + P/N * S_neg) / divisor ; sums[3] = N
-  if (last_block_arrives(reinterpret_cast<unsigned int*>(sums + 4)) && threadIdx.x == 0) {
+  const bool last = last_block_arrives(reinterpret_cast<unsigned int*>(sums + 4));
+  if constexpr (DET) {
+    if (last) {
+      __shared__ double dred[kLossThreads];
+      for (int i = 0; i < 3; ++i) {
+        const double t = block_ordered_sum(sums + 5 + i, static_cast<int>(gridDim.x), 3, dred);
+        if (threadIdx.x == 0) sums[i] = t;
+      }
+    }
+  }
+  if (last && threadIdx.x == 0) {
     const double tot = static_cast<double>(total);
     const double p = __ldcg(sums + 2), nn = tot - p;
     sums[3] = tot;
@@ -120,7 +136,25 @@ extern "C" int osvos_cbce_fwd(const float* output, const float* label, size_t nu
   OSVOS_CHECK_ARG(divisor > 0);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   OSVOS_CHECK_CUDA(cudaMemsetAsync(sums, 0, 5 * sizeof(double), stream));
-  cbce_fwd_kernel<<<loss_grid(numel), kLossThreads, 0, stream>>>(output, label, numel, sums, divisor, loss);
+  cbce_fwd_kernel<false><<<loss_grid(numel), kLossThreads, 0, stream>>>(output, label, numel, sums, divisor, loss);
+  OSVOS_CHECK_CUDA(cudaGetLastError());
+  return OSVOS_OK;
+}
+
+extern "C" size_t osvos_cbce_fwd_deterministic_sums(size_t numel) {
+  if (numel == 0) return 0;
+  return 5 + 3 * static_cast<size_t>(loss_grid(numel));
+}
+
+extern "C" int osvos_cbce_fwd_deterministic(const float* output, const float* label, size_t numel, double divisor,
+                                            double* sums, float* loss, osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(output != nullptr && label != nullptr && sums != nullptr && loss != nullptr && numel > 0);
+  OSVOS_CHECK_ARG(((reinterpret_cast<uintptr_t>(output) | reinterpret_cast<uintptr_t>(label)) & 15) == 0);
+  OSVOS_CHECK_ARG(divisor > 0);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  // the block rows are written in full: only the five leading values (with the arrival counter) need zeroing
+  OSVOS_CHECK_CUDA(cudaMemsetAsync(sums, 0, 5 * sizeof(double), stream));
+  cbce_fwd_kernel<true><<<loss_grid(numel), kLossThreads, 0, stream>>>(output, label, numel, sums, divisor, loss);
   OSVOS_CHECK_CUDA(cudaGetLastError());
   return OSVOS_OK;
 }

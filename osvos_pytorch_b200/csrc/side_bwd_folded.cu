@@ -58,19 +58,27 @@ static_assert(kSwDataBytes % 8 == 0 && ((2 * kSwComputeWarps + 2) * 4) % 8 == 0,
 constexpr int kSwMaxScales = 4;
 struct SwScale {
   const float* dpq;
-  float* g;
+  float* g;                      // DET: partial rows [blocks / (c / 128)][sw_row_pitch(c)], one per chunk stride
   int n, h, w, c;
   int block_begin, blocks;       // this scale's blocks: [block_begin, block_begin + blocks), a multiple of c / 128
 };
+// floats per partial row of the deterministic form: 18 c + 2, padded so that every row keeps the float4 alignment
+__host__ __device__ __forceinline__ size_t sw_row_pitch(int c) { return (static_cast<size_t>(18) * c + 2 + 3) / 4 * 4; }
+
 struct SwParams {
   SwScale sc[kSwMaxScales];
   int count;
   int has_lo;
+  int total_blocks;
 };
 struct SwMaps {
   CUtensorMap hi[kSwMaxScales], lo[kSwMaxScales];
 };
 
+// DET: instead of the vector atomics into G, each block stores its reduced partials into its own row of `g` (the row of
+// its chunk stride `blk`; the slabs of a row are disjoint), and osvos_side_folded_wgrad_multi_deterministic adds the
+// rows in order afterwards.
+template <bool DET = false>
 __global__ void __launch_bounds__(kSwKernelThreads, 2)
 side_folded_wgrad_kernel(const __grid_constant__ SwMaps maps, const __grid_constant__ SwParams p) {
   int sci = 0;
@@ -81,6 +89,9 @@ side_folded_wgrad_kernel(const __grid_constant__ SwMaps maps, const __grid_const
   const float* __restrict__ dpq = L.dpq;
   float* __restrict__ g = L.g;
   const int n = L.n, h = L.h, w = L.w, c = L.c, has_lo = p.has_lo;
+  const size_t grow = DET ? (static_cast<size_t>(static_cast<int>(blockIdx.x) - L.block_begin) / (c / kSwSlab)) *
+                                sw_row_pitch(c)
+                          : 0;   // this block's partial row (DET)
   extern __shared__ uint8_t sw_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(sw_smem_raw) + 127) & ~uintptr_t(127));
   // after the last chunk the ring (+ the slack behind it) is reused for the warps' partial sums: [warp][18][128] floats
@@ -226,13 +237,20 @@ side_folded_wgrad_kernel(const __grid_constant__ SwMaps maps, const __grid_const
       val.x += v.x, val.y += v.y, val.z += v.z, val.w += v.w;
     }
     const int to = i / (kSwSlab / 4), c4 = i % (kSwSlab / 4);
-    atomicAdd(reinterpret_cast<float4*>(g + static_cast<size_t>(to) * c + slab * kSwSlab + c4 * 4), val);
+    float4* dst = reinterpret_cast<float4*>(g + grow + static_cast<size_t>(to) * c + slab * kSwSlab + c4 * 4);
+    if constexpr (DET)
+      *dst = val;
+    else
+      atomicAdd(dst, val);
   }
   if (slab == 0 && threadIdx.x < 2) {
     float v = 0.f;
 #pragma unroll
     for (int wv = 0; wv < kSwComputeWarps; ++wv) v += part_s[2 * wv + threadIdx.x];
-    atomicAdd(g + static_cast<size_t>(18) * c + threadIdx.x, v);
+    if constexpr (DET)
+      g[grow + static_cast<size_t>(18) * c + threadIdx.x] = v;
+    else
+      atomicAdd(g + static_cast<size_t>(18) * c + threadIdx.x, v);
   }
 }
 
@@ -311,16 +329,19 @@ __global__ void __launch_bounds__(kFinThreads) side_grads_finish_kernel(const __
   }
 }
 
+int reduce_rows_launch(const float* rows, int nrows, int ncols, int ld, float* scratch, float* out, int accumulate,
+                       cudaStream_t stream);   // bwd_kernels.cu
+
 }  // namespace osvos
 
 using namespace osvos;
 
 extern "C" size_t osvos_side_folded_wgrad_floats(int c) { return static_cast<size_t>(18) * c + 2; }
 
-extern "C" int osvos_side_folded_wgrad_multi(const osvos_side_wgrad_item* items, int count, osvos_stream_t stream_) {
+// Launch plan of the G kernel: the parameter block, tensor maps and blocks per scale.  `encode` false: no tensor maps
+// (the workspace query of the deterministic form).
+static int side_wgrad_plan(const osvos_side_wgrad_item* items, int count, SwParams& p, SwMaps& maps, bool encode) {
   OSVOS_CHECK_ARG(items != nullptr && count > 0 && count <= kSwMaxScales);
-  SwParams p;
-  SwMaps maps;
   memset(&p, 0, sizeof(p));
   p.count = count;
   p.has_lo = items[0].x_lo != nullptr ? 1 : 0;
@@ -347,6 +368,7 @@ extern "C" int osvos_side_folded_wgrad_multi(const osvos_side_wgrad_item* items,
     const uint64_t dims[2] = {(uint64_t)it.c, (uint64_t)npix};
     const uint64_t strides[1] = {(uint64_t)it.c * 2};
     const uint32_t box[2] = {kSwSlab, kSwChunk};
+    if (!encode) continue;
     int rc = encode_tensor_map(&maps.hi[k], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, 2, it.x_hi, dims, strides, box,
                                CU_TENSOR_MAP_SWIZZLE_NONE);
     if (rc) return rc;
@@ -372,10 +394,71 @@ extern "C" int osvos_side_folded_wgrad_multi(const osvos_side_wgrad_item* items,
     p.sc[k].blocks = static_cast<int>(b * slabs);
     begin += p.sc[k].blocks;
   }
+  p.total_blocks = begin;
+  return OSVOS_OK;
+}
+
+// floats of the deterministic form's workspace: the partial rows of every scale, then the row reduction's scratch
+static size_t side_wgrad_det_floats(const SwParams& p, size_t* rows_floats) {
+  size_t rows = 0, scratch = 0;
+  for (int k = 0; k < p.count; ++k) {
+    const int nrows = p.sc[k].blocks / (p.sc[k].c / kSwSlab);
+    const size_t cols = static_cast<size_t>(18) * p.sc[k].c + 2;
+    rows += nrows * sw_row_pitch(p.sc[k].c);
+    const size_t s = osvos_reduce_rows_scratch_floats(nrows, static_cast<int>(cols));
+    scratch = s > scratch ? s : scratch;
+  }
+  if (rows_floats) *rows_floats = rows;
+  return rows + scratch;
+}
+
+extern "C" int osvos_side_folded_wgrad_multi(const osvos_side_wgrad_item* items, int count, osvos_stream_t stream_) {
+  SwParams p;
+  SwMaps maps;
+  int rc = side_wgrad_plan(items, count, p, maps, true);
+  if (rc) return rc;
   static uint64_t attr_done = 0;
-  OSVOS_CHECK_CUDA(ensure_dynamic_smem(side_folded_wgrad_kernel, kSwSmemBytes, &attr_done));
-  OSVOS_CHECK_CUDA(launch_pdl(side_folded_wgrad_kernel, dim3(begin), dim3(kSwKernelThreads), kSwSmemBytes,
+  OSVOS_CHECK_CUDA(ensure_dynamic_smem(side_folded_wgrad_kernel<false>, kSwSmemBytes, &attr_done));
+  OSVOS_CHECK_CUDA(launch_pdl(side_folded_wgrad_kernel<false>, dim3(p.total_blocks), dim3(kSwKernelThreads), kSwSmemBytes,
                               static_cast<cudaStream_t>(stream_), maps, p));
+  return OSVOS_OK;
+}
+
+extern "C" size_t osvos_side_folded_wgrad_deterministic_workspace_bytes(const osvos_side_wgrad_item* items, int count) {
+  if (items == nullptr || count <= 0 || count > kSwMaxScales) return 0;
+  SwParams p;
+  SwMaps maps;
+  if (side_wgrad_plan(items, count, p, maps, false)) return 0;
+  return side_wgrad_det_floats(p, nullptr) * sizeof(float);
+}
+
+extern "C" int osvos_side_folded_wgrad_multi_deterministic(const osvos_side_wgrad_item* items, int count, void* workspace,
+                                                           osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 15) == 0);
+  SwParams p;
+  SwMaps maps;
+  int rc = side_wgrad_plan(items, count, p, maps, true);
+  if (rc) return rc;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  size_t rows_floats = 0;
+  side_wgrad_det_floats(p, &rows_floats);
+  float* ws = static_cast<float*>(workspace);
+  float* rows[kSwMaxScales];
+  size_t off = 0;
+  for (int k = 0; k < count; ++k) {   // the kernel writes partial rows where the default form adds into G
+    rows[k] = ws + off;
+    p.sc[k].g = rows[k];
+    off += static_cast<size_t>(p.sc[k].blocks / (p.sc[k].c / kSwSlab)) * sw_row_pitch(p.sc[k].c);
+  }
+  static uint64_t attr_done = 0;
+  OSVOS_CHECK_CUDA(ensure_dynamic_smem(side_folded_wgrad_kernel<true>, kSwSmemBytes, &attr_done));
+  OSVOS_CHECK_CUDA(launch_pdl(side_folded_wgrad_kernel<true>, dim3(p.total_blocks), dim3(kSwKernelThreads), kSwSmemBytes,
+                              stream, maps, p));
+  for (int k = 0; k < count; ++k) {   // G += sum of the rows, in row order
+    rc = reduce_rows_launch(rows[k], p.sc[k].blocks / (p.sc[k].c / kSwSlab), 18 * p.sc[k].c + 2,
+                            static_cast<int>(sw_row_pitch(p.sc[k].c)), ws + rows_floats, items[k].g, 1, stream);
+    if (rc) return rc;
+  }
   return OSVOS_OK;
 }
 

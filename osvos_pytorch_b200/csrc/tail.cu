@@ -41,6 +41,13 @@ constexpr int kTailThreads = 256;
 // sums layout (doubles): [2k] / [2k+1] = S_pos / S_neg of map k, [10] = P, [11] = N, [12] / [13] = A_pos / A_neg of the
 // fused map (sum_{y=1} (sigmoid(x) - 1), sum_{y=0} sigmoid(x): d fuse.bias without another pass), [14] = arrival counter
 constexpr int kTailSums = 15;
+constexpr int kTailVals = 13;   // block partials per block in the deterministic form: sums[0..10], [12], [13]
+
+static int tail_fwd_blocks(int n, int h) {
+  size_t blocks = static_cast<size_t>(n) * h;                 // one output row per block iteration
+  const size_t cap = static_cast<size_t>(device_sm_count()) * 8;
+  return static_cast<int>(blocks > cap ? cap : blocks);
+}
 
 __device__ __forceinline__ float softplus_f(float x) { return fmaxf(x, 0.f) + log1pf(__expf(-fabsf(x))); }
 
@@ -49,6 +56,8 @@ __device__ __forceinline__ float softplus_f(float x) { return fmaxf(x, 0.f) + lo
 // Phase 2: a thread takes four consecutive pixels (shifted so that the four are a 16-byte aligned group of the flat map
 // whatever the row length) and blends HORIZONTALLY from shared memory: two LDS.64 and four FMAs per scale and pixel.
 // (The full 2 x 2 gather with its index arithmetic per pixel and scale costs ~850 instructions per pixel group.)
+// DET (OSVOS_FLAG_DETERMINISTIC): block partials go to rows behind the sums, added in a fixed order by the last block.
+template <bool DET = false>
 __global__ void __launch_bounds__(kTailThreads) tail_fwd_kernel(const TailParams p) {
   extern __shared__ float2 vbuf[];     // [scale 0 .. 3][wk_k] vertically blended (p, q)
   pdl_wait();               // side maps, biases and the accumulators all come from earlier kernels (ptx.cuh)
@@ -157,7 +166,7 @@ __global__ void __launch_bounds__(kTailThreads) tail_fwd_kernel(const TailParams
   }
 
   if (p.label && p.sums) {
-    constexpr int kVals = 13;
+    constexpr int kVals = kTailVals;
     __shared__ float red[kTailThreads / 32][kVals];
     float vals[kVals];
 #pragma unroll
@@ -179,14 +188,27 @@ __global__ void __launch_bounds__(kTailThreads) tail_fwd_kernel(const TailParams
       for (int i = 0; i < kVals; ++i) red[warp][i] = vals[i];
     }
     __syncthreads();
+    const int slot = threadIdx.x < 11 ? threadIdx.x : threadIdx.x + 1;
     if (threadIdx.x < kVals) {
       double acc = 0.0;
       for (int wv = 0; wv < kTailThreads / 32; ++wv) acc += static_cast<double>(red[wv][threadIdx.x]);
-      atomicAdd(p.sums + (threadIdx.x < 11 ? threadIdx.x : threadIdx.x + 1), acc);
+      if constexpr (DET) p.sums[kTailSums + static_cast<size_t>(blockIdx.x) * kVals + threadIdx.x] = acc;
+      else atomicAdd(p.sums + slot, acc);
+    }
+    const bool last = last_block_arrives(reinterpret_cast<unsigned int*>(p.sums + 14));
+    if constexpr (DET) {
+      if (last) {   // the block rows in a fixed order (block_ordered_sum), one value at a time
+        __shared__ double dred[kTailThreads];
+        for (int i = 0; i < kVals; ++i) {
+          const double t = block_ordered_sum(p.sums + kTailSums + i, static_cast<int>(gridDim.x), kVals, dred);
+          if (threadIdx.x == 0) p.sums[i < 11 ? i : i + 1] = t;
+        }
+        __syncthreads();
+      }
     }
     // the last block to arrive turns the sums into the five losses and their weighted total:
     // L_k = (Nn/N * S_pos_k + P/N * S_neg_k) / divisor   (layers/osvos_layers.py:38-46)
-    if (last_block_arrives(reinterpret_cast<unsigned int*>(p.sums + 14)) && threadIdx.x == 0) {
+    if (last && threadIdx.x == 0) {
       const double tot = static_cast<double>(total);
       const double pcount = __ldcg(p.sums + 10), nn = tot - pcount;
       p.sums[11] = tot;
@@ -231,7 +253,9 @@ struct TailBwdParams {
 };
 constexpr int kTailBwdCols = 512 + 32;
 
-template <bool LOSS>
+// DET: with several row groups per column, their column sums are added into shared memory in row-group order instead of
+// with shared-memory atomics.
+template <bool LOSS, bool DET = false>
 __global__ void __launch_bounds__(256) tail_bwd2_kernel(const __grid_constant__ TailBwdParams p) {
   __shared__ float colp[kTailBwdCols], colq[kTailBwdCols];
   const int tid = threadIdx.x;
@@ -269,6 +293,8 @@ __global__ void __launch_bounds__(256) tail_bwd2_kernel(const __grid_constant__ 
   const int wpad = min(256, (width + 31) & ~31);
   const int rgroups = 256 / wpad;
   const int r = tid / wpad, c0 = tid - r * wpad;
+  float keep_p = 0.f, keep_q = 0.f;   // DET, rgroups > 1: this thread's (single) column sum
+  bool kept = false;
   if (r < rgroups) {
     for (int c = c0; c < width; c += wpad) {
       const int x = xlo + c;
@@ -304,14 +330,24 @@ __global__ void __launch_bounds__(256) tail_bwd2_kernel(const __grid_constant__ 
         }
       }
       if (rgroups > 1) {
-        atomicAdd(&colp[c], ap);
-        atomicAdd(&colq[c], aq);
+        if constexpr (DET) {
+          keep_p = ap, keep_q = aq, kept = true;   // rgroups > 1 means width <= wpad: one column per thread
+        } else {
+          atomicAdd(&colp[c], ap);
+          atomicAdd(&colq[c], aq);
+        }
       } else {
         colp[c] = ap, colq[c] = aq;
       }
     }
   }
   __syncthreads();
+  if constexpr (DET) {
+    for (int rr = 0; rr < rgroups && rgroups > 1; ++rr) {
+      if (kept && r == rr) colp[c0] += keep_p, colq[c0] += keep_q;
+      __syncthreads();
+    }
+  }
   // phase 2: every low-res pixel of the segment sums its 2s columns; lw = min(32, 2s) lanes per pixel
   const int lw = fs < 32 ? fs : 32;
   const int per_pass = 256 / lw;
@@ -360,6 +396,7 @@ static void fill_tail_scales(TailParams& p, const float* const* pq, int h, int w
 
 extern "C" int osvos_tail_fwd(const osvos_tail_fwd_args* a, osvos_stream_t stream_) {
   OSVOS_CHECK_ARG(a != nullptr && a->n > 0 && a->h > 0 && a->w > 0);
+  OSVOS_CHECK_ARG((a->flags & ~OSVOS_FLAG_DETERMINISTIC) == 0);
   OSVOS_CHECK_ARG(a->label == nullptr || a->sums != nullptr);
   OSVOS_CHECK_ARG(a->losses == nullptr || (a->label != nullptr && a->divisor > 0.f));
   OSVOS_CHECK_ARG(static_cast<size_t>(a->n) * a->h * a->w < (1ull << 31));   // 32-bit element indices in the kernel
@@ -384,14 +421,17 @@ extern "C" int osvos_tail_fwd(const osvos_tail_fwd_args* a, osvos_stream_t strea
   p.h = a->h;
   p.w = a->w;
   if (a->sums) OSVOS_CHECK_CUDA(cudaMemsetAsync(a->sums, 0, kTailSums * sizeof(double), stream));
-  size_t blocks = static_cast<size_t>(a->n) * a->h;                 // one output row per block iteration
-  const size_t cap = static_cast<size_t>(device_sm_count()) * 8;
-  if (blocks > cap) blocks = cap;
+  const size_t blocks = static_cast<size_t>(tail_fwd_blocks(a->n, a->h));
   const size_t smem = sizeof(float2) * (p.sc[0].wk + p.sc[1].wk + p.sc[2].wk + p.sc[3].wk);
   OSVOS_CHECK_ARG(smem <= 48 * 1024);                               // rows up to ~13,000 pixels
   // (with a loss, the memset above is this kernel's stream predecessor: plain launch)
-  if (a->sums) tail_fwd_kernel<<<static_cast<int>(blocks), kTailThreads, smem, stream>>>(p);
-  else OSVOS_CHECK_CUDA(launch_pdl(tail_fwd_kernel, dim3(static_cast<unsigned>(blocks)), dim3(kTailThreads), smem, stream, p));
+  if (a->sums && (a->flags & OSVOS_FLAG_DETERMINISTIC))
+    tail_fwd_kernel<true><<<static_cast<int>(blocks), kTailThreads, smem, stream>>>(p);
+  else if (a->sums)
+    tail_fwd_kernel<false><<<static_cast<int>(blocks), kTailThreads, smem, stream>>>(p);
+  else
+    OSVOS_CHECK_CUDA(launch_pdl(tail_fwd_kernel<false>, dim3(static_cast<unsigned>(blocks)), dim3(kTailThreads), smem,
+                                stream, p));
   OSVOS_CHECK_CUDA(cudaGetLastError());
   return OSVOS_OK;
 }
@@ -422,13 +462,17 @@ static int fill_tail_bwd_scales(TailBwdParams& p, float* const* dpq, int n, int 
 
 extern "C" int osvos_tail_bwd(const osvos_tail_bwd_args* a, osvos_stream_t stream_) {
   OSVOS_CHECK_ARG(a != nullptr && a->n > 0 && a->h > 0 && a->w > 0);
+  OSVOS_CHECK_ARG((a->flags & ~OSVOS_FLAG_DETERMINISTIC) == 0);
   for (int k = 0; k < 4; ++k) OSVOS_CHECK_ARG(a->dpq[k] != nullptr);
   TailBwdParams p;
   memset(&p, 0, sizeof(p));
   const int items = fill_tail_bwd_scales(p, a->dpq, a->n, a->h, a->w);
   for (int k = 0; k < 5; ++k) p.src[k] = a->grad_out[k];
   p.n = a->n, p.h = a->h, p.w = a->w;
-  tail_bwd2_kernel<false><<<items, 256, 0, static_cast<cudaStream_t>(stream_)>>>(p);
+  if (a->flags & OSVOS_FLAG_DETERMINISTIC)
+    tail_bwd2_kernel<false, true><<<items, 256, 0, static_cast<cudaStream_t>(stream_)>>>(p);
+  else
+    tail_bwd2_kernel<false><<<items, 256, 0, static_cast<cudaStream_t>(stream_)>>>(p);
   OSVOS_CHECK_CUDA(cudaGetLastError());
   return OSVOS_OK;
 }
@@ -436,6 +480,7 @@ extern "C" int osvos_tail_bwd(const osvos_tail_bwd_args* a, osvos_stream_t strea
 extern "C" int osvos_tail_loss_bwd(const osvos_tail_loss_bwd_args* a, osvos_stream_t stream_) {
   OSVOS_CHECK_ARG(a != nullptr && a->n > 0 && a->h > 0 && a->w > 0 && a->label != nullptr && a->sums != nullptr);
   OSVOS_CHECK_ARG(a->divisor > 0.f);
+  OSVOS_CHECK_ARG((a->flags & ~OSVOS_FLAG_DETERMINISTIC) == 0);
   for (int k = 0; k < 4; ++k) OSVOS_CHECK_ARG(a->dpq[k] != nullptr);
   for (int k = 0; k < 5; ++k) OSVOS_CHECK_ARG(a->logits[k] != nullptr || a->loss_weights[k] == 0.f);
   TailBwdParams p;
@@ -451,7 +496,15 @@ extern "C" int osvos_tail_loss_bwd(const osvos_tail_loss_bwd_args* a, osvos_stre
   p.inv_divisor = 1.f / a->divisor;
   p.fuse_bias_grad = a->fuse_bias_grad;
   p.n = a->n, p.h = a->h, p.w = a->w;
-  tail_bwd2_kernel<true><<<items, 256, 0, static_cast<cudaStream_t>(stream_)>>>(p);
+  if (a->flags & OSVOS_FLAG_DETERMINISTIC)
+    tail_bwd2_kernel<true, true><<<items, 256, 0, static_cast<cudaStream_t>(stream_)>>>(p);
+  else
+    tail_bwd2_kernel<true><<<items, 256, 0, static_cast<cudaStream_t>(stream_)>>>(p);
   OSVOS_CHECK_CUDA(cudaGetLastError());
   return OSVOS_OK;
+}
+
+extern "C" size_t osvos_tail_fwd_deterministic_sums(int n, int h, int w) {
+  if (n <= 0 || h <= 0 || w <= 0) return 0;
+  return kTailSums + static_cast<size_t>(tail_fwd_blocks(n, h)) * kTailVals;
 }

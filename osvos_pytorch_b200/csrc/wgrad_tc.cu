@@ -18,6 +18,11 @@
 // consumer warpgroups accumulates 64 of the 128 m rows in registers and flushes
 // them with vector atomics (red.global.add.v2.f32) into the zero-initialised
 // workspace, which a small kernel then transposes into the OIHW gradient.
+// Deterministic form (OSVOS_FLAG_DETERMINISTIC, DET = true): every pixel-range split
+// owns a workspace slice ws[split][9][m][n] that its items write with plain stores
+// (each element exactly once), and the finish sums the slices in split order.  The
+// split count then comes from a fixed nominal SM count (kWgNominalSms), so the
+// summation order depends on the shape only.
 //
 // Replaces autograd's weight gradient of nn.Conv2d(k=3, p=1)
 // (reference networks/vgg_osvos.py:41,142; backward triggered at train_online.py:141).
@@ -31,8 +36,10 @@ constexpr int kWgPatchW = 8, kWgPatchH = 8;
 constexpr int kWgBlockK = 64;                  // pixels per K block
 constexpr int kWgBoxBytes = kWgBlockK * 128;   // 8 KiB: 64 pixels x 64 channels of bf16
 
+constexpr int kWgNominalSms = 132;             // split rule of the deterministic form (H100 SXM)
+
 struct WgradParams {
-  float* ws;  // [9][m_total][n_total]
+  float* ws;  // [9][m_total][n_total], or [splits][9][m_total][n_total] in the deterministic form
   int n_img, h, w;
   int m_total, n_total, m_valid;
   int m_blocks, n_blocks, splits;
@@ -69,7 +76,7 @@ __device__ __forceinline__ void wg_decode_item(const WgradParams& p, int item, i
   split = t / p.tap_items;
 }
 
-template <int BLOCK_N, int PLANES>
+template <int BLOCK_N, int PLANES, bool DET>
 __global__ void __launch_bounds__(kWgThreads, 1)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_p_hi, const __grid_constant__ CUtensorMap map_p_lo,
                 const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ CUtensorMap map_q_lo,
@@ -244,14 +251,18 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_p_hi, const __grid_const
             m_out = row & 63;
           }
           if ((m < p.m_valid || p.tap_rows) && chunk_ok) {
-            float* dst = p.ws + (static_cast<size_t>(tap_c) * p.m_total + m_out) * p.n_total +
+            float* dst = p.ws + ((DET ? static_cast<size_t>(split) * 9 : 0) + tap_c) * p.m_total * p.n_total +
+                         static_cast<size_t>(m_out) * p.n_total +
                          ((p.tap_pairs || p.tap_rows) ? -(c & ~63) : nb * BLOCK_N) + c;
             float2 val = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
             if (Cfg::kSplitAcc) {
               val.x += acc[BLOCK_N / 2 + 4 * j + 2 * h];
               val.y += acc[BLOCK_N / 2 + 4 * j + 2 * h + 1];
             }
-            atomicAdd(reinterpret_cast<float2*>(dst), val);
+            if constexpr (DET)
+              *reinterpret_cast<float2*>(dst) = val;   // this split's slice: written once, by this item
+            else
+              atomicAdd(reinterpret_cast<float2*>(dst), val);
           }
         }
       }
@@ -260,14 +271,21 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_p_hi, const __grid_const
 }
 
 // ws[tap][co][ci] -> OIHW gradient (the immediate, non-deferred form of one layer).
+// DET: `splits` workspace slices, summed in split order.
+template <bool DET = false>
 __global__ void wgrad_finish_kernel(const float* __restrict__ ws, float* __restrict__ dw, int cout, int cin, int ld_a,
-                                    int ld_b) {
+                                    int ld_b, int splits) {
   const int total = cout * cin * 9;
+  const size_t slice = static_cast<size_t>(9) * ld_a * ld_b;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int tap = i % 9;
     const int ci = (i / 9) % cin;
     const int co = i / (9 * cin);
-    dw[i] = ws[(static_cast<size_t>(tap) * ld_a + co) * ld_b + ci];
+    const size_t e = (static_cast<size_t>(tap) * ld_a + co) * ld_b + ci;
+    float v = ws[e];
+    if constexpr (DET)
+      for (int s = 1; s < splits; ++s) v += ws[s * slice + e];
+    dw[i] = v;
   }
 }
 
@@ -280,6 +298,7 @@ struct FinishLayer {
   int cout, cin, ld_a, ld_b, accumulate;
   float scale;
   int items;
+  int splits;   // workspace slices, summed in order (1 outside the deterministic form)
 };
 struct FinishTable {
   FinishLayer layer[OSVOS_WGRAD_FINISH_MAX];
@@ -289,6 +308,8 @@ struct FinishTable {
 constexpr int kFinishThreads = 192;
 constexpr int kFinishChunk = 576;
 
+// DET: each layer's L.splits workspace slices are summed in split order.
+template <bool DET = false>
 __global__ void __launch_bounds__(kFinishThreads)
 wgrad_finish_multi_kernel(const __grid_constant__ FinishTable t) {
   __shared__ __align__(16) float tile[9][68];
@@ -308,7 +329,15 @@ wgrad_finish_multi_kernel(const __grid_constant__ FinishTable t) {
     __syncthreads();   // previous item's readers of `tile` are done
     if (threadIdx.x < 144) {   // 9 taps x 16 float4
       const int tap = threadIdx.x >> 4, c4 = threadIdx.x & 15;
-      const float4 v = __ldg(reinterpret_cast<const float4*>(L.ws + (static_cast<size_t>(tap) * L.ld_a + co) * L.ld_b + ci0) + c4);
+      const float4* src = reinterpret_cast<const float4*>(L.ws + (static_cast<size_t>(tap) * L.ld_a + co) * L.ld_b + ci0) + c4;
+      float4 v = __ldg(src);
+      if constexpr (DET) {
+#pragma unroll 4
+        for (int s = 1; s < L.splits; ++s) {   // the split slices in order (loads issued ahead, adds in order)
+          const float4 u = __ldg(src + s * (static_cast<size_t>(9) * L.ld_a * L.ld_b / 4));
+          v.x += u.x, v.y += u.y, v.z += u.z, v.w += u.w;
+        }
+      }
       *reinterpret_cast<float4*>(&tile[tap][c4 * 4]) = v;
     }
     __syncthreads();
@@ -337,22 +366,12 @@ wgrad_finish_multi_kernel(const __grid_constant__ FinishTable t) {
   }
 }
 
-template <int BLOCK_N, int PLANES>
-static int launch_wgrad(const osvos_wgrad_args* a, cudaStream_t stream) {
-  using Cfg = WgCfg<BLOCK_N, PLANES>;
-  // operand roles
-  const void* p_hi = a->dz_hi;
-  const void* p_lo = a->dz_lo;
-  const void* q_hi = a->x_hi;
-  const void* q_lo = a->x_lo;
-  const int cp = a->dz_channels;   // channels of the P tensor
-  const int cq = a->cin;           // channels of the Q tensor
-
-  WgradParams p;
-  p.ws = a->workspace;
-  p.n_img = a->n;
-  p.h = a->h;
-  p.w = a->w;
+// Item geometry and split count of one weight gradient (no device access).
+template <int BLOCK_N>
+static int plan_wgrad(WgradParams& p, int n, int h, int w, int cp, int cq, int sms) {
+  p.n_img = n;
+  p.h = h;
+  p.w = w;
   p.m_total = (cp + 127) / 128 * 128;
   if (p.m_total != cp && cp != 64) return OSVOS_ERR_UNSUPPORTED;
   p.m_total = cp;  // rows actually stored in the workspace
@@ -370,11 +389,10 @@ static int launch_wgrad(const osvos_wgrad_args* a, cudaStream_t stream) {
   p.tap_pairs = (cq == 64 && BLOCK_N == 128 && !p.tap_rows) ? 1 : 0;
   p.tap_items = p.tap_rows ? 3 : p.tap_pairs ? 5 : 9;
   p.n_blocks = (p.tap_pairs || p.tap_rows) ? 1 : cq / BLOCK_N;
-  p.patches_x = (a->w + kWgPatchW - 1) / kWgPatchW;
-  p.patches_y = (a->h + kWgPatchH - 1) / kWgPatchH;
-  p.patches_total = p.patches_x * p.patches_y * a->n;
+  p.patches_x = (w + kWgPatchW - 1) / kWgPatchW;
+  p.patches_y = (h + kWgPatchH - 1) / kWgPatchH;
+  p.patches_total = p.patches_x * p.patches_y * n;
   const int tiles = p.m_blocks * p.n_blocks * p.tap_items;
-  const int sms = device_sm_count();
   // Pixel-range splits: items are dealt round-robin to the persistent CTAs, so the kernel lasts as long as the CTA with
   // the most items - ROUNDS x K blocks per item.  Pick the split count that minimises that (plus ~2 K-block times per
   // item for the accumulator flush that is not hidden behind the next item's MMAs).  A fixed rule such as ceil(2 SMs /
@@ -396,6 +414,25 @@ static int launch_wgrad(const osvos_wgrad_args* a, cudaStream_t stream) {
   p.patches_per_split = (p.patches_total + splits - 1) / splits;
   p.splits = (p.patches_total + p.patches_per_split - 1) / p.patches_per_split;
   p.total_items = tiles * p.splits;
+  return OSVOS_OK;
+}
+
+template <int BLOCK_N, int PLANES, bool DET>
+static int launch_wgrad(const osvos_wgrad_args* a, cudaStream_t stream) {
+  using Cfg = WgCfg<BLOCK_N, PLANES>;
+  // operand roles
+  const void* p_hi = a->dz_hi;
+  const void* p_lo = a->dz_lo;
+  const void* q_hi = a->x_hi;
+  const void* q_lo = a->x_lo;
+  const int cp = a->dz_channels;   // channels of the P tensor
+  const int cq = a->cin;           // channels of the Q tensor
+
+  WgradParams p;
+  const int sms = device_sm_count();
+  int rc = plan_wgrad<BLOCK_N>(p, a->n, a->h, a->w, cp, cq, DET ? kWgNominalSms : sms);
+  if (rc) return rc;
+  p.ws = a->workspace;
 
   CUtensorMap mp_hi, mp_lo, mq_hi, mq_lo;
   auto enc = [&](CUtensorMap* m, const void* base, int c) {
@@ -405,7 +442,6 @@ static int launch_wgrad(const osvos_wgrad_args* a, cudaStream_t stream) {
     return encode_tensor_map(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, 4, base, dims, strides, box,
                              CU_TENSOR_MAP_SWIZZLE_128B);
   };
-  int rc;
   if ((rc = enc(&mp_hi, p_hi, cp))) return rc;
   if ((rc = enc(&mp_lo, PLANES == 2 ? p_lo : p_hi, cp))) return rc;
   if ((rc = enc(&mq_hi, q_hi, cq))) return rc;
@@ -413,19 +449,21 @@ static int launch_wgrad(const osvos_wgrad_args* a, cudaStream_t stream) {
 
   const bool deferred = (a->flags & OSVOS_FLAG_DEFER_FINISH) != 0;
   const size_t ws_bytes = static_cast<size_t>(9) * p.m_total * p.n_total * sizeof(float);
-  if (!deferred) OSVOS_CHECK_CUDA(cudaMemsetAsync(a->workspace, 0, ws_bytes, stream));
-  auto kern = wgrad_tc_kernel<BLOCK_N, PLANES>;
+  if (!deferred && !DET) OSVOS_CHECK_CUDA(cudaMemsetAsync(a->workspace, 0, ws_bytes, stream));
+  auto kern = wgrad_tc_kernel<BLOCK_N, PLANES, DET>;
   static uint64_t attr_done = 0;   // per instantiation: bit d = device d has the shared-memory opt-in
   OSVOS_CHECK_CUDA(ensure_dynamic_smem(kern, Cfg::kSmemBytes, &attr_done));
   const int grid = p.total_items < sms ? p.total_items : sms;
-  if (deferred) {   // (otherwise the memset above is this kernel's stream predecessor: plain launch)
+  if (deferred || DET) {   // (otherwise the memset above is this kernel's stream predecessor: plain launch)
     OSVOS_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kWgThreads), Cfg::kSmemBytes, stream, mp_hi, mp_lo, mq_hi, mq_lo, p));
-    return OSVOS_OK;
+    if (deferred) return OSVOS_OK;
+  } else {
+    kern<<<grid, kWgThreads, Cfg::kSmemBytes, stream>>>(mp_hi, mp_lo, mq_hi, mq_lo, p);
+    OSVOS_CHECK_CUDA(cudaGetLastError());
   }
-  kern<<<grid, kWgThreads, Cfg::kSmemBytes, stream>>>(mp_hi, mp_lo, mq_hi, mq_lo, p);
-  OSVOS_CHECK_CUDA(cudaGetLastError());
   const int total = a->cout * a->cin * 9;
-  wgrad_finish_kernel<<<(total + 255) / 256, 256, 0, stream>>>(a->workspace, a->dw, a->cout, a->cin, p.m_total, p.n_total);
+  wgrad_finish_kernel<DET><<<(total + 255) / 256, 256, 0, stream>>>(a->workspace, a->dw, a->cout, a->cin, p.m_total,
+                                                                    p.n_total, DET ? p.splits : 1);
   OSVOS_CHECK_CUDA(cudaGetLastError());
   return OSVOS_OK;
 }
@@ -438,7 +476,24 @@ extern "C" size_t osvos_wgrad_workspace_bytes(int cout_or_padded, int cin) {
   return static_cast<size_t>(9) * cout_or_padded * cin * sizeof(float);
 }
 
-extern "C" int osvos_wgrad_finish(const osvos_wgrad_finish_item* items, int count, osvos_stream_t stream_) {
+// Split count of the deterministic form (shape only; the tensor-core path's constraints are checked by the launch).
+static int deterministic_splits(int n, int h, int w, int cin, int dz_channels) {
+  if (n <= 0 || h <= 0 || w <= 0 || cin <= 0 || dz_channels <= 0 || dz_channels % 64 != 0) return 0;
+  if (!(cin % 128 == 0 || cin == 64)) return 0;
+  WgradParams p;
+  if (plan_wgrad<128>(p, n, h, w, dz_channels, cin, kWgNominalSms)) return 0;
+  return p.splits;
+}
+
+extern "C" int osvos_wgrad_deterministic_splits(int n, int h, int w, int cin, int dz_channels) {
+  return deterministic_splits(n, h, w, cin, dz_channels);
+}
+
+extern "C" size_t osvos_wgrad_deterministic_workspace_bytes(int n, int h, int w, int cin, int dz_channels) {
+  return static_cast<size_t>(deterministic_splits(n, h, w, cin, dz_channels)) * osvos_wgrad_workspace_bytes(dz_channels, cin);
+}
+
+static int wgrad_finish_impl(const osvos_wgrad_finish_item* items, const int* splits, int count, cudaStream_t stream) {
   OSVOS_CHECK_ARG(items != nullptr && count > 0 && count <= OSVOS_WGRAD_FINISH_MAX);
   FinishTable t;
   t.count = count;
@@ -457,15 +512,30 @@ extern "C" int osvos_wgrad_finish(const osvos_wgrad_finish_item* items, int coun
     L.accumulate = it.accumulate ? 1 : 0;
     L.scale = it.scale;
     L.items = it.cout * (it.cin / 64);
+    L.splits = splits ? splits[i] : 1;
+    OSVOS_CHECK_ARG(L.splits >= 1);
     total_items += L.items;
   }
   OSVOS_CHECK_ARG(total_items < (1ll << 31));
   t.total_items = static_cast<int>(total_items);
   const long long cap = static_cast<long long>(device_sm_count()) * 10;   // 10 x 192 threads resident per SM
   const unsigned grid = static_cast<unsigned>(total_items < cap ? total_items : cap);
-  wgrad_finish_multi_kernel<<<grid, kFinishThreads, 0, static_cast<cudaStream_t>(stream_)>>>(t);
+  if (splits)
+    wgrad_finish_multi_kernel<true><<<grid, kFinishThreads, 0, stream>>>(t);
+  else
+    wgrad_finish_multi_kernel<false><<<grid, kFinishThreads, 0, stream>>>(t);
   OSVOS_CHECK_CUDA(cudaGetLastError());
   return OSVOS_OK;
+}
+
+extern "C" int osvos_wgrad_finish(const osvos_wgrad_finish_item* items, int count, osvos_stream_t stream_) {
+  return wgrad_finish_impl(items, nullptr, count, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int osvos_wgrad_finish_deterministic(const osvos_wgrad_finish_item* items, const int* splits, int count,
+                                                osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(splits != nullptr);
+  return wgrad_finish_impl(items, splits, count, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int osvos_conv3x3_wgrad(const osvos_wgrad_args* a, osvos_stream_t stream_) {
@@ -477,5 +547,7 @@ extern "C" int osvos_conv3x3_wgrad(const osvos_wgrad_args* a, osvos_stream_t str
   OSVOS_CHECK_ARG(a->cin % 128 == 0 || a->cin == 64);     // Cin = 64: tap-pair / tap-row modes of the 128-wide kernel
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const bool fast = (a->flags & OSVOS_FLAG_FAST) != 0;
-  return fast ? launch_wgrad<128, 1>(a, stream) : launch_wgrad<128, 2>(a, stream);
+  if (a->flags & OSVOS_FLAG_DETERMINISTIC)
+    return fast ? launch_wgrad<128, 1, true>(a, stream) : launch_wgrad<128, 2, true>(a, stream);
+  return fast ? launch_wgrad<128, 1, false>(a, stream) : launch_wgrad<128, 2, false>(a, stream);
 }

@@ -41,6 +41,21 @@ class Act:
         return Act(hi, lo)
 
 
+class no_uninitialized_fill:
+    """Under torch.use_deterministic_algorithms torch fills every torch.empty with NaN
+    (torch.utils.deterministic.fill_uninitialized_memory).  The package's workspaces and outputs are written in full
+    by its kernels before they are read, so that fill is pure memory traffic (~0.5 ms per 480x854 backward for the
+    weight-gradient slices alone); this context turns it off around the package's own allocations."""
+    def __enter__(self):
+        import torch.utils.deterministic as d
+        self.prev = d.fill_uninitialized_memory
+        d.fill_uninitialized_memory = False
+
+    def __exit__(self, *exc):
+        import torch.utils.deterministic as d
+        d.fill_uninitialized_memory = self.prev
+
+
 def _require_cuda(t, name):
     if not t.is_cuda:
         raise RuntimeError(f"osvos_pytorch_b200: {name} must be a CUDA tensor; the OSVOS hot path has no CPU fallback "
@@ -194,10 +209,11 @@ def side_folded_multi(xs, folded, fast=False):
 
 
 def conv3x3(x, w_packed, bias, cout, relu=False, fast=False, out_act=True, out_f32=False, mask=None,
-            proj_w=None, proj_b=None, simt=False, pool=False, colsum=None):
+            proj_w=None, proj_b=None, simt=False, pool=False, colsum=None, deterministic=False):
     """3x3 / pad 1 conv of an Act through the wgmma kernel.  Returns (Act|None, f32|None, pq|None), or
     (Act, pooled Act) when pool=True (fused MaxPool2d(2,2,ceil_mode)).  `colsum` ([cout] fp32, pre-zeroed)
-    receives the per-channel sum of the output (fused bias gradient)."""
+    receives the per-channel sum of the output (fused bias gradient); ``deterministic``: added in a fixed order
+    (per-tile partial rows + osvos_reduce_rows) instead of with atomics."""
     lib = nat.load()
     n, h, w, cin = x.shape
     dev = x.hi.device
@@ -215,13 +231,19 @@ def conv3x3(x, w_packed, bias, cout, relu=False, fast=False, out_act=True, out_f
     yp = Act.empty(n, (h + 1) // 2, (w + 1) // 2, cout, dev, fast) if pool else None
     a.pool_hi = nat.ptr(yp.hi) if pool else None
     a.pool_lo = nat.ptr(yp.lo) if pool else None
-    a.colsum = nat.ptr(colsum)
+    rows = None
+    if deterministic and colsum is not None:
+        nrows = lib.osvos_conv3x3_colsum_rows(n, h, w)
+        rows = torch.empty((nrows, cout), dtype=torch.float32, device=dev)
+    a.colsum = nat.ptr(rows if rows is not None else colsum)
     a.n, a.h, a.w, a.cin, a.cout = n, h, w, cin, cout
     a.flags = (nat.FLAG_RELU if relu else 0) | (nat.FLAG_FAST if fast else 0) | \
-              (nat.FLAG_RELU_MASK if mask is not None else 0)
+              (nat.FLAG_RELU_MASK if mask is not None else 0) | (nat.FLAG_DETERMINISTIC if rows is not None else 0)
     fn = lib.osvos_conv3x3_simt if simt else lib.osvos_conv3x3
     _count()
     nat.check(fn(byref(a), _stream()), "osvos_conv3x3")
+    if rows is not None:
+        reduce_rows(rows, colsum, accumulate=True)
     if pool:
         return y, yp
     return y, yf, pq
@@ -248,7 +270,7 @@ def side_project(feat, proj_w, proj_b):
     return pq
 
 
-def tail_fwd(pqs, fuse_bias, n, h, w, label=None, out=None, loss_weights=None, divisor=None):
+def tail_fwd(pqs, fuse_bias, n, h, w, label=None, out=None, loss_weights=None, divisor=None, deterministic=False):
     """Upsample + crop + fuse (+ loss sums, + the five class-balanced BCE losses and their weighted total).
     Returns (out [5,n,1,h,w] fp32, sums [TAIL_SUMS] f64 | None) and, with `loss_weights` (5 floats) and `divisor`,
     additionally losses [6] fp32 = the five per-map losses and sum_k loss_weights[k] * loss_k."""
@@ -258,8 +280,10 @@ def tail_fwd(pqs, fuse_bias, n, h, w, label=None, out=None, loss_weights=None, d
         # each map starts on a 16-byte boundary so the kernel can use 128-bit stores
         per = (n * h * w + 3) // 4 * 4
         out = torch.empty((5, per), dtype=torch.float32, device=dev)[:, :n * h * w].view(5, n, 1, h, w)
-    sums = torch.empty(nat.TAIL_SUMS, dtype=torch.float64, device=dev) if label is not None else None
+    nsums = lib.osvos_tail_fwd_deterministic_sums(n, h, w) if deterministic else nat.TAIL_SUMS
+    sums = torch.empty(nsums, dtype=torch.float64, device=dev) if label is not None else None
     a = nat.TailFwdArgs()
+    a.flags = nat.FLAG_DETERMINISTIC if deterministic else 0
     for k in range(4):
         a.pq[k] = pqs[k].data_ptr()
     for k in range(5):
@@ -284,12 +308,13 @@ def tail_fwd(pqs, fuse_bias, n, h, w, label=None, out=None, loss_weights=None, d
     return out, sums
 
 
-def tail_loss_bwd(out, label, sums, loss_weights, divisor, upstream, n, h, w, want_fuse_bias=True):
+def tail_loss_bwd(out, label, sums, loss_weights, divisor, upstream, n, h, w, want_fuse_bias=True, deterministic=False):
     """Backward of tail + the weighted class-balanced BCE objective in one launch (see include/osvos_b200.h):
     -> (list of 4 dpq tensors [n,hk,wk,2], fuse.bias gradient [1] | None)."""
     lib = nat.load()
     dev = out.device
     a = nat.TailLossBwdArgs()
+    a.flags = nat.FLAG_DETERMINISTIC if deterministic else 0
     for k in range(5):
         a.logits[k] = out[k].data_ptr()
         a.loss_weights[k] = float(loss_weights[k])
@@ -310,14 +335,20 @@ def tail_loss_bwd(out, label, sums, loss_weights, divisor, upstream, n, h, w, wa
 
 
 # ------------------------------------------------------------------ backward ops
-def wgrad_workspace_floats(dz_channels, cin):
+def wgrad_workspace_floats(dz_channels, cin, shape=None, deterministic=False):
+    """Workspace of one weight gradient; ``deterministic`` (needs ``shape`` = (n, h, w)): one slice per pixel-range
+    split, see osvos_wgrad_deterministic_workspace_bytes."""
+    if deterministic:
+        return nat.load().osvos_wgrad_deterministic_workspace_bytes(*shape, cin, dz_channels) // 4
     return nat.load().osvos_wgrad_workspace_bytes(dz_channels, cin) // 4
 
 
-def conv3x3_wgrad(x, dz, cout, fast=False, deferred_ws=None):
+def conv3x3_wgrad(x, dz, cout, fast=False, deferred_ws=None, deterministic=False):
     """dW [cout, cin, 3, 3] of a 3x3 conv from its input act `x` and output-gradient act `dz`.
     With `deferred_ws` (a ZEROED fp32 workspace of wgrad_workspace_floats(dz.channels, cin)) only the tensor-core
-    accumulation is enqueued and a finish item for ops.wgrad_finish is returned instead of dW."""
+    accumulation is enqueued and a finish item for ops.wgrad_finish is returned instead of dW.  ``deterministic``:
+    per-split workspace slices summed in order (the workspace is then wgrad_workspace_floats(..., deterministic=True)
+    floats and needs no zeroing)."""
     lib = nat.load()
     n, h, w, cin = x.shape
     dzc = dz.shape[3]
@@ -325,15 +356,18 @@ def conv3x3_wgrad(x, dz, cout, fast=False, deferred_ws=None):
     a = nat.WgradArgs()
     a.x_hi, a.x_lo, a.dz_hi, a.dz_lo = x.hi.data_ptr(), nat.ptr(x.lo), dz.hi.data_ptr(), nat.ptr(dz.lo)
     a.n, a.h, a.w, a.cin, a.cout, a.dz_channels = n, h, w, cin, cout, dzc
-    a.flags = nat.FLAG_FAST if fast else 0
+    a.flags = (nat.FLAG_FAST if fast else 0) | (nat.FLAG_DETERMINISTIC if deterministic else 0)
     if deferred_ws is not None:
         a.dw, a.workspace = None, deferred_ws.data_ptr()
         a.flags |= nat.FLAG_DEFER_FINISH
         _count(1)
         nat.check(lib.osvos_conv3x3_wgrad(byref(a), _stream()), "osvos_conv3x3_wgrad")
-        return {"ws": deferred_ws, "cout": cout, "cin": cin, "dz_channels": dzc}
+        item = {"ws": deferred_ws, "cout": cout, "cin": cin, "dz_channels": dzc}
+        if deterministic:
+            item["splits"] = lib.osvos_wgrad_deterministic_splits(n, h, w, cin, dzc)
+        return item
     dw = torch.empty((cout, cin, 3, 3), dtype=torch.float32, device=dev)
-    ws = torch.empty(lib.osvos_wgrad_workspace_bytes(dzc, cin) // 4, dtype=torch.float32, device=dev)
+    ws = torch.empty(wgrad_workspace_floats(dzc, cin, (n, h, w), deterministic), dtype=torch.float32, device=dev)
     a.dw, a.workspace = dw.data_ptr(), ws.data_ptr()
     _count(3)
     nat.check(lib.osvos_conv3x3_wgrad(byref(a), _stream()), "osvos_conv3x3_wgrad")
@@ -352,14 +386,20 @@ def wgrad_finish(items):
             f.cout, f.cin, f.dz_channels = it["cout"], it["cin"], it["dz_channels"]
             f.accumulate, f.scale = int(bool(it.get("accumulate"))), 1.0
         _count(1)
-        nat.check(lib.osvos_wgrad_finish(arr, len(part), _stream()), "osvos_wgrad_finish")
+        if any("splits" in it for it in part):           # deterministic workspaces: their split slices in order
+            splits = (nat.c_int * len(part))(*(int(it.get("splits", 1)) for it in part))
+            nat.check(lib.osvos_wgrad_finish_deterministic(arr, splits, len(part), _stream()),
+                      "osvos_wgrad_finish_deterministic")
+        else:
+            nat.check(lib.osvos_wgrad_finish(arr, len(part), _stream()), "osvos_wgrad_finish")
 
 
-def tail_bwd(grads, n, h, w):
+def tail_bwd(grads, n, h, w, deterministic=False):
     """grads: list of 5 tensors [n,1,h,w] or None -> list of 4 dpq tensors [n,hk,wk,2]."""
     lib = nat.load()
     dev = next(g for g in grads if g is not None).device
     a = nat.TailBwdArgs()
+    a.flags = nat.FLAG_DETERMINISTIC if deterministic else 0
     keep = []
     for k in range(5):
         g = grads[k]
@@ -379,9 +419,27 @@ def tail_bwd(grads, n, h, w):
     return dpq
 
 
-def sum_f32(x):
+def reduce_rows(rows, out, accumulate=False):
+    """out[c] = (accumulate ? out[c] : 0) + sum_r rows[r][c] in a fixed order (osvos_reduce_rows); rows [R, C] fp32."""
+    lib = nat.load()
+    nrows, ncols = int(rows.shape[0]), int(rows.shape[1])
+    scratch = torch.empty(lib.osvos_reduce_rows_scratch_floats(nrows, ncols), dtype=torch.float32, device=rows.device)
+    _count(2)
+    nat.check(lib.osvos_reduce_rows(rows.data_ptr(), nrows, ncols, scratch.data_ptr(), out.data_ptr(), int(accumulate),
+                                    _stream()), "osvos_reduce_rows")
+    return out
+
+
+def sum_f32(x, deterministic=False):
     lib = nat.load()
     x = x.contiguous().float()
+    if deterministic:                               # fixed grid of contiguous ranges, totals added in order
+        scratch = torch.empty(lib.osvos_sum_f32_deterministic_scratch_bytes(), dtype=torch.uint8, device=x.device)
+        out = torch.empty(1, dtype=torch.float32, device=x.device)
+        _count(1)
+        nat.check(lib.osvos_sum_f32_deterministic(x.data_ptr(), x.numel(), scratch.data_ptr(), out.data_ptr(),
+                                                  _stream()), "osvos_sum_f32_deterministic")
+        return out
     scratch = torch.empty(2, dtype=torch.float64, device=x.device)
     out = torch.empty(1, dtype=torch.float32, device=x.device)
     _count(1)
@@ -390,7 +448,31 @@ def sum_f32(x):
     return out
 
 
-def unpool_add_mask(dpool, x, dside, colsum=None):
+def _unpool_deterministic(dpool, x, dpq, wfold, colsum):
+    """osvos_unpool_mask_deterministic: the column sums as per-block rows, added into `colsum` in order."""
+    lib = nat.load()
+    n, h, w, c = x.shape
+    dz = Act.empty(n, h, w, c, x.hi.device, x.lo is None)
+    rows = None
+    if colsum is not None:
+        nrows = lib.osvos_unpool_colsum_rows(n, h, w, c, int(dpool is not None), int(dpq is not None))
+        rows = torch.empty((nrows, c), dtype=torch.float32, device=x.hi.device)
+    _count()
+    nat.check(lib.osvos_unpool_mask_deterministic(dpool.hi.data_ptr() if dpool is not None else None,
+                                                  nat.ptr(dpool.lo) if dpool is not None else None, x.hi.data_ptr(),
+                                                  nat.ptr(x.lo), nat.ptr(dpq), nat.ptr(wfold), dz.hi.data_ptr(),
+                                                  nat.ptr(dz.lo), nat.ptr(rows), n, h, w, c, _stream()),
+              "osvos_unpool_mask_deterministic")
+    if rows is not None:
+        reduce_rows(rows, colsum, accumulate=True)
+    return dz
+
+
+def unpool_add_mask(dpool, x, dside, colsum=None, deterministic=False):
+    if deterministic:
+        if dside is not None:
+            raise ValueError("unpool_add_mask: the deterministic form takes no fp32 side gradient map")
+        return _unpool_deterministic(dpool, x, None, None, colsum)
     lib = nat.load()
     n, h, w, c = x.shape
     dz = Act.empty(n, h, w, c, x.hi.device, x.lo is None)
@@ -402,8 +484,10 @@ def unpool_add_mask(dpool, x, dside, colsum=None):
     return dz
 
 
-def unpool_side_mask(dpool, x, dpq, wfold, colsum=None):
+def unpool_side_mask(dpool, x, dpq, wfold, colsum=None, deterministic=False):
     """dz = ReLU'(x) * (unpool(dpool) + folded side gradient of dpq); dpool None: no pooling consumer."""
+    if deterministic:
+        return _unpool_deterministic(dpool, x, dpq, wfold, colsum)
     lib = nat.load()
     n, h, w, c = x.shape
     dz = Act.empty(n, h, w, c, x.hi.device, x.lo is None)
@@ -430,14 +514,25 @@ def side_folded_wgrad(x, dpq, g):
     return g
 
 
-def side_folded_wgrad_multi(xs, dpqs, gs):
-    """side_folded_wgrad of several scales in ONE launch (osvos_side_folded_wgrad_multi)."""
+def side_folded_wgrad_multi(xs, dpqs, gs, deterministic=False):
+    """side_folded_wgrad of several scales in ONE launch (osvos_side_folded_wgrad_multi); ``deterministic``: the
+    blocks' partial rows are added in order (osvos_side_folded_wgrad_multi_deterministic)."""
     lib = nat.load()
     arr = (nat.SideWgradItem * len(xs))()
     for it, x, dpq, g in zip(arr, xs, dpqs, gs):
         n, h, w, c = x.shape
         it.x_hi, it.x_lo, it.dpq, it.g = x.hi.data_ptr(), nat.ptr(x.lo), dpq.data_ptr(), g.data_ptr()
         it.n, it.h, it.w, it.c = n, h, w, c
+    if deterministic:
+        nbytes = lib.osvos_side_folded_wgrad_deterministic_workspace_bytes(arr, len(xs))
+        if nbytes == 0:
+            nat.check(lib.osvos_side_folded_wgrad_multi_deterministic(arr, len(xs), None, _stream()),
+                      "osvos_side_folded_wgrad_multi_deterministic")
+        ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=gs[0].device)
+        _count(1 + 2 * len(xs))
+        nat.check(lib.osvos_side_folded_wgrad_multi_deterministic(arr, len(xs), ws.data_ptr(), _stream()),
+                  "osvos_side_folded_wgrad_multi_deterministic")
+        return
     _count()
     nat.check(lib.osvos_side_folded_wgrad_multi(arr, len(xs), _stream()), "osvos_side_folded_wgrad_multi")
 
@@ -469,11 +564,19 @@ def channel_sum(a):
     return out
 
 
-def conv_first_bwd(x, dz, weight, need_dx):
+def conv_first_bwd(x, dz, weight, need_dx, deterministic=False):
     lib = nat.load()
     n, _, h, w = (int(v) for v in x.shape)
     dw = torch.empty((64, 3, 3, 3), dtype=torch.float32, device=x.device)
     dx = torch.empty_like(x) if need_dx else None
+    if deterministic:                               # one partial slot per block, added in block order
+        ws = torch.empty(lib.osvos_conv_first_bwd_deterministic_workspace_bytes(n, h, w), dtype=torch.uint8,
+                         device=x.device)
+        _count(2 if need_dx else 1)
+        nat.check(lib.osvos_conv_first_bwd_deterministic(x.data_ptr(), dz.hi.data_ptr(), nat.ptr(dz.lo),
+                                                         weight.data_ptr(), dw.data_ptr(), nat.ptr(dx), ws.data_ptr(),
+                                                         n, h, w, _stream()), "osvos_conv_first_bwd_deterministic")
+        return dw, dx
     ws = torch.empty(lib.osvos_conv_first_bwd_workspace_bytes(), dtype=torch.uint8, device=x.device)
     _count(2 if need_dx else 1)
     nat.check(lib.osvos_conv_first_bwd(x.data_ptr(), dz.hi.data_ptr(), nat.ptr(dz.lo), weight.data_ptr(),

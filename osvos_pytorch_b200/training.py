@@ -60,10 +60,14 @@ class GraphedTrainStep:
     layouts are static buffers outside the graph that ``optim.FusedSGD`` rewrites in its update kernel (no
     packing work per micro-batch; only valid with that optimizer).  ``objective(outputs, gts) -> scalar tensor``, or a
     tuple of five loss weights = the package's fused objective (``OSVOS.forward_objective``).
+
+    The graph keeps the kernels of the mode ``torch.are_deterministic_algorithms_enabled()`` had at capture; a replay
+    under the other mode raises instead of silently running those.
     """
 
     def __init__(self, net, objective, sample, grad_scale=1.0, external_pack=False):
         self.net, self.objective, self.grad_scale = net, objective, float(grad_scale)
+        self.deterministic = torch.are_deterministic_algorithms_enabled()
         self.x = sample["image"].detach().clone()
         self.gt = sample["gt"].detach().clone()
         self.params = [p for n, p in net.named_parameters() if not n.startswith("upscale")]
@@ -114,6 +118,10 @@ class GraphedTrainStep:
         return loss.detach()
 
     def __call__(self, sample=None):
+        if torch.are_deterministic_algorithms_enabled() != self.deterministic:
+            raise RuntimeError(
+                "GraphedTrainStep was captured with torch.use_deterministic_algorithms(%s) but is replayed with %s; "
+                "capture a new step after changing the setting" % (self.deterministic, not self.deterministic))
         if sample is not None:
             self.x.copy_(sample["image"], non_blocking=True)
             self.gt.copy_(sample["gt"], non_blocking=True)

@@ -31,6 +31,9 @@ def parse(argv=None):
     ap.add_argument("--lr", type=float, default=None, help="default 1e-8 (reference); 1e-10 with --synthetic, whose "
                     "He-initialised network produces O(10)-scale logits and therefore much larger summed-loss gradients")
     ap.add_argument("--wd", type=float, default=0.0002)
+    ap.add_argument("--deterministic", action="store_true",
+                    help="torch.use_deterministic_algorithms(True) before anything is built: the package's kernels "
+                         "reduce in a fixed order, so two runs on the same device give bit-identical results")
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--gpu-id", type=int, default=0)
     ap.add_argument("--precision", default="exact", choices=["exact", "fast"])
@@ -59,6 +62,8 @@ def parse(argv=None):
 
 def main(argv=None):
     a = parse(argv)
+    if a.deterministic:
+        torch.use_deterministic_algorithms(True)
     iters = a.iters if a.iters is not None else 2000 * a.n_ave_grad
     if a.lr is None:
         a.lr = 1e-10 if a.synthetic else 1e-8

@@ -44,6 +44,9 @@ def parse(argv=None):
     ap.add_argument("--test-interval", type=int, default=5)
     ap.add_argument("--lr", type=float, default=1e-8)
     ap.add_argument("--wd", type=float, default=0.0002)
+    ap.add_argument("--deterministic", action="store_true",
+                    help="torch.use_deterministic_algorithms(True) before anything is built: the package's kernels "
+                         "reduce in a fixed order, so two runs on the same device give bit-identical results")
     ap.add_argument("--pretrained", type=int, default=2, help="2 = Caffe VGG (.mat), 1 = torchvision VGG, 0 = none")
     ap.add_argument("--precision", default="exact", choices=["exact", "fast"])
     ap.add_argument("--synthetic", action="store_true")
@@ -82,6 +85,8 @@ def _val_scores(per_seq):
 
 def main(argv=None):
     a = parse(argv)
+    if a.deterministic:
+        torch.use_deterministic_algorithms(True)
     rank, world, local = parallel.init_distributed()
     device = torch.device("cuda", local)
     torch.cuda.set_device(device)
