@@ -521,6 +521,22 @@ OSVOS_API int osvos_affine_warp_u8_indexed(const uint8_t* image_store, const uin
                                            const int* flips_host, int n, int n_store, int h, int w, float mean_b,
                                            float mean_g, float mean_r, osvos_stream_t stream);
 
+/* ---- resize of decoded frames (dataloaders/davis_2016.py:96-99 inputRes: scipy.misc.imresize, i.e. Pillow's 8-bit
+ * Image.resize; DESIGN.md §17) ----------------------------------------------------------------------------------------
+ *   osvos_resize_u8: src [n][h][w][c] uint8 -> dst [n][out_h][out_w][c] uint8, c = 1 or 3, bit-identical to Pillow's
+ *                    Image.resize((out_w, out_h), BILINEAR) (separable antialiased triangle filter, 22-bit fixed point,
+ *                    horizontal pass first) or NEAREST (ImagingScaleAffine's index walk) of an L / RGB image; channels
+ *                    are independent, so BGR bytes resize as they are.  Equal sizes are a copy.  n < 65536, h, w,
+ *                    out_h, out_w < 32768; src and dst any alignment, not overlapping.  `workspace`:
+ *                    osvos_resize_u8_workspace_bytes(...) bytes (the coefficient or index tables and, when both axes
+ *                    change size under BILINEAR, the horizontal pass's uint8 intermediate), 4-byte aligned, owned by the
+ *                    caller (may be NULL when that is 0); nothing is allocated and nothing waits for the host.
+ *   osvos_resize_u8_workspace_bytes: host query; 0 for invalid arguments.                                            */
+enum { OSVOS_RESIZE_BILINEAR = 0, OSVOS_RESIZE_NEAREST = 1 };
+OSVOS_API size_t osvos_resize_u8_workspace_bytes(int n, int h, int w, int c, int out_h, int out_w, int mode);
+OSVOS_API int osvos_resize_u8(const uint8_t* src, uint8_t* dst, void* workspace, int n, int h, int w, int c, int out_h,
+                              int out_w, int mode, osvos_stream_t stream);
+
 /* ---- DAVIS-2016 region and boundary measures (J and F; DESIGN.md §14) -------------------------------------------
  * Per frame, P = logit > 0 (±0.0 is background, as osvos_logits_to_u8 mode MASK) and G = byte != 0.  The boundary map
  * of a mask is b = seg^E | seg^S | seg^SE (E, S, SE: the right, lower and lower-right neighbour, zeros past the frame),

@@ -98,6 +98,7 @@ class SgdSegment(Structure):
 
 
 U8_PROB, U8_BYTESCALE, U8_MASK = 0, 1, 2
+RESIZE_BILINEAR, RESIZE_NEAREST = 0, 1
 SGD_MAX_SEGMENTS = 64
 
 # name -> (restype, argtypes); mirrors include/osvos_b200.h one to one (tests/test_abi.py checks it)
@@ -153,6 +154,8 @@ SIGNATURES = {
     "osvos_affine_warp_u8_indexed": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int),
                                              POINTER(c_double), POINTER(c_int), c_int, c_int, c_int, c_int, c_float,
                                              c_float, c_float, c_void_p]),
+    "osvos_resize_u8_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
+    "osvos_resize_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "osvos_davis_measures_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "osvos_davis_measures": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "osvos_reduce_rows_scratch_floats": (c_size_t, [c_int, c_int]),

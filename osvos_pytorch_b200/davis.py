@@ -11,8 +11,13 @@ tensors, or the fused warp produces the augmented ones (augment.affine_warp_u8).
 ``DeviceFrames`` decodes a whole split once and keeps the bytes on the device, so parent training decodes once per
 run instead of once per epoch; each batch is then one indexed warp from the store (DESIGN.md §15).
 
-``inputRes`` is not supported: the reference resizes with ``scipy.misc.imresize``, which no longer exists in SciPy, and
-neither entry point sets it.
+``DAVIS2016Frames`` refuses ``inputRes``: its items are the decoded bytes at their stored size.  The reference's
+``inputRes`` (``scipy.misc.imresize``, which no longer exists in SciPy) is a device stage here instead:
+``input_res=`` on ``upload``, ``to_device``, ``DeviceFrames`` and ``inference.SequenceSegmenter`` resizes the image
+(bilinear) and the mask (nearest) right after the upload, bit-identical to scipy 1.0's imresize (ops.resize_u8,
+DESIGN.md §17), before the float conversion, flip and warp, the reference's order.  One deliberate difference: the
+reference builds the all-zero mask of an unannotated frame at the stored size and never resizes it; here that mask
+has the resized size, so that a batch has one size.
 """
 import os
 import random
@@ -138,23 +143,54 @@ def pinned(data):
     return data if data.is_pinned() else data.pin_memory()
 
 
-def upload(batch, device):
-    """One host-to-device copy of a collated batch -> (image uint8 [N,H,W,3], gt uint8 [N,H,W], label stats)."""
+def imresize_size(size, h, w):
+    """The (h', w') that scipy 1.0's ``imresize(arr, size)`` gives a frame of h x w (the reference's ``inputRes``): a
+    tuple is (h', w'), an int is a percentage (int(dim * (size / 100.0))), a float a fraction (int(dim * size))."""
+    if isinstance(size, (bool, np.bool_)):
+        raise TypeError("input_res must be a (height, width) pair, an int percentage or a float fraction")
+    if isinstance(size, (int, np.integer)):
+        pct = int(size) / 100.0
+        out = (int(h * pct), int(w * pct))
+    elif isinstance(size, (float, np.floating)):
+        out = (int(h * float(size)), int(w * float(size)))
+    else:
+        out = tuple(int(v) for v in size)
+        if len(out) != 2:
+            raise ValueError(f"input_res must be (height, width), got {size!r}")
+    if min(out) < 1:
+        raise ValueError(f"input_res {size!r} gives an empty frame {out} for a {h}x{w} frame")
+    return out
+
+
+def resize_pair(img, gt, input_res):
+    """Device frames uint8 [N,H,W,3] and masks [N,H,W] at ``input_res`` (imresize_size): the image bilinear, the mask
+    nearest, as the reference's make_img_gt_pair resizes them (dataloaders/davis_2016.py:96-99)."""
+    h, w = (int(v) for v in img.shape[1:3])
+    size = imresize_size(input_res, h, w)
+    return ops.resize_u8(img, size, "bilinear"), ops.resize_u8(gt, size, "nearest")
+
+
+def upload(batch, device, input_res=None):
+    """One host-to-device copy of a collated batch -> (image uint8 [N,H,W,3], gt uint8 [N,H,W], label stats).
+    ``input_res``: the frames and masks are resized on the device first (resize_pair)."""
     n, h, w = (int(v) for v in batch["size"])
     data = pinned(batch["data"]).to(device, non_blocking=True)
     img, gt = views(data, n, h, w)
+    if input_res is not None:
+        img, gt = resize_pair(img, gt, input_res)
     return img, gt, ops.label_stats_u8(gt)
 
 
-def to_device(batch, device, augment=None, meanval=MEANVAL):
+def to_device(batch, device, augment=None, meanval=MEANVAL, input_res=None):
     """Collated batch -> {'image': f32 [N,3,H,W], 'gt': f32 [N,1,H,W]} on ``device``.
 
     augment None: the reference's make_img_gt_pair + ToTensor, bit for bit (ops.image_from_bgr8, ops.label_from_u8).
     Otherwise RandomHorizontalFlip + ScaleNRotate as the reference composes them, fused with the ingest
     (augment.affine_warp_u8): ``augment`` is a list of per-sample (flip, rot, scale) triples, or a random generator
-    from which augment.draw_params draws them in the reference's order."""
+    from which augment.draw_params draws them in the reference's order.  ``input_res``: the reference's ``inputRes``,
+    applied on the device before all of that (upload)."""
     with torch.cuda.device(device):
-        img, gt, stats = upload(batch, device)
+        img, gt, stats = upload(batch, device, input_res)
         if augment is None:
             return {"image": ops.image_from_bgr8(img, meanval), "gt": ops.label_from_u8(gt, stats)}
         params = augment if isinstance(augment, (list, tuple)) else _augment.draw_params(int(img.shape[0]), rng=augment)
@@ -196,9 +232,14 @@ class DeviceFrames:
 
     ``group``: a torch.distributed process group of R ranks.  Each rank then decodes a 1/R share (``shard``), the
     frame sizes are exchanged with all_gather_object, and the shares are gathered with NCCL all_gather_into_tensor,
-    one call per size group and tensor, so every rank holds the whole store (layout: ``shard_plan``)."""
+    one call per size group and tensor, so every rank holds the whole store (layout: ``shard_plan``).
 
-    def __init__(self, dataset, device, workers=0, group=None):
+    ``input_res``: the reference's ``inputRes`` (imresize_size).  Each frame is resized on the device as it is stored
+    (resize_pair), so the store, its size groups and the memory check are at the resized size; frames of different
+    stored sizes that resize to one size share a group.  With a process group each rank resizes its own share before
+    the gather."""
+
+    def __init__(self, dataset, device, workers=0, group=None, input_res=None):
         import torch.distributed as dist
         from torch.utils.data import DataLoader, Subset
         t0 = time.perf_counter()
@@ -217,7 +258,7 @@ class DeviceFrames:
             metas = [None] * world
             dist.all_gather_object(metas, meta, group=group)
             meta = sorted(m for ms in metas for m in ms)
-        sizes = [m[1] for m in meta]
+        sizes = [m[1] if input_res is None else imresize_size(input_res, *m[1]) for m in meta]
         self.has_gt = [m[2] for m in meta]
         self.fname = [m[3] for m in meta]
         plan = shard_plan(sizes, world)
@@ -232,10 +273,18 @@ class DeviceFrames:
                 img = torch.zeros((world * pad, h, w, 3), dtype=torch.uint8, device=self.device)
                 gt = torch.zeros((world * pad, h, w), dtype=torch.uint8, device=self.device)
                 for j, i in enumerate(members[rank]):
-                    data = pinned(decoded.pop(i)["data"])
-                    src_img, src_gt = views(data, 1, h, w)
-                    img[rank * pad + j].copy_(src_img[0], non_blocking=True)
-                    gt[rank * pad + j].copy_(src_gt[0], non_blocking=True)
+                    item = decoded.pop(i)
+                    data = pinned(item["data"])
+                    s = rank * pad + j
+                    if input_res is None:
+                        src_img, src_gt = views(data, 1, h, w)
+                        img[s].copy_(src_img[0], non_blocking=True)
+                        gt[s].copy_(src_gt[0], non_blocking=True)
+                    else:
+                        h0, w0 = (int(v) for v in item["size"][1:])
+                        src_img, src_gt = views(data.to(self.device, non_blocking=True), 1, h0, w0)
+                        ops.resize_u8(src_img, (h, w), "bilinear", out=img[s:s + 1])
+                        ops.resize_u8(src_gt, (h, w), "nearest", out=gt[s:s + 1])
                 if group is not None:              # in place: this rank's share is already in its slots
                     share = slice(rank * pad, (rank + 1) * pad)
                     dist.all_gather_into_tensor(img, img[share], group=group)

@@ -25,16 +25,25 @@ class SequenceSegmenter:
     ``score=True``: ``frames`` yields ``(frame, gt_u8)`` pairs, ``gt_u8`` the host uint8 annotations [N,H,W] (pinned
     for real overlap).  The mask crosses on the input stream into a ring slot beside the frame, and ops.davis_measures
     scores the fused map on the compute stream right after the forward; the counts stay on the device until
-    ``frame_counts()``.  The results are the same bytes as without scoring."""
+    ``frame_counts()``.  The results are the same bytes as without scoring.
 
-    def __init__(self, net, output="logits", depth=3, frames="nchw_f32", meanval=ops.MEANVAL, score=False):
+    ``input_res`` (``frames="bgr8"`` only): the reference's ``inputRes`` (davis.imresize_size).  Each slot's bytes are
+    resized on the compute stream (ops.resize_u8, bilinear; the mask nearest) into a resized slot of fixed address
+    before the float conversion, so the network, the results and the scores are at that size, as the reference's test
+    loop writes them."""
+
+    def __init__(self, net, output="logits", depth=3, frames="nchw_f32", meanval=ops.MEANVAL, score=False,
+                 input_res=None):
         if output not in ("logits", "bytescale", "prob", "mask"):
             raise ValueError("output must be one of logits / bytescale / prob / mask")
         if frames not in ("nchw_f32", "bgr8"):
             raise ValueError("frames must be nchw_f32 or bgr8")
+        if input_res is not None and frames != "bgr8":
+            raise ValueError("input_res resizes the decoded bytes, as imresize does: it needs frames='bgr8'")
         self.net, self.output, self.depth = net, output, max(2, int(depth))
         self.frames, self.meanval = frames, tuple(meanval)
         self.score = bool(score)
+        self.input_res = input_res
         self._shape = None
         self._counts = []
 
@@ -44,17 +53,24 @@ class SequenceSegmenter:
             self._dev_raw = [torch.empty(shape, dtype=torch.uint8, device=device) for _ in range(self.depth)]
         else:
             n, _, h, w = shape
+        h0, w0 = h, w
+        if self.input_res is not None:
+            from .davis import imresize_size
+            h, w = imresize_size(self.input_res, h0, w0)
+            self._dev_rs = [torch.empty((n, h, w, 3), dtype=torch.uint8, device=device) for _ in range(self.depth)]
         out_dtype = torch.float32 if self.output == "logits" else torch.uint8
         self._dev_in = [torch.empty((n, 3, h, w), dtype=torch.float32, device=device) for _ in range(self.depth)]
         self._dev_out = [torch.empty((n, 1, h, w), dtype=out_dtype, device=device) for _ in range(self.depth)]
         self._host_out = [torch.empty((n, 1, h, w), dtype=out_dtype).pin_memory() for _ in range(self.depth)]
         if self.score:
-            self._dev_gt = [torch.empty((n, h, w), dtype=torch.uint8, device=device) for _ in range(self.depth)]
+            self._dev_gt = [torch.empty((n, h0, w0), dtype=torch.uint8, device=device) for _ in range(self.depth)]
+            if self.input_res is not None:
+                self._dev_gt_rs = [torch.empty((n, h, w), dtype=torch.uint8, device=device) for _ in range(self.depth)]
         self._s_in, self._s_out = torch.cuda.Stream(device), torch.cuda.Stream(device)
         mk = lambda: [torch.cuda.Event() for _ in range(self.depth)]
         self._ev_loaded, self._ev_consumed, self._ev_done, self._ev_host = mk(), mk(), mk(), mk()
         self._shape = tuple(shape)
-        self.h2d_bytes_per_frame = n * 3 * h * w * (1 if self.frames == "bgr8" else 4) + (n * h * w if self.score else 0)
+        self.h2d_bytes_per_frame = n * 3 * h0 * w0 * (1 if self.frames == "bgr8" else 4) + (n * h0 * w0 if self.score else 0)
         self.d2h_bytes_per_frame = n * h * w * (4 if self.output == "logits" else 1)
 
     def _submit(self, i, frame, gt, device):
@@ -71,9 +87,15 @@ class SequenceSegmenter:
         cur.wait_event(self._ev_loaded[k])
         if i >= self.depth:
             cur.wait_event(self._ev_host[k])                    # previous result of this slot is on the host
+        gt_dev = self._dev_gt[k] if self.score else None
         if bgr8:
+            raw = self._dev_raw[k]
+            if self.input_res is not None:
+                raw = ops.resize_u8(raw, self._dev_rs[k].shape[1:3], "bilinear", out=self._dev_rs[k])
+                if self.score:
+                    gt_dev = ops.resize_u8(gt_dev, self._dev_gt_rs[k].shape[1:3], "nearest", out=self._dev_gt_rs[k])
             # same slot address every time this slot comes round, so the engine's direct graph replay still applies
-            ops.image_from_bgr8(self._dev_raw[k], self.meanval, out=self._dev_in[k])
+            ops.image_from_bgr8(raw, self.meanval, out=self._dev_in[k])
         with torch.no_grad():
             eng = getattr(self.net, "_engine", None)
             if eng is not None:
@@ -84,7 +106,7 @@ class SequenceSegmenter:
             else:
                 fused = self.net(self._dev_in[k])[-1]
             if self.score:
-                self._counts.append(ops.davis_measures(fused, self._dev_gt[k]))
+                self._counts.append(ops.davis_measures(fused, gt_dev))
             self._ev_consumed[k].record(cur)                    # after the last read of this slot's frame and mask
             if self.output == "logits":
                 self._dev_out[k].copy_(fused)

@@ -655,6 +655,41 @@ def label_from_u8(masks, stats=None, out=None):
     return out
 
 
+_RESIZE_MODES = {"bilinear": nat.RESIZE_BILINEAR, "nearest": nat.RESIZE_NEAREST}
+
+
+def resize_u8(x, size, mode="bilinear", out=None):
+    """uint8 [N,H,W,C] (C = 3, e.g. BGR frames) or [N,H,W] (C = 1, masks) -> the same layout at ``size`` = (h', w'),
+    bit-identical to scipy 1.0's imresize of each frame (Pillow's Image.resize with ``mode`` 'bilinear' or 'nearest';
+    csrc/resize.cu, DESIGN.md §17).  Equal sizes are a copy.  No host synchronisation."""
+    lib = nat.load()
+    _require_cuda(x, "x")
+    if x.dtype != torch.uint8 or x.dim() not in (3, 4) or (x.dim() == 4 and int(x.shape[3]) not in (1, 3)):
+        raise ValueError(f"x must be uint8 [N,H,W,3], [N,H,W,1] or [N,H,W], got {x.dtype} {tuple(x.shape)}")
+    if mode not in _RESIZE_MODES:
+        raise ValueError("mode must be 'bilinear' or 'nearest'")
+    oh, ow = (int(v) for v in size)
+    x = x.contiguous()
+    n, h, w = (int(v) for v in x.shape[:3])
+    c = int(x.shape[3]) if x.dim() == 4 else 1
+    shape = (n, oh, ow) + tuple(x.shape[3:])
+    if out is None:
+        out = torch.empty(shape, dtype=torch.uint8, device=x.device)
+    elif out.dtype != torch.uint8 or tuple(out.shape) != shape or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous uint8 tensor of shape {shape}")
+    nbytes = lib.osvos_resize_u8_workspace_bytes(n, h, w, c, oh, ow, _RESIZE_MODES[mode])
+    if nbytes == 0 and (oh, ow) != (h, w):
+        raise ValueError(f"cannot resize [{n},{h},{w},{c}] to ({oh}, {ow}): sizes must lie in [1, 32767] and N < 65536")
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device) if nbytes else None
+    if (oh, ow) == (h, w):
+        _count()
+    else:
+        _count(2 if mode == "nearest" else 1 + int(h != oh) + int(w != ow))
+    nat.check(lib.osvos_resize_u8(x.data_ptr(), out.data_ptr(), nat.ptr(ws), n, h, w, c, oh, ow, _RESIZE_MODES[mode],
+                                  _stream()), "osvos_resize_u8")
+    return out
+
+
 def davis_measures(logits, gt_u8, r=None, out=None):
     """DAVIS-2016 J and F counts on the device (csrc/measures.cu, DESIGN.md §14): fused logits fp32 [N,1,H,W] or
     [N,H,W] and annotations uint8 [N,H,W] -> int32 [N,6] = {|P∧G|, |P∨G|, |B(P)|, |B(G)|, fg_match, gt_match} with

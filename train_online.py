@@ -53,10 +53,17 @@ def parse(argv=None):
                     help="score the segmentation against every frame's annotation on the device (DAVIS-2016 J and F, "
                          "osvos_pytorch_b200.evaluation); prints them and writes Results/<seq>_scores.json. "
                          "Needs --loader native")
+    ap.add_argument("--input-res", type=int, nargs=2, default=None, metavar=("H", "W"),
+                    help="the reference's inputRes: resize every frame (bilinear) and annotation (nearest) to H x W on "
+                         "the device before training, segmentation and scoring, as scipy 1.0's imresize does. Needs "
+                         "--loader native (--synthetic has --height / --width)")
     a = ap.parse_args(argv)
     if a.evaluate and (a.synthetic or a.loader != "native"):
         ap.error("--evaluate scores against the DAVIS annotations read by --loader native; it cannot be combined with "
                  + ("--synthetic" if a.synthetic else "--loader reference"))
+    if a.input_res is not None and (a.synthetic or a.loader != "native"):
+        ap.error("--input-res resizes the frames read by --loader native; it cannot be combined with "
+                 + ("--synthetic (use --height / --width)" if a.synthetic else "--loader reference"))
     return a
 
 
@@ -105,7 +112,8 @@ def main(argv=None):
         from torch.utils.data import DataLoader
         from osvos_pytorch_b200 import augment, davis
         first = davis.DAVIS2016Frames(train=True, db_root_dir=Path.db_root_dir(), seq_name=a.seq_name)
-        img_u8, gt_u8, stats = davis.upload(davis.collate([first[0]]), device)
+        input_res = None if a.input_res is None else tuple(a.input_res)
+        img_u8, gt_u8, stats = davis.upload(davis.collate([first[0]]), device, input_res=input_res)
         rng = random.Random(a.seed)
 
         def sample_fn(it):
@@ -177,7 +185,12 @@ def main(argv=None):
             names.append([os.path.basename(s["fname"][jj]) if "fname" in s else f"{ii:05d}_{jj}" for jj in range(n)])
             yield (s["image"], s["gt"]) if a.evaluate else s["image"]
     native = a.loader == "native" and not a.synthetic
-    seg = SequenceSegmenter(net, output="bytescale", frames="bgr8" if native else "nchw_f32", score=a.evaluate)
+    input_res = None if a.input_res is None else tuple(a.input_res)
+    if input_res is not None:
+        print(f"Frames resized to {input_res[0]}x{input_res[1]} (inputRes); results are written at that size"
+              + (", scored against the nearest-resized annotations" if a.evaluate else ""))
+    seg = SequenceSegmenter(net, output="bytescale", frames="bgr8" if native else "nchw_f32", score=a.evaluate,
+                            input_res=input_res)
     for pred in seg(frames()):
         arr = pred.numpy()
         for jj, name in enumerate(names.popleft()):

@@ -65,6 +65,10 @@ def parse(argv=None):
                     help="device: decode the train split once and keep its bytes on every GPU (about 3.4 GB per rank, "
                          "plus 2.3 GB of val frames on rank 0), then augment each batch from there instead of "
                          "decoding every frame in every epoch; needs --loader native")
+    ap.add_argument("--input-res", type=int, nargs=2, default=None, metavar=("H", "W"),
+                    help="the reference's inputRes: resize every frame (bilinear) and annotation (nearest) to H x W on "
+                         "the device, before augmentation and validation, as scipy 1.0's imresize does. Needs --loader "
+                         "native (--synthetic has --height / --width)")
     a = ap.parse_args(argv)
     if a.val_measures and (a.synthetic or a.loader != "native"):
         ap.error("--val-measures scores against the DAVIS annotations read by --loader native; it cannot be combined "
@@ -72,6 +76,9 @@ def parse(argv=None):
     if a.cache == "device" and (a.synthetic or a.loader != "native"):
         ap.error("--cache device keeps the frames decoded by --loader native on the device; it cannot be combined "
                  "with " + ("--synthetic" if a.synthetic else "--loader reference"))
+    if a.input_res is not None and (a.synthetic or a.loader != "native"):
+        ap.error("--input-res resizes the frames read by --loader native; it cannot be combined with "
+                 + ("--synthetic (use --height / --width)" if a.synthetic else "--loader reference"))
     return a
 
 
@@ -125,17 +132,21 @@ def main(argv=None):
         db_train = davis.DAVIS2016Frames(train=True, db_root_dir=Path.db_root_dir())
         sampler = DistributedSampler(db_train, world, rank, shuffle=True, drop_last=True) if world > 1 else None
         db_test = davis.DAVIS2016Frames(train=False, db_root_dir=Path.db_root_dir())
+        res = None if a.input_res is None else tuple(a.input_res)
+        if res is not None and rank == 0:
+            print(f"Frames resized to {res[0]}x{res[1]} (inputRes)"
+                  + ("; validation scored against the nearest-resized annotations" if a.val_measures else ""))
         if a.cache == "device":
             # The stores replace the decoding loaders.  Index loaders with the streaming loaders' batching and sampling
             # and no workers draw from the global RNG as 0-worker streaming loaders do (one base seed per pass, then
             # the sampler's own draw), so a seeded run sees the same batches and the same augmentation draws.
             train_store = davis.DeviceFrames(db_train, device, workers=a.workers,
-                                             group=dist.group.WORLD if world > 1 else None)
+                                             group=dist.group.WORLD if world > 1 else None, input_res=res)
             loader = DataLoader(range(len(db_train)), batch_size=a.batch, shuffle=sampler is None, sampler=sampler,
                                 num_workers=0, drop_last=world > 1)
             val_batches = None
             if rank == 0:                            # only rank 0 validates
-                val_store = davis.DeviceFrames(db_test, device, workers=a.workers)
+                val_store = davis.DeviceFrames(db_test, device, workers=a.workers, input_res=res)
                 val_batches = _Mapped(DataLoader(range(len(db_test)), batch_size=1, shuffle=False, num_workers=0),
                                       lambda b: val_store.ingest(int(b[0])))
                 for name, st in (("train", train_store), ("val", val_store)):
@@ -156,18 +167,18 @@ def main(argv=None):
             if a.val_measures:
                 def val_item(b):                     # davis.to_device without augmentation, keeping the mask bytes
                     with torch.cuda.device(device):
-                        img, gt, stats = davis.upload(b, device)
+                        img, gt, stats = davis.upload(b, device, input_res=res)
                         return {"image": ops.image_from_bgr8(img), "gt": ops.label_from_u8(gt, stats), "gt_u8": gt,
                                 "fname": b["fname"]}
                 val_batches = _Mapped(val_loader, val_item)
             else:
-                val_batches = _Mapped(val_loader, lambda b: davis.to_device(b, device))
+                val_batches = _Mapped(val_loader, lambda b: davis.to_device(b, device, input_res=res))
 
             def epoch_batches(epoch):
                 if sampler is not None:
                     sampler.set_epoch(epoch)
                 for b in loader:      # flip / rotation / scale drawn from Python's random, as the reference's transforms do
-                    yield davis.to_device(b, device, augment=random)
+                    yield davis.to_device(b, device, augment=random, input_res=res)
     else:
         from dataloaders import davis_2016 as db
         from dataloaders import custom_transforms as tr
