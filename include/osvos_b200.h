@@ -537,6 +537,23 @@ OSVOS_API size_t osvos_resize_u8_workspace_bytes(int n, int h, int w, int c, int
 OSVOS_API int osvos_resize_u8(const uint8_t* src, uint8_t* dst, void* workspace, int n, int h, int w, int c, int out_h,
                               int out_w, int mode, osvos_stream_t stream);
 
+/* ---- resize of fp32 maps (fused logits back to the annotations' stored size: scipy 1.0's imresize(..., mode='F'),
+ * i.e. Pillow's 'F' Image.resize; DESIGN.md §18) ----------------------------------------------------------------------
+ *   osvos_resize_f32: src [n][h][w] fp32 -> dst [n][out_h][out_w] fp32, bit-identical to Pillow's
+ *                     Image.resize((out_w, out_h), BILINEAR) of an 'F' image: the bilinear coefficient tables of
+ *                     osvos_resize_u8 kept in double (not rounded to fixed point), horizontal pass first into an fp32
+ *                     intermediate that holds only the source rows the vertical pass reads, each output a double sum
+ *                     of (double)src * k rounded once to fp32; an axis that keeps its size has no pass and equal sizes
+ *                     are a copy.  n < 65536, h, w, out_h, out_w < 32768; src and dst 4-byte aligned, not
+ *                     overlapping.  `workspace`: osvos_resize_f32_workspace_bytes(...) bytes (per axis {xmin, count}
+ *                     and the double weights and, when both axes change size, the fp32 intermediate), 8-byte aligned,
+ *                     owned by the caller (may be NULL when that is 0); nothing is allocated and nothing waits for
+ *                     the host.
+ *   osvos_resize_f32_workspace_bytes: host query; 0 for invalid arguments.                                          */
+OSVOS_API size_t osvos_resize_f32_workspace_bytes(int n, int h, int w, int out_h, int out_w);
+OSVOS_API int osvos_resize_f32(const float* src, float* dst, void* workspace, int n, int h, int w, int out_h, int out_w,
+                               osvos_stream_t stream);
+
 /* ---- DAVIS-2016 region and boundary measures (J and F; DESIGN.md §14) -------------------------------------------
  * Per frame, P = logit > 0 (±0.0 is background, as osvos_logits_to_u8 mode MASK) and G = byte != 0.  The boundary map
  * of a mask is b = seg^E | seg^S | seg^SE (E, S, SE: the right, lower and lower-right neighbour, zeros past the frame),

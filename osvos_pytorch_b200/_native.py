@@ -156,6 +156,8 @@ SIGNATURES = {
                                              c_float, c_float, c_void_p]),
     "osvos_resize_u8_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
     "osvos_resize_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "osvos_resize_f32_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
+    "osvos_resize_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "osvos_davis_measures_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "osvos_davis_measures": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "osvos_reduce_rows_scratch_floats": (c_size_t, [c_int, c_int]),

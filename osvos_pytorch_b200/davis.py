@@ -237,9 +237,14 @@ class DeviceFrames:
     ``input_res``: the reference's ``inputRes`` (imresize_size).  Each frame is resized on the device as it is stored
     (resize_pair), so the store, its size groups and the memory check are at the resized size; frames of different
     stored sizes that resize to one size share a group.  With a process group each rank resizes its own share before
-    the gather."""
+    the gather.
 
-    def __init__(self, dataset, device, workers=0, group=None, input_res=None):
+    ``keep_stored_gt`` (with ``input_res``): the store also keeps every annotation's bytes at its stored size, in
+    groups by stored size (``stored_groups``, each {'size', 'gt'}; ``where_stored[i]`` is index i's (group, slot)), so
+    that segmentations upsampled back to that size (ops.resize_f32) are scored against the original annotations.  The
+    memory check counts them, and ingest returns them as 'gt_u8_stored'."""
+
+    def __init__(self, dataset, device, workers=0, group=None, input_res=None, keep_stored_gt=False):
         import torch.distributed as dist
         from torch.utils.data import DataLoader, Subset
         t0 = time.perf_counter()
@@ -262,13 +267,23 @@ class DeviceFrames:
         self.has_gt = [m[2] for m in meta]
         self.fname = [m[3] for m in meta]
         plan = shard_plan(sizes, world)
+        keep_stored = keep_stored_gt and input_res is not None
+        plan0 = shard_plan([m[1] for m in meta], world) if keep_stored else []
         need = sum(world * pad * (h * w * 4 + 8) for (h, w), pad, _ in plan)
+        need += sum(world * pad * h * w for (h, w), pad, _ in plan0)
         free, _ = torch.cuda.mem_get_info(self.device)
         if need > free:
             raise ValueError(f"DeviceFrames: the {n} decoded frames need {need} bytes on {self.device} but only {free} "
                              "are free")
         self.groups, self.where = [], [None] * n
+        self.stored_groups, self.where_stored = [], [None] * n
         with torch.cuda.device(self.device):
+            for g, ((h, w), pad, members) in enumerate(plan0):
+                self.stored_groups.append({"size": (h, w), "gt": torch.zeros((world * pad, h, w), dtype=torch.uint8,
+                                                                               device=self.device)})
+                for r, m in enumerate(members):
+                    for j, i in enumerate(m):
+                        self.where_stored[i] = (g, r * pad + j)
             for g, ((h, w), pad, members) in enumerate(plan):
                 img = torch.zeros((world * pad, h, w, 3), dtype=torch.uint8, device=self.device)
                 gt = torch.zeros((world * pad, h, w), dtype=torch.uint8, device=self.device)
@@ -285,6 +300,9 @@ class DeviceFrames:
                         src_img, src_gt = views(data.to(self.device, non_blocking=True), 1, h0, w0)
                         ops.resize_u8(src_img, (h, w), "bilinear", out=img[s:s + 1])
                         ops.resize_u8(src_gt, (h, w), "nearest", out=gt[s:s + 1])
+                        if keep_stored:
+                            g0, s0 = self.where_stored[i]
+                            self.stored_groups[g0]["gt"][s0].copy_(src_gt[0])
                 if group is not None:              # in place: this rank's share is already in its slots
                     share = slice(rank * pad, (rank + 1) * pad)
                     dist.all_gather_into_tensor(img, img[share], group=group)
@@ -296,8 +314,12 @@ class DeviceFrames:
                 for r, m in enumerate(members):
                     for j, i in enumerate(m):
                         self.where[i] = (g, r * pad + j)
+            if group is not None:
+                for (_, pad, _), grp in zip(plan0, self.stored_groups):
+                    dist.all_gather_into_tensor(grp["gt"], grp["gt"][rank * pad:(rank + 1) * pad], group=group)
         torch.cuda.synchronize(self.device)
         self.nbytes = sum(t.numel() * t.element_size() for grp in self.groups for t in (grp["img"], grp["gt"], grp["stats"]))
+        self.nbytes += sum(grp["gt"].numel() for grp in self.stored_groups)
         self.build_s = time.perf_counter() - t0
 
     def __len__(self):
@@ -330,11 +352,16 @@ class DeviceFrames:
 
     def ingest(self, i):
         """Frame i without augmentation -> {'image': f32 [1,3,H,W], 'gt': f32 [1,1,H,W], 'gt_u8': uint8 [1,H,W] (a view
-        of the store), 'fname': [name]}; image and gt are bit-identical to to_device(collate([item]), device)."""
+        of the store), 'fname': [name]}; image and gt are bit-identical to to_device(collate([item]), device).  A store
+        built with keep_stored_gt adds 'gt_u8_stored': uint8 [1,H0,W0], the annotation at its stored size (a view)."""
         i = int(i)
         g, s = self._slot(i)
         grp = self.groups[g]
         gt = grp["gt"][s:s + 1]
         with torch.cuda.device(self.device):
-            return {"image": ops.image_from_bgr8(grp["img"][s:s + 1]), "gt": ops.label_from_u8(gt, grp["stats"][s:s + 1]),
+            item = {"image": ops.image_from_bgr8(grp["img"][s:s + 1]), "gt": ops.label_from_u8(gt, grp["stats"][s:s + 1]),
                     "gt_u8": gt, "fname": [self.fname[i]]}
+        if self.stored_groups:
+            g0, s0 = self.where_stored[i]
+            item["gt_u8_stored"] = self.stored_groups[g0]["gt"][s0:s0 + 1]
+        return item

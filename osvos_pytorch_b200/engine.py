@@ -6,6 +6,8 @@ stream handling; all arithmetic is in csrc/.
 Call graph replaced: reference networks/vgg_osvos.py:59-74 (forward) and, in
 training, the autograd graph PyTorch builds for it.
 """
+import contextlib
+import gc
 import os
 
 import torch
@@ -13,6 +15,22 @@ import torch.nn as nn
 
 from . import ops
 from .layers.osvos_layers import bilinear_deconv_weight
+
+
+@contextlib.contextmanager
+def no_collection_during_capture():
+    """Wrap a CUDA graph capture: collect the garbage first, then keep the cyclic collector off until it ends.  A dead
+    reference cycle that still holds a captured graph (an unreferenced network and its engine) would otherwise be
+    collected at a random moment, possibly inside the capture, and destroying a graph is not permitted while a stream
+    captures: it invalidates the capture.  torch.cuda.graph no longer collects before capturing."""
+    gc.collect()
+    enabled = gc.isenabled()
+    gc.disable()
+    try:
+        yield
+    finally:
+        if enabled:
+            gc.enable()
 
 
 class OSVOSEngine:
@@ -237,7 +255,7 @@ class OSVOSEngine:
         static_x = None if direct else x.detach().contiguous().float().clone()
         torch.cuda.synchronize(x.device)
         graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
+        with no_collection_during_capture(), torch.cuda.graph(graph):
             outs = self.forward_inference(x if direct else static_x)
         base = outs[0]._base if outs[0]._base is not None else None
         entry = (graph, static_x, outs, base)

@@ -30,20 +30,30 @@ class SequenceSegmenter:
     ``input_res`` (``frames="bgr8"`` only): the reference's ``inputRes`` (davis.imresize_size).  Each slot's bytes are
     resized on the compute stream (ops.resize_u8, bilinear; the mask nearest) into a resized slot of fixed address
     before the float conversion, so the network, the results and the scores are at that size, as the reference's test
-    loop writes them."""
+    loop writes them.
+
+    ``output_res="stored"`` (with ``input_res``): each fused map is resized back to the frames' stored size on the
+    compute stream (ops.resize_f32, scipy 1.0's imresize(mode='F'); DESIGN.md §18) into a per-slot buffer of fixed
+    address, so the results are [N,1,H0,W0] and the scores are taken against the original annotations, as the
+    DAVIS-2016 benchmark scores 480x854 masks.  ``"network"`` (the default) keeps them at the network resolution.
+    Without ``input_res`` both are the stored size and nothing is resized."""
 
     def __init__(self, net, output="logits", depth=3, frames="nchw_f32", meanval=ops.MEANVAL, score=False,
-                 input_res=None):
+                 input_res=None, output_res="network"):
         if output not in ("logits", "bytescale", "prob", "mask"):
             raise ValueError("output must be one of logits / bytescale / prob / mask")
         if frames not in ("nchw_f32", "bgr8"):
             raise ValueError("frames must be nchw_f32 or bgr8")
         if input_res is not None and frames != "bgr8":
             raise ValueError("input_res resizes the decoded bytes, as imresize does: it needs frames='bgr8'")
+        if output_res not in ("network", "stored"):
+            raise ValueError("output_res must be 'network' or 'stored'")
         self.net, self.output, self.depth = net, output, max(2, int(depth))
         self.frames, self.meanval = frames, tuple(meanval)
         self.score = bool(score)
         self.input_res = input_res
+        self.output_res = output_res
+        self._upsample = input_res is not None and output_res == "stored"
         self._shape = None
         self._counts = []
 
@@ -59,19 +69,22 @@ class SequenceSegmenter:
             h, w = imresize_size(self.input_res, h0, w0)
             self._dev_rs = [torch.empty((n, h, w, 3), dtype=torch.uint8, device=device) for _ in range(self.depth)]
         out_dtype = torch.float32 if self.output == "logits" else torch.uint8
+        rh, rw = (h0, w0) if self._upsample else (h, w)                  # the results' size
         self._dev_in = [torch.empty((n, 3, h, w), dtype=torch.float32, device=device) for _ in range(self.depth)]
-        self._dev_out = [torch.empty((n, 1, h, w), dtype=out_dtype, device=device) for _ in range(self.depth)]
-        self._host_out = [torch.empty((n, 1, h, w), dtype=out_dtype).pin_memory() for _ in range(self.depth)]
+        self._dev_out = [torch.empty((n, 1, rh, rw), dtype=out_dtype, device=device) for _ in range(self.depth)]
+        self._host_out = [torch.empty((n, 1, rh, rw), dtype=out_dtype).pin_memory() for _ in range(self.depth)]
+        if self._upsample:
+            self._dev_up = [torch.empty((n, 1, h0, w0), dtype=torch.float32, device=device) for _ in range(self.depth)]
         if self.score:
             self._dev_gt = [torch.empty((n, h0, w0), dtype=torch.uint8, device=device) for _ in range(self.depth)]
-            if self.input_res is not None:
+            if self.input_res is not None and not self._upsample:
                 self._dev_gt_rs = [torch.empty((n, h, w), dtype=torch.uint8, device=device) for _ in range(self.depth)]
         self._s_in, self._s_out = torch.cuda.Stream(device), torch.cuda.Stream(device)
         mk = lambda: [torch.cuda.Event() for _ in range(self.depth)]
         self._ev_loaded, self._ev_consumed, self._ev_done, self._ev_host = mk(), mk(), mk(), mk()
         self._shape = tuple(shape)
         self.h2d_bytes_per_frame = n * 3 * h0 * w0 * (1 if self.frames == "bgr8" else 4) + (n * h0 * w0 if self.score else 0)
-        self.d2h_bytes_per_frame = n * h * w * (4 if self.output == "logits" else 1)
+        self.d2h_bytes_per_frame = n * rh * rw * (4 if self.output == "logits" else 1)
 
     def _submit(self, i, frame, gt, device):
         k = i % self.depth
@@ -92,7 +105,7 @@ class SequenceSegmenter:
             raw = self._dev_raw[k]
             if self.input_res is not None:
                 raw = ops.resize_u8(raw, self._dev_rs[k].shape[1:3], "bilinear", out=self._dev_rs[k])
-                if self.score:
+                if self.score and not self._upsample:
                     gt_dev = ops.resize_u8(gt_dev, self._dev_gt_rs[k].shape[1:3], "nearest", out=self._dev_gt_rs[k])
             # same slot address every time this slot comes round, so the engine's direct graph replay still applies
             ops.image_from_bgr8(raw, self.meanval, out=self._dev_in[k])
@@ -105,6 +118,8 @@ class SequenceSegmenter:
                 fused = eng.forward(self._dev_in[k], fresh_outputs=False)[-1]
             else:
                 fused = self.net(self._dev_in[k])[-1]
+            if self._upsample:                                  # back to the stored size, before anything reads it
+                fused = ops.resize_f32(fused, self._dev_up[k].shape[2:4], out=self._dev_up[k])
             if self.score:
                 self._counts.append(ops.davis_measures(fused, gt_dev))
             self._ev_consumed[k].record(cur)                    # after the last read of this slot's frame and mask

@@ -690,6 +690,32 @@ def resize_u8(x, size, mode="bilinear", out=None):
     return out
 
 
+def resize_f32(x, size, out=None):
+    """fp32 maps [N,H,W] or [N,1,H,W] (e.g. fused logits) -> the same layout at ``size`` = (h', w'), bit-identical to
+    scipy 1.0's imresize(map, size, interp='bilinear', mode='F') of each map (Pillow's BILINEAR resize of an 'F' image;
+    csrc/resize.cu, DESIGN.md §18).  Equal sizes are a copy.  No host synchronisation."""
+    lib = nat.load()
+    _require_cuda(x, "x")
+    if x.dtype != torch.float32 or x.dim() not in (3, 4) or (x.dim() == 4 and int(x.shape[1]) != 1):
+        raise ValueError(f"x must be fp32 [N,H,W] or [N,1,H,W], got {x.dtype} {tuple(x.shape)}")
+    oh, ow = (int(v) for v in size)
+    x = x.detach().contiguous()
+    n, h, w = int(x.shape[0]), int(x.shape[-2]), int(x.shape[-1])
+    if not (0 < n < 65536 and all(0 < v < 32768 for v in (h, w, oh, ow))):
+        raise ValueError(f"cannot resize [{n},{h},{w}] to ({oh}, {ow}): sizes must lie in [1, 32767] and N < 65536")
+    shape = tuple(x.shape[:-2]) + (oh, ow)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=x.device)
+    elif out.dtype != torch.float32 or tuple(out.shape) != shape or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous fp32 tensor of shape {shape}")
+    nbytes = lib.osvos_resize_f32_workspace_bytes(n, h, w, oh, ow)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device) if nbytes else None
+    _count(1 if (oh, ow) == (h, w) else 1 + int(h != oh) + int(w != ow))
+    nat.check(lib.osvos_resize_f32(x.data_ptr(), out.data_ptr(), nat.ptr(ws), n, h, w, oh, ow, _stream()),
+              "osvos_resize_f32")
+    return out
+
+
 def davis_measures(logits, gt_u8, r=None, out=None):
     """DAVIS-2016 J and F counts on the device (csrc/measures.cu, DESIGN.md §14): fused logits fp32 [N,1,H,W] or
     [N,H,W] and annotations uint8 [N,H,W] -> int32 [N,6] = {|P∧G|, |P∨G|, |B(P)|, |B(G)|, fg_match, gt_match} with

@@ -4,6 +4,7 @@ the online fine-tune loop (train_online.py:112-149 of the reference) and the par
 data-parallel exchange step (train_parent.py:129-176 + parallel.py)."""
 import torch
 
+from .engine import no_collection_during_capture
 from .layers.osvos_layers import class_balanced_cross_entropy_loss
 from .ops import MEANVAL  # noqa: F401  (dataloaders/davis_2016.py:19 of the reference)
 ONLINE_WEIGHTS = (0.0, 0.0, 0.0, 0.0, 1.0)       # train_online.py:127: only the fused map is supervised
@@ -91,7 +92,7 @@ class GraphedTrainStep:
         torch.cuda.synchronize()
         self.graph = torch.cuda.CUDAGraph()
         try:
-            with torch.cuda.graph(self.graph):
+            with no_collection_during_capture(), torch.cuda.graph(self.graph):
                 self.loss = self._body()
         finally:
             # graph-private buffers must not serve eager calls (also after a failed capture: the cached packed layouts

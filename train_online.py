@@ -57,6 +57,11 @@ def parse(argv=None):
                     help="the reference's inputRes: resize every frame (bilinear) and annotation (nearest) to H x W on "
                          "the device before training, segmentation and scoring, as scipy 1.0's imresize does. Needs "
                          "--loader native (--synthetic has --height / --width)")
+    ap.add_argument("--output-res", default="network", choices=["network", "stored"],
+                    help="with --input-res: write (and with --evaluate score) the masks at the network resolution H x W "
+                         "(network), or at each frame's stored size (stored): the fused logits are upsampled on the "
+                         "device as scipy 1.0's imresize(mode='F') does and scored against the original annotations, "
+                         "so the PNGs and J / F compare with the DAVIS-2016 benchmark's")
     a = ap.parse_args(argv)
     if a.evaluate and (a.synthetic or a.loader != "native"):
         ap.error("--evaluate scores against the DAVIS annotations read by --loader native; it cannot be combined with "
@@ -178,19 +183,27 @@ def main(argv=None):
     import collections
     from osvos_pytorch_b200.inference import SequenceSegmenter
     names = collections.deque()
+    native = a.loader == "native" and not a.synthetic
+    input_res = None if a.input_res is None else tuple(a.input_res)
+    upsample = input_res is not None and a.output_res == "stored"
+    stored_hw = []                                      # the sequence's stored size (one size per sequence)
 
     def frames():
         for ii, s in enumerate(test_frames):
             n = int(s["image"].shape[0])
             names.append([os.path.basename(s["fname"][jj]) if "fname" in s else f"{ii:05d}_{jj}" for jj in range(n)])
+            if upsample and not stored_hw:
+                stored_hw.extend(int(v) for v in s["image"].shape[1:3])        # bgr8 [N,H,W,3]
             yield (s["image"], s["gt"]) if a.evaluate else s["image"]
-    native = a.loader == "native" and not a.synthetic
-    input_res = None if a.input_res is None else tuple(a.input_res)
-    if input_res is not None:
+    if upsample:
+        print(f"Frames resized to {input_res[0]}x{input_res[1]} (inputRes); the fused logits are upsampled to the "
+              "stored size, results are written at that size"
+              + (", scored against the original annotations" if a.evaluate else ""))
+    elif input_res is not None:
         print(f"Frames resized to {input_res[0]}x{input_res[1]} (inputRes); results are written at that size"
               + (", scored against the nearest-resized annotations" if a.evaluate else ""))
     seg = SequenceSegmenter(net, output="bytescale", frames="bgr8" if native else "nchw_f32", score=a.evaluate,
-                            input_res=input_res)
+                            input_res=input_res, output_res=a.output_res)
     for pred in seg(frames()):
         arr = pred.numpy()
         for jj, name in enumerate(names.popleft()):
@@ -208,6 +221,8 @@ def main(argv=None):
         st = res["statistics"]
         print("Scores of " + a.seq_name + " (frames 1 .. n-2): "
               + "  ".join(f"{m} M/O/D: {st[m]['M']:.4f} / {st[m]['O']:.4f} / {st[m]['D']:.4f}" for m in ("J", "F")))
+        if upsample:
+            res = dict(network_res=list(input_res), scored_res=stored_hw, **res)
         with open(os.path.join(save_dir, "Results", a.seq_name + "_scores.json"), "w") as f:
             json.dump(dict(sequence=a.seq_name, **res), f, indent=1)
     return history

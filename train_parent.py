@@ -69,6 +69,11 @@ def parse(argv=None):
                     help="the reference's inputRes: resize every frame (bilinear) and annotation (nearest) to H x W on "
                          "the device, before augmentation and validation, as scipy 1.0's imresize does. Needs --loader "
                          "native (--synthetic has --height / --width)")
+    ap.add_argument("--output-res", default="network", choices=["network", "stored"],
+                    help="with --input-res and --val-measures: score J and F at the network resolution against the "
+                         "nearest-resized annotations (network), or upsample the fused logits to each frame's stored "
+                         "size on the device, as scipy 1.0's imresize(mode='F') does, and score them against the "
+                         "original annotations (stored). The validation loss stays at the network resolution")
     a = ap.parse_args(argv)
     if a.val_measures and (a.synthetic or a.loader != "native"):
         ap.error("--val-measures scores against the DAVIS annotations read by --loader native; it cannot be combined "
@@ -114,6 +119,7 @@ def main(argv=None):
     opt = training.make_optimizer(net, "parent", a.lr, a.wd, fused=True)
     bucket = parallel.GradientBucket(parallel.trainable_parameters(net), device)
 
+    stored = False                                   # J and F at the stored size (--input-res --output-res stored)
     if a.synthetic:
         def epoch_batches(epoch):
             # the same number of micro-batches on every rank (a multiple of n_ave): every rank joins every allreduce
@@ -133,9 +139,12 @@ def main(argv=None):
         sampler = DistributedSampler(db_train, world, rank, shuffle=True, drop_last=True) if world > 1 else None
         db_test = davis.DAVIS2016Frames(train=False, db_root_dir=Path.db_root_dir())
         res = None if a.input_res is None else tuple(a.input_res)
+        stored = res is not None and a.val_measures and a.output_res == "stored"
         if res is not None and rank == 0:
             print(f"Frames resized to {res[0]}x{res[1]} (inputRes)"
-                  + ("; validation scored against the nearest-resized annotations" if a.val_measures else ""))
+                  + ("; validation J and F scored at the stored size (fused logits upsampled) against the original "
+                     "annotations" if stored else
+                     "; validation scored against the nearest-resized annotations" if a.val_measures else ""))
         if a.cache == "device":
             # The stores replace the decoding loaders.  Index loaders with the streaming loaders' batching and sampling
             # and no workers draw from the global RNG as 0-worker streaming loaders do (one base seed per pass, then
@@ -146,7 +155,7 @@ def main(argv=None):
                                 num_workers=0, drop_last=world > 1)
             val_batches = None
             if rank == 0:                            # only rank 0 validates
-                val_store = davis.DeviceFrames(db_test, device, workers=a.workers, input_res=res)
+                val_store = davis.DeviceFrames(db_test, device, workers=a.workers, input_res=res, keep_stored_gt=stored)
                 val_batches = _Mapped(DataLoader(range(len(db_test)), batch_size=1, shuffle=False, num_workers=0),
                                       lambda b: val_store.ingest(int(b[0])))
                 for name, st in (("train", train_store), ("val", val_store)):
@@ -167,9 +176,17 @@ def main(argv=None):
             if a.val_measures:
                 def val_item(b):                     # davis.to_device without augmentation, keeping the mask bytes
                     with torch.cuda.device(device):
-                        img, gt, stats = davis.upload(b, device, input_res=res)
+                        if not stored:
+                            img, gt, stats = davis.upload(b, device, input_res=res)
+                            return {"image": ops.image_from_bgr8(img), "gt": ops.label_from_u8(gt, stats), "gt_u8": gt,
+                                    "fname": b["fname"]}
+                        # davis.upload, keeping the collated mask's view at the stored size
+                        n, h, w = (int(v) for v in b["size"])
+                        img0, gt0 = davis.views(davis.pinned(b["data"]).to(device, non_blocking=True), n, h, w)
+                        img, gt = davis.resize_pair(img0, gt0, res)
+                        stats = ops.label_stats_u8(gt)
                         return {"image": ops.image_from_bgr8(img), "gt": ops.label_from_u8(gt, stats), "gt_u8": gt,
-                                "fname": b["fname"]}
+                                "gt_u8_stored": gt0, "fname": b["fname"]}
                 val_batches = _Mapped(val_loader, val_item)
             else:
                 val_batches = _Mapped(val_loader, lambda b: davis.to_device(b, device, input_res=res))
@@ -223,7 +240,11 @@ def main(argv=None):
                     tot += torch.stack([training.class_balanced_cross_entropy_loss(o, s["gt"].to(device),
                                                                                    size_average=False) for o in outs])
                     if a.val_measures:
-                        counts = ops.davis_measures(outs[-1], s["gt_u8"])
+                        if stored:                   # the fused map at the annotation's own size (DESIGN.md §18)
+                            g0 = s["gt_u8_stored"]
+                            counts = ops.davis_measures(ops.resize_f32(outs[-1], g0.shape[1:]), g0)
+                        else:
+                            counts = ops.davis_measures(outs[-1], s["gt_u8"])
                         for i, fname in enumerate(s["fname"]):
                             per_seq.setdefault(fname.split("/")[0], evaluation.SequenceScores()).add(counts[i:i + 1])
             print("***Testing *** " + " ".join(f"Loss {k}: {v:.4f}" for k, v in enumerate((tot / len(val_batches)).tolist())))
