@@ -572,6 +572,36 @@ OSVOS_API size_t osvos_davis_measures_workspace_bytes(int n, int h, int w);
 OSVOS_API int osvos_davis_measures(const float* logits, const uint8_t* masks, int* counts, void* workspace, int n, int h,
                                    int w, int r, osvos_stream_t stream);
 
+/* ---- baseline JPEG decode, bit-identical to cv2.imread (libjpeg-turbo; DESIGN.md §19) ----------------------------
+ *   osvos_jpeg_decode: a batch of n JPEGs of one size h x w, packed by osvos_pytorch_b200.jpeg.pack into `blob`
+ *                      (blob_bytes bytes, 16-byte aligned; headers, tables and de-stuffed entropy-coded segments) ->
+ *                      out [n][h][w][3] uint8 BGR (any alignment) and status [n] int32.  Tables, sampling and quality
+ *                      may differ per image.  Huffman decoding is a self-synchronising parallel decode over chunks of
+ *                      chunk_bits bits (0: the default, OSVOS_JPEG_DEFAULT_CHUNK_BITS; otherwise >= 32), then the
+ *                      DC prefix sums, ISLOW IDCT, fancy upsampling and fixed-point YCbCr -> BGR of libjpeg-turbo.
+ *                      status bits: 1 a bad Huffman code, 2 a zig-zag index past 63, 4 entropy data that ended
+ *                      before the last MCU (bits past a segment's end read as zero, as libjpeg-turbo does), 8 a
+ *                      header inconsistent with the arguments (that image is not decoded).  Output for a stream with
+ *                      bad codes is not specified, but the call reads nothing outside the blob and writes nothing
+ *                      outside out, status and the workspace.  `nseg` is the blob's segment count.  `workspace`:
+ *                      osvos_jpeg_decode_workspace_bytes(...) bytes, 16-byte aligned, owned by the caller; nothing
+ *                      is allocated and nothing waits for the host.  n < 65536, h, w < 32768.
+ *   osvos_jpeg_decode_workspace_bytes: host query; 0 for invalid arguments.                                          */
+#define OSVOS_JPEG_DEFAULT_CHUNK_BITS 512
+typedef struct osvos_jpeg_args {
+  const void* blob;
+  size_t blob_bytes;
+  uint8_t* out;
+  int32_t* status;
+  void* workspace;
+  int n, h, w;
+  int nseg;
+  int chunk_bits;
+  int reserved;
+} osvos_jpeg_args;
+OSVOS_API size_t osvos_jpeg_decode_workspace_bytes(int n, int h, int w, int nseg, size_t blob_bytes, int chunk_bits);
+OSVOS_API int osvos_jpeg_decode(const osvos_jpeg_args* args, osvos_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

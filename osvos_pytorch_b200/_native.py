@@ -97,6 +97,13 @@ class SgdSegment(Structure):
                 ("work_items", c_uint32), ("packed_fwd", c_void_p), ("packed_flip", c_void_p)]
 
 
+class JpegArgs(Structure):
+    """osvos_jpeg_args (include/osvos_b200.h)."""
+    _fields_ = [("blob", c_void_p), ("blob_bytes", c_size_t), ("out", c_void_p), ("status", c_void_p),
+                ("workspace", c_void_p), ("n", c_int), ("h", c_int), ("w", c_int), ("nseg", c_int),
+                ("chunk_bits", c_int), ("reserved", c_int)]
+
+
 U8_PROB, U8_BYTESCALE, U8_MASK = 0, 1, 2
 RESIZE_BILINEAR, RESIZE_NEAREST = 0, 1
 SGD_MAX_SEGMENTS = 64
@@ -179,6 +186,8 @@ SIGNATURES = {
     "osvos_cbce_fwd_deterministic": (c_int, [c_void_p, c_void_p, c_size_t, c_double, c_void_p, c_void_p, c_void_p]),
     "osvos_sum_f32_deterministic_scratch_bytes": (c_size_t, []),
     "osvos_sum_f32_deterministic": (c_int, [c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
+    "osvos_jpeg_decode_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_size_t, c_int]),
+    "osvos_jpeg_decode": (c_int, [POINTER(JpegArgs), c_void_p]),
 }
 
 DAVIS_MAX_RADIUS = 31

@@ -28,6 +28,7 @@ import torch
 from torch.utils.data import Dataset
 
 from . import augment as _augment
+from . import jpeg as _jpeg
 from . import ops
 from .ops import MEANVAL
 
@@ -55,10 +56,18 @@ class DAVIS2016Frames(Dataset):
     ``seq/<file stem>``.
 
     ``all_annotations=True`` (sequence mode): every frame carries its own annotation, as scoring the sequence needs; a
-    sequence whose frame and annotation counts differ raises."""
+    sequence whose frame and annotation counts differ raises.
+
+    ``decode="device"``: the worker reads the frame's file and parses its markers (jpeg.parse) instead of decoding it;
+    the item carries ``jpeg`` (the parsed file) in place of ``image``, and ``collate`` / ``upload`` decode it on the
+    device bit-identically to cv2.imread (ops.decode_jpeg, DESIGN.md §19).  A file outside the decoder's subset is
+    decoded by cv2.imread as with ``decode="host"`` and carries ``image``.  Masks are decoded on the host either way."""
 
     def __init__(self, train=True, db_root_dir=None, seq_name=None, meanval=MEANVAL, inputRes=None,
-                 all_annotations=False):
+                 all_annotations=False, decode="host"):
+        if decode not in ("host", "device"):
+            raise ValueError("decode must be 'host' or 'device'")
+        self.decode = decode
         if inputRes is not None:
             raise NotImplementedError("inputRes: the reference resizes with scipy.misc.imresize, which SciPy no longer "
                                       "has, and neither entry point uses it; frames are read at their stored size")
@@ -103,22 +112,39 @@ class DAVIS2016Frames(Dataset):
         return arr
 
     def __getitem__(self, idx):
-        image = self._read(self.img_list[idx], 1)                      # cv2.IMREAD_COLOR: uint8 [H,W,3] BGR
+        item = {}
+        parsed = None
+        if self.decode == "device":
+            with open(os.path.join(self.db_root_dir, self.img_list[idx]), "rb") as f:
+                parsed = _jpeg.parse(f.read())
+        if isinstance(parsed, _jpeg.Parsed):
+            item["jpeg"] = parsed
+            size = (parsed.h, parsed.w)
+        else:
+            item["image"] = self._read(self.img_list[idx], 1)          # cv2.IMREAD_COLOR: uint8 [H,W,3] BGR
+            size = item["image"].shape[:2]
         has_gt = self.labels[idx] is not None
-        gt = self._read(self.labels[idx], 0) if has_gt else np.zeros(image.shape[:2], dtype=np.uint8)
+        gt = self._read(self.labels[idx], 0) if has_gt else np.zeros(size, dtype=np.uint8)
         if self.seq_name is not None:
             fname = os.path.join(self.seq_name, "%05d" % idx)
         else:
             parts = self.img_list[idx].split("/")
             fname = os.path.join(parts[-2], os.path.splitext(parts[-1])[0])
-        return {"image": image, "gt": gt, "has_gt": has_gt, "fname": fname}
+        item.update(gt=gt, has_gt=has_gt, fname=fname)
+        return item
 
 
 def collate(items):
     """Items of one shape -> {'data': uint8 [N*H*W*4] (the N BGR frames, then the N masks), 'size': (N, H, W),
-    'has_gt': bool [N], 'fname': [N]}.  One buffer, so pinning and the host-to-device copy are one transfer each."""
+    'has_gt': bool [N], 'fname': [N]}.  One buffer, so pinning and the host-to-device copy are one transfer each.
+
+    When any item carries ``jpeg`` (DAVIS2016Frames(decode="device")), 'data' holds instead the N masks, then the
+    frames of the items that carry ``image``, then the packed JPEGs (jpeg.pack, 16-byte aligned), and 'jpeg' says
+    which items are which (``upload`` assembles the frames on the device)."""
     h, w = items[0]["gt"].shape
     n = len(items)
+    if any("jpeg" in it for it in items):
+        return _collate_jpeg(items, n, h, w)
     data = torch.empty(n * h * w * 4, dtype=torch.uint8)
     img, gt = views(data, n, h, w)
     for i, it in enumerate(items):
@@ -128,6 +154,67 @@ def collate(items):
         gt[i] = torch.from_numpy(it["gt"])
     return {"data": data, "size": torch.tensor([n, h, w]), "has_gt": torch.tensor([bool(it["has_gt"]) for it in items]),
             "fname": [it["fname"] for it in items]}
+
+
+def _collate_jpeg(items, n, h, w):
+    dec = [i for i, it in enumerate(items) if "jpeg" in it]
+    fb = [i for i, it in enumerate(items) if "jpeg" not in it]
+    for it in items:
+        size = (it["jpeg"].h, it["jpeg"].w) if "jpeg" in it else it["image"].shape[:2]
+        if tuple(size) != (h, w) or it["gt"].shape != (h, w):
+            raise ValueError("all frames of a batch must share a size")
+    blob = _jpeg.pack([items[i]["jpeg"] for i in dec])
+    blob_off = -(-(n * h * w + len(fb) * h * w * 3) // 16) * 16
+    data = torch.zeros(blob_off + len(blob), dtype=torch.uint8)
+    gt = data[:n * h * w].view(n, h, w)
+    img = data[n * h * w:n * h * w + len(fb) * h * w * 3].view(len(fb), h, w, 3)
+    for i, it in enumerate(items):
+        gt[i] = torch.from_numpy(it["gt"])
+    for k, i in enumerate(fb):
+        img[k] = torch.from_numpy(items[i]["image"])
+    data[blob_off:] = torch.from_numpy(blob)
+    return {"data": data, "size": torch.tensor([n, h, w]), "has_gt": torch.tensor([bool(it["has_gt"]) for it in items]),
+            "fname": [it["fname"] for it in items],
+            "jpeg": {"device": dec, "fallback": fb, "blob_off": blob_off, "nseg": _jpeg.segment_count(blob)}}
+
+
+def _assemble(data, jp, n, h, w, jpeg_status=None, out=None):
+    """The frames [N,H,W,3] (into ``out`` when given), masks [N,H,W] and status words int32 [N] (0 for host-decoded
+    frames) of an uploaded JPEG batch (_collate_jpeg's layout): the packed JPEGs decoded on the device, the
+    host-decoded frames copied into their slots.  ``jpeg_status``: an int32 [1] device tensor the status words are
+    added to."""
+    gt = data[:n * h * w].view(n, h, w)
+    dec, fb = jp["device"], jp["fallback"]
+    img = torch.empty((n, h, w, 3), dtype=torch.uint8, device=data.device) if out is None else out
+    frame_status = torch.zeros(n, dtype=torch.int32, device=data.device)
+    if fb:
+        src = data[n * h * w:n * h * w + len(fb) * h * w * 3].view(len(fb), h, w, 3)
+        if len(fb) == n:
+            img.copy_(src)
+        else:
+            img[torch.tensor(fb, device=data.device)] = src
+    if dec:
+        blob = data[jp["blob_off"]:]
+        out, status = ops.decode_jpeg(blob, len(dec), h, w, out=img if len(dec) == n else None, nseg=jp["nseg"])
+        index = torch.tensor(dec, device=data.device)
+        if len(dec) != n:
+            img[index] = out
+        frame_status[index] = status
+        if jpeg_status is not None:
+            jpeg_status += status.sum(dtype=torch.int32)
+    return img, gt, frame_status
+
+
+def device_views(batch, device, jpeg_status=None):
+    """One host-to-device copy of a collated batch -> (image uint8 [N,H,W,3], gt uint8 [N,H,W], status int32 [N] or
+    None) at the stored size: views of the copy, or for a decode="device" batch the frames decoded on the device
+    (_assemble; status is the decoder's per frame, nonzero for a corrupt or cut-short stream)."""
+    n, h, w = (int(v) for v in batch["size"])
+    data = pinned(batch["data"]).to(device, non_blocking=True)
+    if "jpeg" in batch:
+        return _assemble(data, batch["jpeg"], n, h, w, jpeg_status)
+    img, gt = views(data, n, h, w)
+    return img, gt, None
 
 
 def views(data, n, h, w):
@@ -170,27 +257,27 @@ def resize_pair(img, gt, input_res):
     return ops.resize_u8(img, size, "bilinear"), ops.resize_u8(gt, size, "nearest")
 
 
-def upload(batch, device, input_res=None):
+def upload(batch, device, input_res=None, jpeg_status=None):
     """One host-to-device copy of a collated batch -> (image uint8 [N,H,W,3], gt uint8 [N,H,W], label stats).
-    ``input_res``: the frames and masks are resized on the device first (resize_pair)."""
-    n, h, w = (int(v) for v in batch["size"])
-    data = pinned(batch["data"]).to(device, non_blocking=True)
-    img, gt = views(data, n, h, w)
+    ``input_res``: the frames and masks are resized on the device first (resize_pair).  A batch of
+    DAVIS2016Frames(decode="device") items is decoded on the device first (_assemble; ``jpeg_status``: an int32 [1]
+    device tensor that accumulates the decoder's status words, nonzero when a stream was corrupt or cut short)."""
+    img, gt, _ = device_views(batch, device, jpeg_status)
     if input_res is not None:
         img, gt = resize_pair(img, gt, input_res)
     return img, gt, ops.label_stats_u8(gt)
 
 
-def to_device(batch, device, augment=None, meanval=MEANVAL, input_res=None):
+def to_device(batch, device, augment=None, meanval=MEANVAL, input_res=None, jpeg_status=None):
     """Collated batch -> {'image': f32 [N,3,H,W], 'gt': f32 [N,1,H,W]} on ``device``.
 
     augment None: the reference's make_img_gt_pair + ToTensor, bit for bit (ops.image_from_bgr8, ops.label_from_u8).
     Otherwise RandomHorizontalFlip + ScaleNRotate as the reference composes them, fused with the ingest
     (augment.affine_warp_u8): ``augment`` is a list of per-sample (flip, rot, scale) triples, or a random generator
     from which augment.draw_params draws them in the reference's order.  ``input_res``: the reference's ``inputRes``,
-    applied on the device before all of that (upload)."""
+    applied on the device before all of that (upload, which also decodes a decode="device" batch's JPEGs)."""
     with torch.cuda.device(device):
-        img, gt, stats = upload(batch, device, input_res)
+        img, gt, stats = upload(batch, device, input_res, jpeg_status)
         if augment is None:
             return {"image": ops.image_from_bgr8(img, meanval), "gt": ops.label_from_u8(gt, stats)}
         params = augment if isinstance(augment, (list, tuple)) else _augment.draw_params(int(img.shape[0]), rng=augment)
@@ -242,7 +329,12 @@ class DeviceFrames:
     ``keep_stored_gt`` (with ``input_res``): the store also keeps every annotation's bytes at its stored size, in
     groups by stored size (``stored_groups``, each {'size', 'gt'}; ``where_stored[i]`` is index i's (group, slot)), so
     that segmentations upsampled back to that size (ops.resize_f32) are scored against the original annotations.  The
-    memory check counts them, and ingest returns them as 'gt_u8_stored'."""
+    memory check counts them, and ingest returns them as 'gt_u8_stored'.
+
+    A ``decode="device"`` dataset's frames are decoded on the device (device_views).  Before the store is shared, every
+    frame whose decoder status is nonzero (a corrupt or cut-short stream) is decoded again with cv2.imread, so the store
+    holds cv2's bytes whatever the files.  ``fallback_frames``: frames outside the device decoder's subset (decoded by
+    cv2.imread in the workers); ``redecoded_frames``: frames decoded again after a nonzero status."""
 
     def __init__(self, dataset, device, workers=0, group=None, input_res=None, keep_stored_gt=False):
         import torch.distributed as dist
@@ -277,6 +369,7 @@ class DeviceFrames:
                              "are free")
         self.groups, self.where = [], [None] * n
         self.stored_groups, self.where_stored = [], [None] * n
+        self.fallback_frames = self.redecoded_frames = 0
         with torch.cuda.device(self.device):
             for g, ((h, w), pad, members) in enumerate(plan0):
                 self.stored_groups.append({"size": (h, w), "gt": torch.zeros((world * pad, h, w), dtype=torch.uint8,
@@ -287,22 +380,39 @@ class DeviceFrames:
             for g, ((h, w), pad, members) in enumerate(plan):
                 img = torch.zeros((world * pad, h, w, 3), dtype=torch.uint8, device=self.device)
                 gt = torch.zeros((world * pad, h, w), dtype=torch.uint8, device=self.device)
+                checks = []
                 for j, i in enumerate(members[rank]):
                     item = decoded.pop(i)
-                    data = pinned(item["data"])
                     s = rank * pad + j
+                    if "jpeg" not in item and getattr(dataset, "decode", "host") == "device":
+                        self.fallback_frames += 1
+                    if "jpeg" in item:
+                        src_img, src_gt, st = device_views(item, self.device)
+                        checks.append((i, s, st))
+                    elif input_res is None:
+                        src_img, src_gt = views(pinned(item["data"]), 1, h, w)
+                    else:
+                        h0, w0 = (int(v) for v in item["size"][1:])
+                        src_img, src_gt = views(pinned(item["data"]).to(self.device, non_blocking=True), 1, h0, w0)
                     if input_res is None:
-                        src_img, src_gt = views(data, 1, h, w)
                         img[s].copy_(src_img[0], non_blocking=True)
                         gt[s].copy_(src_gt[0], non_blocking=True)
                     else:
-                        h0, w0 = (int(v) for v in item["size"][1:])
-                        src_img, src_gt = views(data.to(self.device, non_blocking=True), 1, h0, w0)
                         ops.resize_u8(src_img, (h, w), "bilinear", out=img[s:s + 1])
                         ops.resize_u8(src_gt, (h, w), "nearest", out=gt[s:s + 1])
                         if keep_stored:
                             g0, s0 = self.where_stored[i]
                             self.stored_groups[g0]["gt"][s0].copy_(src_gt[0])
+                if checks:                         # one synchronisation per size group, at build time only
+                    flags = torch.cat([st for _, _, st in checks]).cpu()
+                    for (i, s, _), f in zip(checks, flags.tolist()):
+                        if f:
+                            frame = torch.from_numpy(dataset._read(dataset.img_list[i], 1)).to(self.device)[None]
+                            if input_res is None:
+                                img[s:s + 1].copy_(frame)
+                            else:
+                                ops.resize_u8(frame, (h, w), "bilinear", out=img[s:s + 1])
+                            self.redecoded_frames += 1
                 if group is not None:              # in place: this rank's share is already in its slots
                     share = slice(rank * pad, (rank + 1) * pad)
                     dist.all_gather_into_tensor(img, img[share], group=group)

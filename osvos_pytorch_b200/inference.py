@@ -36,16 +36,23 @@ class SequenceSegmenter:
     compute stream (ops.resize_f32, scipy 1.0's imresize(mode='F'); DESIGN.md §18) into a per-slot buffer of fixed
     address, so the results are [N,1,H0,W0] and the scores are taken against the original annotations, as the
     DAVIS-2016 benchmark scores 480x854 masks.  ``"network"`` (the default) keeps them at the network resolution.
-    Without ``input_res`` both are the stored size and nothing is resized."""
+    Without ``input_res`` both are the stored size and nothing is resized.
+
+    ``frames="jpeg"``: ``frames`` yields collated batches (davis.collate) of a DAVIS2016Frames(decode="device")
+    dataset; with ``score=True`` their masks are the annotations (no pairs).  Each batch's buffer crosses PCIe into a
+    per-slot device buffer (grown when a larger batch arrives: the decode is not captured in a graph, only the
+    forward on the fp32 slot is), and the JPEGs are decoded on the compute stream into the slot's bgr8 buffer; from
+    there on it is ``frames="bgr8"``.  ``jpeg_status`` (int32 [1] on the device) sums the decoder's status words
+    over the run: nonzero when a stream was corrupt or cut short."""
 
     def __init__(self, net, output="logits", depth=3, frames="nchw_f32", meanval=ops.MEANVAL, score=False,
                  input_res=None, output_res="network"):
         if output not in ("logits", "bytescale", "prob", "mask"):
             raise ValueError("output must be one of logits / bytescale / prob / mask")
-        if frames not in ("nchw_f32", "bgr8"):
-            raise ValueError("frames must be nchw_f32 or bgr8")
-        if input_res is not None and frames != "bgr8":
-            raise ValueError("input_res resizes the decoded bytes, as imresize does: it needs frames='bgr8'")
+        if frames not in ("nchw_f32", "bgr8", "jpeg"):
+            raise ValueError("frames must be nchw_f32, bgr8 or jpeg")
+        if input_res is not None and frames == "nchw_f32":
+            raise ValueError("input_res resizes the decoded bytes, as imresize does: it needs frames='bgr8' or 'jpeg'")
         if output_res not in ("network", "stored"):
             raise ValueError("output_res must be 'network' or 'stored'")
         self.net, self.output, self.depth = net, output, max(2, int(depth))
@@ -56,10 +63,12 @@ class SequenceSegmenter:
         self._upsample = input_res is not None and output_res == "stored"
         self._shape = None
         self._counts = []
+        self.jpeg_status = None
 
     def _allocate(self, shape, device):
-        if self.frames == "bgr8":
+        if self.frames != "nchw_f32":
             n, h, w, _ = shape
+            self._dev_blob = [None] * self.depth
             self._dev_raw = [torch.empty(shape, dtype=torch.uint8, device=device) for _ in range(self.depth)]
         else:
             n, _, h, w = shape
@@ -83,24 +92,44 @@ class SequenceSegmenter:
         mk = lambda: [torch.cuda.Event() for _ in range(self.depth)]
         self._ev_loaded, self._ev_consumed, self._ev_done, self._ev_host = mk(), mk(), mk(), mk()
         self._shape = tuple(shape)
-        self.h2d_bytes_per_frame = n * 3 * h0 * w0 * (1 if self.frames == "bgr8" else 4) + (n * h0 * w0 if self.score else 0)
+        self.h2d_bytes_per_frame = n * 3 * h0 * w0 * (4 if self.frames == "nchw_f32" else 1) + (n * h0 * w0 if self.score else 0)
         self.d2h_bytes_per_frame = n * rh * rw * (4 if self.output == "logits" else 1)
 
     def _submit(self, i, frame, gt, device):
         k = i % self.depth
         cur = torch.cuda.current_stream(device)
-        bgr8 = self.frames == "bgr8"
+        bgr8 = self.frames != "nchw_f32"
+        jpeg = self.frames == "jpeg"
         with torch.cuda.stream(self._s_in):
             if i >= self.depth:
                 self._s_in.wait_event(self._ev_consumed[k])     # the network has read the previous tenant
-            (self._dev_raw[k] if bgr8 else self._dev_in[k]).copy_(frame, non_blocking=True)
-            if self.score:
+            if jpeg:                                            # the collated buffer: JPEGs, fallback frames, masks
+                from .davis import pinned
+                data = pinned(frame["data"])
+                if self._dev_blob[k] is None or self._dev_blob[k].numel() < data.numel():
+                    self._dev_blob[k] = torch.empty(data.numel(), dtype=torch.uint8, device=device)
+                self._dev_blob[k][:data.numel()].copy_(data, non_blocking=True)
+                self.h2d_bytes_per_frame = data.numel()
+            else:
+                (self._dev_raw[k] if bgr8 else self._dev_in[k]).copy_(frame, non_blocking=True)
+            if self.score and not jpeg:
                 self._dev_gt[k].copy_(gt, non_blocking=True)
             self._ev_loaded[k].record(self._s_in)
         cur.wait_event(self._ev_loaded[k])
         if i >= self.depth:
             cur.wait_event(self._ev_host[k])                    # previous result of this slot is on the host
         gt_dev = self._dev_gt[k] if self.score else None
+        if jpeg:
+            from .davis import _assemble, views
+            n, h, w = (int(v) for v in frame["size"])
+            blob = self._dev_blob[k][:frame["data"].numel()]
+            if "jpeg" in frame:
+                _, gt_view, _ = _assemble(blob, frame["jpeg"], n, h, w, self.jpeg_status, out=self._dev_raw[k])
+            else:                                               # every frame of the batch fell back to cv2.imread
+                img_view, gt_view = views(blob, n, h, w)
+                self._dev_raw[k].copy_(img_view)
+            if self.score:
+                gt_dev = gt_view
         if bgr8:
             raw = self._dev_raw[k]
             if self.input_res is not None:
@@ -140,7 +169,23 @@ class SequenceSegmenter:
         submitted = 0
         self._counts = []
         with torch.cuda.device(device):
+            if self.frames == "jpeg":
+                self.jpeg_status = torch.zeros(1, dtype=torch.int32, device=device)
             for item in frames:
+                if self.frames == "jpeg":
+                    n, h, w = (int(v) for v in item["size"])
+                    if self._shape != (n, h, w, 3):
+                        if submitted:
+                            raise ValueError("all frames of one sequence must share a shape")
+                        self._allocate((n, h, w, 3), device)
+                    self._submit(submitted, item, None, device)
+                    submitted += 1
+                    ready = submitted - self.depth + 1
+                    if ready >= 1:
+                        k = (ready - 1) % self.depth
+                        self._ev_host[k].synchronize()
+                        yield self._host_out[k]
+                    continue
                 frame, gt = item if self.score else (item, None)
                 if frame.dim() == 3:
                     frame = frame.unsqueeze(0)

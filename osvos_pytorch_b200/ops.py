@@ -738,3 +738,40 @@ def davis_measures(logits, gt_u8, r=None, out=None):
     nat.check(lib.osvos_davis_measures(x.data_ptr(), g.data_ptr(), out.data_ptr(), ws.data_ptr(), n, h, w, r, _stream()),
               "osvos_davis_measures")
     return out
+
+
+def decode_jpeg(blob, n, h, w, out=None, status=None, nseg=None, chunk_bits=0):
+    """A batch of n JPEGs of size h x w packed by jpeg.pack (``blob``: uint8 device tensor) -> (out uint8 [n,h,w,3] BGR,
+    bit-identical to cv2.imread; status int32 [n]: 1 bad Huffman code, 2 zig-zag index past 63, 4 data ended before the
+    last MCU, 8 header inconsistent with (n, h, w)).  ``out`` may be any uint8 [n,h,w,3] view with contiguous rows of
+    pixels, e.g. a slot range of a collated buffer.  ``chunk_bits``: the Huffman decoder's chunk size (0: default).
+    No host synchronisation (csrc/jpeg.cu, DESIGN.md §19).  ``nseg`` (required): the blob's segment count,
+    jpeg.segment_count of the host blob.  It sizes the launch, and reading it from the device blob would make the call
+    wait for the device."""
+    if nseg is None:
+        raise ValueError("nseg: pass jpeg.segment_count(host_blob); the device copy is not read back")
+    lib = nat.load()
+    _require_cuda(blob, "blob")
+    if blob.dtype != torch.uint8 or blob.dim() != 1 or not blob.is_contiguous():
+        raise ValueError("blob must be a contiguous 1-D uint8 device tensor from jpeg.pack")
+    if blob.data_ptr() % 16:
+        raise ValueError("blob must be 16-byte aligned")
+    shape = (n, h, w, 3)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.uint8, device=blob.device)
+    elif out.dtype != torch.uint8 or tuple(out.shape) != shape or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous uint8 tensor of shape {shape}")
+    if status is None:
+        status = torch.empty(n, dtype=torch.int32, device=blob.device)
+    elif status.dtype != torch.int32 or tuple(status.shape) != (n,) or not status.is_contiguous():
+        raise ValueError(f"status must be a contiguous int32 tensor of shape ({n},)")
+    nbytes = lib.osvos_jpeg_decode_workspace_bytes(n, h, w, nseg, blob.numel(), chunk_bits)
+    if nbytes == 0:
+        raise ValueError(f"cannot decode [{n},{h},{w}] with {nseg} segments, {blob.numel()} blob bytes, chunk_bits "
+                         f"{chunk_bits}")
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=blob.device)
+    a = nat.JpegArgs(blob.data_ptr(), blob.numel(), out.data_ptr(), status.data_ptr(), ws.data_ptr(), n, h, w, nseg,
+                     chunk_bits, 0)
+    nat.check(lib.osvos_jpeg_decode(byref(a), _stream()), "osvos_jpeg_decode")
+    _count(6)
+    return out, status

@@ -53,6 +53,10 @@ def parse(argv=None):
                     help="score the segmentation against every frame's annotation on the device (DAVIS-2016 J and F, "
                          "osvos_pytorch_b200.evaluation); prints them and writes Results/<seq>_scores.json. "
                          "Needs --loader native")
+    ap.add_argument("--decode", default="host", choices=["host", "device"],
+                    help="--loader native: decode the JPEG frames with cv2.imread in the workers (host), or parse them "
+                         "there and decode them on the GPU, bit-identically (device; files outside the decoder's subset "
+                         "still go through cv2.imread)")
     ap.add_argument("--input-res", type=int, nargs=2, default=None, metavar=("H", "W"),
                     help="the reference's inputRes: resize every frame (bilinear) and annotation (nearest) to H x W on "
                          "the device before training, segmentation and scoring, as scipy 1.0's imresize does. Needs "
@@ -69,6 +73,9 @@ def parse(argv=None):
     if a.input_res is not None and (a.synthetic or a.loader != "native"):
         ap.error("--input-res resizes the frames read by --loader native; it cannot be combined with "
                  + ("--synthetic (use --height / --width)" if a.synthetic else "--loader reference"))
+    if a.decode == "device" and (a.synthetic or a.loader != "native"):
+        ap.error("--decode device decodes the frames read by --loader native; it cannot be combined with "
+                 + ("--synthetic" if a.synthetic else "--loader reference"))
     return a
 
 
@@ -116,7 +123,7 @@ def main(argv=None):
         import random
         from torch.utils.data import DataLoader
         from osvos_pytorch_b200 import augment, davis
-        first = davis.DAVIS2016Frames(train=True, db_root_dir=Path.db_root_dir(), seq_name=a.seq_name)
+        first = davis.DAVIS2016Frames(train=True, db_root_dir=Path.db_root_dir(), seq_name=a.seq_name, decode=a.decode)
         input_res = None if a.input_res is None else tuple(a.input_res)
         img_u8, gt_u8, stats = davis.upload(davis.collate([first[0]]), device, input_res=input_res)
         rng = random.Random(a.seed)
@@ -124,12 +131,15 @@ def main(argv=None):
         def sample_fn(it):
             return augment.affine_warp_u8(img_u8, gt_u8, augment.draw_params(1, rng=rng), stats)
         db_test = davis.DAVIS2016Frames(train=False, db_root_dir=Path.db_root_dir(), seq_name=a.seq_name,
-                                        all_annotations=a.evaluate)
+                                        all_annotations=a.evaluate, decode=a.decode)
         # pinned here, between forwards, not by a loader thread that could allocate during a graph capture; the image
         # and the mask are two views of the one pinned buffer
-        test_frames = (dict(zip(("image", "gt"), davis.views(davis.pinned(b["data"]), *(int(v) for v in b["size"]))),
-                            fname=b["fname"])
-                       for b in DataLoader(db_test, batch_size=1, shuffle=False, num_workers=1, collate_fn=davis.collate))
+        test_loader = DataLoader(db_test, batch_size=1, shuffle=False, num_workers=1, collate_fn=davis.collate)
+        if a.decode == "device":         # collated batches as they are: the segmenter decodes them on the device
+            test_frames = test_loader
+        else:
+            test_frames = (dict(zip(("image", "gt"), davis.views(davis.pinned(b["data"]), *(int(v) for v in b["size"]))),
+                                fname=b["fname"]) for b in test_loader)
     else:
         from dataloaders import davis_2016 as db
         from dataloaders import custom_transforms as tr
@@ -188,13 +198,19 @@ def main(argv=None):
     upsample = input_res is not None and a.output_res == "stored"
     stored_hw = []                                      # the sequence's stored size (one size per sequence)
 
+    jpeg_frames = native and a.decode == "device"
+
     def frames():
         for ii, s in enumerate(test_frames):
-            n = int(s["image"].shape[0])
-            names.append([os.path.basename(s["fname"][jj]) if "fname" in s else f"{ii:05d}_{jj}" for jj in range(n)])
+            shape = tuple(int(v) for v in s["size"]) if jpeg_frames else tuple(s["image"].shape[:3])   # N, H, W
+            names.append([os.path.basename(s["fname"][jj]) if "fname" in s else f"{ii:05d}_{jj}"
+                          for jj in range(shape[0])])
             if upsample and not stored_hw:
-                stored_hw.extend(int(v) for v in s["image"].shape[1:3])        # bgr8 [N,H,W,3]
-            yield (s["image"], s["gt"]) if a.evaluate else s["image"]
+                stored_hw.extend(shape[1:3])
+            if jpeg_frames:                 # a collated batch: the segmenter takes the masks from it
+                yield s
+            else:
+                yield (s["image"], s["gt"]) if a.evaluate else s["image"]
     if upsample:
         print(f"Frames resized to {input_res[0]}x{input_res[1]} (inputRes); the fused logits are upsampled to the "
               "stored size, results are written at that size"
@@ -202,7 +218,8 @@ def main(argv=None):
     elif input_res is not None:
         print(f"Frames resized to {input_res[0]}x{input_res[1]} (inputRes); results are written at that size"
               + (", scored against the nearest-resized annotations" if a.evaluate else ""))
-    seg = SequenceSegmenter(net, output="bytescale", frames="bgr8" if native else "nchw_f32", score=a.evaluate,
+    seg = SequenceSegmenter(net, output="bytescale", frames=("jpeg" if jpeg_frames else "bgr8") if native else "nchw_f32",
+                            score=a.evaluate,
                             input_res=input_res, output_res=a.output_res)
     for pred in seg(frames()):
         arr = pred.numpy()
@@ -212,6 +229,9 @@ def main(argv=None):
                 Image.fromarray(arr[jj, 0], mode="L").save(os.path.join(out_dir, name + ".png"))
             except ImportError:
                 np.save(os.path.join(out_dir, name + ".npy"), arr[jj, 0])
+    if seg.jpeg_status is not None and int(seg.jpeg_status) != 0:     # the segmenter's last wait covered the decodes
+        print(f"WARNING: the device JPEG decoder flagged corrupt or cut-short frames (status sum {int(seg.jpeg_status)}); "
+              "their bytes may differ from cv2.imread's")
     if a.evaluate:
         import json
         from osvos_pytorch_b200.evaluation import SequenceScores

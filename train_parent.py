@@ -65,6 +65,10 @@ def parse(argv=None):
                     help="device: decode the train split once and keep its bytes on every GPU (about 3.4 GB per rank, "
                          "plus 2.3 GB of val frames on rank 0), then augment each batch from there instead of "
                          "decoding every frame in every epoch; needs --loader native")
+    ap.add_argument("--decode", default="host", choices=["host", "device"],
+                    help="--loader native: decode the JPEG frames with cv2.imread in the workers (host), or parse them "
+                         "there and decode them on the GPU, bit-identically (device; files outside the decoder's subset "
+                         "still go through cv2.imread)")
     ap.add_argument("--input-res", type=int, nargs=2, default=None, metavar=("H", "W"),
                     help="the reference's inputRes: resize every frame (bilinear) and annotation (nearest) to H x W on "
                          "the device, before augmentation and validation, as scipy 1.0's imresize does. Needs --loader "
@@ -84,6 +88,9 @@ def parse(argv=None):
     if a.input_res is not None and (a.synthetic or a.loader != "native"):
         ap.error("--input-res resizes the frames read by --loader native; it cannot be combined with "
                  + ("--synthetic (use --height / --width)" if a.synthetic else "--loader reference"))
+    if a.decode == "device" and (a.synthetic or a.loader != "native"):
+        ap.error("--decode device decodes the frames read by --loader native; it cannot be combined with "
+                 + ("--synthetic" if a.synthetic else "--loader reference"))
     return a
 
 
@@ -120,6 +127,7 @@ def main(argv=None):
     bucket = parallel.GradientBucket(parallel.trainable_parameters(net), device)
 
     stored = False                                   # J and F at the stored size (--input-res --output-res stored)
+    jpeg_status = None                               # --decode device, streaming: the decoder's status words, summed
     if a.synthetic:
         def epoch_batches(epoch):
             # the same number of micro-batches on every rank (a multiple of n_ave): every rank joins every allreduce
@@ -135,9 +143,9 @@ def main(argv=None):
         from torch.utils.data import DataLoader
         from torch.utils.data.distributed import DistributedSampler
         from osvos_pytorch_b200 import davis
-        db_train = davis.DAVIS2016Frames(train=True, db_root_dir=Path.db_root_dir())
+        db_train = davis.DAVIS2016Frames(train=True, db_root_dir=Path.db_root_dir(), decode=a.decode)
         sampler = DistributedSampler(db_train, world, rank, shuffle=True, drop_last=True) if world > 1 else None
-        db_test = davis.DAVIS2016Frames(train=False, db_root_dir=Path.db_root_dir())
+        db_test = davis.DAVIS2016Frames(train=False, db_root_dir=Path.db_root_dir(), decode=a.decode)
         res = None if a.input_res is None else tuple(a.input_res)
         stored = res is not None and a.val_measures and a.output_res == "stored"
         if res is not None and rank == 0:
@@ -160,13 +168,17 @@ def main(argv=None):
                                       lambda b: val_store.ingest(int(b[0])))
                 for name, st in (("train", train_store), ("val", val_store)):
                     print(f"Device frame store ({name}): {len(st)} frames, {st.nbytes / 1e9:.2f} GB, built in "
-                          f"{st.build_s:.1f} s")
+                          f"{st.build_s:.1f} s" + (f"; {st.fallback_frames} frames decoded by cv2.imread, "
+                                                   f"{st.redecoded_frames} re-decoded after a decoder status"
+                                                   if a.decode == "device" else ""))
 
             def epoch_batches(epoch):
                 if sampler is not None:
                     sampler.set_epoch(epoch)
                 yield from train_store.batches(loader, rng=random)
         else:
+            if a.decode == "device":
+                jpeg_status = torch.zeros(1, dtype=torch.int32, device=device)
             loader = DataLoader(db_train, batch_size=a.batch, shuffle=sampler is None, sampler=sampler,
                                 num_workers=a.workers, drop_last=world > 1, collate_fn=davis.collate,
                                 persistent_workers=a.workers > 0)
@@ -177,25 +189,25 @@ def main(argv=None):
                 def val_item(b):                     # davis.to_device without augmentation, keeping the mask bytes
                     with torch.cuda.device(device):
                         if not stored:
-                            img, gt, stats = davis.upload(b, device, input_res=res)
+                            img, gt, stats = davis.upload(b, device, input_res=res, jpeg_status=jpeg_status)
                             return {"image": ops.image_from_bgr8(img), "gt": ops.label_from_u8(gt, stats), "gt_u8": gt,
                                     "fname": b["fname"]}
                         # davis.upload, keeping the collated mask's view at the stored size
-                        n, h, w = (int(v) for v in b["size"])
-                        img0, gt0 = davis.views(davis.pinned(b["data"]).to(device, non_blocking=True), n, h, w)
+                        img0, gt0, _ = davis.device_views(b, device, jpeg_status)
                         img, gt = davis.resize_pair(img0, gt0, res)
                         stats = ops.label_stats_u8(gt)
                         return {"image": ops.image_from_bgr8(img), "gt": ops.label_from_u8(gt, stats), "gt_u8": gt,
                                 "gt_u8_stored": gt0, "fname": b["fname"]}
                 val_batches = _Mapped(val_loader, val_item)
             else:
-                val_batches = _Mapped(val_loader, lambda b: davis.to_device(b, device, input_res=res))
+                val_batches = _Mapped(val_loader, lambda b: davis.to_device(b, device, input_res=res,
+                                                                            jpeg_status=jpeg_status))
 
             def epoch_batches(epoch):
                 if sampler is not None:
                     sampler.set_epoch(epoch)
                 for b in loader:      # flip / rotation / scale drawn from Python's random, as the reference's transforms do
-                    yield davis.to_device(b, device, augment=random, input_res=res)
+                    yield davis.to_device(b, device, augment=random, input_res=res, jpeg_status=jpeg_status)
     else:
         from dataloaders import davis_2016 as db
         from dataloaders import custom_transforms as tr
@@ -225,6 +237,10 @@ def main(argv=None):
         t0 = timeit.default_timer()
         losses = training.parent_epoch(net, opt, bucket, epoch_batches(epoch), epoch, a.epochs, n_ave, state=loop_state)
         torch.cuda.synchronize()
+        if jpeg_status is not None and int(jpeg_status) != 0:     # read after the epoch's synchronisation
+            print(f"WARNING: rank {rank}: the device JPEG decoder flagged corrupt or cut-short frames in epoch {epoch} "
+                  f"(status sum {int(jpeg_status)}); their bytes may differ from cv2.imread's")
+            jpeg_status.zero_()
         if rank == 0:
             print(f"[Epoch: {epoch}] " + " ".join(f"Loss {k}: {v:.4f}" for k, v in enumerate(losses.tolist()))
                   + f"  Execution time: {timeit.default_timer() - t0:.2f}")
