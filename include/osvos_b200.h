@@ -602,6 +602,104 @@ typedef struct osvos_jpeg_args {
 OSVOS_API size_t osvos_jpeg_decode_workspace_bytes(int n, int h, int w, int nseg, size_t blob_bytes, int chunk_bits);
 OSVOS_API int osvos_jpeg_decode(const osvos_jpeg_args* args, osvos_stream_t stream);
 
+/* ---- side-branch tail with general deconvolution weights (DESIGN.md §20) ------------------------------------------
+ * The reference's eight ConvTranspose2d layers with ANY weights (networks/vgg_osvos.py:45-46,68-69), their centre crop
+ * (layers/osvos_layers.py:51-56), cat + fuse (:71-72) and, with a label, the class-balanced BCE terms
+ * (layers/osvos_layers.py:28-41); their autograd at train_online.py:141 / train_parent.py:164, including the gradients
+ * of upscale[i] / upscale_[i] that the bilinear path never forms.  Scale k: stride s = 2^(k+1), T_k = (2s)^2 taps
+ * t = ty * 2s + tx; the four scales' taps are concatenated (offsets 0, 16, 80, 336; OSVOS_UPSAMPLING_TAPS in all).
+ *   osvos_upsampling_fold:   vtab [OSVOS_UPSAMPLING_TAPS][16]: V_k[t][ci] = sum_co fuse_w[16k + co] upscale_w[k][ci][co][t]
+ *                            (upscale[k] folded with its slice of fuse), atab [OSVOS_UPSAMPLING_TAPS] = upscale_[k] taps.
+ *                            Pass vtab and atab as ONE buffer (atab = vtab + 16 * OSVOS_UPSAMPLING_TAPS), 16-byte aligned.
+ *   osvos_tail_general_fwd:  out[k<4](y,x) = sum_{<=2x2 src} atab_k[t] p_k(src), out[4] = fuse_bias + sum_k sum_src
+ *                            sum_ci vtab_k[t][ci] feat_k[src][ci], from the 16 side features (osvos_conv3x3 cout == 16,
+ *                            y_f32) and p_k = channel 0 of their pq.  `sums` / `losses`: osvos_tail_fwd's contract and
+ *                            layout, with osvos_tail_general_fwd_sums(n, h, w) doubles (block rows always added in a
+ *                            fixed order).
+ *   osvos_tail_general_bwd:  from the five upstream gradient maps g_k (label NULL; NULL maps count as zero) or, with a
+ *                            label, from dL/dlogit formed on the fly as osvos_tail_loss_bwd does (src = the forward's
+ *                            logits, sums = its sums):
+ *                              df_k [n,h_k,w_k,64] split-bf16 act: channels 0..15 = dF_k[ci] = sum_t g_4 vtab_k[t][ci]
+ *                                   + dp_k score_w[k][ci] with dp_k = sum_t g_k atab_k[t]; channels 16..63 = 0 (the
+ *                                   operand of side_prep's tensor-core weight and data gradients);
+ *                              red_k [17 T_k + 33] = {H[t][ci] = sum g_4 F[ci] (16 T), gA[t] = sum g_k p (T),
+ *                                   sum dp F[ci] (16), sum dp, sum dF[ci] (16)};
+ *                              fuse_bias_grad (label mode only).
+ *                            workspace: osvos_tail_general_bwd_workspace_bytes(n, h, w) bytes, 4-byte aligned.
+ *   osvos_upsampling_grads_finish: d upscale[k][ci][co][t] = fuse_w[16k+co] H_k[t][ci], d upscale_[k] = gA_k,
+ *                            d fuse.weight[16k+co] = sum_{ci,t} upscale_w[k][ci][co][t] H_k[t][ci], d score_dsn[k].weight
+ *                            = sum dp F, .bias = sum dp, d side_prep[k].bias = sum dF; NULL outputs are skipped, with
+ *                            accumulate the values are added to the destinations.
+ *   osvos_unpool_dside_mask: dz = ReLU'(x) * (unpool(dpool) + dside) as osvos_unpool_add_mask, dpool_hi NULL allowed
+ *                            (the deepest stage); OSVOS_FLAG_DETERMINISTIC: colsum is partial rows
+ *                            [osvos_unpool_colsum_rows(n, h, w, c, dpool_hi != NULL, 0)][c].
+ * Every float reduction of these calls is fixed-order (OSVOS_FLAG_DETERMINISTIC is accepted and changes nothing).   */
+#define OSVOS_UPSAMPLING_TAPS 1360
+typedef struct {
+  const float* upscale_w[4];    /* upscale[k].weight [16][16][2s][2s] ([in][out][kH][kW]) */
+  const float* upscale1_w[4];   /* upscale_[k].weight [1][1][2s][2s] */
+  const float* fuse_w;          /* fuse.weight [64] */
+  float* vtab;
+  float* atab;
+} osvos_upsampling_fold_args;
+OSVOS_API int osvos_upsampling_fold(const osvos_upsampling_fold_args* args /* host */, osvos_stream_t stream);
+typedef struct {
+  const float* feat[4];    /* [n,h_k,w_k,16] fp32 */
+  const float* pq[4];      /* [n,h_k,w_k,2] fp32 */
+  const float* vtab;
+  const float* atab;
+  const float* fuse_bias;  /* [1] or NULL */
+  float* out[5];           /* each [n,1,h,w] fp32 or NULL */
+  const float* label;      /* [n,1,h,w] or NULL */
+  double* sums;            /* osvos_tail_general_fwd_sums(n, h, w) doubles (required with label) */
+  float* losses;           /* [6] or NULL */
+  float loss_weights[5];
+  float divisor;
+  int n, h, w;
+  int flags;
+} osvos_tail_general_fwd_args;
+OSVOS_API size_t osvos_tail_general_fwd_sums(int n, int h, int w);
+OSVOS_API int osvos_tail_general_fwd(const osvos_tail_general_fwd_args* args /* host */, osvos_stream_t stream);
+typedef struct {
+  const float* feat[4];
+  const float* pq[4];
+  const float* score_w[4]; /* score_dsn[k].weight [16] */
+  const float* vtab;
+  const float* atab;
+  const float* src[5];     /* gradient maps (label NULL) or the forward's logit maps (label set) */
+  const float* label;
+  const double* sums;      /* the forward's sums (label mode) */
+  const float* upstream;   /* device scalar d(total) or NULL (= 1), label mode */
+  float loss_weights[5];
+  float divisor;
+  void* df_hi[4];          /* [n,h_k,w_k,64] bf16 */
+  void* df_lo[4];          /* or NULL (fast precision) */
+  float* red[4];           /* [17 T_k + 33] */
+  float* fuse_bias_grad;   /* [1] or NULL (label mode) */
+  void* workspace;
+  int n, h, w;
+  int flags;
+} osvos_tail_general_bwd_args;
+OSVOS_API size_t osvos_tail_general_bwd_workspace_bytes(int n, int h, int w);
+OSVOS_API int osvos_tail_general_bwd(const osvos_tail_general_bwd_args* args /* host */, osvos_stream_t stream);
+typedef struct {
+  const float* red[4];
+  const float* upscale_w[4];
+  const float* fuse_w;
+  float* d_upscale_w[4];   /* [16][16][T_k] or NULL */
+  float* d_upscale1_w[4];  /* [T_k] or NULL */
+  float* d_fuse_w;         /* [64] or NULL */
+  float* d_score_w[4];     /* [16] or NULL */
+  float* d_score_b[4];     /* [1] or NULL */
+  float* d_side_b[4];      /* [16] or NULL */
+  int accumulate;
+} osvos_upsampling_grads_args;
+OSVOS_API int osvos_upsampling_grads_finish(const osvos_upsampling_grads_args* args /* host */, osvos_stream_t stream);
+OSVOS_API int osvos_unpool_dside_mask(const void* dpool_hi /* or NULL */, const void* dpool_lo, const void* x_hi,
+                                      const void* x_lo, const float* dside /* [n,h,w,c] fp32 */, void* dz_hi, void* dz_lo,
+                                      float* colsum /* or NULL */, int n, int h, int w, int c, int flags,
+                                      osvos_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -104,6 +104,37 @@ class JpegArgs(Structure):
                 ("chunk_bits", c_int), ("reserved", c_int)]
 
 
+class UpsamplingFoldArgs(Structure):
+    """osvos_upsampling_fold_args (include/osvos_b200.h)."""
+    _fields_ = [("upscale_w", c_void_p * 4), ("upscale1_w", c_void_p * 4), ("fuse_w", c_void_p), ("vtab", c_void_p),
+                ("atab", c_void_p)]
+
+
+class TailGeneralFwdArgs(Structure):
+    """osvos_tail_general_fwd_args (include/osvos_b200.h)."""
+    _fields_ = [("feat", c_void_p * 4), ("pq", c_void_p * 4), ("vtab", c_void_p), ("atab", c_void_p),
+                ("fuse_bias", c_void_p), ("out", c_void_p * 5), ("label", c_void_p), ("sums", c_void_p),
+                ("losses", c_void_p), ("loss_weights", c_float * 5), ("divisor", c_float), ("n", c_int), ("h", c_int),
+                ("w", c_int), ("flags", c_int)]
+
+
+class TailGeneralBwdArgs(Structure):
+    """osvos_tail_general_bwd_args (include/osvos_b200.h)."""
+    _fields_ = [("feat", c_void_p * 4), ("pq", c_void_p * 4), ("score_w", c_void_p * 4), ("vtab", c_void_p),
+                ("atab", c_void_p), ("src", c_void_p * 5), ("label", c_void_p), ("sums", c_void_p),
+                ("upstream", c_void_p), ("loss_weights", c_float * 5), ("divisor", c_float), ("df_hi", c_void_p * 4),
+                ("df_lo", c_void_p * 4), ("red", c_void_p * 4), ("fuse_bias_grad", c_void_p), ("workspace", c_void_p),
+                ("n", c_int), ("h", c_int), ("w", c_int), ("flags", c_int)]
+
+
+class UpsamplingGradsArgs(Structure):
+    """osvos_upsampling_grads_args (include/osvos_b200.h)."""
+    _fields_ = [("red", c_void_p * 4), ("upscale_w", c_void_p * 4), ("fuse_w", c_void_p), ("d_upscale_w", c_void_p * 4),
+                ("d_upscale1_w", c_void_p * 4), ("d_fuse_w", c_void_p), ("d_score_w", c_void_p * 4),
+                ("d_score_b", c_void_p * 4), ("d_side_b", c_void_p * 4), ("accumulate", c_int)]
+
+
+UPSAMPLING_TAPS = 1360
 U8_PROB, U8_BYTESCALE, U8_MASK = 0, 1, 2
 RESIZE_BILINEAR, RESIZE_NEAREST = 0, 1
 SGD_MAX_SEGMENTS = 64
@@ -188,6 +219,14 @@ SIGNATURES = {
     "osvos_sum_f32_deterministic": (c_int, [c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
     "osvos_jpeg_decode_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_size_t, c_int]),
     "osvos_jpeg_decode": (c_int, [POINTER(JpegArgs), c_void_p]),
+    "osvos_upsampling_fold": (c_int, [POINTER(UpsamplingFoldArgs), c_void_p]),
+    "osvos_tail_general_fwd_sums": (c_size_t, [c_int, c_int, c_int]),
+    "osvos_tail_general_fwd": (c_int, [POINTER(TailGeneralFwdArgs), c_void_p]),
+    "osvos_tail_general_bwd_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "osvos_tail_general_bwd": (c_int, [POINTER(TailGeneralBwdArgs), c_void_p]),
+    "osvos_upsampling_grads_finish": (c_int, [POINTER(UpsamplingGradsArgs), c_void_p]),
+    "osvos_unpool_dside_mask": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_int, c_int, c_int, c_int, c_int, c_void_p]),
 }
 
 DAVIS_MAX_RADIUS = 31

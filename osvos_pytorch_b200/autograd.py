@@ -4,8 +4,9 @@ arithmetic).  Replaces the autograd graph of reference networks/vgg_osvos.py:59-
 train_online.py:124 / train_parent.py:140 and walked at :141 / :164.
 
 Gradient bookkeeping mirrors the reference: parameters that do not influence the objective get
-``None`` (e.g. score_dsn.* under the fuse-only online loss, SURVEY.md 8c item 9); the fixed
-bilinear deconvolution weights (lr = 0 in both scripts) receive no gradient.
+``None`` (e.g. score_dsn.* under the fuse-only online loss, SURVEY.md 8c item 9); the eight
+deconvolution weights (lr = 0 in both scripts) receive a gradient only when the module's
+``learn_upsampling`` is set (the general tail, DESIGN.md §20).
 
 Determinism: the forward reads ``torch.are_deterministic_algorithms_enabled()`` once and keeps it on ``ctx``; the loss
 sums of the fused objective and every float reduction of the backward then take their fixed-order forms
@@ -39,7 +40,8 @@ class _OSVOSFunction(torch.autograd.Function):
         `total = sum_k w_k * class_balanced_cross_entropy_loss(map_k, label)` differentiable."""
         m = engine.m
         fast = m.precision == "fast"
-        engine._check_deconvs()
+        general = engine.uses_general_tail()
+        ctx.params = params
         ctx.set_materialize_grads(False)
         det = torch.are_deterministic_algorithms_enabled()      # the backward uses the mode this forward saw
         ctx.det = det
@@ -69,14 +71,27 @@ class _OSVOSFunction(torch.autograd.Function):
             acts.append(stage_acts)
         # side_prep has no ReLU: side_prep o (score_dsn, fuse slice) is ONE 3x3 conv C -> 2 (csrc/side_conv.cu), all four
         # scales in one launch; its backward needs neither the 16 features nor their gradient (csrc/side_bwd_folded.cu)
-        pqs = ops.side_folded_multi([acts[i][-1] for i in range(1, 5)], engine._folded_side_all(), fast=fast)
+        # general deconvolution weights: the 16 side features themselves feed the tail (csrc/tail_general.cu)
+        if general:
+            feats, pqs = engine._side_features([acts[i][-1] for i in range(1, 5)], fast)
+            table = engine._upsampling_table()
+            ctx.general = (feats, pqs, table)
+
+            def tail(**kw):
+                return ops.tail_general_fwd(feats, pqs, table, m.fuse.bias.detach(), n, h, w, **kw)
+        else:
+            pqs = ops.side_folded_multi([acts[i][-1] for i in range(1, 5)], engine._folded_side_all(), fast=fast)
+            ctx.general = None
+
+            def tail(**kw):
+                return ops.tail_fwd(pqs, m.fuse.bias.detach(), n, h, w, **kw)
         ctx.engine = engine
         ctx.dims = (n, h, w)
         ctx.fast = fast
         if getattr(engine, "debug_capture", None) is not None:      # tests: the saved activations of this pass
             engine.debug_capture.update(acts=acts, pooled=pooled)
         if objective is None:
-            out, _ = ops.tail_fwd(pqs, m.fuse.bias.detach(), n, h, w)
+            out, _ = tail()
             ctx.objective = None
             ctx.saved = (xin, acts, pooled)
             return tuple(out[k] for k in range(5))
@@ -85,8 +100,10 @@ class _OSVOSFunction(torch.autograd.Function):
         if label.numel() != n * h * w:
             raise ValueError("objective label must be [N,1,H,W] like the output maps")
         weights = tuple(float(v) for v in weights)
-        out, sums, losses = ops.tail_fwd(pqs, m.fuse.bias.detach(), n, h, w, label=label, loss_weights=weights,
-                                         divisor=divisor, deterministic=det)
+        if general:
+            out, sums, losses = tail(label=label, loss_weights=weights, divisor=divisor)
+        else:
+            out, sums, losses = tail(label=label, loss_weights=weights, divisor=divisor, deterministic=det)
         ctx.objective = (out, label, sums, weights, float(divisor))
         ctx.saved = (xin, acts, pooled)
         maps = tuple(out[k] for k in range(5))
@@ -111,7 +128,7 @@ class _OSVOSFunction(torch.autograd.Function):
             weights = obj[3]
             grads = tuple((True if weights[k] != 0.0 else None) for k in range(5)) if g_total is not None else (None,) * 5
         if all(g is None for g in grads):
-            return (None, None, None) + tuple(None for _ in engine._param_list())
+            return (None, None, None) + tuple(None for _ in ctx.params)
         # ---- weight-gradient plumbing: ONE zeroed arena for all tensor-core wgrad workspaces, ONE finish launch at
         # the end.  In direct mode (engine.accumulate_param_grads_in_place, set by the package's training loops) the
         # finish adds straight into an existing p.grad and the bias column sums are accumulated into p.grad by the
@@ -132,10 +149,17 @@ class _OSVOSFunction(torch.autograd.Function):
                 hs, ws_ = (hs + 1) // 2, (ws_ + 1) // 2
             for c in stage:
                 in_shape[c] = (n, hs, ws_)
-        ws_sizes = [(ops.wgrad_workspace_floats(c.out_channels, c.in_channels, in_shape[c], det) + 3) // 4 * 4
+        general = ctx.general
+        if general is not None:                        # side_prep's weight gradient from the 64-channel dF operand
+            for i, sp in enumerate(m.side_prep):
+                in_shape[sp] = in_shape[convs[i + 1][-1]]
+            wconvs = wconvs + list(m.side_prep)
+        ws_sizes = [(ops.wgrad_workspace_floats(64 if c in m.side_prep else c.out_channels, c.in_channels, in_shape[c],
+                                                det) + 3) // 4 * 4
                     for c in wconvs]
-        # side branch: G [18 C + 2] per scale (rounded up to 16 bytes) behind the wgrad workspaces
-        g_sizes = [(ops.side_folded_wgrad_floats(sp.in_channels) + 3) // 4 * 4 for sp in m.side_prep]
+        # folded side branch: G [18 C + 2] per scale (rounded up to 16 bytes) behind the wgrad workspaces
+        g_sizes = [] if general is not None else [(ops.side_folded_wgrad_floats(sp.in_channels) + 3) // 4 * 4
+                                                  for sp in m.side_prep]
         if det:
             # the per-split slices are written in full: only G needs zeroing
             arena = torch.empty(sum(ws_sizes) + sum(g_sizes), dtype=torch.float32, device=xin.device)
@@ -150,12 +174,21 @@ class _OSVOSFunction(torch.autograd.Function):
         for sz in g_sizes:
             g_of.append(arena[off:off + sz])
             off += sz
-        fresh = [c for c in wconvs if grad_target(c.weight) is None]
-        fresh_buf = torch.empty(sum(c.weight.numel() for c in fresh), dtype=torch.float32, device=xin.device)
+        fresh = [c for c in wconvs if c in m.side_prep or grad_target(c.weight) is None]
+        fresh_buf = torch.empty(sum(c.weight.numel() * (4 if c in m.side_prep else 1) for c in fresh),
+                                dtype=torch.float32, device=xin.device)
         finish_items, off = [], 0
 
         def wgrad(conv, inp, dz_act):
             nonlocal off
+            if conv in m.side_prep:     # dW [64, C, 3, 3] of the zero-padded dF operand: its first 16 rows are side_prep's
+                it = ops.conv3x3_wgrad(inp, dz_act, 64, fast=fast, deferred_ws=ws_of[conv], deterministic=det)
+                nel = 4 * conv.weight.numel()
+                it["dw"], it["accumulate"] = fresh_buf[off:off + nel].view(64, *conv.weight.shape[1:]), False
+                off += nel
+                pg[conv.weight] = it["dw"][:16]
+                finish_items.append(it)
+                return
             it = ops.conv3x3_wgrad(inp, dz_act, conv.out_channels, fast=fast, deferred_ws=ws_of[conv], deterministic=det)
             tgt = grad_target(conv.weight)
             if tgt is not None:
@@ -168,7 +201,22 @@ class _OSVOSFunction(torch.autograd.Function):
                 pg[conv.weight] = it["dw"]
             finish_items.append(it)
 
-        if obj is not None:
+        if general is not None:
+            feats, pqs, table = general
+            score_ws = [sd.weight for sd in m.score_dsn]
+            if obj is not None:
+                out, label, sums, weights, divisor = obj
+                dfs, reds, fb = ops.tail_general_bwd(
+                    feats, pqs, score_ws, table, n, h, w, fast,
+                    objective=(out, label, sums, weights, divisor, g_total.detach().contiguous().float()),
+                    want_fuse_bias=grads[4] is not None)
+                if fb is not None:
+                    pg[m.fuse.bias] = fb.reshape(m.fuse.bias.shape)
+            else:
+                dfs, reds, _ = ops.tail_general_bwd(feats, pqs, score_ws, table, n, h, w, fast, grads=list(grads))
+                if grads[4] is not None:
+                    pg[m.fuse.bias] = ops.sum_f32(grads[4], deterministic=det).reshape(m.fuse.bias.shape)
+        elif obj is not None:
             # tail + loss backward in ONE launch: dL/dlogit is formed on the fly (never written), d fuse.bias comes from
             # the forward's sums
             out, label, sums, weights, divisor = obj
@@ -193,58 +241,90 @@ class _OSVOSFunction(torch.autograd.Function):
 
         def bias_grad(c):                              # None: already accumulated into c.bias.grad
             return None if c in bias_direct else bias_slices[c]
-        # every parameter gradient of the side branch from G[t][o][c] = sum_px dpq[px - t][o] x[px][c] (one pass over
-        # the stage output per scale) and one finish launch for the four scales
-        fold = engine._folded_side_all()
-        side_params = [m.fuse.weight] if grads[4] is not None else []
-        for i in range(4):
-            side_params += [m.side_prep[i].weight, m.side_prep[i].bias]
-            if grads[i] is not None:
-                side_params += [m.score_dsn[i].weight, m.score_dsn[i].bias]
-        in_place = all(grad_target(p) is not None for p in side_params)
-        if not in_place:
-            fresh_small = torch.zeros(4 * 34 + 64, dtype=torch.float32, device=xin.device)
-            fresh_side = torch.empty(sum(sp.weight.numel() for sp in m.side_prep), dtype=torch.float32,
-                                     device=xin.device)
-        ops.side_folded_wgrad_multi([acts[i + 1][-1] for i in range(4)], dpq, g_of, deterministic=det)   # G, one launch
-        entries, off_side = [], 0
-        for i in range(4):
-            sp, sd = m.side_prep[i], m.score_dsn[i]
-            e = {"g": g_of[i], "side_w": sp.weight.detach(), "side_b": sp.bias.detach(), "proj_w": engine._proj(i),
-                 "c": sp.in_channels}
-            if in_place:
-                e["d_side_w"], e["d_side_b"] = sp.weight.grad, sp.bias.grad
-                pg[sp.weight] = pg[sp.bias] = None
+        if general is not None:
+            # every parameter gradient of the tail from H, gA and the source sums (one launch); side_prep's weight
+            # gradient comes from the tensor-core wgrad below, its data gradient from a dgrad conv 16 -> C
+            learn = bool(getattr(m, "learn_upsampling", False))
+            small = torch.zeros(64 + 4 * 33, dtype=torch.float32, device=xin.device)
+            d_up = [torch.empty_like(l.weight) for l in m.upscale] if learn else None
+            d_up1 = [torch.empty_like(l.weight) for l in m.upscale_] if learn else None
+            d_score_w = [small[64 + 33 * i:80 + 33 * i] if grads[i] is not None else None for i in range(4)]
+            d_score_b = [small[80 + 33 * i:81 + 33 * i] if grads[i] is not None else None for i in range(4)]
+            d_side_b = [small[81 + 33 * i:97 + 33 * i] for i in range(4)]
+            ops.upsampling_grads_finish(reds, [l.weight for l in m.upscale], m.fuse.weight, d_up, d_up1,
+                                        small[:64] if grads[4] is not None else None, d_score_w, d_score_b, d_side_b)
+            if grads[4] is not None:
+                pg[m.fuse.weight] = small[:64].view(m.fuse.weight.shape)
+            for i in range(4):
+                pg[m.side_prep[i].bias] = d_side_b[i]
                 if grads[i] is not None:
-                    e["d_score_w"], e["d_score_b"] = sd.weight.grad, sd.bias.grad
-                    pg[sd.weight] = pg[sd.bias] = None
-                if grads[4] is not None:
-                    e["d_fuse_w"] = m.fuse.weight.grad.view(-1)[16 * i:16 * i + 16]
-                    pg[m.fuse.weight] = None
-            else:
-                nel = sp.weight.numel()
-                e["d_side_w"] = fresh_side[off_side:off_side + nel].view(sp.weight.shape)
-                off_side += nel
-                small = fresh_small[34 * i:34 * i + 34]
-                e["d_side_b"] = small[0:16]
-                pg[sp.weight], pg[sp.bias] = e["d_side_w"], e["d_side_b"]
+                    pg[m.score_dsn[i].weight] = d_score_w[i].view(m.score_dsn[i].weight.shape)
+                    pg[m.score_dsn[i].bias] = d_score_b[i].view(m.score_dsn[i].bias.shape)
+                if learn and grads[4] is not None:
+                    pg[m.upscale[i].weight] = d_up[i]
+                if learn and grads[i] is not None:
+                    pg[m.upscale_[i].weight] = d_up1[i]
+                wgrad(m.side_prep[i], acts[i + 1][-1], dfs[i])
+        else:
+            # every parameter gradient of the side branch from G[t][o][c] = sum_px dpq[px - t][o] x[px][c] (one pass over
+            # the stage output per scale) and one finish launch for the four scales
+            fold = engine._folded_side_all()
+            side_params = [m.fuse.weight] if grads[4] is not None else []
+            for i in range(4):
+                side_params += [m.side_prep[i].weight, m.side_prep[i].bias]
                 if grads[i] is not None:
-                    e["d_score_w"], e["d_score_b"] = small[16:32], small[32:33]
-                    pg[sd.weight] = e["d_score_w"].view(sd.weight.shape)
-                    pg[sd.bias] = e["d_score_b"].view(sd.bias.shape)
-                if grads[4] is not None:
-                    e["d_fuse_w"] = fresh_small[136 + 16 * i:136 + 16 * i + 16]
-            entries.append(e)
-        if not in_place and grads[4] is not None:
-            pg[m.fuse.weight] = fresh_small[136:200].view(m.fuse.weight.shape)
-        ops.side_grads_finish(entries, accumulate=in_place)
+                    side_params += [m.score_dsn[i].weight, m.score_dsn[i].bias]
+            in_place = all(grad_target(p) is not None for p in side_params)
+            if not in_place:
+                fresh_small = torch.zeros(4 * 34 + 64, dtype=torch.float32, device=xin.device)
+                fresh_side = torch.empty(sum(sp.weight.numel() for sp in m.side_prep), dtype=torch.float32,
+                                         device=xin.device)
+            ops.side_folded_wgrad_multi([acts[i + 1][-1] for i in range(4)], dpq, g_of, deterministic=det)   # G, one launch
+            entries, off_side = [], 0
+            for i in range(4):
+                sp, sd = m.side_prep[i], m.score_dsn[i]
+                e = {"g": g_of[i], "side_w": sp.weight.detach(), "side_b": sp.bias.detach(), "proj_w": engine._proj(i),
+                     "c": sp.in_channels}
+                if in_place:
+                    e["d_side_w"], e["d_side_b"] = sp.weight.grad, sp.bias.grad
+                    pg[sp.weight] = pg[sp.bias] = None
+                    if grads[i] is not None:
+                        e["d_score_w"], e["d_score_b"] = sd.weight.grad, sd.bias.grad
+                        pg[sd.weight] = pg[sd.bias] = None
+                    if grads[4] is not None:
+                        e["d_fuse_w"] = m.fuse.weight.grad.view(-1)[16 * i:16 * i + 16]
+                        pg[m.fuse.weight] = None
+                else:
+                    nel = sp.weight.numel()
+                    e["d_side_w"] = fresh_side[off_side:off_side + nel].view(sp.weight.shape)
+                    off_side += nel
+                    small = fresh_small[34 * i:34 * i + 34]
+                    e["d_side_b"] = small[0:16]
+                    pg[sp.weight], pg[sp.bias] = e["d_side_w"], e["d_side_b"]
+                    if grads[i] is not None:
+                        e["d_score_w"], e["d_score_b"] = small[16:32], small[32:33]
+                        pg[sd.weight] = e["d_score_w"].view(sd.weight.shape)
+                        pg[sd.bias] = e["d_score_b"].view(sd.bias.shape)
+                    if grads[4] is not None:
+                        e["d_fuse_w"] = fresh_small[136 + 16 * i:136 + 16 * i + 16]
+                entries.append(e)
+            if not in_place and grads[4] is not None:
+                pg[m.fuse.weight] = fresh_small[136:200].view(m.fuse.weight.shape)
+            ops.side_grads_finish(entries, accumulate=in_place)
         dpool = None
         for i in range(4, 0, -1):
             s_out = acts[i][-1]
             last_bias = bias_slices[convs[i][-1]]
             # ReLU'(x) * (unpool(dpool) + side gradient), the latter formed on the fly from dpq and the fp32 folded weights
             # (18 FMAs per element); deepest stage: dpool None, the side branch is the only consumer
-            dz = ops.unpool_side_mask(dpool, s_out, dpq[i - 1], fold[i - 1][2], colsum=last_bias, deterministic=det)
+            if general is not None:
+                sp = m.side_prep[i - 1]
+                _, dside, _ = ops.conv3x3(dfs[i - 1], engine._packed(sp, f"sp{i}", transpose_flip=True), None,
+                                          sp.in_channels, fast=fast, out_act=False, out_f32=True)
+                dz = ops.unpool_dside_mask(dpool, s_out, dside, colsum=last_bias, deterministic=det)
+            else:
+                dz = ops.unpool_side_mask(dpool, s_out, dpq[i - 1], fold[i - 1][2], colsum=last_bias,
+                                          deterministic=det)
             for j in range(len(convs[i]) - 1, -1, -1):
                 conv = convs[i][j]
                 inp = acts[i][j - 1] if j > 0 else pooled[i]
@@ -269,7 +349,10 @@ class _OSVOSFunction(torch.autograd.Function):
         ops.wgrad_finish(finish_items)
         ctx.saved = None
         ctx.objective = None
-        return (None, dx, None) + tuple(pg.get(p) for p in engine._param_list())
+        params = ctx.params
+        ctx.params = None
+        ctx.general = None
+        return (None, dx, None) + tuple(pg.get(p) for p in params)
 
 
 def osvos_apply(engine, x):

@@ -598,6 +598,26 @@ extern "C" int osvos_unpool_side_mask(const void* dpool_hi, const void* dpool_lo
   return launch_unpool<false, true>(nullptr, nullptr, x_hi, x_lo, nullptr, dpq, wfold, dz_hi, dz_lo, colsum, n, h, w, c, stream);
 }
 
+extern "C" int osvos_unpool_dside_mask(const void* dpool_hi, const void* dpool_lo, const void* x_hi, const void* x_lo,
+                                       const float* dside, void* dz_hi, void* dz_lo, float* colsum, int n, int h, int w,
+                                       int c, int flags, osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(x_hi != nullptr && dz_hi != nullptr && dside != nullptr && n > 0 && h > 0 && w > 0 && c % 8 == 0);
+  OSVOS_CHECK_ARG(c <= 2048 && 256 % (c / 8) == 0);
+  OSVOS_CHECK_ARG((flags & ~OSVOS_FLAG_DETERMINISTIC) == 0);
+  OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(dside) & 15) == 0);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const bool det = (flags & OSVOS_FLAG_DETERMINISTIC) != 0;
+  if (dpool_hi != nullptr)
+    return det ? launch_unpool<true, false, true>(dpool_hi, dpool_lo, x_hi, x_lo, dside, nullptr, nullptr, dz_hi, dz_lo,
+                                                  colsum, n, h, w, c, stream)
+               : launch_unpool<true, false>(dpool_hi, dpool_lo, x_hi, x_lo, dside, nullptr, nullptr, dz_hi, dz_lo, colsum,
+                                            n, h, w, c, stream);
+  return det ? launch_unpool<false, false, true>(nullptr, nullptr, x_hi, x_lo, dside, nullptr, nullptr, dz_hi, dz_lo, colsum,
+                                                 n, h, w, c, stream)
+             : launch_unpool<false, false>(nullptr, nullptr, x_hi, x_lo, dside, nullptr, nullptr, dz_hi, dz_lo, colsum, n, h,
+                                           w, c, stream);
+}
+
 extern "C" size_t osvos_sum_f32_deterministic_scratch_bytes(void) { return (kSumBlocks + 1) * sizeof(float); }
 
 extern "C" int osvos_sum_f32_deterministic(const float* x, size_t n, void* scratch, float* out, osvos_stream_t stream_) {

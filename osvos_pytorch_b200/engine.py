@@ -82,8 +82,10 @@ class OSVOSEngine:
                             lambda: ops.pack_conv3x3_weights(conv.weight, transpose_flip, col_pad))
 
     def _tensor_core_convs(self):
-        """(conv module, cache key) of every trunk 3x3 conv that runs on the packed tensor-core path (conv1_1 takes its
-        OIHW weights directly; side_prep is folded with its 1x1 projections instead)."""
+        """(conv module, cache key) of every 3x3 conv that runs on the packed tensor-core path: the trunk convs (conv1_1
+        takes its OIHW weights directly) and, when the general tail runs (uses_general_tail), the four side_prep convs,
+        whose forward and data-gradient convolutions then read packed layouts too.  On the folded path side_prep is
+        folded with its 1x1 projections instead (engine._folded_side_all) and has no packed layout."""
         m = self.m
         out = []
         for i in range(5):
@@ -92,7 +94,9 @@ class OSVOSEngine:
                 if i == 0 and j == 0:
                     continue
                 out.append((conv, f"s{i}c{j}"))
-        return out                # (side_prep runs folded with its projections: engine._folded_side_all)
+        if self.uses_general_tail():
+            out += [(sp, f"sp{i + 1}") for i, sp in enumerate(m.side_prep)]
+        return out
 
     def packed_weight_table(self):
         """[(weight Parameter, forward layout, transposed+flipped layout)] of the tensor-core convs, packed now if
@@ -121,10 +125,13 @@ class OSVOSEngine:
             del self._pack_cache[k]
 
     def _param_list(self):
-        """Parameters the native path differentiates (everything except the fixed deconvolution taps)."""
+        """Parameters the native path differentiates: everything, the eight deconvolution weights only when the module
+        learns its upsampling (otherwise they are fixed taps and their .grad stays None)."""
         m = self.m
+        extra = ([l.weight for l in m.upscale] + [l.weight for l in m.upscale_]
+                 if getattr(m, "learn_upsampling", False) else [])
         return ([p for p in m.stages.parameters()] + [p for p in m.side_prep.parameters()]
-                + [p for p in m.score_dsn.parameters()] + [m.fuse.weight, m.fuse.bias])
+                + [p for p in m.score_dsn.parameters()] + [m.fuse.weight, m.fuse.bias] + extra)
 
     def _proj(self, i):
         m = self.m
@@ -144,24 +151,51 @@ class OSVOSEngine:
             [(m.side_prep[i].weight, m.side_prep[i].bias.detach(), self._proj(i), m.score_dsn[i].bias.detach())
              for i in range(4)]))
 
-    def _check_deconvs(self):
-        """The native tail implements the bilinear deconvolution in closed form; both entry points of
-        the reference keep these weights fixed (lr = 0, train_online.py:84-85, train_parent.py:99-100).
-        Anything else is refused loudly rather than computed wrongly."""
+    def _deconvs_bilinear(self):
+        """True when the eight deconvolution weights are the fixed bilinear taps interp_surgery writes (reference
+        layers/osvos_layers.py:72-85), the only weights the folded tail implements.  Checked once per weight version
+        (a host sync), never inside a graph capture: the eager warm-up before each capture fills the cache."""
         m = self.m
         for name, lst in (("upscale", m.upscale), ("upscale_", m.upscale_)):
             for i, lay in enumerate(lst):
                 w = lay.weight
                 key = (name, i)
                 ver = (w.data_ptr(), w._version)
-                if self._deconv_checked.get(key) == ver:
-                    continue
-                ref = bilinear_deconv_weight(w.shape[0], w.shape[1], w.shape[2]).to(w.device)
-                if tuple(w.shape[2:]) != (2 ** (i + 2),) * 2 or not torch.equal(w.detach().float(), ref):
-                    raise NotImplementedError(
-                        f"{name}.{i}.weight is not the fixed bilinear interpolation kernel written by interp_surgery; "
-                        "the native path only implements that (reference layers/osvos_layers.py:72-85)")
-                self._deconv_checked[key] = ver
+                hit = self._deconv_checked.get(key)
+                if hit is None or hit[0] != ver:
+                    ref = bilinear_deconv_weight(w.shape[0], w.shape[1], w.shape[2]).to(w.device)
+                    ok = tuple(w.shape[2:]) == (2 ** (i + 2),) * 2 and torch.equal(w.detach().float(), ref)
+                    hit = self._deconv_checked[key] = (ver, ok)
+                if not hit[1]:
+                    return False
+        return True
+
+    def uses_general_tail(self):
+        """Which tail runs: the general one (csrc/tail_general.cu, DESIGN.md §20) when the module learns its upsampling
+        or its deconvolution weights are not the bilinear taps, else the folded one (tail.cu).  With learn_upsampling the
+        weight check is skipped, so a training step does not wait for the host."""
+        return bool(getattr(self.m, "learn_upsampling", False)) or not self._deconvs_bilinear()
+
+    def _upsampling_table(self):
+        """V (upscale[k] folded with its slice of fuse.weight) and the upscale_[k] taps in one table, cached on the
+        versions of the nine weights that enter (an optimizer step re-folds)."""
+        m = self.m
+        deps = [m.fuse.weight] + [l.weight for l in m.upscale] + [l.weight for l in m.upscale_]
+        return self._cached(("upsampling",), deps, lambda: ops.upsampling_fold(
+            [l.weight for l in m.upscale], [l.weight for l in m.upscale_], m.fuse.weight))
+
+    def _side_features(self, stage_outs, fast):
+        """(feats, pqs) of the four scales for the general tail: side_prep's 16 fp32 features and their projections."""
+        m = self.m
+        feats, pqs = [], []
+        for i, full in enumerate(stage_outs):
+            sp = m.side_prep[i]
+            _, feat, pq = ops.conv3x3(full, self._packed(sp, f"sp{i + 1}"), sp.bias.detach(), 16, relu=False, fast=fast,
+                                      out_act=False, out_f32=True, proj_w=self._proj(i),
+                                      proj_b=m.score_dsn[i].bias.detach())
+            feats.append(feat)
+            pqs.append(pq)
+        return feats, pqs
 
     # ----------------------------------------------------------------- forward
     def forward(self, x, fresh_outputs=True):
@@ -217,7 +251,7 @@ class OSVOSEngine:
             self._graphs.clear()
             self._buffers_seen.clear()
             self._graphs_pver = pver
-        pkey = (tuple(x.shape), x.device.index, m.precision)
+        pkey = (tuple(x.shape), x.device.index, (m.precision, self.uses_general_tail()))
         direct_ok = x.dtype == torch.float32 and x.is_contiguous() and not x.requires_grad
         entry = None
         if direct_ok:
@@ -277,7 +311,7 @@ class OSVOSEngine:
     def _forward_inference(self, x, simt=False, return_intermediates=False):
         m = self.m
         fast = m.precision == "fast"
-        self._check_deconvs()
+        general = self.uses_general_tail()
         x = x.detach().contiguous().float()
         n, _, h, w = (int(v) for v in x.shape)
         inter = {}
@@ -299,8 +333,8 @@ class OSVOSEngine:
         pqs = []
         # side_prep o (score_dsn, fuse slice) folded into one 3x3 conv C -> 2 (include/osvos_b200.h), the four scales in
         # ONE launch after the last trunk conv; the side features themselves are only computed on request
-        fold = not simt and not return_intermediates
-        stage_outs = []
+        fold = not simt and not return_intermediates and not general
+        stage_outs, feats = [], []
         for i in range(1, 5):
             convs = [c for c in m.stages[i] if isinstance(c, nn.Conv2d)]
             for j, conv in enumerate(convs):
@@ -325,15 +359,19 @@ class OSVOSEngine:
                 continue
             else:
                 _, feat, pq = ops.conv3x3(full, self._packed(sp, f"sp{i}"), sp.bias.detach(), 16, relu=False, fast=fast,
-                                          out_act=False, out_f32=return_intermediates, proj_w=self._proj(i - 1),
-                                          proj_b=m.score_dsn[i - 1].bias.detach())
+                                          out_act=False, out_f32=return_intermediates or general,
+                                          proj_w=self._proj(i - 1), proj_b=m.score_dsn[i - 1].bias.detach())
+            feats.append(feat)
             if return_intermediates:
                 inter[f"side{i}"] = feat
                 inter[f"pq{i}"] = pq
             pqs.append(pq)
         if fold:
             pqs = ops.side_folded_multi(stage_outs, self._folded_side_all(), fast=fast)
-        out, _ = ops.tail_fwd(pqs, m.fuse.bias.detach(), n, h, w)
+        if general:
+            out, _ = ops.tail_general_fwd(feats, pqs, self._upsampling_table(), m.fuse.bias.detach(), n, h, w)
+        else:
+            out, _ = ops.tail_fwd(pqs, m.fuse.bias.detach(), n, h, w)
         outs = [out[k] for k in range(5)]
         if return_intermediates:
             return outs, inter

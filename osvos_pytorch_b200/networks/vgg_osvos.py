@@ -33,11 +33,15 @@ def _make_stage(has_pool, cin, widths):
 class OSVOS(nn.Module):
     """Drop-in for the reference ``OSVOS`` module.
 
-    Extra keyword (not in the reference): ``precision`` = "exact" (default; split
-    bf16, three tensor-core passes, fp32-class results) or "fast" (one bf16 pass).
+    Extra keywords (not in the reference): ``precision`` = "exact" (default; split
+    bf16, three tensor-core passes, fp32-class results) or "fast" (one bf16 pass);
+    ``learn_upsampling`` (default False, also a plain attribute that may be set after
+    load_state_dict): backward writes the gradients of the eight deconvolution weights
+    (upscale / upscale_), as the reference's autograd does.  Deconvolution weights other
+    than interp_surgery's bilinear taps run with or without it (DESIGN.md §20).
     """
 
-    def __init__(self, pretrained=1, precision="exact", verbose=True):
+    def __init__(self, pretrained=1, precision="exact", verbose=True, learn_upsampling=False):
         super().__init__()
         if verbose:
             print("Constructing OSVOS architecture..")
@@ -63,6 +67,7 @@ class OSVOS(nn.Module):
             print("Initializing weights..")
         self._initialize_weights(pretrained, verbose)
         self.precision = precision
+        self.learn_upsampling = bool(learn_upsampling)
         self._engine = OSVOSEngine(self)
 
     # ------------------------------------------------------------------ forward

@@ -334,6 +334,154 @@ def tail_loss_bwd(out, label, sums, loss_weights, divisor, upstream, n, h, w, wa
     return dpq, fb
 
 
+def upsampling_fold(upscale_ws, upscale1_ws, fuse_w):
+    """The eight deconvolution weights and fuse.weight -> one fp32 table [17 * UPSAMPLING_TAPS]: V [taps][16] (each
+    upscale[k] folded with its slice of fuse), then A [taps] (the upscale_[k] taps); osvos_upsampling_fold."""
+    lib = nat.load()
+    ws = [w.detach().contiguous().float() for w in list(upscale_ws) + list(upscale1_ws) + [fuse_w]]
+    for k in range(4):
+        t = 4 << k
+        if tuple(ws[k].shape) != (16, 16, t, t) or tuple(ws[4 + k].shape) != (1, 1, t, t):
+            raise ValueError(f"upscale[{k}] / upscale_[{k}] must be [16,16,{t},{t}] / [1,1,{t},{t}], got "
+                             f"{tuple(ws[k].shape)} / {tuple(ws[4 + k].shape)}")
+    taps = nat.UPSAMPLING_TAPS
+    tab = torch.empty(17 * taps, dtype=torch.float32, device=fuse_w.device)
+    a = nat.UpsamplingFoldArgs()
+    for k in range(4):
+        a.upscale_w[k], a.upscale1_w[k] = ws[k].data_ptr(), ws[4 + k].data_ptr()
+    a.fuse_w, a.vtab, a.atab = ws[8].data_ptr(), tab.data_ptr(), tab[16 * taps:].data_ptr()
+    _count()
+    nat.check(lib.osvos_upsampling_fold(byref(a), _stream()), "osvos_upsampling_fold")
+    return tab
+
+
+def tail_general_fwd(feats, pqs, table, fuse_bias, n, h, w, label=None, loss_weights=None, divisor=None):
+    """tail_fwd with general deconvolution weights: the four 16-channel side features, their pq (p in channel 0) and
+    the upsampling_fold table -> (out [5,n,1,h,w], sums | None[, losses [6]]) with tail_fwd's contract."""
+    lib = nat.load()
+    dev = feats[0].device
+    per = (n * h * w + 3) // 4 * 4
+    out = torch.empty((5, per), dtype=torch.float32, device=dev)[:, :n * h * w].view(5, n, 1, h, w)
+    sums = torch.empty(lib.osvos_tail_general_fwd_sums(n, h, w), dtype=torch.float64, device=dev) \
+        if label is not None else None
+    a = nat.TailGeneralFwdArgs()
+    for k in range(4):
+        a.feat[k], a.pq[k] = feats[k].data_ptr(), pqs[k].data_ptr()
+    for k in range(5):
+        a.out[k] = out[k].data_ptr()
+    taps = nat.UPSAMPLING_TAPS
+    a.vtab, a.atab = table.data_ptr(), table[16 * taps:].data_ptr()
+    a.fuse_bias, a.label, a.sums = nat.ptr(fuse_bias), nat.ptr(label), nat.ptr(sums)
+    losses = None
+    if loss_weights is not None:
+        if label is None or divisor is None:
+            raise ValueError("tail_general_fwd: loss_weights needs label and divisor")
+        losses = torch.empty(6, dtype=torch.float32, device=dev)
+        a.losses = losses.data_ptr()
+        for k in range(5):
+            a.loss_weights[k] = float(loss_weights[k])
+        a.divisor = float(divisor)
+    a.n, a.h, a.w = n, h, w
+    _count(2 if label is not None else 1)
+    nat.check(lib.osvos_tail_general_fwd(byref(a), _stream()), "osvos_tail_general_fwd")
+    if losses is not None:
+        return out, sums, losses
+    return out, sums
+
+
+def tail_general_bwd(feats, pqs, score_ws, table, n, h, w, fast=False, grads=None, objective=None,
+                     want_fuse_bias=False):
+    """Backward of tail_general_fwd (osvos_tail_general_bwd): from the five gradient maps `grads` (None entries are
+    zero), or with `objective` = (logits [5,n,1,h,w], label, sums, loss_weights, divisor, upstream) from dL/dlogit
+    formed on the fly -> (dF acts [n,hk,wk,64] per scale, reduced rows per scale, fuse.bias gradient [1] | None)."""
+    lib = nat.load()
+    dev = feats[0].device
+    a = nat.TailGeneralBwdArgs()
+    taps = nat.UPSAMPLING_TAPS
+    a.vtab, a.atab = table.data_ptr(), table[16 * taps:].data_ptr()
+    keep, dfs, reds = [], [], []
+    for k in range(4):
+        a.feat[k], a.pq[k] = feats[k].data_ptr(), pqs[k].data_ptr()
+        sw = score_ws[k].detach().contiguous().float()
+        keep.append(sw)
+        a.score_w[k] = sw.data_ptr()
+        _, hk, wk, _ = feats[k].shape
+        df = Act.empty(n, hk, wk, 64, dev, fast)
+        dfs.append(df)
+        a.df_hi[k], a.df_lo[k] = df.hi.data_ptr(), nat.ptr(df.lo)
+        t = (4 << k) ** 2
+        red = torch.empty(17 * t + 33, dtype=torch.float32, device=dev)
+        reds.append(red)
+        a.red[k] = red.data_ptr()
+    fb = None
+    if objective is not None:
+        logits, label, sums, weights, divisor, upstream = objective
+        for k in range(5):
+            a.src[k] = logits[k].data_ptr()
+            a.loss_weights[k] = float(weights[k])
+        a.label, a.sums, a.upstream = label.data_ptr(), sums.data_ptr(), nat.ptr(upstream)
+        a.divisor = float(divisor)
+        if want_fuse_bias:
+            fb = torch.empty(1, dtype=torch.float32, device=dev)
+            a.fuse_bias_grad = fb.data_ptr()
+    else:
+        for k in range(5):
+            g = grads[k]
+            if g is not None:
+                g = g.contiguous().float()
+                keep.append(g)
+            a.src[k] = nat.ptr(g)
+    ws = torch.empty((lib.osvos_tail_general_bwd_workspace_bytes(n, h, w) + 3) // 4, dtype=torch.float32, device=dev)
+    a.workspace = ws.data_ptr()
+    a.n, a.h, a.w = n, h, w
+    _count(9)
+    nat.check(lib.osvos_tail_general_bwd(byref(a), _stream()), "osvos_tail_general_bwd")
+    return dfs, reds, fb
+
+
+def upsampling_grads_finish(reds, upscale_ws, fuse_w, d_upscale=None, d_upscale1=None, d_fuse_w=None, d_score_w=None,
+                            d_score_b=None, d_side_b=None, accumulate=False):
+    """Every tail parameter gradient from the reduced rows of tail_general_bwd, one launch
+    (osvos_upsampling_grads_finish).  The d_* arguments are lists of four tensors / None (d_fuse_w: one [64] tensor)."""
+    lib = nat.load()
+    a = nat.UpsamplingGradsArgs()
+    none4 = [None] * 4
+    keep = [u.detach().contiguous().float() for u in upscale_ws] + [fuse_w.detach().contiguous().float()]
+    for k in range(4):
+        a.red[k], a.upscale_w[k] = reds[k].data_ptr(), keep[k].data_ptr()
+        a.d_upscale_w[k] = nat.ptr((d_upscale or none4)[k])
+        a.d_upscale1_w[k] = nat.ptr((d_upscale1 or none4)[k])
+        a.d_score_w[k] = nat.ptr((d_score_w or none4)[k])
+        a.d_score_b[k] = nat.ptr((d_score_b or none4)[k])
+        a.d_side_b[k] = nat.ptr((d_side_b or none4)[k])
+    a.fuse_w, a.d_fuse_w = keep[4].data_ptr(), nat.ptr(d_fuse_w)
+    a.accumulate = 1 if accumulate else 0
+    _count()
+    nat.check(lib.osvos_upsampling_grads_finish(byref(a), _stream()), "osvos_upsampling_grads_finish")
+
+
+def unpool_dside_mask(dpool, x, dside, colsum=None, deterministic=False):
+    """dz = ReLU'(x) * (unpool(dpool) + dside) with an fp32 side gradient map [n,h,w,c]; dpool None: the deepest
+    stage (osvos_unpool_dside_mask)."""
+    lib = nat.load()
+    n, h, w, c = x.shape
+    dz = Act.empty(n, h, w, c, x.hi.device, x.lo is None)
+    rows = None
+    if deterministic and colsum is not None:
+        nrows = lib.osvos_unpool_colsum_rows(n, h, w, c, int(dpool is not None), 0)
+        rows = torch.empty((nrows, c), dtype=torch.float32, device=x.hi.device)
+    _count()
+    nat.check(lib.osvos_unpool_dside_mask(dpool.hi.data_ptr() if dpool is not None else None,
+                                          nat.ptr(dpool.lo) if dpool is not None else None, x.hi.data_ptr(),
+                                          nat.ptr(x.lo), dside.data_ptr(), dz.hi.data_ptr(), nat.ptr(dz.lo),
+                                          nat.ptr(rows if rows is not None else colsum), n, h, w, c,
+                                          nat.FLAG_DETERMINISTIC if deterministic else 0, _stream()),
+              "osvos_unpool_dside_mask")
+    if rows is not None:
+        reduce_rows(rows, colsum, accumulate=True)
+    return dz
+
+
 # ------------------------------------------------------------------ backward ops
 def wgrad_workspace_floats(dz_channels, cin, shape=None, deterministic=False):
     """Workspace of one weight gradient; ``deterministic`` (needs ``shape`` = (n, h, w)): one slice per pixel-range

@@ -68,8 +68,10 @@ class GradientBucket:
 
 
 def trainable_parameters(net):
-    """Everything except the fixed bilinear deconvolution taps (upscale / upscale_)."""
-    return [p for name, p in net.named_parameters() if not name.startswith("upscale")]
+    """Everything except the deconvolution taps (upscale / upscale_), which are trainable only when the net has
+    ``learn_upsampling`` set (backward writes their gradients then)."""
+    learn = bool(getattr(net, "learn_upsampling", False))
+    return [p for name, p in net.named_parameters() if learn or not name.startswith("upscale")]
 
 
 def broadcast_parameters(module, src=0, group=None):

@@ -14,11 +14,17 @@ def _named(module, key):
     return [p for n, p in module.named_parameters() if key in n]
 
 
-def make_optimizer(net, mode, lr=1e-8, wd=0.0002, momentum=0.9, fused=False):
+def make_optimizer(net, mode, lr=1e-8, wd=0.0002, momentum=0.9, fused=False, upsampling_lr=0.0):
     """SGD with the reference's parameter groups (``fused``: optim.FusedSGD - one launch per step, packed conv
     layouts re-emitted in the same pass - instead of torch.optim.SGD).
     online (train_online.py:77-88): stages / side_prep weights (wd) and biases (2 lr), deconvs lr 0,
-    fuse at lr/100; score_dsn is NOT optimised.  parent (train_parent.py:85-103): additionally score_dsn at lr/10."""
+    fuse at lr/100; score_dsn is NOT optimised.  parent (train_parent.py:85-103): additionally score_dsn at lr/10.
+    ``upsampling_lr``: the lr of the two deconvolution groups (the reference's 0 by default; weight decay stays 0).  It
+    only moves the weights when the net has ``learn_upsampling`` set, which makes backward write their gradients; a
+    nonzero value on a net without it is refused rather than ignored."""
+    if upsampling_lr != 0.0 and not getattr(net, "learn_upsampling", False):
+        raise ValueError("upsampling_lr != 0 needs net.learn_upsampling = True: without it backward writes no gradient "
+                         "for upscale / upscale_ and the optimizer would leave them unchanged")
     groups = [
         {"params": _named(net.stages, "weight"), "weight_decay": wd, "initial_lr": lr},
         {"params": _named(net.stages, "bias"), "lr": 2 * lr, "initial_lr": 2 * lr},
@@ -31,8 +37,8 @@ def make_optimizer(net, mode, lr=1e-8, wd=0.0002, momentum=0.9, fused=False):
             {"params": _named(net.score_dsn, "bias"), "lr": 2 * lr / 10, "initial_lr": 2 * lr / 10},
         ]
     groups += [
-        {"params": _named(net.upscale, "weight"), "lr": 0, "initial_lr": 0},
-        {"params": _named(net.upscale_, "weight"), "lr": 0, "initial_lr": 0},
+        {"params": _named(net.upscale, "weight"), "lr": upsampling_lr, "initial_lr": upsampling_lr},
+        {"params": _named(net.upscale_, "weight"), "lr": upsampling_lr, "initial_lr": upsampling_lr},
         {"params": [net.fuse.weight], "lr": lr / 100, "initial_lr": lr / 100, "weight_decay": wd},
         {"params": [net.fuse.bias], "lr": 2 * lr / 100, "initial_lr": 2 * lr / 100},
     ]
@@ -71,7 +77,8 @@ class GraphedTrainStep:
         self.deterministic = torch.are_deterministic_algorithms_enabled()
         self.x = sample["image"].detach().clone()
         self.gt = sample["gt"].detach().clone()
-        self.params = [p for n, p in net.named_parameters() if not n.startswith("upscale")]
+        from .parallel import trainable_parameters
+        self.params = trainable_parameters(net)
         for p in self.params:
             if p.grad is None:
                 p.grad = torch.zeros_like(p)
@@ -138,7 +145,7 @@ class GraphedTrainStep:
 
 
 def online_finetune(net, sample_fn, iters, n_ave_grad=5, lr=1e-8, wd=0.0002, log_every=0, log=print, use_graph=True,
-                    fused_optimizer=True):
+                    fused_optimizer=True, upsampling_lr=0.0):
     """`iters` forward/backward passes on the annotated frame, SGD step every `n_ave_grad` (reference
     train_online.py:112-149).  Losses are kept on the device; one host read per `log_every` iterations
     instead of the reference's per-iteration .item() sync.  With `use_graph` the fwd+loss+bwd of a micro-batch
@@ -146,7 +153,7 @@ def online_finetune(net, sample_fn, iters, n_ave_grad=5, lr=1e-8, wd=0.0002, log
     the gradient zeroing and the repack of the conv weights are one kernel (optim.FusedSGD).  Returns the list of
     logged losses."""
     net.train()
-    opt = make_optimizer(net, "online", lr, wd, fused=fused_optimizer)
+    opt = make_optimizer(net, "online", lr, wd, fused=fused_optimizer, upsampling_lr=upsampling_lr)
     opt.zero_grad()
     opt_params = [p for g in opt.param_groups for p in g["params"]]
     history, running = [], None

@@ -31,6 +31,9 @@ def parse(argv=None):
     ap.add_argument("--lr", type=float, default=None, help="default 1e-8 (reference); 1e-10 with --synthetic, whose "
                     "He-initialised network produces O(10)-scale logits and therefore much larger summed-loss gradients")
     ap.add_argument("--wd", type=float, default=0.0002)
+    ap.add_argument("--upsampling-lr", type=float, default=0.0,
+                    help="lr of the side-output deconvolutions (upscale / upscale_); 0 keeps them fixed as the reference "
+                         "does, a nonzero value trains them (the net learns its upsampling)")
     ap.add_argument("--deterministic", action="store_true",
                     help="torch.use_deterministic_algorithms(True) before anything is built: the package's kernels "
                          "reduce in a fixed order, so two runs on the same device give bit-identical results")
@@ -92,7 +95,7 @@ def main(argv=None):
     device = torch.device(f"cuda:{a.gpu_id}")
     torch.cuda.set_device(device)
 
-    net = vo.OSVOS(pretrained=0, precision=a.precision)
+    net = vo.OSVOS(pretrained=0, precision=a.precision, learn_upsampling=a.upsampling_lr != 0.0)
     if a.synthetic:
         vo.he_init_(net, seed=a.seed)
         with torch.no_grad():               # keep the synthetic logits O(10): scale the side branch down
@@ -174,7 +177,8 @@ def main(argv=None):
 
     print("Start of Online Training, sequence: " + a.seq_name)
     t0 = timeit.default_timer()
-    history = training.online_finetune(net, sample_fn, iters, a.n_ave_grad, a.lr, a.wd, log_every)
+    history = training.online_finetune(net, sample_fn, iters, a.n_ave_grad, a.lr, a.wd, log_every,
+                                       upsampling_lr=a.upsampling_lr)
     torch.cuda.synchronize()
     dt = timeit.default_timer() - t0
     print(f"Online training time: {dt:.2f} s ({iters / dt:.1f} fwd+bwd/s, {iters / a.n_ave_grad / dt:.1f} SGD steps/s)")

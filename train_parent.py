@@ -44,6 +44,9 @@ def parse(argv=None):
     ap.add_argument("--test-interval", type=int, default=5)
     ap.add_argument("--lr", type=float, default=1e-8)
     ap.add_argument("--wd", type=float, default=0.0002)
+    ap.add_argument("--upsampling-lr", type=float, default=0.0,
+                    help="lr of the side-output deconvolutions (upscale / upscale_); 0 keeps them fixed as the reference "
+                         "does, a nonzero value trains them (the net learns its upsampling)")
     ap.add_argument("--deterministic", action="store_true",
                     help="torch.use_deterministic_algorithms(True) before anything is built: the package's kernels "
                          "reduce in a fixed order, so two runs on the same device give bit-identical results")
@@ -114,16 +117,17 @@ def main(argv=None):
     os.makedirs(save_dir, exist_ok=True)
 
     if a.resume_epoch == 0:
-        net = vo.OSVOS(pretrained=0 if a.synthetic else a.pretrained, precision=a.precision, verbose=rank == 0)
+        net = vo.OSVOS(pretrained=0 if a.synthetic else a.pretrained, precision=a.precision, verbose=rank == 0,
+                       learn_upsampling=a.upsampling_lr != 0.0)
         if a.synthetic:
             vo.he_init_(net, seed=0)
     else:
-        net = vo.OSVOS(pretrained=0, precision=a.precision, verbose=rank == 0)
+        net = vo.OSVOS(pretrained=0, precision=a.precision, verbose=rank == 0, learn_upsampling=a.upsampling_lr != 0.0)
         ckpt = os.path.join(save_dir, f"{a.model_name}_epoch-{a.resume_epoch - 1}.pth")
         net.load_state_dict(torch.load(ckpt, map_location="cpu"))
     net.to(device)
     parallel.broadcast_parameters(net, src=0)        # replicas must be ONE model (the reference's init is unseeded)
-    opt = training.make_optimizer(net, "parent", a.lr, a.wd, fused=True)
+    opt = training.make_optimizer(net, "parent", a.lr, a.wd, fused=True, upsampling_lr=a.upsampling_lr)
     bucket = parallel.GradientBucket(parallel.trainable_parameters(net), device)
 
     stored = False                                   # J and F at the stored size (--input-res --output-res stored)
