@@ -602,7 +602,23 @@ typedef struct osvos_jpeg_args {
 OSVOS_API size_t osvos_jpeg_decode_workspace_bytes(int n, int h, int w, int nseg, size_t blob_bytes, int chunk_bits);
 OSVOS_API int osvos_jpeg_decode(const osvos_jpeg_args* args, osvos_stream_t stream);
 
-/* ---- side-branch tail with general deconvolution weights (DESIGN.md §20) ------------------------------------------
+/* ---- PNG encoding of 8-bit maps (the result files of train_online.py:187, sm.imsave; DESIGN.md §21) ---------------
+ *   osvos_png_encode: src [n][h][w] uint8 (any alignment) -> one complete 8-bit grayscale PNG per frame in
+ *                     out [n][osvos_png_max_bytes(h, w)] (frame i's file is out + i * max_bytes, lengths[i] bytes long;
+ *                     lengths int64 [n], 8-byte aligned).  Colour type 0, bit depth 8, no interlace, no ancillary
+ *                     chunks; the row filter is the least-sum-of-residuals heuristic, the zlib stream uses literals
+ *                     and distance-1 matches in one dynamic-Huffman or stored block per segment of filtered rows,
+ *                     each segment its own IDAT chunk.  The bytes are a function of the frame alone (not of n, the
+ *                     stream or the run).  `workspace`: osvos_png_encode_workspace_bytes(n, h, w) bytes, 16-byte
+ *                     aligned, owned by the caller; nothing is allocated and nothing waits for the host.  n < 65536.
+ *   osvos_png_max_bytes: the per-frame capacity (every segment stored); 0 unless 1 <= h, w <= 32767.
+ *   osvos_png_encode_workspace_bytes: host query; 0 for invalid arguments.                                          */
+OSVOS_API size_t osvos_png_max_bytes(int h, int w);
+OSVOS_API size_t osvos_png_encode_workspace_bytes(int n, int h, int w);
+OSVOS_API int osvos_png_encode(const uint8_t* src, uint8_t* out, int64_t* lengths, void* workspace, int n, int h, int w,
+                               osvos_stream_t stream);
+
+/* ---- side-branch tail with general deconvolution weights (DESIGN.md §20)------------------------------------------
  * The reference's eight ConvTranspose2d layers with ANY weights (networks/vgg_osvos.py:45-46,68-69), their centre crop
  * (layers/osvos_layers.py:51-56), cat + fuse (:71-72) and, with a label, the class-balanced BCE terms
  * (layers/osvos_layers.py:28-41); their autograd at train_online.py:141 / train_parent.py:164, including the gradients

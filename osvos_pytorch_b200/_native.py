@@ -227,6 +227,10 @@ SIGNATURES = {
     "osvos_upsampling_grads_finish": (c_int, [POINTER(UpsamplingGradsArgs), c_void_p]),
     "osvos_unpool_dside_mask": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                         c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    # train_online.py:187 (sm.imsave of each result) on the device
+    "osvos_png_max_bytes": (c_size_t, [c_int, c_int]),
+    "osvos_png_encode_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "osvos_png_encode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
 }
 
 DAVIS_MAX_RADIUS = 31

@@ -43,10 +43,16 @@ class SequenceSegmenter:
     per-slot device buffer (grown when a larger batch arrives: the decode is not captured in a graph, only the
     forward on the fp32 slot is), and the JPEGs are decoded on the compute stream into the slot's bgr8 buffer; from
     there on it is ``frames="bgr8"``.  ``jpeg_status`` (int32 [1] on the device) sums the decoder's status words
-    over the run: nonzero when a stream was corrupt or cut short."""
+    over the run: nonzero when a stream was corrupt or cut short.
+
+    ``encode="png"`` (``output`` bytescale / prob / mask): each uint8 result is encoded on the compute stream
+    (ops.encode_png, DESIGN.md §21) into a per-slot buffer of fixed address, and the whole buffer (the per-frame
+    capacity, so no size is read back first) and the file lengths cross device->host instead of the maps.  Each result
+    is then a list of N ``memoryview``s, each one complete PNG file (what Image.fromarray(map, "L").save writes, other
+    deflate bytes) backed by the pinned slot and valid as long as the maps are without it."""
 
     def __init__(self, net, output="logits", depth=3, frames="nchw_f32", meanval=ops.MEANVAL, score=False,
-                 input_res=None, output_res="network"):
+                 input_res=None, output_res="network", encode=None):
         if output not in ("logits", "bytescale", "prob", "mask"):
             raise ValueError("output must be one of logits / bytescale / prob / mask")
         if frames not in ("nchw_f32", "bgr8", "jpeg"):
@@ -55,12 +61,17 @@ class SequenceSegmenter:
             raise ValueError("input_res resizes the decoded bytes, as imresize does: it needs frames='bgr8' or 'jpeg'")
         if output_res not in ("network", "stored"):
             raise ValueError("output_res must be 'network' or 'stored'")
+        if encode not in (None, "png"):
+            raise ValueError("encode must be None or 'png'")
+        if encode == "png" and output == "logits":
+            raise ValueError("encode='png' writes 8-bit maps: it needs output bytescale, prob or mask")
         self.net, self.output, self.depth = net, output, max(2, int(depth))
         self.frames, self.meanval = frames, tuple(meanval)
         self.score = bool(score)
         self.input_res = input_res
         self.output_res = output_res
         self._upsample = input_res is not None and output_res == "stored"
+        self.encode = encode
         self._shape = None
         self._counts = []
         self.jpeg_status = None
@@ -81,7 +92,14 @@ class SequenceSegmenter:
         rh, rw = (h0, w0) if self._upsample else (h, w)                  # the results' size
         self._dev_in = [torch.empty((n, 3, h, w), dtype=torch.float32, device=device) for _ in range(self.depth)]
         self._dev_out = [torch.empty((n, 1, rh, rw), dtype=out_dtype, device=device) for _ in range(self.depth)]
-        self._host_out = [torch.empty((n, 1, rh, rw), dtype=out_dtype).pin_memory() for _ in range(self.depth)]
+        if self.encode == "png":
+            cap = ops.png_max_bytes(rh, rw)
+            self._dev_png = [torch.empty((n, cap), dtype=torch.uint8, device=device) for _ in range(self.depth)]
+            self._dev_len = [torch.empty(n, dtype=torch.int64, device=device) for _ in range(self.depth)]
+            self._host_png = [torch.empty((n, cap), dtype=torch.uint8).pin_memory() for _ in range(self.depth)]
+            self._host_len = [torch.empty(n, dtype=torch.int64).pin_memory() for _ in range(self.depth)]
+        else:
+            self._host_out = [torch.empty((n, 1, rh, rw), dtype=out_dtype).pin_memory() for _ in range(self.depth)]
         if self._upsample:
             self._dev_up = [torch.empty((n, 1, h0, w0), dtype=torch.float32, device=device) for _ in range(self.depth)]
         if self.score:
@@ -94,6 +112,8 @@ class SequenceSegmenter:
         self._shape = tuple(shape)
         self.h2d_bytes_per_frame = n * 3 * h0 * w0 * (4 if self.frames == "nchw_f32" else 1) + (n * h0 * w0 if self.score else 0)
         self.d2h_bytes_per_frame = n * rh * rw * (4 if self.output == "logits" else 1)
+        if self.encode == "png":
+            self.d2h_bytes_per_frame = n * (cap + 8)
 
     def _submit(self, i, frame, gt, device):
         k = i % self.depth
@@ -156,11 +176,24 @@ class SequenceSegmenter:
                 self._dev_out[k].copy_(fused)
             else:
                 ops.logits_to_u8(fused, self.output, out=self._dev_out[k])
+                if self.encode == "png":
+                    ops.encode_png(self._dev_out[k], out=self._dev_png[k], lengths=self._dev_len[k])
         self._ev_done[k].record(cur)
         with torch.cuda.stream(self._s_out):
             self._s_out.wait_event(self._ev_done[k])
-            self._host_out[k].copy_(self._dev_out[k], non_blocking=True)
+            if self.encode == "png":
+                self._host_png[k].copy_(self._dev_png[k], non_blocking=True)
+                self._host_len[k].copy_(self._dev_len[k], non_blocking=True)
+            else:
+                self._host_out[k].copy_(self._dev_out[k], non_blocking=True)
             self._ev_host[k].record(self._s_out)
+
+    def _result(self, k):
+        self._ev_host[k].synchronize()
+        if self.encode != "png":
+            return self._host_out[k]
+        files = self._host_png[k].numpy()
+        return [memoryview(files[j, :int(ln)]) for j, ln in enumerate(self._host_len[k].tolist())]
 
     def __call__(self, frames):
         device = next(self.net.parameters()).device
@@ -183,8 +216,7 @@ class SequenceSegmenter:
                     ready = submitted - self.depth + 1
                     if ready >= 1:
                         k = (ready - 1) % self.depth
-                        self._ev_host[k].synchronize()
-                        yield self._host_out[k]
+                        yield self._result(k)
                     continue
                 frame, gt = item if self.score else (item, None)
                 if frame.dim() == 3:
@@ -207,12 +239,10 @@ class SequenceSegmenter:
                 ready = submitted - self.depth + 1              # keep depth-1 frames in flight
                 if ready >= 1:
                     k = (ready - 1) % self.depth
-                    self._ev_host[k].synchronize()
-                    yield self._host_out[k]
+                    yield self._result(k)
             for j in range(max(0, submitted - self.depth + 1), submitted):
                 k = j % self.depth
-                self._ev_host[k].synchronize()
-                yield self._host_out[k]
+                yield self._result(k)
 
     def frame_counts(self):
         """int32 [frames*N, 6] host tensor of the last run's ops.davis_measures counts, frame order (score=True);

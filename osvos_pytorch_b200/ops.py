@@ -864,6 +864,41 @@ def resize_f32(x, size, out=None):
     return out
 
 
+def png_max_bytes(h, w):
+    """Capacity of one encoded frame (osvos_png_max_bytes): the size with every segment stored."""
+    return int(nat.load().osvos_png_max_bytes(int(h), int(w)))
+
+
+def encode_png(maps, out=None, lengths=None):
+    """uint8 maps [N,H,W] or [N,1,H,W] -> (out uint8 [N, png_max_bytes(H, W)], lengths int64 [N]): frame i's 8-bit
+    grayscale PNG file is out[i, :lengths[i]], what the reference's sm.imsave (train_online.py:187) or
+    Image.fromarray(map, "L").save writes, with other (deterministic) deflate bytes (csrc/png.cu, DESIGN.md §21).
+    No host synchronisation."""
+    lib = nat.load()
+    _require_cuda(maps, "maps")
+    if maps.dtype != torch.uint8 or maps.dim() not in (3, 4) or (maps.dim() == 4 and int(maps.shape[1]) != 1):
+        raise ValueError(f"maps must be uint8 [N,H,W] or [N,1,H,W], got {maps.dtype} {tuple(maps.shape)}")
+    x = maps.contiguous()
+    n, h, w = int(x.shape[0]), int(x.shape[-2]), int(x.shape[-1])
+    cap = lib.osvos_png_max_bytes(h, w)
+    nbytes = lib.osvos_png_encode_workspace_bytes(n, h, w)
+    if cap == 0 or nbytes == 0:
+        raise ValueError(f"cannot encode [{n},{h},{w}]: sizes must lie in [1, 32767] and 0 < N < 65536")
+    if out is None:
+        out = torch.empty((n, cap), dtype=torch.uint8, device=x.device)
+    elif out.dtype != torch.uint8 or tuple(out.shape) != (n, cap) or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous uint8 tensor of shape ({n}, {cap})")
+    if lengths is None:
+        lengths = torch.empty(n, dtype=torch.int64, device=x.device)
+    elif lengths.dtype != torch.int64 or tuple(lengths.shape) != (n,) or not lengths.is_contiguous():
+        raise ValueError(f"lengths must be a contiguous int64 tensor of shape ({n},)")
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    _count(3)
+    nat.check(lib.osvos_png_encode(x.data_ptr(), out.data_ptr(), lengths.data_ptr(), ws.data_ptr(), n, h, w, _stream()),
+              "osvos_png_encode")
+    return out, lengths
+
+
 def davis_measures(logits, gt_u8, r=None, out=None):
     """DAVIS-2016 J and F counts on the device (csrc/measures.cu, DESIGN.md §14): fused logits fp32 [N,1,H,W] or
     [N,H,W] and annotations uint8 [N,H,W] -> int32 [N,6] = {|P∧G|, |P∨G|, |B(P)|, |B(G)|, fg_match, gt_match} with

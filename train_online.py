@@ -69,6 +69,9 @@ def parse(argv=None):
                          "(network), or at each frame's stored size (stored): the fused logits are upsampled on the "
                          "device as scipy 1.0's imresize(mode='F') does and scored against the original annotations, "
                          "so the PNGs and J / F compare with the DAVIS-2016 benchmark's")
+    ap.add_argument("--encode", default="host", choices=["host", "device"],
+                    help="write the result PNGs with Pillow on the host (host), or encode them on the GPU "
+                         "(device: SequenceSegmenter(encode='png'); the bytes are written as they come, no Pillow)")
     a = ap.parse_args(argv)
     if a.evaluate and (a.synthetic or a.loader != "native"):
         ap.error("--evaluate scores against the DAVIS annotations read by --loader native; it cannot be combined with "
@@ -224,8 +227,14 @@ def main(argv=None):
               + (", scored against the nearest-resized annotations" if a.evaluate else ""))
     seg = SequenceSegmenter(net, output="bytescale", frames=("jpeg" if jpeg_frames else "bgr8") if native else "nchw_f32",
                             score=a.evaluate,
-                            input_res=input_res, output_res=a.output_res)
+                            input_res=input_res, output_res=a.output_res,
+                            encode="png" if a.encode == "device" else None)
     for pred in seg(frames()):
+        if a.encode == "device":                        # one complete PNG file per frame
+            for jj, name in enumerate(names.popleft()):
+                with open(os.path.join(out_dir, name + ".png"), "wb") as f:
+                    f.write(pred[jj])
+            continue
         arr = pred.numpy()
         for jj, name in enumerate(names.popleft()):
             try:
