@@ -618,6 +618,36 @@ OSVOS_API size_t osvos_png_encode_workspace_bytes(int n, int h, int w);
 OSVOS_API int osvos_png_encode(const uint8_t* src, uint8_t* out, int64_t* lengths, void* workspace, int n, int h, int w,
                                osvos_stream_t stream);
 
+/* ---- PNG decoding of 8-bit and 1-bit grayscale files (result and annotation masks; DESIGN.md §22) ------------------
+ *   osvos_png_decode: a batch of n PNG files of one size h x w, parsed and packed by osvos_pytorch_b200.png.pack into
+ *                     `blob` (blob_bytes bytes, 16-byte aligned: per-file records, segment records, the concatenated
+ *                     IDAT payloads) -> out [n][h][w] uint8 (any alignment; depth 1 as 0 / 255) and status [n] int32.
+ *                     Each zlib stream is inflated by one warp per segment when the cuts the host proposed (after an
+ *                     IDAT payload ending in 00 00 FF FF) are proven by a counting pass, otherwise by one warp in order;
+ *                     a wrong proposal changes neither pixels nor status.  Then the Adler-32 check and the row filters.
+ *                     status bits: 1 an invalid block type, code-length set or undefined code, 2 a distance beyond the
+ *                     bytes written, 4 a stream that ended early or an output that is not h * (rowbytes + 1) bytes,
+ *                     8 an Adler-32 mismatch, 16 a filter type above 4, 32 a header inconsistent with the arguments
+ *                     (that file is not decoded).  Pixels of a flagged file are not specified, but the call reads
+ *                     nothing outside the blob and writes nothing outside out, status, path and the workspace.
+ *                     `path` (int32 [n] or NULL): which pass wrote each file, 1 the segment passes, 2 the in-order
+ *                     pass, 0 neither.  `nseg` is the blob's segment count.  `workspace`:
+ *                     osvos_png_decode_workspace_bytes(...) bytes, 16-byte aligned, owned by the caller; nothing is
+ *                     allocated and nothing waits for the host.  n < 65536, h, w < 32768, blob_bytes < 2^31.
+ *   osvos_png_decode_workspace_bytes: host query; 0 for invalid arguments.                                          */
+typedef struct osvos_png_decode_args {
+  const void* blob;
+  size_t blob_bytes;
+  uint8_t* out;
+  int32_t* status;
+  void* workspace;
+  int32_t* path;
+  int n, h, w;
+  int nseg;
+} osvos_png_decode_args;
+OSVOS_API size_t osvos_png_decode_workspace_bytes(int n, int h, int w, int nseg, size_t blob_bytes);
+OSVOS_API int osvos_png_decode(const osvos_png_decode_args* args, osvos_stream_t stream);
+
 /* ---- side-branch tail with general deconvolution weights (DESIGN.md §20)------------------------------------------
  * The reference's eight ConvTranspose2d layers with ANY weights (networks/vgg_osvos.py:45-46,68-69), their centre crop
  * (layers/osvos_layers.py:51-56), cat + fuse (:71-72) and, with a label, the class-balanced BCE terms

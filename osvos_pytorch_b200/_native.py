@@ -104,6 +104,12 @@ class JpegArgs(Structure):
                 ("chunk_bits", c_int), ("reserved", c_int)]
 
 
+class PngDecodeArgs(Structure):
+    """osvos_png_decode_args (include/osvos_b200.h)."""
+    _fields_ = [("blob", c_void_p), ("blob_bytes", c_size_t), ("out", c_void_p), ("status", c_void_p),
+                ("workspace", c_void_p), ("path", c_void_p), ("n", c_int), ("h", c_int), ("w", c_int), ("nseg", c_int)]
+
+
 class UpsamplingFoldArgs(Structure):
     """osvos_upsampling_fold_args (include/osvos_b200.h)."""
     _fields_ = [("upscale_w", c_void_p * 4), ("upscale1_w", c_void_p * 4), ("fuse_w", c_void_p), ("vtab", c_void_p),
@@ -231,6 +237,8 @@ SIGNATURES = {
     "osvos_png_max_bytes": (c_size_t, [c_int, c_int]),
     "osvos_png_encode_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "osvos_png_encode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "osvos_png_decode_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_size_t]),
+    "osvos_png_decode": (c_int, [POINTER(PngDecodeArgs), c_void_p]),
 }
 
 DAVIS_MAX_RADIUS = 31

@@ -69,3 +69,104 @@ class SequenceScores:
         j, f = j_and_f(counts)
         return {"J": j.tolist(), "F": f.tolist(), "counts": counts.tolist(),
                 "statistics": {"J": statistics(j), "F": statistics(f)}}
+
+
+def dataset_scores(per_seq):
+    """{sequence: SequenceScores or its result()} -> the dataset figures {'J': {M, O, D}, 'F': {M, O, D}}: the mean over
+    sequences of the per-sequence statistics (NaN without sequences)."""
+    stats = [(sc.result() if isinstance(sc, SequenceScores) else sc)["statistics"] for sc in per_seq.values()]
+    return {m: {k: float(np.mean([st[m][k] for st in stats])) if stats else float("nan") for k in "MOD"}
+            for m in ("J", "F")}
+
+
+def _png_stems(folder):
+    import os
+    return sorted(f[:-4] for f in os.listdir(folder) if f.lower().endswith(".png"))
+
+
+def score_results(results_dir, db_root_dir=None, sequences=None, threshold=128, device="cuda", batch=16,
+                  decode="device", readers=4):
+    """Scores a folder of result PNGs against the DAVIS-2016 annotations (DESIGN.md §22).
+
+    ``results_dir/<seq>/<stem>.png`` is paired with ``db_root_dir/Annotations/480p/<seq>/<stem>.png`` by file stem;
+    a missing result, a missing annotation or differing sizes raise ValueError.  ``sequences``: the sequences to score
+    (default: those of ``val_seqs.txt`` that have a folder under ``results_dir``).  The prediction is
+    ``byte >= threshold`` (128 is logit > 0 for "mask" and "prob" files), the annotation ``byte != 0``, scored by
+    ops.davis_measures with no per-frame synchronisation.  ``decode``: "device" reads and parses the files in
+    ``readers`` threads and decodes them with png.decode_files (cv2 for files outside its subset or flagged by it),
+    "host" decodes every file with cv2; both give the same counts.
+
+    Returns {'sequences': {seq: SequenceScores.result()}, 'dataset': dataset_scores(...), 'frames', 'fallback_files',
+    'redecoded_files'}."""
+    import os
+    from concurrent.futures import ThreadPoolExecutor
+
+    from . import ops, png
+    if decode not in ("device", "host"):
+        raise ValueError(f"decode must be 'device' or 'host', got {decode!r}")
+    if db_root_dir is None:
+        from mypath import Path
+        db_root_dir = Path.db_root_dir()
+    ann_root = os.path.join(db_root_dir, "Annotations", "480p")
+    if sequences is None:
+        with open(os.path.join(db_root_dir, "val_seqs.txt")) as f:
+            sequences = [s.strip() for s in f if s.strip()]
+        sequences = [s for s in sequences if os.path.isdir(os.path.join(results_dir, s))]
+        if not sequences:
+            raise ValueError(f"no sequence of val_seqs.txt has a folder under {results_dir}")
+    pairs = []                                               # (sequence, result path, annotation path)
+    for seq in sequences:
+        res_dir, ann_dir = os.path.join(results_dir, seq), os.path.join(ann_root, seq)
+        if not os.path.isdir(res_dir) or not os.path.isdir(ann_dir):
+            raise ValueError(f"unknown sequence {seq!r}: no folder " + (res_dir if not os.path.isdir(res_dir) else ann_dir))
+        have, want = set(_png_stems(res_dir)), _png_stems(ann_dir)
+        missing = [s for s in want if s not in have]
+        if missing:
+            raise ValueError(f"sequence {seq!r}: no result for frame(s) {', '.join(missing[:5])} in {res_dir}")
+        extra = sorted(have - set(want))
+        if extra:
+            raise ValueError(f"sequence {seq!r}: no annotation for result(s) {', '.join(extra[:5])} in {ann_dir}")
+        pairs.extend((seq, os.path.join(res_dir, s + ".png"), os.path.join(ann_dir, s + ".png")) for s in want)
+
+    def read(path):
+        with open(path, "rb") as f:
+            data = f.read()
+        return (data, png.parse(data)) if decode == "device" else (png.decode_host(data), None)
+
+    def to_device(items):
+        if decode == "device":
+            return png.decode_files([d for d, _ in items], device, parsed=[p for _, p in items])
+        if len({m.shape for m, _ in items}) != 1:
+            raise ValueError("the files differ in size")
+        return torch.from_numpy(np.stack([m for m, _ in items])).to(device), 0, 0
+
+    scores = {seq: SequenceScores() for seq in sequences}
+    fallback = redecoded = 0
+    threshold = int(threshold)
+    with ThreadPoolExecutor(max(1, int(readers))) as pool:
+        loaded = pool.map(lambda pr: (read(pr[1]), read(pr[2])), pairs)
+        # one batch never mixes sequences: a sequence has one size, the dataset need not
+        start = 0
+        while start < len(pairs):
+            seq = pairs[start][0]
+            stop = start
+            while stop < len(pairs) and stop - start < batch and pairs[stop][0] == seq:
+                stop += 1
+            items = [next(loaded) for _ in range(stop - start)]
+            try:
+                res, fb_r, rd_r = to_device([it[0] for it in items])
+                ann, fb_a, rd_a = to_device([it[1] for it in items])
+            except ValueError as e:
+                raise ValueError(f"sequence {seq!r}, frames {os.path.basename(pairs[start][1])} .. "
+                                 f"{os.path.basename(pairs[stop - 1][1])}: {e}") from e
+            if res.shape != ann.shape:
+                raise ValueError(f"sequence {seq!r}: results are {res.shape[1]}x{res.shape[2]}, annotations "
+                                 f"{ann.shape[1]}x{ann.shape[2]}")
+            fallback += fb_r + fb_a
+            redecoded += rd_r + rd_a
+            pred = torch.where(res >= threshold, 1.0, -1.0).to(torch.float32)
+            scores[seq].add(ops.davis_measures(pred, ann))
+            start = stop
+    per_seq = {seq: sc.result() for seq, sc in scores.items()}
+    return {"sequences": per_seq, "dataset": dataset_scores(per_seq), "frames": len(pairs),
+            "fallback_files": fallback, "redecoded_files": redecoded}

@@ -958,3 +958,42 @@ def decode_jpeg(blob, n, h, w, out=None, status=None, nseg=None, chunk_bits=0):
     nat.check(lib.osvos_jpeg_decode(byref(a), _stream()), "osvos_jpeg_decode")
     _count(6)
     return out, status
+
+
+def decode_png(blob, n, h, w, nseg, out=None, status=None, path=None):
+    """A batch of n grayscale PNGs of size h x w packed by png.pack (``blob``: uint8 device tensor) -> (out uint8
+    [n,h,w], what cv2.imread(path, 0) gives, 1-bit files as 0 / 255; status int32 [n]: 1 invalid block type, code
+    lengths or code, 2 distance beyond the bytes written, 4 stream ended early or wrong output size, 8 Adler-32
+    mismatch, 16 filter type above 4, 32 header inconsistent with (n, h, w)).  ``out`` may be any contiguous uint8
+    [n,h,w] tensor, at any alignment.  ``nseg`` (required): the blob's segment count, png.segment_count of the host
+    blob; it sizes the launch, and reading it from the device blob would make the call wait for the device.
+    ``path``: optional int32 [n] that receives which pass wrote each file (1 the per-segment passes over proven cuts,
+    2 the in-order pass).  No host synchronisation (csrc/png_decode.cu, DESIGN.md §22)."""
+    if nseg is None:
+        raise ValueError("nseg: pass png.segment_count(host_blob); the device copy is not read back")
+    lib = nat.load()
+    _require_cuda(blob, "blob")
+    if blob.dtype != torch.uint8 or blob.dim() != 1 or not blob.is_contiguous():
+        raise ValueError("blob must be a contiguous 1-D uint8 device tensor from png.pack")
+    if blob.data_ptr() % 16:
+        raise ValueError("blob must be 16-byte aligned")
+    shape = (n, h, w)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.uint8, device=blob.device)
+    elif out.dtype != torch.uint8 or tuple(out.shape) != shape or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous uint8 tensor of shape {shape}")
+    if status is None:
+        status = torch.empty(n, dtype=torch.int32, device=blob.device)
+    elif status.dtype != torch.int32 or tuple(status.shape) != (n,) or not status.is_contiguous():
+        raise ValueError(f"status must be a contiguous int32 tensor of shape ({n},)")
+    if path is not None and (path.dtype != torch.int32 or tuple(path.shape) != (n,) or not path.is_contiguous()):
+        raise ValueError(f"path must be a contiguous int32 tensor of shape ({n},)")
+    nbytes = lib.osvos_png_decode_workspace_bytes(n, h, w, nseg, blob.numel())
+    if nbytes == 0:
+        raise ValueError(f"cannot decode [{n},{h},{w}] with {nseg} segments, {blob.numel()} blob bytes")
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=blob.device)
+    a = nat.PngDecodeArgs(blob.data_ptr(), blob.numel(), out.data_ptr(), status.data_ptr(), ws.data_ptr(), nat.ptr(path),
+                          n, h, w, nseg)
+    nat.check(lib.osvos_png_decode(byref(a), _stream()), "osvos_png_decode")
+    _count(5 if nseg == n else 7)
+    return out, status

@@ -97,14 +97,6 @@ def parse(argv=None):
     return a
 
 
-def _val_scores(per_seq):
-    """{sequence: SequenceScores} -> the dataset means over sequences of the J and F statistics."""
-    import numpy as np
-    stats = [sc.result()["statistics"] for sc in per_seq.values()]
-    return {m: {k: float(np.mean([st[m][k] for st in stats])) if stats else float("nan") for k in "MOD"}
-            for m in ("J", "F")}
-
-
 def main(argv=None):
     a = parse(argv)
     if a.deterministic:
@@ -269,7 +261,7 @@ def main(argv=None):
                             per_seq.setdefault(fname.split("/")[0], evaluation.SequenceScores()).add(counts[i:i + 1])
             print("***Testing *** " + " ".join(f"Loss {k}: {v:.4f}" for k, v in enumerate((tot / len(val_batches)).tolist())))
             if a.val_measures:
-                sc = _val_scores(per_seq)
+                sc = evaluation.dataset_scores(per_seq)
                 print("***Testing *** " + "  ".join(f"{m} M/O/D: {sc[m]['M']:.4f} / {sc[m]['O']:.4f} / {sc[m]['D']:.4f}"
                                                     for m in ("J", "F")) + f"  ({len(per_seq)} sequences)")
     if world > 1:
