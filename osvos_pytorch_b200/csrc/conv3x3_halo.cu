@@ -308,13 +308,17 @@ static int conv3x3_halo_dispatch(const osvos_conv3x3_args* a, cudaStream_t strea
     if (lean) return launch_halo<64, 2, true>(a, stream);
     return fast ? launch_halo<64, 1, false, DET>(a, stream) : launch_halo<64, 2, false, DET>(a, stream);
   }
-  // N = 256 tiles whenever that does not cost a wave.  The cost model per (tap, 64-channel) step (N = 128 ~ 1000 cycles
-  // for 2 + 1 instructions, N = 256 ~ 2200 exact) is carried over from the first tensor-core generation this was tuned on;
-  // on an H100 the choice measured neutral at 480x854 (552-553 frames/s with 256-wide tiles and with 128-wide ones only).
-  const bool prefer256 = fast ? waves256 * 1100 < waves128 * 700 : waves256 * 2200 < waves128 * 1000;
-  if (a->cout % 256 == 0 && prefer256)
-    return fast ? launch_halo<256, 1, false, DET>(a, stream) : launch_halo<256, 2, false, DET>(a, stream);
-  if (fast) return launch_halo<128, 1, false, DET>(a, stream);
+  // Fast mode: N = 256 tiles whenever that does not cost a wave.  The cost model per (tap, 64-channel) step (N = 128 ~ 700
+  // cycles, N = 256 ~ 1100, one instruction each) is carried over from the first tensor-core generation this was tuned on;
+  // the fast-mode choice has not been measured on an H100.
+  // Exact mode never takes N = 256: at ~2200 cycles against ~1000 it would need waves256 * 2.2 < waves128, and
+  // waves128 = ceil(2T / S) <= 2 ceil(T / S) = 2 waves256 for any T tiles of 256 on S SMs.  (So the exact-mode A/B in
+  // DESIGN.md section 8, 552-553 frames/s with and without 256-wide tiles, ran the same kernels in both arms.)
+  if (fast) {
+    const bool prefer256 = waves256 * 1100 < waves128 * 700;
+    if (a->cout % 256 == 0 && prefer256) return launch_halo<256, 1, false, DET>(a, stream);
+    return launch_halo<128, 1, false, DET>(a, stream);
+  }
   if (lean) return launch_halo<128, 2, true>(a, stream);
   return launch_halo<128, 2, false, DET>(a, stream);
 }
