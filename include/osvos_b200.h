@@ -648,6 +648,31 @@ typedef struct osvos_png_decode_args {
 OSVOS_API size_t osvos_png_decode_workspace_bytes(int n, int h, int w, int nseg, size_t blob_bytes);
 OSVOS_API int osvos_png_decode(const osvos_png_decode_args* args, osvos_stream_t stream);
 
+/* ---- segmentation overlays as JPEG files (replaces the reference's display: dataloaders/helpers.py:15-40
+ *      overlay_mask and the vis_res window of train_online.py:160-205; DESIGN.md §23) ---------------------------------
+ *   osvos_overlay_mask: frames [n][h][w][3] uint8 BGR (any alignment) and logits [n][h][w] fp32 (4-byte aligned) ->
+ *                     out [n][h][w][3] uint8 (may be frames itself).  fg = logit > 0 (+-0 and NaN are background);
+ *                     edge = fg with a 4-neighbour in the background or outside the frame (the pixels
+ *                     cv2.drawContours(findContours(mask, RETR_TREE, CHAIN_APPROX_SIMPLE), -1, 0, 1) paints).  Each
+ *                     pixel is (0, 0, 0) on the edge, (v + c + 1) >> 1 per channel on the rest of fg (c0, c1, c2 the
+ *                     colour in the frame's channel order, 0..255), v elsewhere.
+ *   osvos_jpeg_encode: src [n][h][w][3] uint8 BGR (any alignment) -> one baseline JPEG file per frame in
+ *                     out [n][osvos_jpeg_max_bytes(h, w)] (frame i's file is out + i * max_bytes, lengths[i] bytes long;
+ *                     lengths int64 [n], 8-byte aligned), the bytes cv2.imencode('.jpg', frame,
+ *                     [IMWRITE_JPEG_QUALITY, quality]) writes: JFIF, 4:2:0, ISLOW FDCT, the Annex K Huffman tables,
+ *                     no restart interval.  1 <= quality <= 100, 1 <= h, w <= 65500, n < 65536.  `workspace`:
+ *                     osvos_jpeg_encode_workspace_bytes(n, h, w) bytes, 16-byte aligned, owned by the caller; nothing
+ *                     is allocated and nothing waits for the host.
+ *   osvos_jpeg_max_bytes: the per-frame capacity: header and EOI plus twice the largest scan (every block at
+ *                     22 + 63 x 26 bits, every byte stuffed); 0 for invalid sizes.
+ *   osvos_jpeg_encode_workspace_bytes: host query; 0 for invalid arguments.                                          */
+OSVOS_API int osvos_overlay_mask(const uint8_t* frames, const float* logits, uint8_t* out, int n, int h, int w, int c0,
+                                 int c1, int c2, osvos_stream_t stream);
+OSVOS_API size_t osvos_jpeg_max_bytes(int h, int w);
+OSVOS_API size_t osvos_jpeg_encode_workspace_bytes(int n, int h, int w);
+OSVOS_API int osvos_jpeg_encode(const uint8_t* src, uint8_t* out, int64_t* lengths, void* workspace, int n, int h, int w,
+                                int quality, osvos_stream_t stream);
+
 /* ---- side-branch tail with general deconvolution weights (DESIGN.md §20)------------------------------------------
  * The reference's eight ConvTranspose2d layers with ANY weights (networks/vgg_osvos.py:45-46,68-69), their centre crop
  * (layers/osvos_layers.py:51-56), cat + fuse (:71-72) and, with a label, the class-balanced BCE terms

@@ -239,6 +239,11 @@ SIGNATURES = {
     "osvos_png_encode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "osvos_png_decode_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_size_t]),
     "osvos_png_decode": (c_int, [POINTER(PngDecodeArgs), c_void_p]),
+    # helpers.py:15-40 overlay_mask and the vis_res display of train_online.py:160-205, written as JPEG files
+    "osvos_overlay_mask": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "osvos_jpeg_max_bytes": (c_size_t, [c_int, c_int]),
+    "osvos_jpeg_encode_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "osvos_jpeg_encode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
 }
 
 DAVIS_MAX_RADIUS = 31

@@ -49,10 +49,18 @@ class SequenceSegmenter:
     (ops.encode_png, DESIGN.md §21) into a per-slot buffer of fixed address, and the whole buffer (the per-frame
     capacity, so no size is read back first) and the file lengths cross device->host instead of the maps.  Each result
     is then a list of N ``memoryview``s, each one complete PNG file (what Image.fromarray(map, "L").save writes, other
-    deflate bytes) backed by the pinned slot and valid as long as the maps are without it."""
+    deflate bytes) backed by the pinned slot and valid as long as the maps are without it.
+
+    ``overlay="jpeg"`` (``frames="bgr8"`` or ``"jpeg"``): each frame's mask drawn over its bytes (ops.overlay_mask: the
+    frame at the results' size, i.e. the resized slot under ``input_res`` or the stored bytes under
+    ``output_res="stored"``, and the fused map after any resize) and encoded as the JPEG cv2.imencode would write at
+    ``overlay_quality`` (ops.encode_jpeg, DESIGN.md §23), on the compute stream before the slot is released, into a
+    per-slot buffer of fixed address that crosses device->host at its capacity with the file lengths.  Each yielded
+    item is then ``(result, overlays)``, ``overlays`` a list of N ``memoryview``s, one complete JPEG file each, valid
+    as long as the result is."""
 
     def __init__(self, net, output="logits", depth=3, frames="nchw_f32", meanval=ops.MEANVAL, score=False,
-                 input_res=None, output_res="network", encode=None):
+                 input_res=None, output_res="network", encode=None, overlay=None, overlay_quality=95):
         if output not in ("logits", "bytescale", "prob", "mask"):
             raise ValueError("output must be one of logits / bytescale / prob / mask")
         if frames not in ("nchw_f32", "bgr8", "jpeg"):
@@ -65,6 +73,12 @@ class SequenceSegmenter:
             raise ValueError("encode must be None or 'png'")
         if encode == "png" and output == "logits":
             raise ValueError("encode='png' writes 8-bit maps: it needs output bytescale, prob or mask")
+        if overlay not in (None, "jpeg"):
+            raise ValueError("overlay must be None or 'jpeg'")
+        if overlay == "jpeg" and frames == "nchw_f32":
+            raise ValueError("overlay='jpeg' draws over the frames' bytes: it needs frames='bgr8' or 'jpeg'")
+        if not 1 <= int(overlay_quality) <= 100:
+            raise ValueError("overlay_quality must lie in 1..100")
         self.net, self.output, self.depth = net, output, max(2, int(depth))
         self.frames, self.meanval = frames, tuple(meanval)
         self.score = bool(score)
@@ -72,6 +86,7 @@ class SequenceSegmenter:
         self.output_res = output_res
         self._upsample = input_res is not None and output_res == "stored"
         self.encode = encode
+        self.overlay, self.overlay_quality = overlay, int(overlay_quality)
         self._shape = None
         self._counts = []
         self.jpeg_status = None
@@ -100,6 +115,13 @@ class SequenceSegmenter:
             self._host_len = [torch.empty(n, dtype=torch.int64).pin_memory() for _ in range(self.depth)]
         else:
             self._host_out = [torch.empty((n, 1, rh, rw), dtype=out_dtype).pin_memory() for _ in range(self.depth)]
+        if self.overlay == "jpeg":
+            ocap = ops.jpeg_max_bytes(rh, rw)
+            self._dev_ovl = torch.empty((n, rh, rw, 3), dtype=torch.uint8, device=device)   # compute stream only
+            self._dev_jpg = [torch.empty((n, ocap), dtype=torch.uint8, device=device) for _ in range(self.depth)]
+            self._dev_jlen = [torch.empty(n, dtype=torch.int64, device=device) for _ in range(self.depth)]
+            self._host_jpg = [torch.empty((n, ocap), dtype=torch.uint8).pin_memory() for _ in range(self.depth)]
+            self._host_jlen = [torch.empty(n, dtype=torch.int64).pin_memory() for _ in range(self.depth)]
         if self._upsample:
             self._dev_up = [torch.empty((n, 1, h0, w0), dtype=torch.float32, device=device) for _ in range(self.depth)]
         if self.score:
@@ -114,6 +136,8 @@ class SequenceSegmenter:
         self.d2h_bytes_per_frame = n * rh * rw * (4 if self.output == "logits" else 1)
         if self.encode == "png":
             self.d2h_bytes_per_frame = n * (cap + 8)
+        if self.overlay == "jpeg":
+            self.d2h_bytes_per_frame += n * (ocap + 8)
 
     def _submit(self, i, frame, gt, device):
         k = i % self.depth
@@ -171,6 +195,9 @@ class SequenceSegmenter:
                 fused = ops.resize_f32(fused, self._dev_up[k].shape[2:4], out=self._dev_up[k])
             if self.score:
                 self._counts.append(ops.davis_measures(fused, gt_dev))
+            if self.overlay == "jpeg":                          # reads the slot's frame: before the slot is released
+                img = ops.overlay_mask(self._dev_raw[k] if self._upsample else raw, fused, out=self._dev_ovl)
+                ops.encode_jpeg(img, self.overlay_quality, out=self._dev_jpg[k], lengths=self._dev_jlen[k])
             self._ev_consumed[k].record(cur)                    # after the last read of this slot's frame and mask
             if self.output == "logits":
                 self._dev_out[k].copy_(fused)
@@ -186,14 +213,22 @@ class SequenceSegmenter:
                 self._host_len[k].copy_(self._dev_len[k], non_blocking=True)
             else:
                 self._host_out[k].copy_(self._dev_out[k], non_blocking=True)
+            if self.overlay == "jpeg":
+                self._host_jpg[k].copy_(self._dev_jpg[k], non_blocking=True)
+                self._host_jlen[k].copy_(self._dev_jlen[k], non_blocking=True)
             self._ev_host[k].record(self._s_out)
 
     def _result(self, k):
         self._ev_host[k].synchronize()
         if self.encode != "png":
-            return self._host_out[k]
-        files = self._host_png[k].numpy()
-        return [memoryview(files[j, :int(ln)]) for j, ln in enumerate(self._host_len[k].tolist())]
+            res = self._host_out[k]
+        else:
+            files = self._host_png[k].numpy()
+            res = [memoryview(files[j, :int(ln)]) for j, ln in enumerate(self._host_len[k].tolist())]
+        if self.overlay != "jpeg":
+            return res
+        files = self._host_jpg[k].numpy()
+        return res, [memoryview(files[j, :int(ln)]) for j, ln in enumerate(self._host_jlen[k].tolist())]
 
     def __call__(self, frames):
         device = next(self.net.parameters()).device

@@ -997,3 +997,68 @@ def decode_png(blob, n, h, w, nseg, out=None, status=None, path=None):
     nat.check(lib.osvos_png_decode(byref(a), _stream()), "osvos_png_decode")
     _count(5 if nseg == n else 7)
     return out, status
+
+
+def overlay_mask(frames, logits, color=(0, 0, 255), out=None):
+    """The mask drawn over the frame (the reference's helpers.overlay_mask, shown by train_online.py's vis_res):
+    frames uint8 [N,H,W,3] BGR and fused logits fp32 [N,1,H,W] or [N,H,W] -> uint8 [N,H,W,3].  fg = logit > 0 (+-0
+    and NaN are background); fg pixels with a 4-neighbour in the background or outside the frame (the contour
+    cv2.drawContours draws) are black, the rest of fg is (v + c + 1) >> 1 per channel with ``color`` in BGR order, the
+    background keeps its bytes.  ``out`` may be ``frames`` itself.  No host synchronisation (DESIGN.md §23)."""
+    lib = nat.load()
+    x = _require_u8(frames, "frames", 4)
+    n, h, w, c = (int(v) for v in x.shape)
+    if c != 3:
+        raise ValueError("frames must be [N,H,W,3]")
+    _require_cuda(logits, "logits")
+    if logits.dtype != torch.float32 or logits.numel() != n * h * w or tuple(logits.shape[-2:]) != (h, w):
+        raise ValueError(f"logits must be fp32 [N,1,H,W] or [N,H,W] matching frames {tuple(x.shape)}, got "
+                         f"{logits.dtype} {tuple(logits.shape)}")
+    col = tuple(int(v) for v in color)
+    if len(col) != 3 or not all(0 <= v <= 255 for v in col):
+        raise ValueError(f"color must be three values in 0..255, got {color}")
+    lg = logits.detach().contiguous()
+    if out is None:
+        out = torch.empty_like(x)
+    elif out.dtype != torch.uint8 or tuple(out.shape) != (n, h, w, 3) or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous uint8 tensor of shape {(n, h, w, 3)}")
+    _count()
+    nat.check(lib.osvos_overlay_mask(x.data_ptr(), lg.data_ptr(), out.data_ptr(), n, h, w, *col, _stream()),
+              "osvos_overlay_mask")
+    return out
+
+
+def jpeg_max_bytes(h, w):
+    """Capacity of one encoded frame (osvos_jpeg_max_bytes): header and EOI plus twice the largest possible scan."""
+    return int(nat.load().osvos_jpeg_max_bytes(int(h), int(w)))
+
+
+def encode_jpeg(frames, quality=95, out=None, lengths=None):
+    """uint8 BGR frames [N,H,W,3] -> (out uint8 [N, jpeg_max_bytes(H, W)], lengths int64 [N]): frame i's JPEG file is
+    out[i, :lengths[i]], byte for byte what cv2.imencode('.jpg', frame, [cv2.IMWRITE_JPEG_QUALITY, quality]) writes
+    (quality 95 is cv2.imwrite's default; csrc/jpeg_encode.cu, DESIGN.md §23).  No host synchronisation."""
+    lib = nat.load()
+    x = _require_u8(frames, "frames", 4)
+    n, h, w, c = (int(v) for v in x.shape)
+    if c != 3:
+        raise ValueError("frames must be [N,H,W,3]")
+    q = int(quality)
+    if not 1 <= q <= 100:
+        raise ValueError(f"quality must lie in 1..100, got {quality}")
+    cap = lib.osvos_jpeg_max_bytes(h, w)
+    nbytes = lib.osvos_jpeg_encode_workspace_bytes(n, h, w)
+    if cap == 0 or nbytes == 0:
+        raise ValueError(f"cannot encode [{n},{h},{w},3]: sizes must lie in [1, 65500] and 0 < N < 65536")
+    if out is None:
+        out = torch.empty((n, cap), dtype=torch.uint8, device=x.device)
+    elif out.dtype != torch.uint8 or tuple(out.shape) != (n, cap) or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous uint8 tensor of shape ({n}, {cap})")
+    if lengths is None:
+        lengths = torch.empty(n, dtype=torch.int64, device=x.device)
+    elif lengths.dtype != torch.int64 or tuple(lengths.shape) != (n,) or not lengths.is_contiguous():
+        raise ValueError(f"lengths must be a contiguous int64 tensor of shape ({n},)")
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    _count(7)
+    nat.check(lib.osvos_jpeg_encode(x.data_ptr(), out.data_ptr(), lengths.data_ptr(), ws.data_ptr(), n, h, w, q,
+                                    _stream()), "osvos_jpeg_encode")
+    return out, lengths

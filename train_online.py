@@ -72,6 +72,11 @@ def parse(argv=None):
     ap.add_argument("--encode", default="host", choices=["host", "device"],
                     help="write the result PNGs with Pillow on the host (host), or encode them on the GPU "
                          "(device: SequenceSegmenter(encode='png'); the bytes are written as they come, no Pillow)")
+    ap.add_argument("--overlay", action="store_true",
+                    help="also write each frame with its mask drawn over it (the reference's vis_res picture: the "
+                         "foreground blended 50/50 with red, its outline black) as Results/<seq>_overlay/<frame>.jpg, "
+                         "drawn and JPEG-encoded on the GPU (the bytes cv2.imwrite would write). Needs --loader native")
+    ap.add_argument("--overlay-quality", type=int, default=95, help="JPEG quality of --overlay (1..100)")
     a = ap.parse_args(argv)
     if a.evaluate and (a.synthetic or a.loader != "native"):
         ap.error("--evaluate scores against the DAVIS annotations read by --loader native; it cannot be combined with "
@@ -82,6 +87,11 @@ def parse(argv=None):
     if a.decode == "device" and (a.synthetic or a.loader != "native"):
         ap.error("--decode device decodes the frames read by --loader native; it cannot be combined with "
                  + ("--synthetic" if a.synthetic else "--loader reference"))
+    if a.overlay and (a.synthetic or a.loader != "native"):
+        ap.error("--overlay draws over the frames read by --loader native; it cannot be combined with "
+                 + ("--synthetic" if a.synthetic else "--loader reference"))
+    if not 1 <= a.overlay_quality <= 100:
+        ap.error("--overlay-quality must lie in 1..100")
     return a
 
 
@@ -228,15 +238,25 @@ def main(argv=None):
     seg = SequenceSegmenter(net, output="bytescale", frames=("jpeg" if jpeg_frames else "bgr8") if native else "nchw_f32",
                             score=a.evaluate,
                             input_res=input_res, output_res=a.output_res,
-                            encode="png" if a.encode == "device" else None)
+                            encode="png" if a.encode == "device" else None,
+                            overlay="jpeg" if a.overlay else None, overlay_quality=a.overlay_quality)
+    if a.overlay:
+        overlay_dir = os.path.join(save_dir, "Results", a.seq_name + "_overlay")
+        os.makedirs(overlay_dir, exist_ok=True)
     for pred in seg(frames()):
+        batch_names = names.popleft()
+        if a.overlay:                                   # one complete JPEG file per frame
+            pred, overlays = pred
+            for jj, name in enumerate(batch_names):
+                with open(os.path.join(overlay_dir, name + ".jpg"), "wb") as f:
+                    f.write(overlays[jj])
         if a.encode == "device":                        # one complete PNG file per frame
-            for jj, name in enumerate(names.popleft()):
+            for jj, name in enumerate(batch_names):
                 with open(os.path.join(out_dir, name + ".png"), "wb") as f:
                     f.write(pred[jj])
             continue
         arr = pred.numpy()
-        for jj, name in enumerate(names.popleft()):
+        for jj, name in enumerate(batch_names):
             try:
                 from PIL import Image
                 Image.fromarray(arr[jj, 0], mode="L").save(os.path.join(out_dir, name + ".png"))
