@@ -572,6 +572,25 @@ OSVOS_API size_t osvos_davis_measures_workspace_bytes(int n, int h, int w);
 OSVOS_API int osvos_davis_measures(const float* logits, const uint8_t* masks, int* counts, void* workspace, int n, int h,
                                    int w, int r, osvos_stream_t stream);
 
+/* ---- DAVIS-2017 per-object measures and the merge of per-object maps (DESIGN.md §24) ------------------------------
+ *   osvos_davis_measures_objects: label maps [n][h][w] uint8 and annotations gt [n][h][w] uint8 (both any alignment) ->
+ *                         counts [n][k][6] int32 (4-byte aligned), row (f, j) the six counts of osvos_davis_measures for
+ *                         object j + 1 with P = label == j + 1 and G = gt == j + 1, both cleared where gt == 255 (void).
+ *                         Boundaries, radius and disk as osvos_davis_measures.  1 <= k <= OSVOS_DAVIS_MAX_OBJECTS,
+ *                         n * k < 65536, h, w < 32768.  `workspace`: osvos_davis_measures_objects_workspace_bytes(n, k,
+ *                         h, w) bytes, 4-byte aligned, owned by the caller.  Zeroes counts itself.  Integer counts: the
+ *                         result does not depend on the launch configuration.
+ *   osvos_davis_measures_objects_workspace_bytes: host query; 0 for a non-positive dimension.
+ *   osvos_merge_objects:  `maps` (host array of k device pointers, each to `pixels` fp32 values, 4-byte aligned) ->
+ *                         out [pixels] uint8 (any alignment): 1 + the first k of the largest value where that value is
+ *                         > 0, else 0 (±0 and NaN never win).  1 <= k <= OSVOS_MERGE_MAX_OBJECTS.                    */
+#define OSVOS_DAVIS_MAX_OBJECTS 254
+#define OSVOS_MERGE_MAX_OBJECTS 254
+OSVOS_API size_t osvos_davis_measures_objects_workspace_bytes(int n, int k, int h, int w);
+OSVOS_API int osvos_davis_measures_objects(const uint8_t* labels, const uint8_t* gt, int* counts, void* workspace, int n,
+                                           int k, int h, int w, int r, osvos_stream_t stream);
+OSVOS_API int osvos_merge_objects(const float* const* maps, int k, uint8_t* out, size_t pixels, osvos_stream_t stream);
+
 /* ---- baseline JPEG decode, bit-identical to cv2.imread (libjpeg-turbo; DESIGN.md §19) ----------------------------
  *   osvos_jpeg_decode: a batch of n JPEGs of one size h x w, packed by osvos_pytorch_b200.jpeg.pack into `blob`
  *                      (blob_bytes bytes, 16-byte aligned; headers, tables and de-stuffed entropy-coded segments) ->
@@ -617,11 +636,21 @@ OSVOS_API size_t osvos_png_max_bytes(int h, int w);
 OSVOS_API size_t osvos_png_encode_workspace_bytes(int n, int h, int w);
 OSVOS_API int osvos_png_encode(const uint8_t* src, uint8_t* out, int64_t* lengths, void* workspace, int n, int h, int w,
                                osvos_stream_t stream);
+/*   osvos_png_encode_palette: osvos_png_encode with IHDR colour type 3 (depth 8) and a PLTE chunk of `palette` (host
+ *                     memory, 3 * entries bytes RGB, 1 <= entries <= 256) after it; the bytes of each map are written as
+ *                     palette indices.  Everything after the PLTE chunk is identical to osvos_png_encode's file of the
+ *                     same map.  out [n][osvos_png_max_bytes_palette(h, w, entries)]; the workspace is
+ *                     osvos_png_encode_workspace_bytes(n, h, w).
+ *   osvos_png_max_bytes_palette: osvos_png_max_bytes(h, w) + 12 + 3 * entries; 0 for invalid arguments.              */
+OSVOS_API size_t osvos_png_max_bytes_palette(int h, int w, int entries);
+OSVOS_API int osvos_png_encode_palette(const uint8_t* src, const uint8_t* palette, int entries, uint8_t* out,
+                                       int64_t* lengths, void* workspace, int n, int h, int w, osvos_stream_t stream);
 
-/* ---- PNG decoding of 8-bit and 1-bit grayscale files (result and annotation masks; DESIGN.md §22) ------------------
+/* ---- PNG decoding of 8-bit and 1-bit grayscale files and palette files (result and annotation masks; §22, §24) ----
  *   osvos_png_decode: a batch of n PNG files of one size h x w, parsed and packed by osvos_pytorch_b200.png.pack into
  *                     `blob` (blob_bytes bytes, 16-byte aligned: per-file records, segment records, the concatenated
- *                     IDAT payloads) -> out [n][h][w] uint8 (any alignment; depth 1 as 0 / 255) and status [n] int32.
+ *                     IDAT payloads) -> out [n][h][w] uint8 (any alignment; gray depth 1 as 0 / 255, palette files at
+ *                     depth 1, 2, 4 or 8 as their raw indices, samples MSB first) and status [n] int32.
  *                     Each zlib stream is inflated by one warp per segment when the cuts the host proposed (after an
  *                     IDAT payload ending in 00 00 FF FF) are proven by a counting pass, otherwise by one warp in order;
  *                     a wrong proposal changes neither pixels nor status.  Then the Adler-32 check and the row filters.

@@ -239,6 +239,14 @@ SIGNATURES = {
     "osvos_png_encode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "osvos_png_decode_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_size_t]),
     "osvos_png_decode": (c_int, [POINTER(PngDecodeArgs), c_void_p]),
+    # DAVIS-2017: palette label files, the merge of per-object maps and per-object measures (DESIGN.md §24)
+    "osvos_png_max_bytes_palette": (c_size_t, [c_int, c_int, c_int]),
+    "osvos_png_encode_palette": (c_int, [c_void_p, c_char_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                         c_void_p]),
+    "osvos_merge_objects": (c_int, [POINTER(c_void_p), c_int, c_void_p, c_size_t, c_void_p]),
+    "osvos_davis_measures_objects_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "osvos_davis_measures_objects": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                             c_void_p]),
     # helpers.py:15-40 overlay_mask and the vis_res display of train_online.py:160-205, written as JPEG files
     "osvos_overlay_mask": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "osvos_jpeg_max_bytes": (c_size_t, [c_int, c_int]),
@@ -247,6 +255,7 @@ SIGNATURES = {
 }
 
 DAVIS_MAX_RADIUS = 31
+DAVIS_MAX_OBJECTS = 254
 
 _lib = None
 

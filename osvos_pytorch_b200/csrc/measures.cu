@@ -182,9 +182,168 @@ measures_match_kernel(MeasureMaps maps, int* __restrict__ counts, int h, int w, 
   block_add2(fg_match, gt_match, counts + 6 * f + 4);
 }
 
+// Per-object form (DESIGN.md §24): blockIdx.y = frame f of n; every lane reads its label and annotation byte once and
+// the warp forms the K (P, G) words of object k = 1..K, P = label == k, G = gt == k, both cleared where gt == 255
+// (void).  Plane f * K + (k - 1) of each map, so the boundary and match kernels run over n * K planes unchanged and
+// their counts land in [n][K][6].  |P∧G| and |P∨G| are summed per object in shared memory, one atomicAdd per block,
+// object and count.
+__global__ void __launch_bounds__(kMeasureThreads)
+measures_pack_objects_kernel(const uint8_t* __restrict__ labels, const uint8_t* __restrict__ gt, MeasureMaps maps,
+                             int* __restrict__ counts, int nobj, int h, int w) {
+  __shared__ int part[2 * OSVOS_DAVIS_MAX_OBJECTS];
+  const int f = blockIdx.y;
+  const int ww = measure_words(w);
+  const int words = h * ww;
+  const size_t hw = static_cast<size_t>(h) * w;
+  const uint8_t* lf = labels + f * hw;
+  const uint8_t* gf = gt + f * hw;
+  const int lane = threadIdx.x & 31;
+  for (int i = threadIdx.x; i < 2 * nobj; i += kMeasureThreads) part[i] = 0;
+  __syncthreads();
+  for (int i = blockIdx.x * kMeasureWarps + (threadIdx.x >> 5); i < words; i += gridDim.x * kMeasureWarps) {
+    const int y = i / ww;
+    const int x = ((i - y * ww) << 5) + lane;
+    int lab = 0, g = 0;
+    if (x < w) {
+      const size_t o = static_cast<size_t>(y) * w + x;
+      lab = __ldg(lf + o);
+      g = __ldg(gf + o);
+      if (g == 255) lab = g = 0;                    // void: in neither mask
+    }
+    // objects present in this word: skip the ballots of the others, their words are zero
+    const uint32_t any = __reduce_or_sync(0xffffffffu, (lab <= nobj ? 1u << (lab & 31) : 0u) |
+                                                             (g <= nobj ? 1u << (g & 31) : 0u));
+    for (int k = 1; k <= nobj; ++k) {
+      uint32_t pw = 0, gw = 0;
+      if (k >= 32 || (any >> k) & 1u) {
+        pw = __ballot_sync(0xffffffffu, lab == k);
+        gw = __ballot_sync(0xffffffffu, g == k);
+      }
+      if (lane == 0) {
+        const size_t plane = static_cast<size_t>(f) * nobj + (k - 1);
+        maps.p[plane * words + i] = pw;
+        maps.g[plane * words + i] = gw;
+        const int in = __popc(pw & gw), un = __popc(pw | gw);
+        if (in) atomicAdd(&part[2 * (k - 1)], in);
+        if (un) atomicAdd(&part[2 * (k - 1) + 1], un);
+      }
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < 2 * nobj; i += kMeasureThreads)
+    if (part[i]) atomicAdd(counts + 6 * (static_cast<size_t>(f) * nobj + (i >> 1)) + (i & 1), part[i]);
+}
+
 }  // namespace osvos
 
 using namespace osvos;
+
+extern "C" size_t osvos_davis_measures_objects_workspace_bytes(int n, int k, int h, int w) {
+  if (n <= 0 || k <= 0 || h <= 0 || w <= 0) return 0;
+  return 4 * sizeof(uint32_t) * static_cast<size_t>(n) * k * h * measure_words(w);
+}
+
+extern "C" int osvos_davis_measures_objects(const uint8_t* labels, const uint8_t* gt, int* counts, void* workspace,
+                                            int n, int k, int h, int w, int r, osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(labels != nullptr && gt != nullptr && counts != nullptr && workspace != nullptr);
+  OSVOS_CHECK_ARG(k >= 1 && k <= OSVOS_DAVIS_MAX_OBJECTS);
+  OSVOS_CHECK_ARG(n > 0 && static_cast<long long>(n) * k < 65536 && h > 0 && w > 0 && h < 32768 && w < 32768);
+  OSVOS_CHECK_ARG(r >= 1 && r <= OSVOS_DAVIS_MAX_RADIUS);
+  OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 3) == 0 && (reinterpret_cast<uintptr_t>(counts) & 3) == 0);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const int planes = n * k;
+  const size_t plane = static_cast<size_t>(planes) * h * measure_words(w);
+  uint32_t* ws = static_cast<uint32_t*>(workspace);
+  const MeasureMaps maps{ws, ws + plane, ws + 2 * plane, ws + 3 * plane};
+  const int words = h * measure_words(w);
+  const int sms = device_sm_count();
+  const int per_frame = max(1, (8 * sms + n - 1) / n);
+  const int per_plane = max(1, (8 * sms + planes - 1) / planes);
+  const dim3 grid_pack(min(per_frame, (words + kMeasureWarps - 1) / kMeasureWarps), n);
+  const dim3 grid_word(min(per_plane, (words + kMeasureThreads - 1) / kMeasureThreads), planes);
+  const dim3 grid_match(min(per_plane, (2 * words + kMeasureThreads - 1) / kMeasureThreads), planes);
+  OSVOS_CHECK_CUDA(cudaMemsetAsync(counts, 0, sizeof(int) * 6 * static_cast<size_t>(planes), stream));
+  measures_pack_objects_kernel<<<grid_pack, kMeasureThreads, 0, stream>>>(labels, gt, maps, counts, k, h, w);
+  OSVOS_CHECK_CUDA(cudaGetLastError());
+  measures_boundary_kernel<<<grid_word, kMeasureThreads, 0, stream>>>(maps, counts, h, w);
+  OSVOS_CHECK_CUDA(cudaGetLastError());
+  measures_match_kernel<<<grid_match, kMeasureThreads, 0, stream>>>(maps, counts, h, w, r);
+  OSVOS_CHECK_CUDA(cudaGetLastError());
+  return OSVOS_OK;
+}
+
+// ---- merge of per-object fused maps (DESIGN.md §24) ------------------------------------------------------------------
+
+namespace osvos {
+
+struct MergeMaps {
+  const float* map[OSVOS_MERGE_MAX_OBJECTS];
+};
+
+// label = 1 + the first k of the largest logit if that logit is > 0, else 0: `best` starts at +0 and only a strictly
+// larger value replaces it, so ±0 and NaN never win and ties go to the lowest k.  Four pixels per thread; float4 loads
+// when every map is 16-byte aligned (vec), one 32-bit store when out is 4-byte aligned too.
+template <bool VEC>
+__global__ void __launch_bounds__(256) merge_objects_kernel(MergeMaps maps, int nobj, uint8_t* __restrict__ out,
+                                                            long long pixels) {
+  const long long quads = (pixels + 3) >> 2;
+  const bool out_aligned = (reinterpret_cast<uintptr_t>(out) & 3) == 0;
+  for (long long q = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; q < quads;
+       q += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long i0 = q << 2;
+    float best[4] = {0.f, 0.f, 0.f, 0.f};
+    uint32_t lab[4] = {0, 0, 0, 0};
+    const bool full = i0 + 4 <= pixels;
+    for (int k = 0; k < nobj; ++k) {
+      float v[4];
+      if (VEC && full) {
+        const float4 t = __ldg(reinterpret_cast<const float4*>(maps.map[k] + i0));
+        v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+      } else {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) v[j] = i0 + j < pixels ? __ldg(maps.map[k] + i0 + j) : 0.f;
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        if (v[j] > best[j]) {
+          best[j] = v[j];
+          lab[j] = k + 1;
+        }
+      }
+    }
+    if (full && out_aligned) {
+      *reinterpret_cast<uint32_t*>(out + i0) = lab[0] | (lab[1] << 8) | (lab[2] << 16) | (lab[3] << 24);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (i0 + j < pixels) out[i0 + j] = static_cast<uint8_t>(lab[j]);
+    }
+  }
+}
+
+}  // namespace osvos
+
+extern "C" int osvos_merge_objects(const float* const* maps, int k, uint8_t* out, size_t pixels,
+                                   osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(maps != nullptr && out != nullptr && pixels > 0);
+  OSVOS_CHECK_ARG(k >= 1 && k <= OSVOS_MERGE_MAX_OBJECTS);
+  MergeMaps m{};
+  bool vec = true;
+  for (int i = 0; i < k; ++i) {
+    OSVOS_CHECK_ARG(maps[i] != nullptr && (reinterpret_cast<uintptr_t>(maps[i]) & 3) == 0);
+    vec = vec && (reinterpret_cast<uintptr_t>(maps[i]) & 15) == 0;
+    m.map[i] = maps[i];
+  }
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const long long quads = (static_cast<long long>(pixels) + 3) >> 2;
+  const unsigned blocks = static_cast<unsigned>(min(static_cast<long long>(16 * device_sm_count()), (quads + 255) / 256));
+  if (vec)
+    merge_objects_kernel<true><<<blocks, 256, 0, stream>>>(m, k, out, static_cast<long long>(pixels));
+  else
+    merge_objects_kernel<false><<<blocks, 256, 0, stream>>>(m, k, out, static_cast<long long>(pixels));
+  OSVOS_CHECK_CUDA(cudaGetLastError());
+  return OSVOS_OK;
+}
 
 extern "C" size_t osvos_davis_measures_workspace_bytes(int n, int h, int w) {
   if (n <= 0 || h <= 0 || w <= 0) return 0;

@@ -1,5 +1,7 @@
 // PNG encoder for 8-bit grayscale maps (the files the reference writes with sm.imsave, train_online.py:187; DESIGN.md
-// §21).  The format is restricted so that every part is parallel and the bytes are a function of the frame alone:
+// §21), and for 8-bit palette maps (DAVIS-2017 label files, §24: IHDR colour type 3 and a PLTE chunk, everything
+// after the header identical to the grayscale file of the same bytes).  The format is restricted so that every part
+// is parallel and the bytes are a function of the frame alone:
 //   filter:   per row the type 0-4 of least sum(min(v, 256 - v)) over the filtered bytes, ties to the lower type;
 //   segments: R = max(1, kPngSegmentBytes / (w + 1)) filtered rows each, one IDAT chunk per segment, compressed on
 //             their own (no match crosses a segment start) into one dynamic-Huffman block or one stored block,
@@ -556,10 +558,17 @@ __device__ __forceinline__ void put_be32(uint8_t* p, uint32_t v) {
   p[3] = static_cast<uint8_t>(v);
 }
 
+// The whole PLTE chunk of a palette file (length, type, 3 * entries bytes, CRC), built on the host; bytes == 0: a
+// grayscale file.
+struct PngPlte {
+  uint8_t chunk[12 + 3 * 256];
+  int bytes;
+};
+
 __global__ void __launch_bounds__(256) png_assemble_kernel(const uint8_t* __restrict__ slots, const int* __restrict__ sizes,
                                                            const uint32_t* __restrict__ adler, uint8_t* out,
                                                            long long* lengths, int h, int w, int rows, int nseg,
-                                                           int seg_cap, size_t max_bytes) {
+                                                           int seg_cap, size_t max_bytes, PngPlte plte) {
   __shared__ unsigned long long red[3][8];
   __shared__ uint8_t tail[30];
   const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
@@ -586,7 +595,7 @@ __global__ void __launch_bounds__(256) png_assemble_kernel(const uint8_t* __rest
   }
   if (lane == 0) { red[0][wid] = off; red[1][wid] = s1; red[2][wid] = s2; }
   __syncthreads();
-  off = 33;                                        // signature + IHDR
+  off = 33 + plte.bytes;                           // signature + IHDR (+ PLTE)
   s1 = 1;
   s2 = N % kAdlerMod;
   for (int k = 0; k < 8; ++k) { off += red[0][k]; s1 += red[1][k]; s2 += red[2][k]; }
@@ -598,11 +607,14 @@ __global__ void __launch_bounds__(256) png_assemble_kernel(const uint8_t* __rest
     uint8_t hdr[33] = {0x89, 'P', 'N', 'G', '\r', '\n', 0x1A, '\n', 0, 0, 0, 13, 'I', 'H', 'D', 'R'};
     put_be32(hdr + 16, static_cast<uint32_t>(w));
     put_be32(hdr + 20, static_cast<uint32_t>(h));
-    hdr[24] = 8;                                   // bit depth; colour type 0 (grey), no interlace
-    hdr[25] = hdr[26] = hdr[27] = hdr[28] = 0;
+    hdr[24] = 8;                                   // bit depth; colour type 0 (grey) or 3 (palette), no interlace
+    hdr[25] = plte.bytes ? 3 : 0;
+    hdr[26] = hdr[27] = hdr[28] = 0;
     put_be32(hdr + 29, crc32_bytes(hdr + 12, 17));
     for (int i = 0; i < 33; ++i) file[i] = hdr[i];
   }
+  if (seg == 0)
+    for (int i = t; i < plte.bytes; i += 256) file[33 + i] = plte.chunk[i];
   if (last && t == 0) {
     const uint32_t a = static_cast<uint32_t>(((s2 % kAdlerMod) << 16) | (s1 % kAdlerMod));
     const uint8_t fixed[14] = {0, 0, 0, 6, 'I', 'D', 'A', 'T', 0x03, 0x00};
@@ -628,8 +640,21 @@ extern "C" size_t osvos_png_encode_workspace_bytes(int n, int h, int w) {
   return png_plan(n, h, w).bytes;
 }
 
-extern "C" int osvos_png_encode(const uint8_t* src, uint8_t* out, int64_t* lengths, void* workspace, int n, int h, int w,
-                                osvos_stream_t stream_) {
+extern "C" size_t osvos_png_max_bytes_palette(int h, int w, int entries) {
+  return png_dims_ok(h, w) && entries >= 1 && entries <= 256 ? png_max_bytes(h, w) + 12 + 3 * entries : 0;
+}
+
+static uint32_t png_host_crc32(const uint8_t* p, int n) {
+  uint32_t c = 0xFFFFFFFFu;
+  for (int i = 0; i < n; ++i) {
+    c ^= p[i];
+    for (int k = 0; k < 8; ++k) c = (c & 1) ? (c >> 1) ^ kCrcPoly : c >> 1;
+  }
+  return ~c;
+}
+
+static int png_encode_impl(const uint8_t* src, const PngPlte& plte, uint8_t* out, int64_t* lengths, void* workspace,
+                           int n, int h, int w, size_t max_bytes, osvos_stream_t stream_) {
   OSVOS_CHECK_ARG(src != nullptr && out != nullptr && lengths != nullptr && workspace != nullptr);
   OSVOS_CHECK_ARG(n > 0 && n < 65536 && png_dims_ok(h, w));
   OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 15) == 0 && (reinterpret_cast<uintptr_t>(lengths) & 7) == 0);
@@ -650,7 +675,30 @@ extern "C" int osvos_png_encode(const uint8_t* src, uint8_t* out, int64_t* lengt
                                                                     p.seg_cap, seg_bytes_cap);
   OSVOS_CHECK_CUDA(cudaGetLastError());
   png_assemble_kernel<<<dim3(p.nseg, n), 256, 0, stream>>>(slots, sizes, adler, out, reinterpret_cast<long long*>(lengths),
-                                                           h, w, p.rows, p.nseg, p.seg_cap, png_max_bytes(h, w));
+                                                           h, w, p.rows, p.nseg, p.seg_cap, max_bytes, plte);
   OSVOS_CHECK_CUDA(cudaGetLastError());
   return OSVOS_OK;
+}
+
+extern "C" int osvos_png_encode(const uint8_t* src, uint8_t* out, int64_t* lengths, void* workspace, int n, int h, int w,
+                                osvos_stream_t stream) {
+  PngPlte plte{};
+  return png_encode_impl(src, plte, out, lengths, workspace, n, h, w, png_dims_ok(h, w) ? png_max_bytes(h, w) : 0,
+                         stream);
+}
+
+extern "C" int osvos_png_encode_palette(const uint8_t* src, const uint8_t* palette, int entries, uint8_t* out,
+                                        int64_t* lengths, void* workspace, int n, int h, int w, osvos_stream_t stream) {
+  OSVOS_CHECK_ARG(palette != nullptr && entries >= 1 && entries <= 256);
+  PngPlte plte{};
+  const int len = 3 * entries;
+  plte.chunk[0] = plte.chunk[1] = 0;
+  plte.chunk[2] = static_cast<uint8_t>(len >> 8);
+  plte.chunk[3] = static_cast<uint8_t>(len);
+  memcpy(plte.chunk + 4, "PLTE", 4);
+  memcpy(plte.chunk + 8, palette, len);
+  const uint32_t crc = png_host_crc32(plte.chunk + 4, 4 + len);
+  for (int k = 0; k < 4; ++k) plte.chunk[8 + len + k] = static_cast<uint8_t>(crc >> (24 - 8 * k));
+  plte.bytes = 12 + len;
+  return png_encode_impl(src, plte, out, lengths, workspace, n, h, w, osvos_png_max_bytes_palette(h, w, entries), stream);
 }

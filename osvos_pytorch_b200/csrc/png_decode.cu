@@ -1,5 +1,6 @@
-// PNG decoder for 8-bit and 1-bit grayscale files (DESIGN.md §22): the inverse of csrc/png.cu, and of any other encoder
-// that stays inside the subset osvos_pytorch_b200/png.py parses (colour type 0, depth 8 or 1, no interlace).
+// PNG decoder for 8-bit and 1-bit grayscale files and 1/2/4/8-bit palette files (DESIGN.md §22, §24): the inverse of
+// csrc/png.cu, and of any other encoder that stays inside the subset osvos_pytorch_b200/png.py parses (colour type 0 at
+// depth 8 or 1, or, when the caller asks for indices, colour type 3 at depth 1, 2, 4 or 8; no interlace).
 //
 // The host walks the chunks, checks the CRCs, concatenates the IDAT payloads into one zlib stream per file and PROPOSES
 // cuts of that stream: positions just after an IDAT payload that ends in 00 00 FF FF, where a full flush would leave the
@@ -24,7 +25,8 @@
 //                        filters in place, rows in order: runs of Sub rows one warp per row (prefix sum), runs of Up
 //                        rows one thread per column, runs of Average / Paeth rows as a skewed wavefront in one warp
 //                        (lane j on row r + j, one pixel behind lane j - 1, the row above handed down by shuffle);
-//   png_expand_kernel    the rows without their type bytes into out; depth 1 expanded to 0 / 255.
+//   png_expand_kernel    the rows without their type bytes into out; gray depth 1 expanded to 0 / 255, palette
+//                        samples unpacked MSB first to their raw index.
 // Inflate is one warp per stream with every lane running the same control flow on the same bits: the Huffman tables are
 // built by the warp in shared memory (canonical codes, a first-level lookup plus the per-length counts for longer
 // codes), lane 0 writes literals and all lanes copy matches.  Every read is bounded by the segment's end and every
@@ -47,7 +49,7 @@ struct PngBlobHeader {
   int64_t files_off, segs_off, data_off, data_bytes;
 };
 struct PngBlobFile {
-  int32_t h, w, depth, seg0, nseg, pad[3];
+  int32_t h, w, depth, seg0, nseg, colour, pad[2];   // colour: PNG colour type, 0 (grayscale) or 3 (palette)
   int64_t stream_off, stream_len;    // the zlib stream (header, deflate data, Adler-32) inside the data area
 };
 struct PngBlobSegment {
@@ -97,7 +99,12 @@ __device__ PngLayout png_layout(const PngDecodeParams& p) {
   return l;
 }
 
-__device__ __forceinline__ int png_row_bytes(int depth, int w) { return depth == 8 ? w : (w + 7) >> 3; }
+__device__ __forceinline__ int png_row_bytes(int depth, int w) { return (w * depth + 7) >> 3; }
+
+// grayscale at depth 8 or 1, palette at depth 1, 2, 4 or 8
+__device__ __forceinline__ bool png_format_ok(int colour, int depth) {
+  return colour == 0 ? (depth == 8 || depth == 1) : colour == 3 && (depth == 1 || depth == 2 || depth == 4 || depth == 8);
+}
 
 // ---- validate -------------------------------------------------------------------------------------------------------
 
@@ -110,7 +117,7 @@ __global__ void png_validate_kernel(PngDecodeParams p) {
   if (ok) {
     const PngBlobFile F = l.files[f];
     const int64_t prev_end = f == 0 ? 0 : static_cast<int64_t>(l.files[f - 1].seg0) + l.files[f - 1].nseg;
-    ok = F.h == p.h && F.w == p.w && (F.depth == 8 || F.depth == 1) && F.nseg >= 1 && F.seg0 >= 0 &&
+    ok = F.h == p.h && F.w == p.w && png_format_ok(F.colour, F.depth) && F.nseg >= 1 && F.seg0 >= 0 &&
          F.seg0 == prev_end && static_cast<int64_t>(F.seg0) + F.nseg <= p.nseg &&
          (f + 1 < p.n || static_cast<int64_t>(F.seg0) + F.nseg == p.nseg) && F.stream_off >= 0 && F.stream_len >= 6 &&
          F.stream_off <= l.data_bytes && F.stream_len <= l.data_bytes - F.stream_off;
@@ -675,7 +682,10 @@ __global__ void __launch_bounds__(256) png_expand_kernel(PngDecodeParams p) {
   const PngLayout l = png_layout(p);
   if (!l.ok || p.status[f] != 0) return;
   const int depth = l.files[f].depth;
+  const bool gray = l.files[f].colour == 0;
   const int rb = png_row_bytes(depth, p.w), stride = rb + 1;
+  const int per_byte_log2 = depth == 1 ? 3 : depth == 2 ? 2 : depth == 4 ? 1 : 0;
+  const int mask = (1 << depth) - 1;
   const uint8_t* fb = p.filt + static_cast<size_t>(f) * p.fstride;
   uint8_t* out = p.out + static_cast<size_t>(f) * p.h * p.w;
   const long long total = static_cast<long long>(p.h) * p.w;
@@ -683,7 +693,10 @@ __global__ void __launch_bounds__(256) png_expand_kernel(PngDecodeParams p) {
        i += static_cast<long long>(gridDim.x) * 256) {
     const int y = static_cast<int>(i / p.w), x = static_cast<int>(i - static_cast<long long>(y) * p.w);
     const uint8_t* row = fb + static_cast<size_t>(y) * stride + 1;
-    out[i] = depth == 8 ? row[x] : (((row[x >> 3] >> (7 - (x & 7))) & 1) ? 255 : 0);
+    // samples MSB first; a palette sample is its index, a 1-bit gray sample 0 / 255
+    const int shift = 8 - depth * ((x & ((1 << per_byte_log2) - 1)) + 1);
+    const int v = (row[x >> per_byte_log2] >> shift) & mask;
+    out[i] = static_cast<uint8_t>(gray && depth == 1 ? v * 255 : v);
   }
 }
 

@@ -30,6 +30,8 @@ from torch.utils.data import Dataset
 from . import augment as _augment
 from . import jpeg as _jpeg
 from . import ops
+from . import png as _png
+from .evaluation import n_objects as _n_objects
 from .ops import MEANVAL
 
 
@@ -111,6 +113,9 @@ class DAVIS2016Frames(Dataset):
             raise FileNotFoundError(f"cv2.imread could not read {os.path.join(self.db_root_dir, rel)}")
         return arr
 
+    def _read_gt(self, rel):
+        return self._read(rel, 0)
+
     def __getitem__(self, idx):
         item = {}
         parsed = None
@@ -124,13 +129,70 @@ class DAVIS2016Frames(Dataset):
             item["image"] = self._read(self.img_list[idx], 1)          # cv2.IMREAD_COLOR: uint8 [H,W,3] BGR
             size = item["image"].shape[:2]
         has_gt = self.labels[idx] is not None
-        gt = self._read(self.labels[idx], 0) if has_gt else np.zeros(size, dtype=np.uint8)
+        gt = self._read_gt(self.labels[idx]) if has_gt else np.zeros(size, dtype=np.uint8)
         if self.seq_name is not None:
             fname = os.path.join(self.seq_name, "%05d" % idx)
         else:
             parts = self.img_list[idx].split("/")
             fname = os.path.join(parts[-2], os.path.splitext(parts[-1])[0])
         item.update(gt=gt, has_gt=has_gt, fname=fname)
+        return item
+
+
+class DAVIS2017Frames(DAVIS2016Frames):
+    """DAVIS-2017 (semi-supervised), items as DAVIS2016Frames' with ``gt`` = the annotation's object ids and
+    ``n_objects`` (DESIGN.md §24).
+
+    The sequences are those of ``ImageSets/2017/<split>.txt`` (``split`` "train" or "val"), frames from
+    ``JPEGImages/480p/<seq>/`` and annotations from ``Annotations/480p/<seq>/``, which are 8-bit palette PNGs: 0
+    background, 1 .. K the objects, 255 void.  Each annotation is read as its indices (np.array(PIL.Image.open(f)), the
+    toolkit's reader), never converted to gray.  A sequence's objects are 1 .. K with K = evaluation.n_objects of its
+    first annotation, and ``palettes[seq]`` is that annotation's PLTE bytes (png.palette_of), the palette to write the
+    sequence's results with.  ``seq_name`` and ``all_annotations`` are DAVIS2016Frames' sequence mode (only the first
+    frame annotated unless ``all_annotations``); ``decode`` applies to the JPEG frames as there."""
+
+    def __init__(self, split="val", db_root_dir=None, seq_name=None, all_annotations=False, decode="host"):
+        if split not in ("train", "val"):
+            raise ValueError("split must be 'train' or 'val'")
+        if decode not in ("host", "device"):
+            raise ValueError("decode must be 'host' or 'device'")
+        self.decode, self.train, self.split, self.seq_name, self.meanval = decode, False, split, seq_name, MEANVAL
+        self.db_root_dir = default_db_root() if db_root_dir is None else db_root_dir
+        root = self.db_root_dir
+        if seq_name is None:
+            with open(os.path.join(root, "ImageSets", "2017", split + ".txt")) as f:
+                seqs = [x.strip() for x in f if x.strip()]
+        else:
+            seqs = [str(seq_name)]
+        img_list, labels, self.seq_of = [], [], []
+        self.n_objects, self.palettes = {}, {}
+        for seq in seqs:
+            images = np.sort(os.listdir(os.path.join(root, "JPEGImages/480p/", seq)))
+            anns = np.sort([x for x in os.listdir(os.path.join(root, "Annotations/480p/", seq)) if x.endswith(".png")])
+            if not len(anns):
+                raise ValueError(f"{root}: sequence {seq} has no annotation")
+            if seq_name is None or all_annotations:
+                if len(anns) != len(images):
+                    raise ValueError(f"{root}: sequence {seq} has {len(images)} frames but {len(anns)} annotations")
+                labs = [os.path.join("Annotations/480p/", seq, x) for x in anns]
+            else:
+                labs = [os.path.join("Annotations/480p/", seq, anns[0])] + [None] * (len(images) - 1)
+            img_list.extend(os.path.join("JPEGImages/480p/", seq, x) for x in images)
+            labels.extend(labs)
+            self.seq_of.extend([seq] * len(images))
+            with open(os.path.join(root, labs[0]), "rb") as f:
+                first = f.read()
+            self.n_objects[seq] = _n_objects(_png.decode_host_index(first))
+            self.palettes[seq] = _png.palette_of(first)
+        self.img_list, self.labels = img_list, labels
+
+    def _read_gt(self, rel):
+        with open(os.path.join(self.db_root_dir, rel), "rb") as f:
+            return _png.decode_host_index(f.read())
+
+    def __getitem__(self, idx):
+        item = super().__getitem__(idx)
+        item["n_objects"] = self.n_objects[self.seq_of[idx]]
         return item
 
 

@@ -1,4 +1,5 @@
-"""DAVIS-2016 region (J) and boundary (F) scores from the device counts of ``ops.davis_measures`` (DESIGN.md §14).
+"""DAVIS-2016 region (J) and boundary (F) scores from the device counts of ``ops.davis_measures`` (DESIGN.md §14), and
+their DAVIS-2017 per-object form from ``ops.davis_measures_objects`` (``ObjectScores``, DESIGN.md §24).
 
 The kernel produces six integers per frame; this module turns them into J and F (on the device, no synchronisation)
 and a sequence's per-frame series into the benchmark's statistics: mean M, recall O and decay D.  As the DAVIS-2016
@@ -79,14 +80,69 @@ def dataset_scores(per_seq):
             for m in ("J", "F")}
 
 
+def n_objects(first_gt):
+    """The object ids of a DAVIS-2017 sequence are 1 .. K, K = the largest value of its first annotation other than 255
+    (void): the toolkit's rule.  ``first_gt``: uint8 array or tensor [H,W]."""
+    g = torch.as_tensor(np.asarray(first_gt.cpu() if torch.is_tensor(first_gt) else first_gt))
+    g = torch.where(g == 255, torch.zeros_like(g), g)
+    return int(g.max()) if g.numel() else 0
+
+
+class ObjectScores:
+    """SequenceScores for DAVIS-2017: accumulates per-object device counts [N,K,6] (ops.davis_measures_objects) frame by
+    frame without synchronising; ``result()`` reads them back once."""
+
+    def __init__(self, n_objects):
+        self.n_objects = int(n_objects)
+        self._counts = []
+
+    def add(self, counts):
+        self._counts.append(counts.reshape(-1, self.n_objects, 6))
+
+    def result(self):
+        """{'objects': {object id: {'J', 'F' (per-frame lists), 'statistics': {'J': {M, O, D}, 'F': {M, O, D}}}},
+        'counts': per-frame lists of K lists of six ints}.  An object absent from a frame is scored on that frame."""
+        if not self._counts:
+            counts = torch.zeros((0, self.n_objects, 6), dtype=torch.int32)
+        else:
+            counts = torch.cat([c.to(self._counts[0].device) for c in self._counts]).cpu()
+        j, f = j_and_f(counts)                                     # [frames, K]
+        objects = {}
+        for k in range(self.n_objects):
+            objects[k + 1] = {"J": j[:, k].tolist(), "F": f[:, k].tolist(),
+                              "statistics": {"J": statistics(j[:, k]), "F": statistics(f[:, k])}}
+        return {"objects": objects, "counts": counts.tolist()}
+
+
+def dataset_scores_objects(per_seq):
+    """{sequence: ObjectScores or its result()} -> the DAVIS-2017 global figures: {'J': {M, O, D}, 'F': {M, O, D},
+    'J&F': (J_M + F_M) / 2, 'objects': count}, every mean taken over all objects of all sequences (not over sequences),
+    as the toolkit's global table does (NaN without objects)."""
+    stats = [ob["statistics"] for sc in per_seq.values()
+             for ob in (sc.result() if isinstance(sc, ObjectScores) else sc)["objects"].values()]
+    out = {m: {k: float(np.mean([st[m][k] for st in stats])) if stats else float("nan") for k in "MOD"}
+           for m in ("J", "F")}
+    out["J&F"] = (out["J"]["M"] + out["F"]["M"]) / 2
+    out["objects"] = len(stats)
+    return out
+
+
 def _png_stems(folder):
     import os
     return sorted(f[:-4] for f in os.listdir(folder) if f.lower().endswith(".png"))
 
 
 def score_results(results_dir, db_root_dir=None, sequences=None, threshold=128, device="cuda", batch=16,
-                  decode="device", readers=4):
+                  decode="device", readers=4, davis="2016"):
     """Scores a folder of result PNGs against the DAVIS-2016 annotations (DESIGN.md §22).
+
+    ``davis="2017"`` (DESIGN.md §24): results and annotations are palette (or grayscale) PNGs of object ids, both
+    decoded to their indices (``png.parse(..., palette="index")``: on the device, Pillow for files outside its subset;
+    ``decode="host"``: Pillow for every file).  The default sequences are those of ``ImageSets/2017/val.txt`` that have
+    a folder under ``results_dir``; each sequence's objects are 1 .. n_objects(first annotation), scored per object
+    with ops.davis_measures_objects (void pixels, 255, ignored).  ``threshold`` does not apply.  Returns
+    {'sequences': {seq: ObjectScores.result()}, 'dataset': dataset_scores_objects(...), 'frames', 'fallback_files',
+    'redecoded_files'}.
 
     ``results_dir/<seq>/<stem>.png`` is paired with ``db_root_dir/Annotations/480p/<seq>/<stem>.png`` by file stem;
     a missing result, a missing annotation or differing sizes raise ValueError.  ``sequences``: the sequences to score
@@ -104,16 +160,20 @@ def score_results(results_dir, db_root_dir=None, sequences=None, threshold=128, 
     from . import ops, png
     if decode not in ("device", "host"):
         raise ValueError(f"decode must be 'device' or 'host', got {decode!r}")
+    if davis not in ("2016", "2017"):
+        raise ValueError(f"davis must be '2016' or '2017', got {davis!r}")
+    multi = davis == "2017"
     if db_root_dir is None:
         from mypath import Path
         db_root_dir = Path.db_root_dir()
     ann_root = os.path.join(db_root_dir, "Annotations", "480p")
     if sequences is None:
-        with open(os.path.join(db_root_dir, "val_seqs.txt")) as f:
+        listing = os.path.join("ImageSets", "2017", "val.txt") if multi else "val_seqs.txt"
+        with open(os.path.join(db_root_dir, listing)) as f:
             sequences = [s.strip() for s in f if s.strip()]
         sequences = [s for s in sequences if os.path.isdir(os.path.join(results_dir, s))]
         if not sequences:
-            raise ValueError(f"no sequence of val_seqs.txt has a folder under {results_dir}")
+            raise ValueError(f"no sequence of {listing} has a folder under {results_dir}")
     pairs = []                                               # (sequence, result path, annotation path)
     for seq in sequences:
         res_dir, ann_dir = os.path.join(results_dir, seq), os.path.join(ann_root, seq)
@@ -128,19 +188,23 @@ def score_results(results_dir, db_root_dir=None, sequences=None, threshold=128, 
             raise ValueError(f"sequence {seq!r}: no annotation for result(s) {', '.join(extra[:5])} in {ann_dir}")
         pairs.extend((seq, os.path.join(res_dir, s + ".png"), os.path.join(ann_dir, s + ".png")) for s in want)
 
+    mode = "index" if multi else None
+
     def read(path):
         with open(path, "rb") as f:
             data = f.read()
-        return (data, png.parse(data)) if decode == "device" else (png.decode_host(data), None)
+        if decode == "device":
+            return data, png.parse(data, palette=mode)
+        return (png.decode_host_index(data) if multi else png.decode_host(data)), None
 
     def to_device(items):
         if decode == "device":
-            return png.decode_files([d for d, _ in items], device, parsed=[p for _, p in items])
+            return png.decode_files([d for d, _ in items], device, parsed=[p for _, p in items], palette=mode)
         if len({m.shape for m, _ in items}) != 1:
             raise ValueError("the files differ in size")
         return torch.from_numpy(np.stack([m for m, _ in items])).to(device), 0, 0
 
-    scores = {seq: SequenceScores() for seq in sequences}
+    scores = {} if multi else {seq: SequenceScores() for seq in sequences}
     fallback = redecoded = 0
     threshold = int(threshold)
     with ThreadPoolExecutor(max(1, int(readers))) as pool:
@@ -164,9 +228,18 @@ def score_results(results_dir, db_root_dir=None, sequences=None, threshold=128, 
                                  f"{ann.shape[1]}x{ann.shape[2]}")
             fallback += fb_r + fb_a
             redecoded += rd_r + rd_a
-            pred = torch.where(res >= threshold, 1.0, -1.0).to(torch.float32)
-            scores[seq].add(ops.davis_measures(pred, ann))
+            if multi:
+                if seq not in scores:                        # the batch starts the sequence: ann[0] is its first frame
+                    k = n_objects(ann[0])
+                    if k == 0:
+                        raise ValueError(f"sequence {seq!r}: the first annotation has no object")
+                    scores[seq] = ObjectScores(k)
+                scores[seq].add(ops.davis_measures_objects(res, ann, scores[seq].n_objects))
+            else:
+                pred = torch.where(res >= threshold, 1.0, -1.0).to(torch.float32)
+                scores[seq].add(ops.davis_measures(pred, ann))
             start = stop
     per_seq = {seq: sc.result() for seq, sc in scores.items()}
-    return {"sequences": per_seq, "dataset": dataset_scores(per_seq), "frames": len(pairs),
+    dataset = dataset_scores_objects(per_seq) if multi else dataset_scores(per_seq)
+    return {"sequences": per_seq, "dataset": dataset, "frames": len(pairs),
             "fallback_files": fallback, "redecoded_files": redecoded}

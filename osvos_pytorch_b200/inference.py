@@ -57,12 +57,32 @@ class SequenceSegmenter:
     ``overlay_quality`` (ops.encode_jpeg, DESIGN.md §23), on the compute stream before the slot is released, into a
     per-slot buffer of fixed address that crosses device->host at its capacity with the file lengths.  Each yielded
     item is then ``(result, overlays)``, ``overlays`` a list of N ``memoryview``s, one complete JPEG file each, valid
-    as long as the result is."""
+    as long as the result is.
 
-    def __init__(self, net, output="logits", depth=3, frames="nchw_f32", meanval=ops.MEANVAL, score=False,
-                 input_res=None, output_res="network", encode=None, overlay=None, overlay_quality=95):
-        if output not in ("logits", "bytescale", "prob", "mask"):
-            raise ValueError("output must be one of logits / bytescale / prob / mask")
+    ``nets=[net_1, ..., net_K]`` with ``output="labels"`` (DAVIS-2017, one fine-tuned network per object; DESIGN.md
+    §24): per frame every net's forward runs on the same fp32 slot and ops.merge_objects turns the K fused maps into
+    the slot's uint8 label map (1 + the object of the largest positive logit, 0 background), so each result is uint8
+    [N,1,H,W] of object ids.  ``score=True`` scores it with ops.davis_measures_objects against the slot's annotation
+    (object ids, 255 void) and ``frame_counts()`` returns [frames*N, K, 6].  ``encode="png"`` with ``palette`` (the
+    PLTE bytes, e.g. the first annotation's) writes palette files.  ``input_res``, ``output_res="stored"`` and
+    ``overlay`` are not available with labels."""
+
+    def __init__(self, net=None, output="logits", depth=3, frames="nchw_f32", meanval=ops.MEANVAL, score=False,
+                 input_res=None, output_res="network", encode=None, overlay=None, overlay_quality=95, nets=None,
+                 palette=None):
+        if (net is None) == (nets is None):
+            raise ValueError("pass either net or nets")
+        nets = [net] if nets is None else list(nets)
+        if not 1 <= len(nets) <= 254 or len({id(m) for m in nets}) != len(nets):
+            raise ValueError("nets must be 1 .. 254 distinct networks")
+        if output not in ("logits", "bytescale", "prob", "mask", "labels"):
+            raise ValueError("output must be one of logits / bytescale / prob / mask / labels")
+        if len(nets) > 1 and output != "labels":
+            raise ValueError("several nets are merged into a label map: they need output='labels'")
+        if output == "labels" and (input_res is not None or output_res != "network" or overlay is not None):
+            raise ValueError("output='labels' does not take input_res, output_res='stored' or overlay")
+        if palette is not None and (output != "labels" or encode != "png"):
+            raise ValueError("palette writes label maps as palette PNGs: it needs output='labels' and encode='png'")
         if frames not in ("nchw_f32", "bgr8", "jpeg"):
             raise ValueError("frames must be nchw_f32, bgr8 or jpeg")
         if input_res is not None and frames == "nchw_f32":
@@ -79,7 +99,8 @@ class SequenceSegmenter:
             raise ValueError("overlay='jpeg' draws over the frames' bytes: it needs frames='bgr8' or 'jpeg'")
         if not 1 <= int(overlay_quality) <= 100:
             raise ValueError("overlay_quality must lie in 1..100")
-        self.net, self.output, self.depth = net, output, max(2, int(depth))
+        self.nets, self.net, self.output, self.depth = nets, nets[0], output, max(2, int(depth))
+        self.palette = None if palette is None else bytes(palette)
         self.frames, self.meanval = frames, tuple(meanval)
         self.score = bool(score)
         self.input_res = input_res
@@ -108,7 +129,7 @@ class SequenceSegmenter:
         self._dev_in = [torch.empty((n, 3, h, w), dtype=torch.float32, device=device) for _ in range(self.depth)]
         self._dev_out = [torch.empty((n, 1, rh, rw), dtype=out_dtype, device=device) for _ in range(self.depth)]
         if self.encode == "png":
-            cap = ops.png_max_bytes(rh, rw)
+            cap = ops.png_max_bytes(rh, rw, self.palette)
             self._dev_png = [torch.empty((n, cap), dtype=torch.uint8, device=device) for _ in range(self.depth)]
             self._dev_len = [torch.empty(n, dtype=torch.int64, device=device) for _ in range(self.depth)]
             self._host_png = [torch.empty((n, cap), dtype=torch.uint8).pin_memory() for _ in range(self.depth)]
@@ -183,17 +204,25 @@ class SequenceSegmenter:
             # same slot address every time this slot comes round, so the engine's direct graph replay still applies
             ops.image_from_bgr8(raw, self.meanval, out=self._dev_in[k])
         with torch.no_grad():
-            eng = getattr(self.net, "_engine", None)
-            if eng is not None:
-                # the ring slot is a buffer that comes back: from its second frame on the engine replays a graph captured on
-                # the slot itself (no input copy), and the fused map is read out of the graph's static output right here on
-                # the same stream (no copy of the five maps into fresh tensors)
-                fused = eng.forward(self._dev_in[k], fresh_outputs=False)[-1]
-            else:
-                fused = self.net(self._dev_in[k])[-1]
+            fused_maps = []
+            for net in self.nets:
+                eng = getattr(net, "_engine", None)
+                if eng is not None:
+                    # the ring slot is a buffer that comes back: from its second frame on the engine replays a graph
+                    # captured on the slot itself (no input copy), and the fused map is read out of the graph's static
+                    # output right here on the same stream (no copy of the five maps into fresh tensors); each net has
+                    # its own engine, so the K static outputs stay valid until the merge below
+                    fused_maps.append(eng.forward(self._dev_in[k], fresh_outputs=False)[-1])
+                else:
+                    fused_maps.append(net(self._dev_in[k])[-1])
+            fused = fused_maps[0]
             if self._upsample:                                  # back to the stored size, before anything reads it
                 fused = ops.resize_f32(fused, self._dev_up[k].shape[2:4], out=self._dev_up[k])
-            if self.score:
+            if self.output == "labels":
+                labels = ops.merge_objects(fused_maps, out=self._dev_out[k])
+                if self.score:
+                    self._counts.append(ops.davis_measures_objects(labels, gt_dev, len(self.nets)))
+            elif self.score:
                 self._counts.append(ops.davis_measures(fused, gt_dev))
             if self.overlay == "jpeg":                          # reads the slot's frame: before the slot is released
                 img = ops.overlay_mask(self._dev_raw[k] if self._upsample else raw, fused, out=self._dev_ovl)
@@ -202,9 +231,10 @@ class SequenceSegmenter:
             if self.output == "logits":
                 self._dev_out[k].copy_(fused)
             else:
-                ops.logits_to_u8(fused, self.output, out=self._dev_out[k])
+                if self.output != "labels":
+                    ops.logits_to_u8(fused, self.output, out=self._dev_out[k])
                 if self.encode == "png":
-                    ops.encode_png(self._dev_out[k], out=self._dev_png[k], lengths=self._dev_len[k])
+                    ops.encode_png(self._dev_out[k], out=self._dev_png[k], lengths=self._dev_len[k], palette=self.palette)
         self._ev_done[k].record(cur)
         with torch.cuda.stream(self._s_out):
             self._s_out.wait_event(self._ev_done[k])
@@ -281,11 +311,11 @@ class SequenceSegmenter:
 
     def frame_counts(self):
         """int32 [frames*N, 6] host tensor of the last run's ops.davis_measures counts, frame order (score=True);
-        one synchronisation."""
+        [frames*N, K, 6] of ops.davis_measures_objects with output="labels".  One synchronisation."""
         if not self.score:
             raise RuntimeError("frame_counts() needs SequenceSegmenter(..., score=True)")
         if not self._counts:
-            return torch.zeros((0, 6), dtype=torch.int32)
+            return torch.zeros((0, len(self.nets), 6) if self.output == "labels" else (0, 6), dtype=torch.int32)
         return torch.cat(self._counts).cpu()
 
     def join_current_stream(self):

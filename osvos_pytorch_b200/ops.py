@@ -1,7 +1,7 @@
 """Tensor-level wrappers over the C ABI: they allocate outputs with torch (device
 memory + stream plumbing only) and enqueue the native kernels on the current
 torch stream.  No arithmetic happens in Python / PyTorch here."""
-from ctypes import byref
+from ctypes import byref, c_void_p
 
 import torch
 
@@ -864,23 +864,36 @@ def resize_f32(x, size, out=None):
     return out
 
 
-def png_max_bytes(h, w):
-    """Capacity of one encoded frame (osvos_png_max_bytes): the size with every segment stored."""
-    return int(nat.load().osvos_png_max_bytes(int(h), int(w)))
+def _palette_bytes(palette):
+    pal = bytes(palette)
+    if not pal or len(pal) % 3 or len(pal) > 768:
+        raise ValueError(f"palette must be 3 * n bytes with 1 <= n <= 256 (the PLTE chunk's RGB triples), got {len(pal)}")
+    return pal
 
 
-def encode_png(maps, out=None, lengths=None):
+def png_max_bytes(h, w, palette=None):
+    """Capacity of one encoded frame (osvos_png_max_bytes): the size with every segment stored.  With ``palette`` (the
+    PLTE bytes of encode_png) the PLTE chunk is added (osvos_png_max_bytes_palette)."""
+    if palette is None:
+        return int(nat.load().osvos_png_max_bytes(int(h), int(w)))
+    return int(nat.load().osvos_png_max_bytes_palette(int(h), int(w), len(_palette_bytes(palette)) // 3))
+
+
+def encode_png(maps, out=None, lengths=None, palette=None):
     """uint8 maps [N,H,W] or [N,1,H,W] -> (out uint8 [N, png_max_bytes(H, W)], lengths int64 [N]): frame i's 8-bit
     grayscale PNG file is out[i, :lengths[i]], what the reference's sm.imsave (train_online.py:187) or
     Image.fromarray(map, "L").save writes, with other (deterministic) deflate bytes (csrc/png.cu, DESIGN.md §21).
-    No host synchronisation."""
+    ``palette`` (3 * n bytes of RGB triples, 1 <= n <= 256, e.g. png.palette_of a DAVIS-2017 annotation): palette
+    files instead, the bytes as indices (IHDR colour type 3 and a PLTE chunk; the rest of the file is the grayscale
+    one's; out is then [N, png_max_bytes(H, W, palette)], DESIGN.md §24).  No host synchronisation."""
     lib = nat.load()
     _require_cuda(maps, "maps")
     if maps.dtype != torch.uint8 or maps.dim() not in (3, 4) or (maps.dim() == 4 and int(maps.shape[1]) != 1):
         raise ValueError(f"maps must be uint8 [N,H,W] or [N,1,H,W], got {maps.dtype} {tuple(maps.shape)}")
+    pal = None if palette is None else _palette_bytes(palette)
     x = maps.contiguous()
     n, h, w = int(x.shape[0]), int(x.shape[-2]), int(x.shape[-1])
-    cap = lib.osvos_png_max_bytes(h, w)
+    cap = lib.osvos_png_max_bytes(h, w) if pal is None else lib.osvos_png_max_bytes_palette(h, w, len(pal) // 3)
     nbytes = lib.osvos_png_encode_workspace_bytes(n, h, w)
     if cap == 0 or nbytes == 0:
         raise ValueError(f"cannot encode [{n},{h},{w}]: sizes must lie in [1, 32767] and 0 < N < 65536")
@@ -894,8 +907,12 @@ def encode_png(maps, out=None, lengths=None):
         raise ValueError(f"lengths must be a contiguous int64 tensor of shape ({n},)")
     ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
     _count(3)
-    nat.check(lib.osvos_png_encode(x.data_ptr(), out.data_ptr(), lengths.data_ptr(), ws.data_ptr(), n, h, w, _stream()),
-              "osvos_png_encode")
+    if pal is None:
+        nat.check(lib.osvos_png_encode(x.data_ptr(), out.data_ptr(), lengths.data_ptr(), ws.data_ptr(), n, h, w,
+                                       _stream()), "osvos_png_encode")
+    else:
+        nat.check(lib.osvos_png_encode_palette(x.data_ptr(), pal, len(pal) // 3, out.data_ptr(), lengths.data_ptr(),
+                                               ws.data_ptr(), n, h, w, _stream()), "osvos_png_encode_palette")
     return out, lengths
 
 
@@ -920,6 +937,63 @@ def davis_measures(logits, gt_u8, r=None, out=None):
     _count(4)
     nat.check(lib.osvos_davis_measures(x.data_ptr(), g.data_ptr(), out.data_ptr(), ws.data_ptr(), n, h, w, r, _stream()),
               "osvos_davis_measures")
+    return out
+
+
+def merge_objects(maps, out=None):
+    """Per-object fused logit maps -> uint8 label map [N,H,W] (csrc/measures.cu, DESIGN.md §24): label = 1 + argmax_k
+    logit_k where that maximum is > 0, else 0; ties go to the lowest k, NaN never wins and ±0 is background.  ``maps``:
+    a list of K fp32 tensors of one shape [N,1,H,W] or [N,H,W], or one fp32 tensor [K,N,1,H,W] / [K,N,H,W];
+    1 <= K <= 254.  ``out`` may be any contiguous uint8 [N,H,W] tensor (e.g. a view of a [N,1,H,W] buffer), at any
+    alignment.  No host synchronisation."""
+    lib = nat.load()
+    items = list(maps.unbind(0)) if torch.is_tensor(maps) else list(maps)
+    if not 1 <= len(items) <= nat.DAVIS_MAX_OBJECTS:
+        raise ValueError(f"merge_objects takes 1 .. {nat.DAVIS_MAX_OBJECTS} maps, got {len(items)}")
+    shape = tuple(items[0].shape)
+    if len(shape) not in (3, 4) or (len(shape) == 4 and shape[1] != 1):
+        raise ValueError(f"maps must be fp32 [N,1,H,W] or [N,H,W], got {shape}")
+    keep = []
+    for t in items:
+        _require_cuda(t, "maps")
+        if t.dtype != torch.float32 or tuple(t.shape) != shape or t.device != items[0].device:
+            raise ValueError(f"every map must be fp32 {shape} on one device, got {t.dtype} {tuple(t.shape)}")
+        keep.append(t.detach().contiguous())
+    n, h, w = shape[0], shape[-2], shape[-1]
+    if out is None:
+        out = torch.empty((n, h, w), dtype=torch.uint8, device=keep[0].device)
+    elif out.dtype != torch.uint8 or out.numel() != n * h * w or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous uint8 tensor of {n * h * w} elements, e.g. [{n},{h},{w}]")
+    ptrs = (c_void_p * len(keep))(*(t.data_ptr() for t in keep))
+    _count()
+    nat.check(lib.osvos_merge_objects(ptrs, len(keep), out.data_ptr(), n * h * w, _stream()), "osvos_merge_objects")
+    return out
+
+
+def davis_measures_objects(labels, gt, n_objects, r=None, out=None):
+    """DAVIS-2017 per-object J and F counts on the device (csrc/measures.cu, DESIGN.md §24): label maps uint8 [N,H,W]
+    (or [N,1,H,W]) and index annotations uint8 [N,H,W] -> int32 [N,K,6], K = ``n_objects``; row (i, k-1) holds the six
+    counts of davis_measures with P = label == k and G = gt == k, both cleared where gt == 255 (void).  ``r``:
+    boundary tolerance, default evaluation.bound_pix(H, W).  No host synchronisation."""
+    from .evaluation import bound_pix
+    lib = nat.load()
+    g = _require_u8(gt, "gt", 3)
+    n, h, w = (int(v) for v in g.shape)
+    _require_cuda(labels, "labels")
+    if labels.dtype != torch.uint8 or labels.numel() != n * h * w or tuple(labels.shape[-2:]) != (h, w):
+        raise ValueError(f"labels must be uint8 [N,H,W] or [N,1,H,W] matching gt {tuple(g.shape)}, got "
+                         f"{labels.dtype} {tuple(labels.shape)}")
+    k = int(n_objects)
+    if not 1 <= k <= nat.DAVIS_MAX_OBJECTS or n * k >= 65536:
+        raise ValueError(f"n_objects must lie in 1 .. {nat.DAVIS_MAX_OBJECTS} with N * K < 65536, got K = {k}, N = {n}")
+    lab = labels.contiguous()
+    r = bound_pix(h, w) if r is None else int(r)
+    if out is None:
+        out = torch.empty((n, k, 6), dtype=torch.int32, device=g.device)
+    ws = torch.empty(lib.osvos_davis_measures_objects_workspace_bytes(n, k, h, w), dtype=torch.uint8, device=g.device)
+    _count(4)
+    nat.check(lib.osvos_davis_measures_objects(lab.data_ptr(), g.data_ptr(), out.data_ptr(), ws.data_ptr(), n, k, h, w,
+                                               r, _stream()), "osvos_davis_measures_objects")
     return out
 
 
@@ -962,7 +1036,8 @@ def decode_jpeg(blob, n, h, w, out=None, status=None, nseg=None, chunk_bits=0):
 
 def decode_png(blob, n, h, w, nseg, out=None, status=None, path=None):
     """A batch of n grayscale PNGs of size h x w packed by png.pack (``blob``: uint8 device tensor) -> (out uint8
-    [n,h,w], what cv2.imread(path, 0) gives, 1-bit files as 0 / 255; status int32 [n]: 1 invalid block type, code
+    [n,h,w], what cv2.imread(path, 0) gives, 1-bit files as 0 / 255; palette files parsed with palette="index" as
+    their raw indices, what np.array(PIL.Image.open(f)) gives (DESIGN.md §24); status int32 [n]: 1 invalid block type, code
     lengths or code, 2 distance beyond the bytes written, 4 stream ended early or wrong output size, 8 Adler-32
     mismatch, 16 filter type above 4, 32 header inconsistent with (n, h, w)).  ``out`` may be any contiguous uint8
     [n,h,w] tensor, at any alignment.  ``nseg`` (required): the blob's segment count, png.segment_count of the host

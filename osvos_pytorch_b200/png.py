@@ -6,6 +6,11 @@ is outside the subset the device decodes: colour type 0 (grayscale), bit depth 8
 ancillary chunks, any split of the zlib stream over ``IDAT`` chunks.  Everything else is decoded by
 ``cv2.imdecode(..., 0)`` on the host.  Bit depth 1 decodes to 0 / 255, as cv2 gives.
 
+``parse(data, palette="index")`` (DAVIS-2017 label files, DESIGN.md §24) also accepts colour type 3 (palette) at bit
+depths 1, 2, 4 and 8, with or without ``tRNS`` (transparency does not change the indices); the device writes each
+pixel's raw index, what ``np.array(PIL.Image.open(f))`` gives.  In that mode the host fallback is Pillow, never cv2,
+whose conversion to gray would lose the indices.
+
 Proposed cuts: a zlib stream can be inflated in independent pieces where a full flush happened: the stream is on a
 byte boundary there, the bytes before it are ``00 00 FF FF`` and no match reaches back across it.  The project's own
 encoder (csrc/png.cu) ends every ``IDAT`` that way.  ``parse`` proposes a cut after every ``IDAT`` payload that ends
@@ -31,7 +36,8 @@ import numpy as np
 
 MAGIC = 0x31474E50                      # "PNG1"
 HEADER = struct.Struct("<8i4q")
-FILE = np.dtype([("h", "<i4"), ("w", "<i4"), ("depth", "<i4"), ("seg0", "<i4"), ("nseg", "<i4"), ("pad", "<i4", 3),
+FILE = np.dtype([("h", "<i4"), ("w", "<i4"), ("depth", "<i4"), ("seg0", "<i4"), ("nseg", "<i4"), ("colour", "<i4"),
+                 ("pad", "<i4", 2),
                  ("stream_off", "<i8"), ("stream_len", "<i8")])
 SEGMENT = np.dtype([("beg", "<i8"), ("end", "<i8"), ("file", "<i4"), ("index", "<i4")])
 SIGNATURE = b"\x89PNG\r\n\x1a\n"
@@ -53,20 +59,26 @@ class Parsed:
     depth: int
     stream: bytes                                   # the zlib stream: the IDAT payloads concatenated
     cuts: list = field(default_factory=list)        # proposed segment starts after the first, offsets in ``stream``
+    colour: int = 0                                 # PNG colour type: 0 grayscale, 3 palette
+    palette: bytes = None                           # the PLTE chunk's bytes (RGB triples) of a palette file
 
     @property
     def rowbytes(self):
-        return self.w if self.depth == 8 else -(-self.w // 8)
+        return -(-self.w * self.depth // 8)
 
 
-def parse(data):
-    """Parse a PNG file's bytes -> Parsed, or Fallback(reason) for a file outside the device subset."""
+def parse(data, palette=None):
+    """Parse a PNG file's bytes -> Parsed, or Fallback(reason) for a file outside the device subset.  ``palette``:
+    None (grayscale files only) or "index" (palette files too, decoded to their indices)."""
+    if palette not in (None, "index"):
+        raise ValueError(f"palette must be None or 'index', got {palette!r}")
     data = bytes(data)
     if data[:8] != SIGNATURE:
         return Fallback("not a PNG (no signature)")
     p, n = 8, len(data)
     ihdr = None
     payloads = []
+    plte = trns = None
     ended = False
     while p < n:
         if p + 12 > n:
@@ -85,18 +97,28 @@ def parse(data):
             ihdr = struct.unpack(">IIBBBBB", body)
         elif kind == b"IDAT":
             payloads.append(body)
+        elif kind == b"PLTE":
+            plte = body
         elif kind == b"tRNS":
-            return Fallback("tRNS")
+            trns = body
         elif kind == b"IEND":
             ended = True
             break
     if ihdr is None or not ended:
         return Fallback("truncated")
     w, h, depth, colour, compression, filtering, interlace = ihdr
-    if colour != 0:
-        return Fallback(_COLOUR.get(colour, f"colour type {colour}"))
-    if depth not in (1, 8):
-        return Fallback(f"{depth}-bit")
+    if colour == 3 and palette == "index":
+        if depth not in (1, 2, 4, 8):
+            return Fallback(f"{depth}-bit")
+        if plte is None or not plte or len(plte) % 3 or len(plte) > 768:
+            return Fallback("no valid PLTE")
+    else:
+        if colour != 0:
+            return Fallback(_COLOUR.get(colour, f"colour type {colour}"))
+        if trns is not None:
+            return Fallback("tRNS")
+        if depth not in (1, 8):
+            return Fallback(f"{depth}-bit")
     if interlace != 0:
         return Fallback("interlaced")
     if compression != 0 or filtering != 0:
@@ -116,7 +138,7 @@ def parse(data):
         at += len(body)
         if at >= 6 and at < len(stream) and stream[at - 4:at] == FLUSH and (not cuts or cuts[-1] != at):
             cuts.append(at)
-    return Parsed(h, w, depth, stream, cuts)
+    return Parsed(h, w, depth, stream, cuts, colour, plte if colour == 3 else None)
 
 
 def pack(parsed_list):
@@ -131,7 +153,7 @@ def pack(parsed_list):
     off = 0
     for i, p in enumerate(parsed_list):
         bounds = [2] + list(p.cuts) + [len(p.stream)]
-        files[i] = (h, w, p.depth, len(segs), len(bounds) - 1, 0, off, len(p.stream))
+        files[i] = (h, w, p.depth, len(segs), len(bounds) - 1, p.colour, 0, off, len(p.stream))
         segs.extend((off + bounds[k], off + bounds[k + 1], i, k) for k in range(len(bounds) - 1))
         off += len(p.stream)
     parts = [files.tobytes(), np.array(segs, dtype=SEGMENT).tobytes()]
@@ -162,20 +184,50 @@ def decode_host(data):
     return m
 
 
-def decode_files(datas, device, parsed=None):
+def decode_host_index(data):
+    """One file's bytes -> uint8 [h, w] as np.array(PIL.Image.open(f)) gives: a palette file's indices, a grayscale
+    file's values (depth 1 as 0 / 255).  Other colour types raise ValueError."""
+    import io
+
+    from PIL import Image
+    img = Image.open(io.BytesIO(bytes(data)))
+    if img.mode == "1":
+        img = img.convert("L")
+    if img.mode not in ("P", "L"):
+        raise ValueError(f"an index or grayscale PNG is needed, got mode {img.mode}")
+    return np.array(img, dtype=np.uint8)
+
+
+def palette_of(data):
+    """The PLTE chunk's bytes (RGB triples) of a PNG file, or None when it has none."""
+    data = bytes(data)
+    p = 8
+    while p + 8 <= len(data):
+        ln, = struct.unpack(">I", data[p:p + 4])
+        kind = data[p + 4:p + 8]
+        if kind == b"PLTE":
+            return data[p + 8:p + 8 + ln]
+        if kind in (b"IDAT", b"IEND"):
+            return None
+        p += 12 + ln
+    return None
+
+
+def decode_files(datas, device, parsed=None, palette=None):
     """A list of PNG files' bytes, all of one size -> (uint8 [n,h,w] on ``device``, fallback count, re-decoded count).
 
     Files inside the subset are decoded on the device (ops.decode_png); Fallback files, and after one read of the
-    status words the files the decoder flagged, are decoded by cv2 on the host.  ``parsed``: the files' ``parse``
-    results when the caller has them already (reader threads)."""
+    status words the files the decoder flagged, are decoded by cv2 on the host (Pillow with ``palette="index"``,
+    see ``parse``).  ``parsed``: the files' ``parse`` results when the caller has them already (reader threads)."""
     import torch
 
     from . import ops
     if parsed is None:
-        parsed = [parse(d) for d in datas]
+        parsed = [parse(d, palette=palette) for d in datas]
+    host_decode = decode_host_index if palette == "index" else decode_host
     n = len(datas)
     sub = [i for i, p in enumerate(parsed) if isinstance(p, Parsed)]
-    host = {i: decode_host(datas[i]) for i in range(n) if not isinstance(parsed[i], Parsed)}
+    host = {i: host_decode(datas[i]) for i in range(n) if not isinstance(parsed[i], Parsed)}
     fallback = len(host)
     sizes = {(parsed[i].h, parsed[i].w) for i in sub} | {m.shape for m in host.values()}
     if len(sizes) != 1:
@@ -189,7 +241,7 @@ def decode_files(datas, device, parsed=None):
         if len(sub) != n:
             out[torch.tensor(sub, device=device)] = got
         for j in torch.nonzero(status.cpu()).flatten().tolist():
-            host[sub[j]] = decode_host(datas[sub[j]])
+            host[sub[j]] = host_decode(datas[sub[j]])
             if host[sub[j]].shape != (h, w):
                 raise ValueError("the files differ in size")
     if host:

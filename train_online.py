@@ -5,6 +5,7 @@ first frame with SGD(lr 1e-8, momentum .9), save the weights, then segment the s
 
     SEQ_NAME=blackswan python train_online.py --loader native # DAVIS on disk (needs cv2 + the dataset)
     SEQ_NAME=blackswan python train_online.py --loader native --evaluate   # ... and score the masks (J and F)
+    SEQ_NAME=dogs-jump python train_online.py --loader native --davis 2017 --evaluate   # DAVIS-2017, one net per object
     SEQ_NAME=blackswan python train_online.py                 # the same through the reference's dataloaders package
     python train_online.py --synthetic --iters 200            # synthetic 480x854 frame, no dataset
 
@@ -13,12 +14,14 @@ import argparse
 import os
 import timeit
 
+import collections
+
 import numpy as np
 import torch
 
 import networks.vgg_osvos as vo
 from mypath import Path
-from osvos_pytorch_b200 import training
+from osvos_pytorch_b200 import ops, training
 
 
 def parse(argv=None):
@@ -77,6 +80,12 @@ def parse(argv=None):
                          "foreground blended 50/50 with red, its outline black) as Results/<seq>_overlay/<frame>.jpg, "
                          "drawn and JPEG-encoded on the GPU (the bytes cv2.imwrite would write). Needs --loader native")
     ap.add_argument("--overlay-quality", type=int, default=95, help="JPEG quality of --overlay (1..100)")
+    ap.add_argument("--davis", default="2016", choices=["2016", "2017"],
+                    help="2017: a DAVIS-2017 sequence (palette annotations of K objects). The parent is fine-tuned once "
+                         "per object on the first frame with that object's mask, every frame goes through the K nets "
+                         "and each pixel takes the object of the largest positive fused logit; the results are palette "
+                         "PNGs of object ids (the first annotation's palette) and --evaluate scores every object. "
+                         "Needs --loader native; K fine-tunes take K times as long")
     a = ap.parse_args(argv)
     if a.evaluate and (a.synthetic or a.loader != "native"):
         ap.error("--evaluate scores against the DAVIS annotations read by --loader native; it cannot be combined with "
@@ -92,6 +101,12 @@ def parse(argv=None):
                  + ("--synthetic" if a.synthetic else "--loader reference"))
     if not 1 <= a.overlay_quality <= 100:
         ap.error("--overlay-quality must lie in 1..100")
+    if a.davis == "2017":
+        if a.synthetic or a.loader != "native":
+            ap.error("--davis 2017 reads the sequence with --loader native; it cannot be combined with "
+                     + ("--synthetic" if a.synthetic else "--loader reference"))
+        if a.input_res is not None or a.overlay:
+            ap.error("--davis 2017 writes label maps at the stored size: --input-res and --overlay do not apply")
     return a
 
 
@@ -117,6 +132,8 @@ def main(argv=None):
     else:
         ckpt = os.path.join(save_dir, f"{a.parent_name}_epoch-{a.parent_epoch - 1}.pth")
         net.load_state_dict(torch.load(ckpt, map_location="cpu"))
+    if a.davis == "2017":
+        return online_2017(a, net.state_dict(), device, save_dir, iters, log_every)
     net.to(device)
 
     if a.synthetic:
@@ -207,7 +224,6 @@ def main(argv=None):
     # The reference's test loop (train_online.py:172-187): forward -> numpy sigmoid -> scipy.misc.imsave, which min-max
     # bytescales each frame.  Same payload here, produced on the device (ops.logits_to_u8 mode "bytescale") with the
     # H2D / forward / D2H legs of consecutive frames overlapped (inference.SequenceSegmenter).
-    import collections
     from osvos_pytorch_b200.inference import SequenceSegmenter
     names = collections.deque()
     native = a.loader == "native" and not a.synthetic
@@ -278,6 +294,95 @@ def main(argv=None):
             res = dict(network_res=list(input_res), scored_res=stored_hw, **res)
         with open(os.path.join(save_dir, "Results", a.seq_name + "_scores.json"), "w") as f:
             json.dump(dict(sequence=a.seq_name, **res), f, indent=1)
+    return history
+
+
+def online_2017(a, parent, device, save_dir, iters, log_every):
+    """DAVIS-2017 semi-supervised (DESIGN.md §24): one fine-tune of the parent weights ``parent`` per object of the
+    first annotation, then the sequence segmented by the K nets and merged into label maps."""
+    import json
+    import random
+    from torch.utils.data import DataLoader
+    from osvos_pytorch_b200 import augment, davis
+    from osvos_pytorch_b200.evaluation import ObjectScores
+    from osvos_pytorch_b200.inference import SequenceSegmenter
+    first_ds = davis.DAVIS2017Frames(db_root_dir=Path.db_root_dir(), seq_name=a.seq_name, decode=a.decode)
+    first = first_ds[0]                              # read once: every object trains on these bytes
+    k_objects, palette = first["n_objects"], first_ds.palettes[a.seq_name]
+    if k_objects < 1:
+        raise SystemExit(f"sequence {a.seq_name}: the first annotation has no object")
+    img_u8, ids_u8, _ = davis.upload(davis.collate([first]), device)
+    print(f"Start of Online Training, sequence: {a.seq_name}, {k_objects} object(s)")
+    nets, history = [], []
+    t0 = timeit.default_timer()
+    for k in range(1, k_objects + 1):
+        net = vo.OSVOS(pretrained=0, precision=a.precision, learn_upsampling=a.upsampling_lr != 0.0)
+        net.load_state_dict(parent)
+        net.to(device)
+        gt_k = torch.where(ids_u8 == k, 255, 0).to(torch.uint8)          # the object's binary mask as 0 / 255 bytes
+        stats_k = ops.label_stats_u8(gt_k)
+        rng = random.Random(a.seed)
+
+        def sample_fn(it, gt_k=gt_k, stats_k=stats_k, rng=rng):
+            return augment.affine_warp_u8(img_u8, gt_k, augment.draw_params(1, rng=rng), stats_k)
+        hist = training.online_finetune(net, sample_fn, iters, a.n_ave_grad, a.lr, a.wd, log_every,
+                                        upsampling_lr=a.upsampling_lr)
+        if hist and not all(v == v and abs(v) != float("inf") for v in hist):
+            print(f"WARNING: object {k}: non-finite loss - lower --lr for this initialisation")
+        history.append(hist)
+        if not a.no_save:
+            torch.save(net.state_dict(), os.path.join(save_dir, f"{a.seq_name}_object-{k}_epoch-{iters - 1}.pth"))
+        net.eval()
+        nets.append(net)
+    torch.cuda.synchronize()
+    dt = timeit.default_timer() - t0
+    print(f"Online training time: {dt:.2f} s for {k_objects} object(s) ({k_objects * iters / dt:.1f} fwd+bwd/s)")
+
+    print("Testing Network")
+    out_dir = os.path.join(save_dir, "Results", a.seq_name)
+    os.makedirs(out_dir, exist_ok=True)
+    db_test = davis.DAVIS2017Frames(db_root_dir=Path.db_root_dir(), seq_name=a.seq_name, all_annotations=a.evaluate,
+                                    decode=a.decode)
+    test_loader = DataLoader(db_test, batch_size=1, shuffle=False, num_workers=1, collate_fn=davis.collate)
+    jpeg_frames = a.decode == "device"
+    names = collections.deque()
+
+    def frames():
+        for b in test_loader:
+            names.append([os.path.basename(f) for f in b["fname"]])
+            if jpeg_frames:
+                yield b
+            else:
+                img, gt = davis.views(davis.pinned(b["data"]), *(int(v) for v in b["size"]))
+                yield (img, gt) if a.evaluate else img
+    encode = a.encode == "device"
+    seg = SequenceSegmenter(nets=nets, output="labels", frames="jpeg" if jpeg_frames else "bgr8", score=a.evaluate,
+                            encode="png" if encode else None, palette=palette if encode else None)
+    for pred in seg(frames()):
+        batch_names = names.popleft()
+        for jj, name in enumerate(batch_names):
+            path = os.path.join(out_dir, name + ".png")
+            if encode:                                  # one complete palette PNG file per frame
+                with open(path, "wb") as f:
+                    f.write(pred[jj])
+            else:
+                from PIL import Image
+                im = Image.fromarray(pred.numpy()[jj, 0], mode="P")
+                if palette is not None:
+                    im.putpalette(palette)
+                im.save(path)
+    if seg.jpeg_status is not None and int(seg.jpeg_status) != 0:
+        print(f"WARNING: the device JPEG decoder flagged corrupt or cut-short frames (status sum {int(seg.jpeg_status)})")
+    if a.evaluate:
+        scores = ObjectScores(k_objects)
+        scores.add(seg.frame_counts())
+        res = scores.result()
+        for k, ob in res["objects"].items():
+            st = ob["statistics"]
+            print(f"Scores of {a.seq_name} object {k} (frames 1 .. n-2): "
+                  + "  ".join(f"{m} M/O/D: {st[m]['M']:.4f} / {st[m]['O']:.4f} / {st[m]['D']:.4f}" for m in ("J", "F")))
+        with open(os.path.join(save_dir, "Results", a.seq_name + "_scores.json"), "w") as f:
+            json.dump(dict(sequence=a.seq_name, davis="2017", n_objects=k_objects, **res), f, indent=1)
     return history
 
 
