@@ -240,7 +240,8 @@ def wgrad_cases(sms):
 
 
 # ------------------------------------------------------------------------------------------------ kernel names
-_TEMPLATE_ARGS = re.compile(r"(conv3x3_halo_kernel|wgrad_tc_kernel)<([^<>]*)>")
+# kernel name -> number of leading integer template arguments (the rest are bool)
+CONV_KERNELS = {"conv3x3_halo_kernel": 2, "wgrad_tc_kernel": 2}
 
 
 def _template_value(tok):
@@ -250,13 +251,16 @@ def _template_value(tok):
     return int(tok.rstrip("uU"))
 
 
-def parse_kernel_name(name):
-    """Demangled kernel name -> (kernel, template-argument tuple), or None for other kernels.  Accepts both demangled
-    spellings: ``<128, 2, true, false, ...>`` and ``<(int)128, (int)2, (bool)1, ...>``.  Integer arguments come back as
-    int; the boolean positions (from the third on) as bool."""
-    m = _TEMPLATE_ARGS.search(name)
+def parse_kernel_name(name, kernels=None):
+    """Demangled kernel name -> (kernel, template-argument tuple), or None for kernels not in ``kernels`` ({name: number
+    of leading integer arguments}, default CONV_KERNELS).  Accepts both demangled spellings: ``<128, 2, true, false,
+    ...>`` and ``<(int)128, (int)2, (bool)1, ...>``.  The leading integer arguments come back as int, the boolean
+    positions after them as bool."""
+    kernels = CONV_KERNELS if kernels is None else kernels
+    m = re.search(r"\b(" + "|".join(map(re.escape, kernels)) + r")<([^<>]*)>", name)
     if m is None:
         return None
+    n_int = kernels[m.group(1)]
     vals = [_template_value(t) for t in m.group(2).split(",")]
-    vals = vals[:2] + [bool(v) for v in vals[2:]]
+    vals = vals[:n_int] + [bool(v) for v in vals[n_int:]]
     return m.group(1), tuple(vals)

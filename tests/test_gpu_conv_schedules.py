@@ -51,8 +51,12 @@ def sms(dev):
 
 
 class KernelsRan:
-    """Counts the conv3x3_halo_kernel / wgrad_tc_kernel instantiations the device ran inside the block, by their
-    demangled names in a torch.profiler trace of CUDA activity."""
+    """Counts the conv3x3_halo_kernel / wgrad_tc_kernel instantiations (or those ``parse`` recognises) the device ran
+    inside the block, by their demangled names in a torch.profiler trace of CUDA activity; ``seen`` lists every record
+    of the window as (name, device type, count)."""
+    def __init__(self, parse=cdr.parse_kernel_name):
+        self.parse = parse
+
     def __enter__(self):
         from torch.profiler import ProfilerActivity, profile
         torch.cuda.synchronize()
@@ -64,25 +68,27 @@ class KernelsRan:
         torch.cuda.synchronize()
         self.prof.__exit__(*exc)
         self.counts = Counter()
+        self.seen = []
         for ev in self.prof.key_averages():
+            self.seen.append((ev.key[:60], ev.device_type.name, ev.count))
             if ev.device_type.name != "CUDA":
                 continue
-            parsed = cdr.parse_kernel_name(ev.key)
+            parsed = self.parse(ev.key)
             if parsed is not None:
                 self.counts[parsed] += ev.count
         return False
 
 
-def profiled(fn, expected):
-    """fn() under KernelsRan; its kernels must be exactly ``expected`` ({(kernel, template args): launches}).  The
-    profiler occasionally loses a kernel record from a window (a count below the launches made, seen on the H100 at
+def profiled(fn, expected, parse=cdr.parse_kernel_name):
+    """fn() under KernelsRan(parse); its kernels must be exactly ``expected`` ({(kernel, template args): launches}).
+    The profiler occasionally loses a kernel record from a window (a count below the launches made, seen on the H100 at
     about one window in 50); such a window is run again, at most twice.  A wrong instantiation fails either way."""
     for _ in range(3):
-        with KernelsRan() as k:
+        with KernelsRan(parse) as k:
             out = fn()
         if sum(k.counts.values()) >= sum(expected.values()):
             break
-    assert k.counts == expected, k.counts
+    assert k.counts == expected, (k.counts, k.seen[:12])
     return out
 
 
