@@ -130,19 +130,17 @@ OSVOS_API int osvos_conv3x3(const osvos_conv3x3_args* args /* host */, osvos_str
 /* ---- folded side branch (inference and training) ---------------------------------------
  * side_prep has no ReLU (networks/vgg_osvos.py:67), so side_prep followed by score_dsn and this scale's slice of
  * fuse (:44,54,69,72) is ONE 3x3 convolution C -> 2:  W'[o][ci][tap] = sum_co proj_w[16 o + co] * side_w[co][ci][tap],
- * b'[o] = (o == 0 ? proj_b : 0) + sum_co proj_w[16 o + co] * side_b[co].  This writes W' in the packed operand layout
- * (osvos_packed_weight_bytes(2, cin) bytes) and b' (2 floats); osvos_conv3x3 with cout == 2, w_packed = packed,
- * bias = bias2 and pq set then produces the same pq as the cout == 16 call with projections, at 1/8 of the columns. */
-OSVOS_API int osvos_fold_side_weights(const float* side_w /* [16,cin,3,3] */, const float* side_b /* [16] or NULL */,
-                                      const float* proj_w /* [32] */, const float* proj_b /* [1] or NULL */, void* packed,
-                                      float* bias2 /* [2] */, int cin, osvos_stream_t stream);
+ * b'[o] = (o == 0 ? proj_b : 0) + sum_co proj_w[16 o + co] * side_b[co].  osvos_fold_side_weights_multi (below) writes
+ * W' in the packed operand layout (osvos_packed_weight_bytes(2, cin) bytes) and b' (2 floats); osvos_conv3x3 with
+ * cout == 2, w_packed = packed, bias = bias2 and pq set then produces the same pq as the cout == 16 call with
+ * projections, at 1/8 of the columns. */
 /* The folded side convolutions (cout == 2 calls of osvos_conv3x3) of up to four scales in ONE launch: `args` is an array
  * of `count` argument blocks, each exactly what the single call takes; results are identical.  Inference runs the four
  * scales this way after the last trunk convolution (networks/vgg_osvos.py:67,69,72 for all four stages at once). */
 OSVOS_API int osvos_side_folded_multi(const osvos_conv3x3_args* args /* host array */, int count, osvos_stream_t stream);
 
-/* The same fold for up to four scales in ONE launch (training re-folds after every optimizer step), optionally with an
- * fp32 copy of W' in [tap][o][ci] order (18 * cin floats) - the operand of the folded backward below.              */
+/* The fold of up to four scales in ONE launch (training re-folds after every optimizer step), optionally with an fp32
+ * copy of W' in [tap][o][ci] order (18 * cin floats) - the operand of the folded backward below.                   */
 typedef struct {
   const float* side_w;   /* [16,cin,3,3] */
   const float* side_b;   /* [16] or NULL */
@@ -219,12 +217,13 @@ OSVOS_API int osvos_side_project(const float* feat /* [n,h,w,16] */, const float
                        int n, int h, int w, osvos_stream_t stream);
 
 /* ---- class_balanced_cross_entropy_loss (layers/osvos_layers.py:19-48) -----------
- * forward: sums[0..3] = {S_pos, S_neg, P, N} (5 doubles, zeroed by the call; sums[4] is an arrival counter), loss[0] =
- * (Nn/N*S_pos + P/N*S_neg)/divisor with divisor = numel (size_average), batch
+ * forward: sums[0..3] = {S_pos, S_neg, P, N} (osvos_cbce_fwd_sums(numel, flags) doubles; the call zeroes the first 5,
+ * sums[4] is an arrival counter), loss[0] = (Nn/N*S_pos + P/N*S_neg)/divisor with divisor = numel (size_average), batch
  * (batch_average) or 1.  backward: grad_in = grad_out[0] * w * (sigmoid(x) - y) / divisor
  * (grad_out == NULL means 1).                                                        */
+OSVOS_API size_t osvos_cbce_fwd_sums(size_t numel, int flags);
 OSVOS_API int osvos_cbce_fwd(const float* output, const float* label, size_t numel, double divisor, double* sums,
-                             float* loss, osvos_stream_t stream);
+                             float* loss, int flags, osvos_stream_t stream);
 OSVOS_API int osvos_cbce_bwd(const float* output, const float* label, const double* sums, const float* grad_out,
                              double divisor, size_t numel, float* grad_in, osvos_stream_t stream);
 
@@ -235,8 +234,9 @@ OSVOS_API int osvos_cbce_bwd(const float* output, const float* label, const doub
  * networks/vgg_osvos.py:41,142; backward at train_online.py:141 / train_parent.py:164):
  *   dw[co][ci][r][s] = sum_px dz[px][co] * x[px + (r-1, s-1)][ci]
  * dz has `cout` channels (dz_channels == cout, a multiple of 64).  (side_prep's weight gradient does not come through
- * here: osvos_side_folded_wgrad / osvos_side_grads_finish.)
- * workspace: osvos_wgrad_workspace_bytes(dz_channels, cin) bytes, contents destroyed.  */
+ * here: osvos_side_folded_wgrad_multi / osvos_side_grads_finish.)
+ * workspace: osvos_wgrad_workspace_bytes(n, h, w, cin, dz_channels, flags & OSVOS_FLAG_DETERMINISTIC) bytes, contents
+ * destroyed.  */
 typedef struct {
   const void* x_hi;   /* layer input act [n,h,w,cin]        */
   const void* x_lo;
@@ -246,14 +246,15 @@ typedef struct {
   float* workspace;
   int n, h, w, cin, cout, dz_channels;
   int flags;          /* OSVOS_FLAG_FAST | OSVOS_FLAG_DEFER_FINISH (then dw may be NULL) | OSVOS_FLAG_DETERMINISTIC (then
-                         the workspace is osvos_wgrad_deterministic_workspace_bytes and needs no zeroing) */
+                         the workspace needs no zeroing) */
 } osvos_wgrad_args;
-OSVOS_API size_t osvos_wgrad_workspace_bytes(int dz_channels, int cin);
+OSVOS_API size_t osvos_wgrad_workspace_bytes(int n, int h, int w, int cin, int dz_channels, int flags);
 OSVOS_API int osvos_conv3x3_wgrad(const osvos_wgrad_args* args /* host */, osvos_stream_t stream);
 
 /* Deferred finish of up to OSVOS_WGRAD_FINISH_MAX weight gradients in ONE launch: workspace [9][a][b] -> OIHW,
  * dw = (accumulate ? dw : 0) + scale * ws.  With accumulate the destination can be the parameter's .grad itself
- * (what autograd's AccumulateGrad would do with a separate add kernel, train_online.py:141).                    */
+ * (what autograd's AccumulateGrad would do with a separate add kernel, train_online.py:141).  `splits` (host,
+ * [count]): the osvos_wgrad_deterministic_splits of each item's shape with OSVOS_FLAG_DETERMINISTIC, NULL without. */
 #define OSVOS_WGRAD_FINISH_MAX 24
 typedef struct {
   const float* workspace;  /* as passed to osvos_conv3x3_wgrad with OSVOS_FLAG_DEFER_FINISH */
@@ -262,7 +263,8 @@ typedef struct {
   int accumulate;
   float scale;
 } osvos_wgrad_finish_item;
-OSVOS_API int osvos_wgrad_finish(const osvos_wgrad_finish_item* items /* host */, int count, osvos_stream_t stream);
+OSVOS_API int osvos_wgrad_finish(const osvos_wgrad_finish_item* items /* host */, const int* splits, int count, int flags,
+                                 osvos_stream_t stream);
 
 /* ---- adjoint of the tail: gradients of the five maps -> low-res dp/dq ------------
  * Backward of osvos_tail_fwd (autograd of networks/vgg_osvos.py:68-72): strided bilinear
@@ -296,36 +298,42 @@ typedef struct {
 } osvos_tail_loss_bwd_args;
 OSVOS_API int osvos_tail_loss_bwd(const osvos_tail_loss_bwd_args* args /* host */, osvos_stream_t stream);
 
-/* out[0] = sum(x[0:n]) (fuse.bias gradient); scratch: 2 doubles (total, arrival counter).  */
-OSVOS_API int osvos_sum_f32(const float* x, size_t n, double* scratch, float* out, osvos_stream_t stream);
+/* out[0] = sum(x[0:n]) (fuse.bias gradient); scratch: osvos_sum_f32_scratch_bytes(flags) bytes, 8-byte aligned.  */
+OSVOS_API size_t osvos_sum_f32_scratch_bytes(int flags);
+OSVOS_API int osvos_sum_f32(const float* x, size_t n, void* scratch, float* out, int flags, osvos_stream_t stream);
 
-/* ---- max-unpool + side-branch add + ReLU mask (autograd of networks/vgg_osvos.py:140,143) */
-OSVOS_API int osvos_unpool_add_mask(const void* dpool_hi, const void* dpool_lo, const void* x_hi, const void* x_lo,
-                                    const float* dside /* [n,h,w,c] fp32 or NULL */, void* dz_hi, void* dz_lo,
-                                    float* colsum /* [c] accumulated per-channel sum of dz, or NULL */, int n,
-                                    int h, int w, int c, osvos_stream_t stream);
+/* ---- max-unpool + side-branch add + ReLU mask (autograd of networks/vgg_osvos.py:140,143) ------------------------
+ * dz = ReLU'(x) * (unpool(dpool) + side-branch gradient), the side-branch gradient being one of
+ *   dside:      an fp32 map [n,h,w,c], 16-byte aligned;
+ *   dpq, wfold: the folded form dX[px][c] = sum_{t,o} wfold[t][o][c] dpq[px - t][o] (see the folded side branch
+ *               backward below), computed on the fly; dpq [n,h,w,2], wfold [9][2][c] fp32 16-byte aligned, h*w < 2^30;
+ *   neither:    zero (stage 1).
+ * dpool_hi NULL: no pooling consumer (the deepest stage); at least one of dpool_hi, dside and dpq is set, and dside
+ * excludes dpq.  colsum: [c] per-channel sum of dz (the bias gradient), accumulated, or NULL.  c: a multiple of 8 up
+ * to 2048 with 256 % (c / 8) == 0.                                                                                  */
+OSVOS_API int osvos_unpool_mask(const void* dpool_hi /* or NULL */, const void* dpool_lo, const void* x_hi,
+                                const void* x_lo, const float* dside /* or NULL */, const float* dpq /* or NULL */,
+                                const float* wfold /* or NULL */, void* dz_hi, void* dz_lo, float* colsum /* or NULL */,
+                                int n, int h, int w, int c, int flags, osvos_stream_t stream);
 
 /* ---- side branch backward in folded (rank-2) form -------------------------------------------------------------
  * Autograd of networks/vgg_osvos.py:67,69,72 (side_prep -> score_dsn / fuse slice) expressed on the folded 3x3
- * convolution C -> 2 (see osvos_fold_side_weights): the branch's backward only sees the two gradient channels
+ * convolution C -> 2 (see osvos_fold_side_weights_multi): the branch's backward only sees the two gradient channels
  * dpq = (dL/dp, dL/dq).
- *   osvos_side_folded_wgrad:  g[t][o][c] += sum_px dpq[px - t][o] * x[px][c]  (t = 3r + s <-> offset (r-1, s-1)),
+ *   osvos_side_folded_wgrad_multi: for up to four scales in one launch (x_lo either set for all items or for none),
+ *                             g[t][o][c] += sum_px dpq[px - t][o] * x[px][c]  (t = 3r + s <-> offset (r-1, s-1)),
  *                             g[18 c + o] += sum_px dpq[px][o];   g: osvos_side_folded_wgrad_floats(c) floats, PRE-ZEROED,
- *                             16-byte aligned; c a multiple of 128.
+ *                             16-byte aligned; c a multiple of 128.  workspace: osvos_side_folded_wgrad_workspace_bytes(
+ *                             items, count, flags) bytes, 16-byte aligned (0 in the default form: workspace may be NULL).
  *   osvos_side_grads_finish:  every parameter gradient of up to four scales from g, one launch:
  *                             d side_prep.weight[f][c][t] = proj[f] g[t][0][c] + proj[16+f] g[t][1][c],
  *                             d side_prep.bias[f] = proj[f] S0 + proj[16+f] S1,
  *                             d score_dsn.weight[f] = <side_w[f], g[.][0][.]> + side_b[f] S0, d score_dsn.bias = S0,
  *                             d fuse.weight slice[f] = <side_w[f], g[.][1][.]> + side_b[f] S1
  *                             (NULL outputs are skipped; accumulate: add to the destinations instead of overwriting).
- *   osvos_unpool_side_mask:   dz = ReLU'(x) * (unpool(dpool) + dX),  dX[px][c] = sum_{t,o} wfold[t][o][c] dpq[px - t][o]
- *                             - osvos_unpool_add_mask with the side gradient computed on the fly from dpq and the fp32
- *                             folded weights (osvos_fold_side_weights_multi) instead of read from an fp32 map;
- *                             dpool_hi NULL: no pooling consumer (deepest stage).                                    */
+ *   osvos_unpool_mask with dpq and wfold (the fp32 folded weights of osvos_fold_side_weights_multi): the gradient
+ *                             w.r.t. the stage output, dX[px][c] = sum_{t,o} wfold[t][o][c] dpq[px - t][o].          */
 OSVOS_API size_t osvos_side_folded_wgrad_floats(int c);
-OSVOS_API int osvos_side_folded_wgrad(const void* x_hi, const void* x_lo /* or NULL */, const float* dpq /* [n,h,w,2] */,
-                                      float* g, int n, int h, int w, int c, osvos_stream_t stream);
-/* The same for up to four scales in one launch (x_lo either set for all items or for none). */
 typedef struct {
   const void* x_hi;
   const void* x_lo;
@@ -333,9 +341,12 @@ typedef struct {
   float* g;
   int n, h, w, c;
 } osvos_side_wgrad_item;
-OSVOS_API int osvos_side_folded_wgrad_multi(const osvos_side_wgrad_item* items /* host */, int count, osvos_stream_t stream);
+OSVOS_API size_t osvos_side_folded_wgrad_workspace_bytes(const osvos_side_wgrad_item* items /* host */, int count,
+                                                         int flags);
+OSVOS_API int osvos_side_folded_wgrad_multi(const osvos_side_wgrad_item* items /* host */, int count, void* workspace,
+                                            int flags, osvos_stream_t stream);
 typedef struct {
-  const float* g;        /* as filled by osvos_side_folded_wgrad */
+  const float* g;        /* as filled by osvos_side_folded_wgrad_multi */
   const float* side_w;   /* [16,c,3,3] */
   const float* side_b;   /* [16] or NULL */
   const float* proj_w;   /* [32] */
@@ -348,78 +359,42 @@ typedef struct {
   int accumulate;
 } osvos_side_grads_item;
 OSVOS_API int osvos_side_grads_finish(const osvos_side_grads_item* items /* host */, int count, osvos_stream_t stream);
-OSVOS_API int osvos_unpool_side_mask(const void* dpool_hi /* or NULL */, const void* dpool_lo, const void* x_hi,
-                                     const void* x_lo, const float* dpq /* [n,h,w,2] */,
-                                     const float* wfold /* [9][2][c] fp32 */, void* dz_hi, void* dz_lo,
-                                     float* colsum /* or NULL */, int n, int h, int w, int c, osvos_stream_t stream);
-
-/* ---- bias gradient: out[c] = sum over pixels of an act ----------------------------- */
-OSVOS_API int osvos_channel_sum(const void* act_hi, const void* act_lo, float* out, size_t npix, int c,
-                                osvos_stream_t stream);
 
 /* ---- conv1_1 backward: dw [64][3][3][3] and (optionally) dx [n,3,h,w] ---------------
- * workspace: osvos_conv_first_bwd_workspace_bytes() bytes (replicated partial sums + arrival counter; zeroed by
- * the call).                                                                                  */
-OSVOS_API size_t osvos_conv_first_bwd_workspace_bytes(void);
+ * workspace: osvos_conv_first_bwd_workspace_bytes(n, h, w, flags) bytes (default form: replicated partial sums +
+ * arrival counter, zeroed by the call).                                                       */
+OSVOS_API size_t osvos_conv_first_bwd_workspace_bytes(int n, int h, int w, int flags);
 OSVOS_API int osvos_conv_first_bwd(const float* x_nchw, const void* dz_hi, const void* dz_lo, const float* w_oihw,
                                    float* dw, float* dx_nchw /* or NULL */, void* workspace, int n, int h, int w,
-                                   osvos_stream_t stream);
+                                   int flags, osvos_stream_t stream);
 
 /* ---- Deterministic forms (OSVOS_FLAG_DETERMINISTIC; torch.use_deterministic_algorithms in the package) ----------
  * Every float reduction of the training path has a form whose summation order depends on the shapes (and, where a
- * grid is sized by it, the device's SM count) only, so two runs on one device give bit-identical results:
- *   osvos_reduce_rows:      out[c] = (accumulate ? out[c] : 0) + sum_r rows[r][c], rows [nrows][ncols] fp32, in a fixed
- *                           order (up to 64 row segments, each summed by 8 interleaved row lanes); scratch:
- *                           osvos_reduce_rows_scratch_floats(nrows, ncols) floats.
- *   osvos_conv3x3_colsum_rows: rows of the colsum partials of osvos_conv3x3 with OSVOS_FLAG_DETERMINISTIC (8 per
- *                           128-pixel tile).
- *   osvos_conv3x3_wgrad with the flag: one workspace slice per pixel-range split, written with plain stores; the split
- *                           count comes from a nominal 132-SM device (osvos_wgrad_deterministic_splits), so it does not
- *                           depend on the H100 variant.  osvos_wgrad_finish_deterministic sums the splits[i] slices of
- *                           item i in order before it scales and accumulates.
- *   osvos_unpool_mask_deterministic: osvos_unpool_side_mask (dpq, wfold set) or osvos_unpool_add_mask without dside (dpq,
- *                           wfold NULL) whose column sums go to partial rows [osvos_unpool_colsum_rows(n, h, w, c, pool,
- *                           side)][c], one per block (pool = dpool_hi != NULL, side = dpq != NULL), or nowhere (NULL).
- *   osvos_side_folded_wgrad_multi_deterministic: G += the blocks' partial rows in order; workspace
- *                           osvos_side_folded_wgrad_deterministic_workspace_bytes(items, count) bytes, 16-byte aligned.
- *   osvos_conv_first_bwd_deterministic: one partial slot per block, added by the ordered row reduction; workspace
- *                           osvos_conv_first_bwd_deterministic_workspace_bytes(n, h, w) bytes.
- *   osvos_cbce_fwd_deterministic: osvos_cbce_fwd with one row of block sums per block behind sums[0..4], added in a
- *                           fixed order by the last block; `sums` holds osvos_cbce_fwd_deterministic_sums(numel) doubles
- *                           (osvos_cbce_bwd reads sums[0..4] as before).
- *   osvos_sum_f32_deterministic: osvos_sum_f32 over a fixed grid of 256 contiguous ranges, their totals added in order
- *                           by the last block; scratch: osvos_sum_f32_deterministic_scratch_bytes() bytes.
+ * grid is sized by it, the device's SM count) only, so two runs on one device give bit-identical results.  What the
+ * flag changes, per entry point (the size queries take the same flags and return 0 for shapes the calls refuse):
+ *   osvos_conv3x3:              colsum is partial rows [osvos_conv3x3_colsum_rows(n, h, w)][cout], 8 per 128-pixel tile.
+ *   osvos_conv3x3_wgrad:        one workspace slice per pixel-range split, written with plain stores; the split count
+ *                               (osvos_wgrad_deterministic_splits) comes from a nominal 132-SM device, not the H100 variant.
+ *   osvos_wgrad_finish:         adds the splits[i] slices of item i in order before it scales and accumulates.
+ *   osvos_unpool_mask:          colsum is partial rows [osvos_unpool_colsum_rows(n, h, w, c, pool, side)][c], one per
+ *                               block (pool = dpool_hi != NULL, side = dpq != NULL).
+ *   osvos_side_folded_wgrad_multi: G += the blocks' partial rows in order, through the workspace.
+ *   osvos_conv_first_bwd:       one partial slot per block in the workspace, added by the ordered row reduction.
+ *   osvos_cbce_fwd:             one row of block sums per block behind sums[0..4], added in a fixed order by the last
+ *                               block (osvos_cbce_bwd reads sums[0..4] either way).
+ *   osvos_sum_f32:              a fixed grid of 256 contiguous ranges, their totals added in order by the last block.
  *   osvos_tail_fwd / osvos_tail_bwd / osvos_tail_loss_bwd: the `flags` member of their argument blocks (appended:
- *                           callers zero-initialise the blocks).
- * The queries return 0 for shapes the entry points refuse.                                                        */
+ *                               callers zero-initialise the blocks); tail_fwd's sums: osvos_tail_fwd_deterministic_sums.
+ * osvos_reduce_rows adds such partial rows: out[c] = (accumulate ? out[c] : 0) + sum_r rows[r][c], rows [nrows][ncols]
+ * fp32, in a fixed order (up to 64 row segments, each summed by 8 interleaved row lanes); scratch:
+ * osvos_reduce_rows_scratch_floats(nrows, ncols) floats.                                                            */
 OSVOS_API size_t osvos_reduce_rows_scratch_floats(int nrows, int ncols);
 OSVOS_API int osvos_reduce_rows(const float* rows, int nrows, int ncols, float* scratch, float* out, int accumulate,
                                 osvos_stream_t stream);
 OSVOS_API size_t osvos_conv3x3_colsum_rows(int n, int h, int w);
 OSVOS_API int osvos_wgrad_deterministic_splits(int n, int h, int w, int cin, int dz_channels);
-OSVOS_API size_t osvos_wgrad_deterministic_workspace_bytes(int n, int h, int w, int cin, int dz_channels);
-OSVOS_API int osvos_wgrad_finish_deterministic(const osvos_wgrad_finish_item* items /* host */,
-                                               const int* splits /* host, [count] */, int count, osvos_stream_t stream);
 OSVOS_API size_t osvos_unpool_colsum_rows(int n, int h, int w, int c, int pool, int side);
-OSVOS_API int osvos_unpool_mask_deterministic(const void* dpool_hi /* or NULL */, const void* dpool_lo, const void* x_hi,
-                                              const void* x_lo, const float* dpq /* or NULL */,
-                                              const float* wfold /* or NULL */, void* dz_hi, void* dz_lo,
-                                              float* colsum_rows /* or NULL */, int n, int h, int w, int c,
-                                              osvos_stream_t stream);
-OSVOS_API size_t osvos_side_folded_wgrad_deterministic_workspace_bytes(const osvos_side_wgrad_item* items /* host */,
-                                                                       int count);
-OSVOS_API int osvos_side_folded_wgrad_multi_deterministic(const osvos_side_wgrad_item* items /* host */, int count,
-                                                          void* workspace, osvos_stream_t stream);
-OSVOS_API size_t osvos_conv_first_bwd_deterministic_workspace_bytes(int n, int h, int w);
-OSVOS_API int osvos_conv_first_bwd_deterministic(const float* x_nchw, const void* dz_hi, const void* dz_lo,
-                                                 const float* w_oihw, float* dw, float* dx_nchw /* or NULL */,
-                                                 void* workspace, int n, int h, int w, osvos_stream_t stream);
 OSVOS_API size_t osvos_tail_fwd_deterministic_sums(int n, int h, int w);
-OSVOS_API size_t osvos_cbce_fwd_deterministic_sums(size_t numel);
-OSVOS_API int osvos_cbce_fwd_deterministic(const float* output, const float* label, size_t numel, double divisor,
-                                           double* sums, float* loss, osvos_stream_t stream);
-OSVOS_API size_t osvos_sum_f32_deterministic_scratch_bytes(void);
-OSVOS_API int osvos_sum_f32_deterministic(const float* x, size_t n, void* scratch, float* out, osvos_stream_t stream);
 
 /* ===================== SURVEY.md 8(f) "next" rows: callers either side ===================== */
 
@@ -730,10 +705,8 @@ OSVOS_API int osvos_jpeg_encode(const uint8_t* src, uint8_t* out, int64_t* lengt
  *                            d fuse.weight[16k+co] = sum_{ci,t} upscale_w[k][ci][co][t] H_k[t][ci], d score_dsn[k].weight
  *                            = sum dp F, .bias = sum dp, d side_prep[k].bias = sum dF; NULL outputs are skipped, with
  *                            accumulate the values are added to the destinations.
- *   osvos_unpool_dside_mask: dz = ReLU'(x) * (unpool(dpool) + dside) as osvos_unpool_add_mask, dpool_hi NULL allowed
- *                            (the deepest stage); OSVOS_FLAG_DETERMINISTIC: colsum is partial rows
- *                            [osvos_unpool_colsum_rows(n, h, w, c, dpool_hi != NULL, 0)][c].
- * Every float reduction of these calls is fixed-order (OSVOS_FLAG_DETERMINISTIC is accepted and changes nothing).   */
+ * Every float reduction of these calls is fixed-order (OSVOS_FLAG_DETERMINISTIC is accepted and changes nothing).  On
+ * this path the side branch's gradient w.r.t. a stage output enters the trunk as osvos_unpool_mask's fp32 dside map. */
 #define OSVOS_UPSAMPLING_TAPS 1360
 typedef struct {
   const float* upscale_w[4];    /* upscale[k].weight [16][16][2s][2s] ([in][out][kH][kW]) */
@@ -795,10 +768,6 @@ typedef struct {
   int accumulate;
 } osvos_upsampling_grads_args;
 OSVOS_API int osvos_upsampling_grads_finish(const osvos_upsampling_grads_args* args /* host */, osvos_stream_t stream);
-OSVOS_API int osvos_unpool_dside_mask(const void* dpool_hi /* or NULL */, const void* dpool_lo, const void* x_hi,
-                                      const void* x_lo, const float* dside /* [n,h,w,c] fp32 */, void* dz_hi, void* dz_lo,
-                                      float* colsum /* or NULL */, int n, int h, int w, int c, int flags,
-                                      osvos_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -158,32 +158,30 @@ SIGNATURES = {
     "osvos_conv3x3": (c_int, [POINTER(Conv3x3Args), c_void_p]),
     "osvos_stage1_fused": (c_int, [POINTER(Stage1Args), c_void_p]),
     "osvos_set_pdl": (c_int, [c_int]),
-    "osvos_fold_side_weights": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "osvos_side_folded_multi": (c_int, [POINTER(Conv3x3Args), c_int, c_void_p]),
     "osvos_fold_side_weights_multi": (c_int, [POINTER(FoldItem), c_int, c_void_p]),
     "osvos_conv3x3_simt": (c_int, [POINTER(Conv3x3Args), c_void_p]),
     "osvos_maxpool2x2_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "osvos_tail_fwd": (c_int, [POINTER(TailFwdArgs), c_void_p]),
-    "osvos_cbce_fwd": (c_int, [c_void_p, c_void_p, c_size_t, c_double, c_void_p, c_void_p, c_void_p]),
+    "osvos_cbce_fwd_sums": (c_size_t, [c_size_t, c_int]),
+    "osvos_cbce_fwd": (c_int, [c_void_p, c_void_p, c_size_t, c_double, c_void_p, c_void_p, c_int, c_void_p]),
     "osvos_cbce_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_double, c_size_t, c_void_p, c_void_p]),
-    "osvos_wgrad_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "osvos_wgrad_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "osvos_conv3x3_wgrad": (c_int, [POINTER(WgradArgs), c_void_p]),
-    "osvos_wgrad_finish": (c_int, [POINTER(WgradFinishItem), c_int, c_void_p]),
+    "osvos_wgrad_finish": (c_int, [POINTER(WgradFinishItem), POINTER(c_int), c_int, c_int, c_void_p]),
     "osvos_tail_bwd": (c_int, [POINTER(TailBwdArgs), c_void_p]),
     "osvos_tail_loss_bwd": (c_int, [POINTER(TailLossBwdArgs), c_void_p]),
-    "osvos_sum_f32": (c_int, [c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
-    "osvos_unpool_add_mask": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                      c_int, c_int, c_int, c_int, c_void_p]),
+    "osvos_sum_f32_scratch_bytes": (c_size_t, [c_int]),
+    "osvos_sum_f32": (c_int, [c_void_p, c_size_t, c_void_p, c_void_p, c_int, c_void_p]),
+    "osvos_unpool_mask": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                  c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "osvos_side_folded_wgrad_floats": (c_size_t, [c_int]),
-    "osvos_side_folded_wgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
-    "osvos_side_folded_wgrad_multi": (c_int, [POINTER(SideWgradItem), c_int, c_void_p]),
+    "osvos_side_folded_wgrad_workspace_bytes": (c_size_t, [POINTER(SideWgradItem), c_int, c_int]),
+    "osvos_side_folded_wgrad_multi": (c_int, [POINTER(SideWgradItem), c_int, c_void_p, c_int, c_void_p]),
     "osvos_side_grads_finish": (c_int, [POINTER(SideGradsItem), c_int, c_void_p]),
-    "osvos_unpool_side_mask": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                       c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
-    "osvos_channel_sum": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_void_p]),
-    "osvos_conv_first_bwd_workspace_bytes": (c_size_t, []),
+    "osvos_conv_first_bwd_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "osvos_conv_first_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
-                                     c_void_p]),
+                                     c_int, c_void_p]),
     "osvos_side_project": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "osvos_logits_to_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_size_t, c_int, c_void_p]),
     "osvos_sgd_work_items": (c_uint32, [c_uint64, c_int, c_int]),
@@ -208,21 +206,8 @@ SIGNATURES = {
     "osvos_reduce_rows": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     "osvos_conv3x3_colsum_rows": (c_size_t, [c_int, c_int, c_int]),
     "osvos_wgrad_deterministic_splits": (c_int, [c_int, c_int, c_int, c_int, c_int]),
-    "osvos_wgrad_deterministic_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
-    "osvos_wgrad_finish_deterministic": (c_int, [POINTER(WgradFinishItem), POINTER(c_int), c_int, c_void_p]),
     "osvos_unpool_colsum_rows": (c_size_t, [c_int, c_int, c_int, c_int, c_int, c_int]),
-    "osvos_unpool_mask_deterministic": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
-    "osvos_side_folded_wgrad_deterministic_workspace_bytes": (c_size_t, [POINTER(SideWgradItem), c_int]),
-    "osvos_side_folded_wgrad_multi_deterministic": (c_int, [POINTER(SideWgradItem), c_int, c_void_p, c_void_p]),
-    "osvos_conv_first_bwd_deterministic_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
-    "osvos_conv_first_bwd_deterministic": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                   c_int, c_int, c_int, c_void_p]),
     "osvos_tail_fwd_deterministic_sums": (c_size_t, [c_int, c_int, c_int]),
-    "osvos_cbce_fwd_deterministic_sums": (c_size_t, [c_size_t]),
-    "osvos_cbce_fwd_deterministic": (c_int, [c_void_p, c_void_p, c_size_t, c_double, c_void_p, c_void_p, c_void_p]),
-    "osvos_sum_f32_deterministic_scratch_bytes": (c_size_t, []),
-    "osvos_sum_f32_deterministic": (c_int, [c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
     "osvos_jpeg_decode_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_size_t, c_int]),
     "osvos_jpeg_decode": (c_int, [POINTER(JpegArgs), c_void_p]),
     "osvos_upsampling_fold": (c_int, [POINTER(UpsamplingFoldArgs), c_void_p]),
@@ -231,8 +216,6 @@ SIGNATURES = {
     "osvos_tail_general_bwd_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "osvos_tail_general_bwd": (c_int, [POINTER(TailGeneralBwdArgs), c_void_p]),
     "osvos_upsampling_grads_finish": (c_int, [POINTER(UpsamplingGradsArgs), c_void_p]),
-    "osvos_unpool_dside_mask": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                        c_int, c_int, c_int, c_int, c_int, c_void_p]),
     # train_online.py:187 (sm.imsave of each result) on the device
     "osvos_png_max_bytes": (c_size_t, [c_int, c_int]),
     "osvos_png_encode_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),

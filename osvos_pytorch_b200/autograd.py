@@ -321,10 +321,10 @@ class _OSVOSFunction(torch.autograd.Function):
                 sp = m.side_prep[i - 1]
                 _, dside, _ = ops.conv3x3(dfs[i - 1], engine._packed(sp, f"sp{i}", transpose_flip=True), None,
                                           sp.in_channels, fast=fast, out_act=False, out_f32=True)
-                dz = ops.unpool_dside_mask(dpool, s_out, dside, colsum=last_bias, deterministic=det)
+                dz = ops.unpool_mask(dpool, s_out, dside=dside, colsum=last_bias, deterministic=det)
             else:
-                dz = ops.unpool_side_mask(dpool, s_out, dpq[i - 1], fold[i - 1][2], colsum=last_bias,
-                                          deterministic=det)
+                dz = ops.unpool_mask(dpool, s_out, dpq=dpq[i - 1], wfold=fold[i - 1][2], colsum=last_bias,
+                                     deterministic=det)
             for j in range(len(convs[i]) - 1, -1, -1):
                 conv = convs[i][j]
                 inp = acts[i][j - 1] if j > 0 else pooled[i]
@@ -338,7 +338,7 @@ class _OSVOSFunction(torch.autograd.Function):
                     dpool, _, _ = ops.conv3x3(dz, wt, None, conv.in_channels, fast=fast)
         # stage 1 (no side branch)
         c12, c11 = convs[0][1], convs[0][0]
-        dz = ops.unpool_add_mask(dpool, acts[0][1], None, colsum=bias_slices[c12], deterministic=det)
+        dz = ops.unpool_mask(dpool, acts[0][1], colsum=bias_slices[c12], deterministic=det)
         wgrad(c12, acts[0][0], dz)
         pg[c12.bias] = bias_grad(c12)
         dz, _, _ = ops.conv3x3(dz, engine._packed(c12, "s0c1", transpose_flip=True), None, 64, fast=fast,

@@ -1,6 +1,6 @@
 // Bandwidth-bound backward kernels around the tensor-core dgrad / wgrad GEMMs:
-// max-unpool + ReLU mask (+ the side branch's folded gradient), per-channel
-// bias-gradient sums and the conv1_1 (Cin = 3) backward.
+// max-unpool + ReLU mask (+ the side branch's folded gradient, + the fused
+// bias-gradient column sums), ordered sums and the conv1_1 (Cin = 3) backward.
 // They replace the autograd graph PyTorch builds for reference
 // networks/vgg_osvos.py:59-74 (triggered at train_online.py:141, train_parent.py:164).
 #include "common.cuh"
@@ -273,41 +273,6 @@ unpool_add_mask_kernel(const __nv_bfloat16* __restrict__ dp_hi, const __nv_bfloa
   }
 }
 
-// ------------------------------------------------- per-channel sums of an act
-// out[c] += sum_px (hi + lo)[px][c]   (bias gradient; out zeroed by the caller)
-__global__ void __launch_bounds__(256)
-channel_sum_kernel(const __nv_bfloat16* __restrict__ hi, const __nv_bfloat16* __restrict__ lo, size_t npix, int c,
-                   float* __restrict__ out) {
-  const int groups = c / 8;               // threads across channels (8 channels each)
-  const int rows = 256 / groups;          // pixel rows handled concurrently by the block
-  const int g = threadIdx.x % groups, ry = threadIdx.x / groups;
-  float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  if (ry < rows) {
-    for (size_t px = blockIdx.x * static_cast<size_t>(rows) + ry; px < npix; px += static_cast<size_t>(gridDim.x) * rows) {
-      const uint4 vh = __ldg(reinterpret_cast<const uint4*>(hi + px * c + g * 8));
-      uint4 vl = make_uint4(0, 0, 0, 0);
-      if (lo) vl = __ldg(reinterpret_cast<const uint4*>(lo + px * c + g * 8));
-      const uint32_t hw[4] = {vh.x, vh.y, vh.z, vh.w};
-      const uint32_t lw[4] = {vl.x, vl.y, vl.z, vl.w};
-#pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        acc[2 * t] += bf16_lo_to_float(hw[t]) + bf16_lo_to_float(lw[t]);
-        acc[2 * t + 1] += bf16_hi_to_float(hw[t]) + bf16_hi_to_float(lw[t]);
-      }
-    }
-  }
-  extern __shared__ float sm[];  // [256][8]
-#pragma unroll
-  for (int j = 0; j < 8; ++j) sm[threadIdx.x * 8 + j] = acc[j];
-  __syncthreads();
-  for (int ch = threadIdx.x; ch < c; ch += 256) {
-    const int gg = ch / 8, j = ch % 8;
-    float t = 0.f;
-    for (int r = 0; r < rows; ++r) t += sm[(r * groups + gg) * 8 + j];
-    atomicAdd(out + ch, t);
-  }
-}
-
 // -------------------------------------------------------------- conv1_1 bwd
 // dW[co][ci][r][s] = sum_px dz[px][co] * x[ci][px + (r-1, s-1)]: a [32 (27 used) x 64] output with the whole image
 // as reduction axis - 1.4 GFLOP at 480x854 against 105 MB of dz, i.e. HBM-bound once the arithmetic is cheap.  The
@@ -537,11 +502,26 @@ static inline int grid_cap(size_t blocks, int per_sm) {
 
 using namespace osvos;
 
-extern "C" int osvos_sum_f32(const float* x, size_t n, double* scratch, float* out, osvos_stream_t stream_) {
+extern "C" size_t osvos_sum_f32_scratch_bytes(int flags) {
+  if ((flags & ~OSVOS_FLAG_DETERMINISTIC) != 0) return 0;
+  // deterministic: the block partials and the arrival counter; default: the fp64 total and the arrival counter
+  return (flags & OSVOS_FLAG_DETERMINISTIC) ? (kSumBlocks + 1) * sizeof(float) : 2 * sizeof(double);
+}
+
+extern "C" int osvos_sum_f32(const float* x, size_t n, void* scratch, float* out, int flags, osvos_stream_t stream_) {
   OSVOS_CHECK_ARG(x != nullptr && scratch != nullptr && out != nullptr && n > 0);
+  OSVOS_CHECK_ARG((flags & ~OSVOS_FLAG_DETERMINISTIC) == 0);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  OSVOS_CHECK_CUDA(cudaMemsetAsync(scratch, 0, 2 * sizeof(double), stream));
-  sum_f32_kernel<<<grid_cap((n + 255) / 256, 4), 256, 0, stream>>>(x, n, scratch, out);
+  if (flags & OSVOS_FLAG_DETERMINISTIC) {
+    float* part = static_cast<float*>(scratch);
+    // the block partials are written in full: only the arrival counter behind them is zeroed
+    OSVOS_CHECK_CUDA(cudaMemsetAsync(part + kSumBlocks, 0, sizeof(float), stream));
+    sum_f32_det_kernel<<<kSumBlocks, 256, 0, stream>>>(x, n, (n + kSumBlocks - 1) / kSumBlocks, part, out);
+  } else {
+    double* total = static_cast<double*>(scratch);
+    OSVOS_CHECK_CUDA(cudaMemsetAsync(total, 0, 2 * sizeof(double), stream));
+    sum_f32_kernel<<<grid_cap((n + 255) / 256, 4), 256, 0, stream>>>(x, n, total, out);
+  }
   OSVOS_CHECK_CUDA(cudaGetLastError());
   return OSVOS_OK;
 }
@@ -552,83 +532,59 @@ static size_t unpool_tiles(int n, int h, int w, int c, bool pool) {
   return static_cast<size_t>(n) * oh * ((ow + ppb - 1) / ppb);
 }
 
-template <bool POOL, bool SIDE, bool DET = false>
-static int launch_unpool(const void* dpool_hi, const void* dpool_lo, const void* x_hi, const void* x_lo, const float* dside,
-                         const float* dpq, const float* wfold, void* dz_hi, void* dz_lo, float* colsum, int n, int h, int w,
-                         int c, cudaStream_t stream) {
-  const int oh = POOL ? (h + 1) / 2 : h, ow = POOL ? (w + 1) / 2 : w;
-  const size_t tiles = unpool_tiles(n, h, w, c, POOL);
+struct UnpoolCall {
+  const void *dpool_hi, *dpool_lo, *x_hi, *x_lo;
+  const float *dside, *dpq, *wfold;
+  void *dz_hi, *dz_lo;
+  float* colsum;
+  int n, h, w, c;
+};
+
+template <bool POOL, bool SIDE, bool DET>
+static int launch_unpool(const UnpoolCall& a, cudaStream_t stream) {
+  const int oh = POOL ? (a.h + 1) / 2 : a.h, ow = POOL ? (a.w + 1) / 2 : a.w;
+  const size_t tiles = unpool_tiles(a.n, a.h, a.w, a.c, POOL);
   OSVOS_CHECK_ARG(tiles < (static_cast<size_t>(1) << 31));
   const int grid = grid_cap(tiles, SIDE ? 2 : 4);
   // the folded weights go to shared memory when every block has tiles enough to amortise the copy
   const int wf_in_smem = (SIDE && tiles >= static_cast<size_t>(grid) * 4) ? 1 : 0;
-  const size_t smem = static_cast<size_t>(c) * sizeof(float) * (wf_in_smem ? 19 : 1) + (DET ? 256 * 8 * sizeof(float) : 0);
+  const size_t smem = static_cast<size_t>(a.c) * sizeof(float) * (wf_in_smem ? 19 : 1) + (DET ? 256 * 8 * sizeof(float) : 0);
   auto kern = unpool_add_mask_kernel<POOL, SIDE, DET>;
   static uint64_t attr_done = 0;
   if (smem > 48 * 1024)
     OSVOS_CHECK_CUDA(ensure_dynamic_smem(kern, (19 * 2048 + (DET ? 256 * 8 : 0)) * sizeof(float), &attr_done));
   OSVOS_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(256), smem, stream,
-                              static_cast<const __nv_bfloat16*>(dpool_hi), static_cast<const __nv_bfloat16*>(dpool_lo),
-                              static_cast<const __nv_bfloat16*>(x_hi), static_cast<const __nv_bfloat16*>(x_lo), dside, dpq,
-                              wfold, static_cast<__nv_bfloat16*>(dz_hi), static_cast<__nv_bfloat16*>(dz_lo), colsum, n, h, w,
-                              c, oh, ow, wf_in_smem));
+                              static_cast<const __nv_bfloat16*>(a.dpool_hi), static_cast<const __nv_bfloat16*>(a.dpool_lo),
+                              static_cast<const __nv_bfloat16*>(a.x_hi), static_cast<const __nv_bfloat16*>(a.x_lo), a.dside,
+                              a.dpq, a.wfold, static_cast<__nv_bfloat16*>(a.dz_hi), static_cast<__nv_bfloat16*>(a.dz_lo),
+                              a.colsum, a.n, a.h, a.w, a.c, oh, ow, wf_in_smem));
   return OSVOS_OK;
 }
 
-extern "C" int osvos_unpool_add_mask(const void* dpool_hi, const void* dpool_lo, const void* x_hi, const void* x_lo,
-                                     const float* dside, void* dz_hi, void* dz_lo, float* colsum, int n, int h, int w,
-                                     int c, osvos_stream_t stream_) {
-  OSVOS_CHECK_ARG(dpool_hi != nullptr && x_hi != nullptr && dz_hi != nullptr && n > 0 && h > 0 && w > 0 && c % 8 == 0);
-  OSVOS_CHECK_ARG(c <= 2048 && 256 % (c / 8) == 0);
-  return launch_unpool<true, false>(dpool_hi, dpool_lo, x_hi, x_lo, dside, nullptr, nullptr, dz_hi, dz_lo, colsum, n, h, w, c,
-                             static_cast<cudaStream_t>(stream_));
-}
-
-extern "C" int osvos_unpool_side_mask(const void* dpool_hi, const void* dpool_lo, const void* x_hi, const void* x_lo,
-                                      const float* dpq, const float* wfold, void* dz_hi, void* dz_lo, float* colsum, int n,
-                                      int h, int w, int c, osvos_stream_t stream_) {
-  OSVOS_CHECK_ARG(x_hi != nullptr && dz_hi != nullptr && dpq != nullptr && wfold != nullptr && n > 0 && h > 0 && w > 0 &&
-                  c % 8 == 0);
-  OSVOS_CHECK_ARG(c <= 2048 && 256 % (c / 8) == 0);
-  OSVOS_CHECK_ARG(static_cast<long>(h) * w < (1l << 30));
-  OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(wfold) & 15) == 0);
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (dpool_hi != nullptr)
-    return launch_unpool<true, true>(dpool_hi, dpool_lo, x_hi, x_lo, nullptr, dpq, wfold, dz_hi, dz_lo, colsum, n, h, w, c, stream);
-  return launch_unpool<false, true>(nullptr, nullptr, x_hi, x_lo, nullptr, dpq, wfold, dz_hi, dz_lo, colsum, n, h, w, c, stream);
-}
-
-extern "C" int osvos_unpool_dside_mask(const void* dpool_hi, const void* dpool_lo, const void* x_hi, const void* x_lo,
-                                       const float* dside, void* dz_hi, void* dz_lo, float* colsum, int n, int h, int w,
-                                       int c, int flags, osvos_stream_t stream_) {
-  OSVOS_CHECK_ARG(x_hi != nullptr && dz_hi != nullptr && dside != nullptr && n > 0 && h > 0 && w > 0 && c % 8 == 0);
+extern "C" int osvos_unpool_mask(const void* dpool_hi, const void* dpool_lo, const void* x_hi, const void* x_lo,
+                                 const float* dside, const float* dpq, const float* wfold, void* dz_hi, void* dz_lo,
+                                 float* colsum, int n, int h, int w, int c, int flags, osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(x_hi != nullptr && dz_hi != nullptr && n > 0 && h > 0 && w > 0 && c >= 8 && c % 8 == 0);
   OSVOS_CHECK_ARG(c <= 2048 && 256 % (c / 8) == 0);
   OSVOS_CHECK_ARG((flags & ~OSVOS_FLAG_DETERMINISTIC) == 0);
+  OSVOS_CHECK_ARG((dpq == nullptr) == (wfold == nullptr));
+  OSVOS_CHECK_ARG(dside == nullptr || dpq == nullptr);
+  OSVOS_CHECK_ARG(dpool_hi != nullptr || dside != nullptr || dpq != nullptr);
   OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(dside) & 15) == 0);
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  const bool det = (flags & OSVOS_FLAG_DETERMINISTIC) != 0;
-  if (dpool_hi != nullptr)
-    return det ? launch_unpool<true, false, true>(dpool_hi, dpool_lo, x_hi, x_lo, dside, nullptr, nullptr, dz_hi, dz_lo,
-                                                  colsum, n, h, w, c, stream)
-               : launch_unpool<true, false>(dpool_hi, dpool_lo, x_hi, x_lo, dside, nullptr, nullptr, dz_hi, dz_lo, colsum,
-                                            n, h, w, c, stream);
-  return det ? launch_unpool<false, false, true>(nullptr, nullptr, x_hi, x_lo, dside, nullptr, nullptr, dz_hi, dz_lo, colsum,
-                                                 n, h, w, c, stream)
-             : launch_unpool<false, false>(nullptr, nullptr, x_hi, x_lo, dside, nullptr, nullptr, dz_hi, dz_lo, colsum, n, h,
-                                           w, c, stream);
-}
-
-extern "C" size_t osvos_sum_f32_deterministic_scratch_bytes(void) { return (kSumBlocks + 1) * sizeof(float); }
-
-extern "C" int osvos_sum_f32_deterministic(const float* x, size_t n, void* scratch, float* out, osvos_stream_t stream_) {
-  OSVOS_CHECK_ARG(x != nullptr && scratch != nullptr && out != nullptr && n > 0);
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  float* part = static_cast<float*>(scratch);
-  // the block partials are written in full: only the arrival counter behind them is zeroed
-  OSVOS_CHECK_CUDA(cudaMemsetAsync(part + kSumBlocks, 0, sizeof(float), stream));
-  sum_f32_det_kernel<<<kSumBlocks, 256, 0, stream>>>(x, n, (n + kSumBlocks - 1) / kSumBlocks, part, out);
-  OSVOS_CHECK_CUDA(cudaGetLastError());
-  return OSVOS_OK;
+  if (dpq != nullptr) {
+    OSVOS_CHECK_ARG(static_cast<long>(h) * w < (1l << 30));
+    OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(wfold) & 15) == 0);
+  }
+  const bool pool = dpool_hi != nullptr, side = dpq != nullptr, det = (flags & OSVOS_FLAG_DETERMINISTIC) != 0;
+  const UnpoolCall a = {dpool_hi, pool ? dpool_lo : nullptr, x_hi, x_lo, dside, dpq, wfold, dz_hi, dz_lo, colsum,
+                        n, h, w, c};
+  using Launch = int (*)(const UnpoolCall&, cudaStream_t);
+  static const Launch launch[2][2][2] = {   // [POOL][SIDE][DET]
+      {{launch_unpool<false, false, false>, launch_unpool<false, false, true>},
+       {launch_unpool<false, true, false>, launch_unpool<false, true, true>}},
+      {{launch_unpool<true, false, false>, launch_unpool<true, false, true>},
+       {launch_unpool<true, true, false>, launch_unpool<true, true, true>}}};
+  return launch[pool][side][det](a, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" size_t osvos_reduce_rows_scratch_floats(int nrows, int ncols) {
@@ -647,91 +603,40 @@ extern "C" size_t osvos_unpool_colsum_rows(int n, int h, int w, int c, int pool,
   return static_cast<size_t>(grid_cap(unpool_tiles(n, h, w, c, pool != 0), side ? 2 : 4));
 }
 
-extern "C" int osvos_unpool_mask_deterministic(const void* dpool_hi, const void* dpool_lo, const void* x_hi,
-                                               const void* x_lo, const float* dpq, const float* wfold, void* dz_hi,
-                                               void* dz_lo, float* colsum_rows, int n, int h, int w, int c,
-                                               osvos_stream_t stream_) {
-  OSVOS_CHECK_ARG(x_hi != nullptr && dz_hi != nullptr && n > 0 && h > 0 && w > 0 && c % 8 == 0);
-  OSVOS_CHECK_ARG(c <= 2048 && 256 % (c / 8) == 0);
-  OSVOS_CHECK_ARG((dpq == nullptr) == (wfold == nullptr));
-  OSVOS_CHECK_ARG(dpq != nullptr || dpool_hi != nullptr);
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (dpq == nullptr)
-    return launch_unpool<true, false, true>(dpool_hi, dpool_lo, x_hi, x_lo, nullptr, nullptr, nullptr, dz_hi, dz_lo,
-                                            colsum_rows, n, h, w, c, stream);
-  OSVOS_CHECK_ARG(static_cast<long>(h) * w < (1l << 30));
-  OSVOS_CHECK_ARG((reinterpret_cast<uintptr_t>(wfold) & 15) == 0);
-  if (dpool_hi != nullptr)
-    return launch_unpool<true, true, true>(dpool_hi, dpool_lo, x_hi, x_lo, nullptr, dpq, wfold, dz_hi, dz_lo, colsum_rows,
-                                           n, h, w, c, stream);
-  return launch_unpool<false, true, true>(nullptr, nullptr, x_hi, x_lo, nullptr, dpq, wfold, dz_hi, dz_lo, colsum_rows, n,
-                                          h, w, c, stream);
-}
-
-extern "C" int osvos_channel_sum(const void* act_hi, const void* act_lo, float* out, size_t npix, int c,
-                                 osvos_stream_t stream_) {
-  OSVOS_CHECK_ARG(act_hi != nullptr && out != nullptr && npix > 0 && c % 8 == 0 && c >= 8 && c <= 2048 &&
-                  256 % (c / 8) == 0);
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  OSVOS_CHECK_CUDA(cudaMemsetAsync(out, 0, c * sizeof(float), stream));
-  const int rows = 256 / (c / 8);
-  const size_t blocks = (npix + rows - 1) / rows;
-  channel_sum_kernel<<<grid_cap(blocks, 4), 256, 256 * 8 * sizeof(float), stream>>>(
-      static_cast<const __nv_bfloat16*>(act_hi), static_cast<const __nv_bfloat16*>(act_lo), npix, c, out);
-  OSVOS_CHECK_CUDA(cudaGetLastError());
-  return OSVOS_OK;
-}
-
-extern "C" size_t osvos_conv_first_bwd_workspace_bytes(void) { return (kFwCopies * 64 * 27 + 4) * sizeof(float); }
-
-extern "C" int osvos_conv_first_bwd(const float* x_nchw, const void* dz_hi, const void* dz_lo, const float* w_oihw,
-                                    float* dw, float* dx_nchw, void* workspace, int n, int h, int w,
-                                    osvos_stream_t stream_) {
-  OSVOS_CHECK_ARG(x_nchw != nullptr && dz_hi != nullptr && dw != nullptr && workspace != nullptr && n > 0 && h > 0 &&
-                  w > 0);
-  OSVOS_CHECK_ARG(dx_nchw == nullptr || w_oihw != nullptr);
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  OSVOS_CHECK_CUDA(cudaMemsetAsync(workspace, 0, osvos_conv_first_bwd_workspace_bytes(), stream));
-  const size_t tiles = static_cast<size_t>(n) * h * ((w + kFwPix - 1) / kFwPix);
-  conv_first_wgrad_kernel<false><<<grid_cap(tiles, 4), 256, 0, stream>>>(
-      x_nchw, static_cast<const __nv_bfloat16*>(dz_hi), static_cast<const __nv_bfloat16*>(dz_lo), dw,
-      static_cast<float*>(workspace), n, h, w);
-  if (dx_nchw) {
-    dim3 grid((w + 127) / 128, h, n);
-    conv_first_dgrad_kernel<<<grid, 128, 0, stream>>>(static_cast<const __nv_bfloat16*>(dz_hi),
-                                                       static_cast<const __nv_bfloat16*>(dz_lo), w_oihw, dx_nchw, n, h,
-                                                       w);
-  }
-  OSVOS_CHECK_CUDA(cudaGetLastError());
-  return OSVOS_OK;
-}
-
 static size_t conv_first_tiles(int n, int h, int w) {
   return static_cast<size_t>(n) * h * ((w + kFwPix - 1) / kFwPix);
 }
 
-extern "C" size_t osvos_conv_first_bwd_deterministic_workspace_bytes(int n, int h, int w) {
-  if (n <= 0 || h <= 0 || w <= 0) return 0;
+extern "C" size_t osvos_conv_first_bwd_workspace_bytes(int n, int h, int w, int flags) {
+  if (n <= 0 || h <= 0 || w <= 0 || (flags & ~OSVOS_FLAG_DETERMINISTIC) != 0) return 0;
+  if (!(flags & OSVOS_FLAG_DETERMINISTIC)) return (kFwCopies * 64 * 27 + 4) * sizeof(float);
   const int grid = grid_cap(conv_first_tiles(n, h, w), 4);
   // the blocks' slots, then the ordered reduction's scratch
   return (static_cast<size_t>(grid) * 64 * 27 + osvos_reduce_rows_scratch_floats(grid, 64 * 27)) * sizeof(float);
 }
 
-extern "C" int osvos_conv_first_bwd_deterministic(const float* x_nchw, const void* dz_hi, const void* dz_lo,
-                                                  const float* w_oihw, float* dw, float* dx_nchw, void* workspace, int n,
-                                                  int h, int w, osvos_stream_t stream_) {
+extern "C" int osvos_conv_first_bwd(const float* x_nchw, const void* dz_hi, const void* dz_lo, const float* w_oihw,
+                                    float* dw, float* dx_nchw, void* workspace, int n, int h, int w, int flags,
+                                    osvos_stream_t stream_) {
   OSVOS_CHECK_ARG(x_nchw != nullptr && dz_hi != nullptr && dw != nullptr && workspace != nullptr && n > 0 && h > 0 &&
                   w > 0);
   OSVOS_CHECK_ARG(dx_nchw == nullptr || w_oihw != nullptr);
+  OSVOS_CHECK_ARG((flags & ~OSVOS_FLAG_DETERMINISTIC) == 0);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const int grid = grid_cap(conv_first_tiles(n, h, w), 4);
-  float* slots = static_cast<float*>(workspace);
-  // every slot is written in full by its block (no zeroing); the slots are then added in block order
-  conv_first_wgrad_kernel<true><<<grid, 256, 0, stream>>>(
-      x_nchw, static_cast<const __nv_bfloat16*>(dz_hi), static_cast<const __nv_bfloat16*>(dz_lo), dw, slots, n, h, w);
-  OSVOS_CHECK_CUDA(cudaGetLastError());
-  int rc = reduce_rows_launch(slots, grid, 64 * 27, 64 * 27, slots + static_cast<size_t>(grid) * 64 * 27, dw, 0, stream);
-  if (rc) return rc;
+  float* ws = static_cast<float*>(workspace);
+  if (flags & OSVOS_FLAG_DETERMINISTIC) {
+    // every slot is written in full by its block (no zeroing); the slots are then added in block order
+    conv_first_wgrad_kernel<true><<<grid, 256, 0, stream>>>(
+        x_nchw, static_cast<const __nv_bfloat16*>(dz_hi), static_cast<const __nv_bfloat16*>(dz_lo), dw, ws, n, h, w);
+    OSVOS_CHECK_CUDA(cudaGetLastError());
+    int rc = reduce_rows_launch(ws, grid, 64 * 27, 64 * 27, ws + static_cast<size_t>(grid) * 64 * 27, dw, 0, stream);
+    if (rc) return rc;
+  } else {
+    OSVOS_CHECK_CUDA(cudaMemsetAsync(workspace, 0, osvos_conv_first_bwd_workspace_bytes(n, h, w, 0), stream));
+    conv_first_wgrad_kernel<false><<<grid, 256, 0, stream>>>(
+        x_nchw, static_cast<const __nv_bfloat16*>(dz_hi), static_cast<const __nv_bfloat16*>(dz_lo), dw, ws, n, h, w);
+  }
   if (dx_nchw) {
     dim3 dgrid((w + 127) / 128, h, n);
     conv_first_dgrad_kernel<<<dgrid, 128, 0, stream>>>(static_cast<const __nv_bfloat16*>(dz_hi),

@@ -328,7 +328,7 @@ static int check_conv_args(const osvos_conv3x3_args* a) {
   OSVOS_CHECK_ARG(a->n > 0 && a->h > 0 && a->w > 0);
   OSVOS_CHECK_ARG(a->cin >= 64 && a->cin % 64 == 0);
   OSVOS_CHECK_ARG(a->cout == 2 || a->cout == 16 || a->cout == 64 || (a->cout > 0 && a->cout % 128 == 0));
-  // cout == 2: the folded side branch (osvos_fold_side_weights) - pq is the only output, bias = the 2 folded biases
+  // cout == 2: the folded side branch (osvos_fold_side_weights_multi) - pq is the only output, bias = the 2 folded biases
   OSVOS_CHECK_ARG(a->cout != 2 || (a->pq != nullptr && a->y_hi == nullptr && a->y_f32 == nullptr && a->pool_hi == nullptr &&
                                    a->colsum == nullptr && !(a->flags & (OSVOS_FLAG_RELU | OSVOS_FLAG_RELU_MASK))));
   // cout == 16: side_prep - fp32 features and / or projections only (no pool or colsum either, below)

@@ -38,32 +38,6 @@ __global__ void pack_weights_kernel(const float* __restrict__ w, __nv_bfloat16* 
 // linear 3x3 convolution C -> 2 (networks/vgg_osvos.py:41,44,54 run at :67,69,72):
 //   W'[o][ci][tap] = sum_co proj_w[16 o + co] * w_side[co][ci][tap],  b'[o] = (o == 0 ? proj_b : 0) + sum_co proj_w[16 o + co] * b_side[co]
 // written straight in the packed split-bf16 operand layout [plane][tap][o][ci] the side kernel's weight box reads.
-__global__ void fold_side_weights_kernel(const float* __restrict__ w_side, const float* __restrict__ b_side,
-                                         const float* __restrict__ proj_w, const float* __restrict__ proj_b,
-                                         __nv_bfloat16* __restrict__ out, float* __restrict__ bias2, int cin) {
-  const int plane = 9 * 2 * cin;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < plane; i += gridDim.x * blockDim.x) {
-    const int ci = i % cin;
-    const int o = (i / cin) & 1;
-    const int tap = i / (2 * cin);
-    float v = 0.f;
-#pragma unroll
-    for (int co = 0; co < 16; ++co) v = fmaf(__ldg(proj_w + 16 * o + co), __ldg(w_side + (static_cast<size_t>(co) * cin + ci) * 9 + tap), v);
-    __nv_bfloat16 hi, lo;
-    split_bf16(v, hi, lo);
-    out[i] = hi;
-    out[plane + i] = lo;
-  }
-  if (blockIdx.x == 0 && threadIdx.x < 2) {
-    const int o = threadIdx.x;
-    float b = (o == 0 && proj_b) ? __ldg(proj_b) : 0.f;
-    if (b_side) {
-      for (int co = 0; co < 16; ++co) b = fmaf(__ldg(proj_w + 16 * o + co), __ldg(b_side + co), b);
-    }
-    bias2[o] = b;
-  }
-}
-
 // All scales of the side branch in ONE launch (training re-folds after every optimizer step), optionally with an fp32
 // copy of W' in the same [tap][o][ci] order for the folded backward (side_bwd_folded.cu, bwd_kernels.cu).
 struct FoldScale {
@@ -296,16 +270,6 @@ extern "C" int osvos_pack_conv3x3_weights(const float* w, void* packed, int cout
   const size_t plane = static_cast<size_t>(9) * rows * colp;
   pack_weights_kernel<<<grid_for(plane, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       w, static_cast<__nv_bfloat16*>(packed), cout, cin, rows, cols, colp, transpose_flip);
-  OSVOS_CHECK_CUDA(cudaGetLastError());
-  return OSVOS_OK;
-}
-
-extern "C" int osvos_fold_side_weights(const float* side_w, const float* side_b, const float* proj_w, const float* proj_b,
-                                       void* packed, float* bias2, int cin, osvos_stream_t stream) {
-  OSVOS_CHECK_ARG(side_w != nullptr && proj_w != nullptr && packed != nullptr && bias2 != nullptr);
-  OSVOS_CHECK_ARG(cin >= 64 && cin % 64 == 0);
-  fold_side_weights_kernel<<<grid_for(static_cast<size_t>(18) * cin, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      side_w, side_b, proj_w, proj_b, static_cast<__nv_bfloat16*>(packed), bias2, cin);
   OSVOS_CHECK_CUDA(cudaGetLastError());
   return OSVOS_OK;
 }

@@ -129,32 +129,25 @@ static int loss_grid(size_t total) {
   return static_cast<int>(blocks);
 }
 
+extern "C" size_t osvos_cbce_fwd_sums(size_t numel, int flags) {
+  if (numel == 0 || (flags & ~OSVOS_FLAG_DETERMINISTIC) != 0) return 0;
+  return (flags & OSVOS_FLAG_DETERMINISTIC) ? 5 + 3 * static_cast<size_t>(loss_grid(numel)) : 5;
+}
+
 extern "C" int osvos_cbce_fwd(const float* output, const float* label, size_t numel, double divisor, double* sums,
-                              float* loss, osvos_stream_t stream_) {
+                              float* loss, int flags, osvos_stream_t stream_) {
   OSVOS_CHECK_ARG(output != nullptr && label != nullptr && sums != nullptr && loss != nullptr && numel > 0);
   OSVOS_CHECK_ARG(((reinterpret_cast<uintptr_t>(output) | reinterpret_cast<uintptr_t>(label)) & 15) == 0);
   OSVOS_CHECK_ARG(divisor > 0);
+  OSVOS_CHECK_ARG((flags & ~OSVOS_FLAG_DETERMINISTIC) == 0);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  // deterministic: the block rows are written in full, so in both forms only the five leading values (with the arrival
+  // counter) need zeroing
   OSVOS_CHECK_CUDA(cudaMemsetAsync(sums, 0, 5 * sizeof(double), stream));
-  cbce_fwd_kernel<false><<<loss_grid(numel), kLossThreads, 0, stream>>>(output, label, numel, sums, divisor, loss);
-  OSVOS_CHECK_CUDA(cudaGetLastError());
-  return OSVOS_OK;
-}
-
-extern "C" size_t osvos_cbce_fwd_deterministic_sums(size_t numel) {
-  if (numel == 0) return 0;
-  return 5 + 3 * static_cast<size_t>(loss_grid(numel));
-}
-
-extern "C" int osvos_cbce_fwd_deterministic(const float* output, const float* label, size_t numel, double divisor,
-                                            double* sums, float* loss, osvos_stream_t stream_) {
-  OSVOS_CHECK_ARG(output != nullptr && label != nullptr && sums != nullptr && loss != nullptr && numel > 0);
-  OSVOS_CHECK_ARG(((reinterpret_cast<uintptr_t>(output) | reinterpret_cast<uintptr_t>(label)) & 15) == 0);
-  OSVOS_CHECK_ARG(divisor > 0);
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  // the block rows are written in full: only the five leading values (with the arrival counter) need zeroing
-  OSVOS_CHECK_CUDA(cudaMemsetAsync(sums, 0, 5 * sizeof(double), stream));
-  cbce_fwd_kernel<true><<<loss_grid(numel), kLossThreads, 0, stream>>>(output, label, numel, sums, divisor, loss);
+  if (flags & OSVOS_FLAG_DETERMINISTIC)
+    cbce_fwd_kernel<true><<<loss_grid(numel), kLossThreads, 0, stream>>>(output, label, numel, sums, divisor, loss);
+  else
+    cbce_fwd_kernel<false><<<loss_grid(numel), kLossThreads, 0, stream>>>(output, label, numel, sums, divisor, loss);
   OSVOS_CHECK_CUDA(cudaGetLastError());
   return OSVOS_OK;
 }

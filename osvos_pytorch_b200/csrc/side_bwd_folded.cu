@@ -3,7 +3,7 @@
 // side_prep[i] has no ReLU (reference networks/vgg_osvos.py:67), so the whole side branch of a scale,
 //   feat = side_prep(x);  p = score_dsn(feat);  q = fuse_slice . feat            (:41,44,54 run at :67,69,72)
 // is ONE linear 3x3 convolution C -> 2 with weights W'[o][c][t] = sum_f proj[o][f] * W_side[f][c][t] (the inference
-// path already runs it that way, osvos_fold_side_weights).  Its backward therefore only ever sees the TWO gradient
+// path already runs it that way, osvos_fold_side_weights_multi).  Its backward therefore only ever sees the TWO gradient
 // channels dpq = (dL/dp, dL/dq) - not the 16 feature gradients autograd materialises:
 //
 //   G[t][o][c] = sum_px dpq[px - t][o] * x[px][c]        "folded weight gradient": 18 numbers per channel     (1)
@@ -76,8 +76,8 @@ struct SwMaps {
 };
 
 // DET: instead of the vector atomics into G, each block stores its reduced partials into its own row of `g` (the row of
-// its chunk stride `blk`; the slabs of a row are disjoint), and osvos_side_folded_wgrad_multi_deterministic adds the
-// rows in order afterwards.
+// its chunk stride `blk`; the slabs of a row are disjoint), and the deterministic form of osvos_side_folded_wgrad_multi
+// adds the rows in order afterwards.
 template <bool DET = false>
 __global__ void __launch_bounds__(kSwKernelThreads, 2)
 side_folded_wgrad_kernel(const __grid_constant__ SwMaps maps, const __grid_constant__ SwParams p) {
@@ -412,34 +412,31 @@ static size_t side_wgrad_det_floats(const SwParams& p, size_t* rows_floats) {
   return rows + scratch;
 }
 
-extern "C" int osvos_side_folded_wgrad_multi(const osvos_side_wgrad_item* items, int count, osvos_stream_t stream_) {
-  SwParams p;
-  SwMaps maps;
-  int rc = side_wgrad_plan(items, count, p, maps, true);
-  if (rc) return rc;
-  static uint64_t attr_done = 0;
-  OSVOS_CHECK_CUDA(ensure_dynamic_smem(side_folded_wgrad_kernel<false>, kSwSmemBytes, &attr_done));
-  OSVOS_CHECK_CUDA(launch_pdl(side_folded_wgrad_kernel<false>, dim3(p.total_blocks), dim3(kSwKernelThreads), kSwSmemBytes,
-                              static_cast<cudaStream_t>(stream_), maps, p));
-  return OSVOS_OK;
-}
-
-extern "C" size_t osvos_side_folded_wgrad_deterministic_workspace_bytes(const osvos_side_wgrad_item* items, int count) {
-  if (items == nullptr || count <= 0 || count > kSwMaxScales) return 0;
+extern "C" size_t osvos_side_folded_wgrad_workspace_bytes(const osvos_side_wgrad_item* items, int count, int flags) {
+  if (items == nullptr || count <= 0 || count > kSwMaxScales || flags != OSVOS_FLAG_DETERMINISTIC) return 0;
   SwParams p;
   SwMaps maps;
   if (side_wgrad_plan(items, count, p, maps, false)) return 0;
   return side_wgrad_det_floats(p, nullptr) * sizeof(float);
 }
 
-extern "C" int osvos_side_folded_wgrad_multi_deterministic(const osvos_side_wgrad_item* items, int count, void* workspace,
-                                                           osvos_stream_t stream_) {
-  OSVOS_CHECK_ARG(workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 15) == 0);
+extern "C" int osvos_side_folded_wgrad_multi(const osvos_side_wgrad_item* items, int count, void* workspace, int flags,
+                                             osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG((flags & ~OSVOS_FLAG_DETERMINISTIC) == 0);
+  const bool det = (flags & OSVOS_FLAG_DETERMINISTIC) != 0;
+  if (det) OSVOS_CHECK_ARG(workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 15) == 0);
   SwParams p;
   SwMaps maps;
   int rc = side_wgrad_plan(items, count, p, maps, true);
   if (rc) return rc;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!det) {
+    static uint64_t attr_done = 0;
+    OSVOS_CHECK_CUDA(ensure_dynamic_smem(side_folded_wgrad_kernel<false>, kSwSmemBytes, &attr_done));
+    OSVOS_CHECK_CUDA(launch_pdl(side_folded_wgrad_kernel<false>, dim3(p.total_blocks), dim3(kSwKernelThreads),
+                                kSwSmemBytes, stream, maps, p));
+    return OSVOS_OK;
+  }
   size_t rows_floats = 0;
   side_wgrad_det_floats(p, &rows_floats);
   float* ws = static_cast<float*>(workspace);
@@ -460,20 +457,6 @@ extern "C" int osvos_side_folded_wgrad_multi_deterministic(const osvos_side_wgra
     if (rc) return rc;
   }
   return OSVOS_OK;
-}
-
-extern "C" int osvos_side_folded_wgrad(const void* x_hi, const void* x_lo, const float* dpq, float* g, int n, int h,
-                                       int w, int c, osvos_stream_t stream_) {
-  osvos_side_wgrad_item it;
-  it.x_hi = x_hi;
-  it.x_lo = x_lo;
-  it.dpq = dpq;
-  it.g = g;
-  it.n = n;
-  it.h = h;
-  it.w = w;
-  it.c = c;
-  return osvos_side_folded_wgrad_multi(&it, 1, stream_);
 }
 
 extern "C" int osvos_side_grads_finish(const osvos_side_grads_item* items, int count, osvos_stream_t stream_) {

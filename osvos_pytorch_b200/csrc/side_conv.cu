@@ -13,7 +13,7 @@
 //
 // NCO = 2 - the FOLDED side branch (inference and training): side_prep has no ReLU, so side_prep followed by the two 1x1 projections
 // (score_dsn, this scale's slice of fuse) is ONE linear 3x3 convolution C -> 2 whose weights are
-// W'[o][ci][tap] = sum_co proj[o][co] * W_side[co][ci][tap] (osvos_fold_side_weights).  The same kernel then runs with
+// W'[o][ci][tap] = sum_co proj[o][co] * W_side[co][ci][tap] (osvos_fold_side_weights_multi).  The same kernel then runs with
 // N = 32 (18 used) instead of 144: 1/8 of the accumulator columns to exchange, 1/4.5 of the weight bytes to stream,
 // a third less tensor time.  The backward of the folded form needs no features either (side_bwd_folded.cu); NCO = 16 stays
 // for osvos_conv3x3 calls with cout == 16 (the literal side_prep op).
@@ -358,7 +358,7 @@ static int launch_side(const osvos_conv3x3_args* const* args, int count, cudaStr
 
 int side_conv_dispatch(const osvos_conv3x3_args* a, cudaStream_t stream) {
   const osvos_conv3x3_args* one[1] = {a};
-  if (a->cout == 2)   // folded projections (osvos_fold_side_weights): pq only
+  if (a->cout == 2)   // folded projections (osvos_fold_side_weights_multi): pq only
     return (a->flags & OSVOS_FLAG_FAST) ? launch_side<1, 2>(one, 1, stream) : launch_side<2, 2>(one, 1, stream);
   return (a->flags & OSVOS_FLAG_FAST) ? launch_side<1, 16>(one, 1, stream) : launch_side<2, 16>(one, 1, stream);
 }

@@ -472,10 +472,6 @@ static int launch_wgrad(const osvos_wgrad_args* a, cudaStream_t stream) {
 
 using namespace osvos;
 
-extern "C" size_t osvos_wgrad_workspace_bytes(int cout_or_padded, int cin) {
-  return static_cast<size_t>(9) * cout_or_padded * cin * sizeof(float);
-}
-
 // Split count of the deterministic form (shape only; the tensor-core path's constraints are checked by the launch).
 static int deterministic_splits(int n, int h, int w, int cin, int dz_channels) {
   if (n <= 0 || h <= 0 || w <= 0 || cin <= 0 || dz_channels <= 0 || dz_channels % 64 != 0) return 0;
@@ -489,12 +485,19 @@ extern "C" int osvos_wgrad_deterministic_splits(int n, int h, int w, int cin, in
   return deterministic_splits(n, h, w, cin, dz_channels);
 }
 
-extern "C" size_t osvos_wgrad_deterministic_workspace_bytes(int n, int h, int w, int cin, int dz_channels) {
-  return static_cast<size_t>(deterministic_splits(n, h, w, cin, dz_channels)) * osvos_wgrad_workspace_bytes(dz_channels, cin);
+extern "C" size_t osvos_wgrad_workspace_bytes(int n, int h, int w, int cin, int dz_channels, int flags) {
+  if (n <= 0 || h <= 0 || w <= 0 || cin <= 0 || dz_channels <= 0 || (flags & ~OSVOS_FLAG_DETERMINISTIC) != 0) return 0;
+  const size_t slice = static_cast<size_t>(9) * dz_channels * cin * sizeof(float);
+  if (!(flags & OSVOS_FLAG_DETERMINISTIC)) return slice;
+  return static_cast<size_t>(deterministic_splits(n, h, w, cin, dz_channels)) * slice;
 }
 
-static int wgrad_finish_impl(const osvos_wgrad_finish_item* items, const int* splits, int count, cudaStream_t stream) {
+extern "C" int osvos_wgrad_finish(const osvos_wgrad_finish_item* items, const int* splits, int count, int flags,
+                                  osvos_stream_t stream_) {
   OSVOS_CHECK_ARG(items != nullptr && count > 0 && count <= OSVOS_WGRAD_FINISH_MAX);
+  OSVOS_CHECK_ARG((flags & ~OSVOS_FLAG_DETERMINISTIC) == 0);
+  const bool det = (flags & OSVOS_FLAG_DETERMINISTIC) != 0;
+  OSVOS_CHECK_ARG((splits != nullptr) == det);
   FinishTable t;
   t.count = count;
   long long total_items = 0;
@@ -512,7 +515,7 @@ static int wgrad_finish_impl(const osvos_wgrad_finish_item* items, const int* sp
     L.accumulate = it.accumulate ? 1 : 0;
     L.scale = it.scale;
     L.items = it.cout * (it.cin / 64);
-    L.splits = splits ? splits[i] : 1;
+    L.splits = det ? splits[i] : 1;
     OSVOS_CHECK_ARG(L.splits >= 1);
     total_items += L.items;
   }
@@ -520,22 +523,13 @@ static int wgrad_finish_impl(const osvos_wgrad_finish_item* items, const int* sp
   t.total_items = static_cast<int>(total_items);
   const long long cap = static_cast<long long>(device_sm_count()) * 10;   // 10 x 192 threads resident per SM
   const unsigned grid = static_cast<unsigned>(total_items < cap ? total_items : cap);
-  if (splits)
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (det)
     wgrad_finish_multi_kernel<true><<<grid, kFinishThreads, 0, stream>>>(t);
   else
     wgrad_finish_multi_kernel<false><<<grid, kFinishThreads, 0, stream>>>(t);
   OSVOS_CHECK_CUDA(cudaGetLastError());
   return OSVOS_OK;
-}
-
-extern "C" int osvos_wgrad_finish(const osvos_wgrad_finish_item* items, int count, osvos_stream_t stream_) {
-  return wgrad_finish_impl(items, nullptr, count, static_cast<cudaStream_t>(stream_));
-}
-
-extern "C" int osvos_wgrad_finish_deterministic(const osvos_wgrad_finish_item* items, const int* splits, int count,
-                                                osvos_stream_t stream_) {
-  OSVOS_CHECK_ARG(splits != nullptr);
-  return wgrad_finish_impl(items, splits, count, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int osvos_conv3x3_wgrad(const osvos_wgrad_args* a, osvos_stream_t stream_) {

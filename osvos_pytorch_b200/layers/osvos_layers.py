@@ -72,16 +72,11 @@ class _ClassBalancedBCE(torch.autograd.Function):
         assert x.numel() == y.numel()
         loss = torch.empty((), dtype=torch.float32, device=x.device)   # 0-dim, not a view: `loss /= k` must work
         stream = torch.cuda.current_stream().cuda_stream
-        if torch.are_deterministic_algorithms_enabled():
-            # block sums added in a fixed order instead of with fp64 atomics (rows behind sums[0..4])
-            sums = torch.empty(lib.osvos_cbce_fwd_deterministic_sums(x.numel()), dtype=torch.float64, device=x.device)
-            nat.check(lib.osvos_cbce_fwd_deterministic(x.data_ptr(), y.data_ptr(), x.numel(), float(divisor),
-                                                       sums.data_ptr(), loss.data_ptr(), stream),
-                      "osvos_cbce_fwd_deterministic")
-        else:
-            sums = torch.empty(5, dtype=torch.float64, device=x.device)
-            nat.check(lib.osvos_cbce_fwd(x.data_ptr(), y.data_ptr(), x.numel(), float(divisor), sums.data_ptr(),
-                                         loss.data_ptr(), stream), "osvos_cbce_fwd")
+        # deterministic: block sums added in a fixed order instead of with fp64 atomics (rows behind sums[0..4])
+        flags = nat.FLAG_DETERMINISTIC if torch.are_deterministic_algorithms_enabled() else 0
+        sums = torch.empty(lib.osvos_cbce_fwd_sums(x.numel(), flags), dtype=torch.float64, device=x.device)
+        nat.check(lib.osvos_cbce_fwd(x.data_ptr(), y.data_ptr(), x.numel(), float(divisor), sums.data_ptr(),
+                                     loss.data_ptr(), flags, stream), "osvos_cbce_fwd")
         ctx.save_for_backward(x, y, sums)
         ctx.divisor = float(divisor)
         ctx.shape = output.shape

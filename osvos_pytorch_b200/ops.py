@@ -114,19 +114,6 @@ def conv_first(x, weight, bias, relu=True, fast=False):
     return y
 
 
-def fold_side_weights(side_w, side_b, proj_w, proj_b):
-    """side_prep o {score_dsn, fuse slice} -> (packed [2, cin, 3, 3] operand, bias2 [2]); see include/osvos_b200.h."""
-    lib = nat.load()
-    side_w = side_w.detach().contiguous().float()
-    cin = int(side_w.shape[1])
-    packed = torch.empty(lib.osvos_packed_weight_bytes(2, cin) // 2, dtype=torch.bfloat16, device=side_w.device)
-    bias2 = torch.empty(2, dtype=torch.float32, device=side_w.device)
-    _count()
-    nat.check(lib.osvos_fold_side_weights(side_w.data_ptr(), nat.ptr(side_b), proj_w.data_ptr(), nat.ptr(proj_b),
-                                          packed.data_ptr(), bias2.data_ptr(), cin, _stream()), "osvos_fold_side_weights")
-    return packed, bias2
-
-
 def fold_side_weights_multi(entries, want_f32=True):
     """All side scales folded in ONE launch.  entries: [(side_w, side_b, proj_w [32], proj_b)] ->
     [(packed, bias2, folded_f32 [9, 2, cin] | None)]; see include/osvos_b200.h (osvos_fold_side_weights_multi)."""
@@ -460,40 +447,41 @@ def upsampling_grads_finish(reds, upscale_ws, fuse_w, d_upscale=None, d_upscale1
     nat.check(lib.osvos_upsampling_grads_finish(byref(a), _stream()), "osvos_upsampling_grads_finish")
 
 
-def unpool_dside_mask(dpool, x, dside, colsum=None, deterministic=False):
-    """dz = ReLU'(x) * (unpool(dpool) + dside) with an fp32 side gradient map [n,h,w,c]; dpool None: the deepest
-    stage (osvos_unpool_dside_mask)."""
+def unpool_mask(dpool, x, dside=None, dpq=None, wfold=None, colsum=None, deterministic=False):
+    """dz = ReLU'(x) * (unpool(dpool) + side-branch gradient) (osvos_unpool_mask).  The side-branch gradient is the
+    fp32 map `dside` [n,h,w,c], the folded form of `dpq` [n,h,w,2] and `wfold` [9,2,c], or none; dpool None: the
+    deepest stage (no pooling consumer).  `colsum` [c] accumulates the per-channel sums of dz (the bias gradient);
+    ``deterministic``: they go to per-block rows that are added in order."""
     lib = nat.load()
     n, h, w, c = x.shape
     dz = Act.empty(n, h, w, c, x.hi.device, x.lo is None)
+    flags = nat.FLAG_DETERMINISTIC if deterministic else 0
     rows = None
     if deterministic and colsum is not None:
-        nrows = lib.osvos_unpool_colsum_rows(n, h, w, c, int(dpool is not None), 0)
+        nrows = lib.osvos_unpool_colsum_rows(n, h, w, c, int(dpool is not None), int(dpq is not None))
         rows = torch.empty((nrows, c), dtype=torch.float32, device=x.hi.device)
     _count()
-    nat.check(lib.osvos_unpool_dside_mask(dpool.hi.data_ptr() if dpool is not None else None,
-                                          nat.ptr(dpool.lo) if dpool is not None else None, x.hi.data_ptr(),
-                                          nat.ptr(x.lo), dside.data_ptr(), dz.hi.data_ptr(), nat.ptr(dz.lo),
-                                          nat.ptr(rows if rows is not None else colsum), n, h, w, c,
-                                          nat.FLAG_DETERMINISTIC if deterministic else 0, _stream()),
-              "osvos_unpool_dside_mask")
+    nat.check(lib.osvos_unpool_mask(dpool.hi.data_ptr() if dpool is not None else None,
+                                    nat.ptr(dpool.lo) if dpool is not None else None, x.hi.data_ptr(), nat.ptr(x.lo),
+                                    nat.ptr(dside), nat.ptr(dpq), nat.ptr(wfold), dz.hi.data_ptr(), nat.ptr(dz.lo),
+                                    nat.ptr(rows if rows is not None else colsum), n, h, w, c, flags, _stream()),
+              "osvos_unpool_mask")
     if rows is not None:
         reduce_rows(rows, colsum, accumulate=True)
     return dz
 
 
 # ------------------------------------------------------------------ backward ops
-def wgrad_workspace_floats(dz_channels, cin, shape=None, deterministic=False):
-    """Workspace of one weight gradient; ``deterministic`` (needs ``shape`` = (n, h, w)): one slice per pixel-range
-    split, see osvos_wgrad_deterministic_workspace_bytes."""
-    if deterministic:
-        return nat.load().osvos_wgrad_deterministic_workspace_bytes(*shape, cin, dz_channels) // 4
-    return nat.load().osvos_wgrad_workspace_bytes(dz_channels, cin) // 4
+def wgrad_workspace_floats(dz_channels, cin, shape, deterministic=False):
+    """Workspace of one weight gradient over an input of ``shape`` = (n, h, w) (osvos_wgrad_workspace_bytes);
+    ``deterministic``: one slice per pixel-range split."""
+    flags = nat.FLAG_DETERMINISTIC if deterministic else 0
+    return nat.load().osvos_wgrad_workspace_bytes(*shape, cin, dz_channels, flags) // 4
 
 
 def conv3x3_wgrad(x, dz, cout, fast=False, deferred_ws=None, deterministic=False):
     """dW [cout, cin, 3, 3] of a 3x3 conv from its input act `x` and output-gradient act `dz`.
-    With `deferred_ws` (a ZEROED fp32 workspace of wgrad_workspace_floats(dz.channels, cin)) only the tensor-core
+    With `deferred_ws` (a ZEROED fp32 workspace of wgrad_workspace_floats(dz.channels, cin, shape)) only the tensor-core
     accumulation is enqueued and a finish item for ops.wgrad_finish is returned instead of dW.  ``deterministic``:
     per-split workspace slices summed in order (the workspace is then wgrad_workspace_floats(..., deterministic=True)
     floats and needs no zeroing)."""
@@ -533,13 +521,11 @@ def wgrad_finish(items):
             f.workspace, f.dw = it["ws"].data_ptr(), it["dw"].data_ptr()
             f.cout, f.cin, f.dz_channels = it["cout"], it["cin"], it["dz_channels"]
             f.accumulate, f.scale = int(bool(it.get("accumulate"))), 1.0
+        det = any("splits" in it for it in part)         # deterministic workspaces: their split slices in order
+        splits = (nat.c_int * len(part))(*(int(it.get("splits", 1)) for it in part)) if det else None
         _count(1)
-        if any("splits" in it for it in part):           # deterministic workspaces: their split slices in order
-            splits = (nat.c_int * len(part))(*(int(it.get("splits", 1)) for it in part))
-            nat.check(lib.osvos_wgrad_finish_deterministic(arr, splits, len(part), _stream()),
-                      "osvos_wgrad_finish_deterministic")
-        else:
-            nat.check(lib.osvos_wgrad_finish(arr, len(part), _stream()), "osvos_wgrad_finish")
+        nat.check(lib.osvos_wgrad_finish(arr, splits, len(part), nat.FLAG_DETERMINISTIC if det else 0, _stream()),
+                  "osvos_wgrad_finish")
 
 
 def tail_bwd(grads, n, h, w, deterministic=False):
@@ -579,110 +565,38 @@ def reduce_rows(rows, out, accumulate=False):
 
 
 def sum_f32(x, deterministic=False):
+    """sum(x) as a [1] fp32 tensor (osvos_sum_f32); ``deterministic``: fixed grid of contiguous ranges, totals added in
+    order."""
     lib = nat.load()
     x = x.contiguous().float()
-    if deterministic:                               # fixed grid of contiguous ranges, totals added in order
-        scratch = torch.empty(lib.osvos_sum_f32_deterministic_scratch_bytes(), dtype=torch.uint8, device=x.device)
-        out = torch.empty(1, dtype=torch.float32, device=x.device)
-        _count(1)
-        nat.check(lib.osvos_sum_f32_deterministic(x.data_ptr(), x.numel(), scratch.data_ptr(), out.data_ptr(),
-                                                  _stream()), "osvos_sum_f32_deterministic")
-        return out
-    scratch = torch.empty(2, dtype=torch.float64, device=x.device)
+    flags = nat.FLAG_DETERMINISTIC if deterministic else 0
+    scratch = torch.empty(lib.osvos_sum_f32_scratch_bytes(flags), dtype=torch.uint8, device=x.device)
     out = torch.empty(1, dtype=torch.float32, device=x.device)
     _count(1)
-    nat.check(lib.osvos_sum_f32(x.data_ptr(), x.numel(), scratch.data_ptr(), out.data_ptr(), _stream()),
+    nat.check(lib.osvos_sum_f32(x.data_ptr(), x.numel(), scratch.data_ptr(), out.data_ptr(), flags, _stream()),
               "osvos_sum_f32")
     return out
-
-
-def _unpool_deterministic(dpool, x, dpq, wfold, colsum):
-    """osvos_unpool_mask_deterministic: the column sums as per-block rows, added into `colsum` in order."""
-    lib = nat.load()
-    n, h, w, c = x.shape
-    dz = Act.empty(n, h, w, c, x.hi.device, x.lo is None)
-    rows = None
-    if colsum is not None:
-        nrows = lib.osvos_unpool_colsum_rows(n, h, w, c, int(dpool is not None), int(dpq is not None))
-        rows = torch.empty((nrows, c), dtype=torch.float32, device=x.hi.device)
-    _count()
-    nat.check(lib.osvos_unpool_mask_deterministic(dpool.hi.data_ptr() if dpool is not None else None,
-                                                  nat.ptr(dpool.lo) if dpool is not None else None, x.hi.data_ptr(),
-                                                  nat.ptr(x.lo), nat.ptr(dpq), nat.ptr(wfold), dz.hi.data_ptr(),
-                                                  nat.ptr(dz.lo), nat.ptr(rows), n, h, w, c, _stream()),
-              "osvos_unpool_mask_deterministic")
-    if rows is not None:
-        reduce_rows(rows, colsum, accumulate=True)
-    return dz
-
-
-def unpool_add_mask(dpool, x, dside, colsum=None, deterministic=False):
-    if deterministic:
-        if dside is not None:
-            raise ValueError("unpool_add_mask: the deterministic form takes no fp32 side gradient map")
-        return _unpool_deterministic(dpool, x, None, None, colsum)
-    lib = nat.load()
-    n, h, w, c = x.shape
-    dz = Act.empty(n, h, w, c, x.hi.device, x.lo is None)
-    _count()
-    nat.check(lib.osvos_unpool_add_mask(dpool.hi.data_ptr(), nat.ptr(dpool.lo), x.hi.data_ptr(), nat.ptr(x.lo),
-                                        nat.ptr(dside), dz.hi.data_ptr(), nat.ptr(dz.lo), nat.ptr(colsum), n, h, w, c,
-                                        _stream()),
-              "osvos_unpool_add_mask")
-    return dz
-
-
-def unpool_side_mask(dpool, x, dpq, wfold, colsum=None, deterministic=False):
-    """dz = ReLU'(x) * (unpool(dpool) + folded side gradient of dpq); dpool None: no pooling consumer."""
-    if deterministic:
-        return _unpool_deterministic(dpool, x, dpq, wfold, colsum)
-    lib = nat.load()
-    n, h, w, c = x.shape
-    dz = Act.empty(n, h, w, c, x.hi.device, x.lo is None)
-    _count()
-    nat.check(lib.osvos_unpool_side_mask(dpool.hi.data_ptr() if dpool is not None else None,
-                                         nat.ptr(dpool.lo) if dpool is not None else None, x.hi.data_ptr(), nat.ptr(x.lo),
-                                         dpq.data_ptr(), wfold.data_ptr(), dz.hi.data_ptr(), nat.ptr(dz.lo),
-                                         nat.ptr(colsum), n, h, w, c, _stream()),
-              "osvos_unpool_side_mask")
-    return dz
 
 
 def side_folded_wgrad_floats(c):
     return int(nat.load().osvos_side_folded_wgrad_floats(c))
 
 
-def side_folded_wgrad(x, dpq, g):
-    """g ([18 c + 2] fp32, PRE-ZEROED) += folded weight gradient of the side branch (include/osvos_b200.h)."""
-    lib = nat.load()
-    n, h, w, c = x.shape
-    _count()
-    nat.check(lib.osvos_side_folded_wgrad(x.hi.data_ptr(), nat.ptr(x.lo), dpq.data_ptr(), g.data_ptr(), n, h, w, c,
-                                          _stream()), "osvos_side_folded_wgrad")
-    return g
-
-
 def side_folded_wgrad_multi(xs, dpqs, gs, deterministic=False):
-    """side_folded_wgrad of several scales in ONE launch (osvos_side_folded_wgrad_multi); ``deterministic``: the
-    blocks' partial rows are added in order (osvos_side_folded_wgrad_multi_deterministic)."""
+    """gs[k] ([18 c + 2] fp32, PRE-ZEROED) += folded weight gradient of the side branch of scale k, all scales in ONE
+    launch (osvos_side_folded_wgrad_multi); ``deterministic``: the blocks' partial rows are added in order."""
     lib = nat.load()
     arr = (nat.SideWgradItem * len(xs))()
     for it, x, dpq, g in zip(arr, xs, dpqs, gs):
         n, h, w, c = x.shape
         it.x_hi, it.x_lo, it.dpq, it.g = x.hi.data_ptr(), nat.ptr(x.lo), dpq.data_ptr(), g.data_ptr()
         it.n, it.h, it.w, it.c = n, h, w, c
-    if deterministic:
-        nbytes = lib.osvos_side_folded_wgrad_deterministic_workspace_bytes(arr, len(xs))
-        if nbytes == 0:
-            nat.check(lib.osvos_side_folded_wgrad_multi_deterministic(arr, len(xs), None, _stream()),
-                      "osvos_side_folded_wgrad_multi_deterministic")
-        ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=gs[0].device)
-        _count(1 + 2 * len(xs))
-        nat.check(lib.osvos_side_folded_wgrad_multi_deterministic(arr, len(xs), ws.data_ptr(), _stream()),
-                  "osvos_side_folded_wgrad_multi_deterministic")
-        return
-    _count()
-    nat.check(lib.osvos_side_folded_wgrad_multi(arr, len(xs), _stream()), "osvos_side_folded_wgrad_multi")
+    flags = nat.FLAG_DETERMINISTIC if deterministic else 0
+    nbytes = lib.osvos_side_folded_wgrad_workspace_bytes(arr, len(xs), flags)
+    ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=gs[0].device) if nbytes else None
+    _count(1 + 2 * len(xs) if deterministic else 1)
+    nat.check(lib.osvos_side_folded_wgrad_multi(arr, len(xs), nat.ptr(ws), flags, _stream()),
+              "osvos_side_folded_wgrad_multi")
 
 
 def side_grads_finish(entries, accumulate):
@@ -702,33 +616,16 @@ def side_grads_finish(entries, accumulate):
     nat.check(lib.osvos_side_grads_finish(items, len(entries), _stream()), "osvos_side_grads_finish")
 
 
-def channel_sum(a):
-    lib = nat.load()
-    n, h, w, c = a.shape
-    out = torch.empty(c, dtype=torch.float32, device=a.hi.device)
-    _count()
-    nat.check(lib.osvos_channel_sum(a.hi.data_ptr(), nat.ptr(a.lo), out.data_ptr(), n * h * w, c, _stream()),
-              "osvos_channel_sum")
-    return out
-
-
 def conv_first_bwd(x, dz, weight, need_dx, deterministic=False):
     lib = nat.load()
     n, _, h, w = (int(v) for v in x.shape)
     dw = torch.empty((64, 3, 3, 3), dtype=torch.float32, device=x.device)
     dx = torch.empty_like(x) if need_dx else None
-    if deterministic:                               # one partial slot per block, added in block order
-        ws = torch.empty(lib.osvos_conv_first_bwd_deterministic_workspace_bytes(n, h, w), dtype=torch.uint8,
-                         device=x.device)
-        _count(2 if need_dx else 1)
-        nat.check(lib.osvos_conv_first_bwd_deterministic(x.data_ptr(), dz.hi.data_ptr(), nat.ptr(dz.lo),
-                                                         weight.data_ptr(), dw.data_ptr(), nat.ptr(dx), ws.data_ptr(),
-                                                         n, h, w, _stream()), "osvos_conv_first_bwd_deterministic")
-        return dw, dx
-    ws = torch.empty(lib.osvos_conv_first_bwd_workspace_bytes(), dtype=torch.uint8, device=x.device)
+    flags = nat.FLAG_DETERMINISTIC if deterministic else 0   # deterministic: one partial slot per block, added in order
+    ws = torch.empty(lib.osvos_conv_first_bwd_workspace_bytes(n, h, w, flags), dtype=torch.uint8, device=x.device)
     _count(2 if need_dx else 1)
     nat.check(lib.osvos_conv_first_bwd(x.data_ptr(), dz.hi.data_ptr(), nat.ptr(dz.lo), weight.data_ptr(),
-                                       dw.data_ptr(), nat.ptr(dx), ws.data_ptr(), n, h, w, _stream()),
+                                       dw.data_ptr(), nat.ptr(dx), ws.data_ptr(), n, h, w, flags, _stream()),
               "osvos_conv_first_bwd")
     return dw, dx
 

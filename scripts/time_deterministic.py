@@ -120,10 +120,11 @@ def workspace_bytes(n):
         for _ in range(s):
             h, w = (h + 1) // 2, (w + 1) // 2
         if cin > 3:
-            wg += lib.osvos_wgrad_deterministic_workspace_bytes(n, h, w, cin, cout) - lib.osvos_wgrad_workspace_bytes(cout, cin)
+            wg += (lib.osvos_wgrad_workspace_bytes(n, h, w, cin, cout, nat.FLAG_DETERMINISTIC)
+                   - lib.osvos_wgrad_workspace_bytes(n, h, w, cin, cout, 0))
         colsum += lib.osvos_conv3x3_colsum_rows(n, h, w) * cout * 4
     return {"wgrad_slices": int(wg), "colsum_rows_upper_bound": int(colsum),
-            "conv1_1_slots": int(lib.osvos_conv_first_bwd_deterministic_workspace_bytes(n, H, W)),
+            "conv1_1_slots": int(lib.osvos_conv_first_bwd_workspace_bytes(n, H, W, nat.FLAG_DETERMINISTIC)),
             "tail_rows": int(lib.osvos_tail_fwd_deterministic_sums(n, H, W) * 8)}
 
 

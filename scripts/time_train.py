@@ -31,8 +31,8 @@ ms = e0.elapsed_time(e1) / reps
 print(f"fwd+bwd {h}x{w} {prec}: {ms:.3f} ms/frame = {1000/ms:.1f} fps; conv TFLOP/s (algorithmic, 3x fwd flops) {3*oc.conv_flops(h, w)/ms/1e9:.1f}")
 rec = []
 names = ["conv_first", "conv3x3", "maxpool2x2", "tail_fwd", "conv3x3_wgrad", "tail_bwd", "sum_f32", "side_folded_multi",
-         "side_folded_wgrad_multi", "side_grads_finish", "unpool_side_mask", "unpool_add_mask", "channel_sum",
-         "conv_first_bwd", "pack_conv3x3_weights", "fold_side_weights_multi"]
+         "side_folded_wgrad_multi", "side_grads_finish", "unpool_mask", "conv_first_bwd", "pack_conv3x3_weights",
+         "fold_side_weights_multi"]
 def wrap(name):
     f = getattr(O, name)
     def g(*a, **k):

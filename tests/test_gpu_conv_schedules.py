@@ -359,18 +359,18 @@ def test_wgrad_deferred_finish_accumulates(dev, sms):
 
 @pytest.mark.parametrize("det", [False, True])
 @pytest.mark.parametrize("fast", [False, True])
-def test_wgrad_refuses_dz_channels_192(dev, fast, det):
+def test_wgrad_refuses_192_output_channels(dev, fast, det):
     """192 output channels are not a whole number of 128-row m blocks.  With a workspace present the launch reaches
     plan_wgrad, which refuses it as OSVOS_ERR_UNSUPPORTED (status 3) before anything is enqueued: no kernel runs and
     the workspace keeps its contents.  The deterministic workspace size of such a shape is 0
-    (osvos_wgrad_deterministic_workspace_bytes), so the immediate deterministic call has no workspace and is refused
-    earlier, as an invalid argument (status 1)."""
+    (osvos_wgrad_workspace_bytes with OSVOS_FLAG_DETERMINISTIC), so the immediate deterministic call has no workspace
+    and is refused earlier, as an invalid argument (status 1)."""
     from osvos_pytorch_b200 import _native as nat, ops
     g = torch.Generator().manual_seed(3)
     x = ops.nchw_to_act(torch.randn(1, 128, 9, 11, generator=g).to(dev), fast)
     dz = ops.nchw_to_act(torch.randn(1, 192, 9, 11, generator=g).to(dev), fast)
-    assert nat.load().osvos_wgrad_deterministic_workspace_bytes(1, 9, 11, 128, 192) == 0
-    ws = torch.full((ops.wgrad_workspace_floats(192, 128),), 7.0, device=dev)
+    assert nat.load().osvos_wgrad_workspace_bytes(1, 9, 11, 128, 192, nat.FLAG_DETERMINISTIC) == 0
+    ws = torch.full((ops.wgrad_workspace_floats(192, 128, (1, 9, 11)),), 7.0, device=dev)
     with KernelsRan() as k:
         with pytest.raises(nat.NativeLibraryError, match="failed with status 3"):
             ops.conv3x3_wgrad(x, dz, 192, fast=fast, deferred_ws=ws, deterministic=det)

@@ -65,7 +65,7 @@ def xa_ref(act):
     return ops.act_to_nchw(act).double().cpu()
 
 
-def test_wgrad_workspace_figures():
+def test_deterministic_wgrad_workspace_figures():
     """The deterministic workspace of every trunk layer at 480x854, batch 1 (printed; DESIGN.md §16 quotes them)."""
     from osvos_pytorch_b200 import _native as nat
     lib = nat.load()
@@ -74,8 +74,9 @@ def test_wgrad_workspace_figures():
     total = 0
     for cin, cout, s in layers:
         h, w = -(-480 // s), -(-854 // s)
-        nb = lib.osvos_wgrad_deterministic_workspace_bytes(1, h, w, cin, cout)
-        assert nb == lib.osvos_wgrad_deterministic_splits(1, h, w, cin, cout) * lib.osvos_wgrad_workspace_bytes(cout, cin)
+        nb = lib.osvos_wgrad_workspace_bytes(1, h, w, cin, cout, nat.FLAG_DETERMINISTIC)
+        assert nb == lib.osvos_wgrad_deterministic_splits(1, h, w, cin, cout) * lib.osvos_wgrad_workspace_bytes(1, h, w, cin,
+                                                                                                              cout, 0)
         total += nb
         print(f"{cin}->{cout} at {h}x{w}: {lib.osvos_wgrad_deterministic_splits(1, h, w, cin, cout)} splits, "
               f"{nb / 2**20:.1f} MiB")

@@ -42,10 +42,10 @@ def test_dgrad_column_sums(n, h, w, cin, cout, fast):
 @pytest.mark.parametrize("n,h,w,c", [(1, 40, 56, 64), (2, 67, 93, 128), (1, 120, 214, 256), (1, 31, 55, 512)])
 @pytest.mark.parametrize("side", [False, True])
 @pytest.mark.parametrize("pool", [True, False])
-def test_unpool_column_sums(n, h, w, c, side, pool):
+def test_unpool_mask_column_sums(n, h, w, c, side, pool):
     from osvos_pytorch_b200 import ops
     if not side and not pool:
-        pytest.skip("the add form always has a pooling consumer")
+        pytest.skip("without the side branch the call needs a pooling consumer")
     x = _act(_rand((n, c, h, w), 4))
     dpool = _act(_rand((n, c, (h + 1) // 2, (w + 1) // 2), 5, 0.1)) if pool else None
     dpq = _rand((n, h, w, 2), 6, 0.1).cuda() if side else None
@@ -53,10 +53,7 @@ def test_unpool_column_sums(n, h, w, c, side, pool):
     outs = []
     for det in (True, True, False):
         cs = torch.zeros(c, device="cuda")
-        if side:
-            dz = ops.unpool_side_mask(dpool, x, dpq, wfold, colsum=cs, deterministic=det)
-        else:
-            dz = ops.unpool_add_mask(dpool, x, None, colsum=cs, deterministic=det)
+        dz = ops.unpool_mask(dpool, x, dpq=dpq, wfold=wfold, colsum=cs, deterministic=det)
         outs.append((cs, ops.act_to_nchw(dz)))
     assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[2][1])   # dz itself is unchanged
     assert maxrel(outs[0][0], outs[2][0]) < 1e-5

@@ -161,8 +161,8 @@ def test_stage1_fused_equals_conv1_1_then_conv1_2(dev, n, h, w):
     assert maxrel(ops.act_to_nchw(pool1).cpu(), ops.act_to_nchw(pool0).cpu()) < 2e-5
 
 
-def test_side_branch_folded_into_one_conv(dev):
-    """side_prep (no ReLU) + score_dsn + fuse slice == ONE 3x3 conv C -> 2 (osvos_fold_side_weights): same pq as the
+def test_side_branch_multi_fold_is_one_conv(dev):
+    """side_prep (no ReLU) + score_dsn + fuse slice == ONE 3x3 conv C -> 2 (osvos_fold_side_weights_multi): same pq as the
     16-feature kernel with fused projections, to fp32 reassociation."""
     from osvos_pytorch_b200 import ops
     for n, h, w, cin in [(1, 30, 27, 128), (2, 17, 13, 256), (1, 60, 107, 512), (1, 5, 3, 512), (1, 120, 214, 128)]:
@@ -175,7 +175,8 @@ def test_side_branch_folded_into_one_conv(dev):
         a = ops.nchw_to_act(x.to(dev))
         _, _, pq16 = ops.conv3x3(a, ops.pack_conv3x3_weights(wt.to(dev)), bs.to(dev), 16, out_act=False, proj_w=proj.to(dev),
                                  proj_b=pb.to(dev))
-        packed, bias2 = ops.fold_side_weights(wt.to(dev), bs.to(dev), proj.to(dev), pb.to(dev))
+        (packed, bias2, _), = ops.fold_side_weights_multi([(wt.to(dev), bs.to(dev), proj.to(dev), pb.to(dev))],
+                                                          want_f32=False)
         pq2 = ops.side_folded(a, packed, bias2)
         torch.cuda.synchronize()
         feat = F.conv2d(x.double(), wt.double(), bs.double(), padding=1)

@@ -30,7 +30,7 @@ def _literal_branch(x, side_w, side_b, ws, bs, wf, dp, dq):
 
 
 @pytest.mark.parametrize("n,h,w,c", [(1, 9, 14, 128), (2, 7, 5, 128), (1, 33, 45, 256), (1, 4, 6, 512), (1, 40, 70, 128)])
-def test_folded_side_backward_kernels(dev, n, h, w, c):
+def test_folded_side_backward(dev, n, h, w, c):
     from osvos_pytorch_b200 import ops
     g = torch.Generator().manual_seed(h * w + c)
     x = split_round(torch.randn(n, c, h, w, generator=g).clamp(min=0) * 2)       # a post-ReLU stage output
@@ -44,17 +44,22 @@ def test_folded_side_backward_kernels(dev, n, h, w, c):
 
     proj = torch.cat([ws, wf]).to(dev)
     (packed, bias2, wfold), = ops.fold_side_weights_multi([(side_w.to(dev), side_b.to(dev), proj, bs.to(dev))])
-    # the fold itself: W'[t][o][c] = sum_f proj[o][f] side_w[f][c][t], same operand / bias as the single-scale entry point
+    # the fold itself: W'[t][o][c] = sum_f proj[o][f] side_w[f][c][t]; the packed operand is the split-bf16 packing of
+    # that same fp32 fold (as OIHW [2, c, 3, 3]), bit for bit
     want_fold = torch.einsum("of,fct->toc", torch.stack([ws, wf]).double(), side_w.double().reshape(16, c, 9))
     assert maxrel(wfold, want_fold) < 1e-6
-    packed1, bias1 = ops.fold_side_weights(side_w.to(dev), side_b.to(dev), proj, bs.to(dev))
-    assert torch.equal(packed1, packed) and torch.equal(bias1, bias2)
+    assert torch.equal(packed, ops.pack_conv3x3_weights(wfold.permute(1, 2, 0).reshape(2, c, 3, 3)))
+    # b'[o] = (o == 0 ? proj_b : 0) + sum_f proj[o][f] side_b[f]: 16 fp32 FMAs after the proj_b term
+    terms = torch.stack([ws, wf]).double() * side_b.double()
+    want_b = terms.sum(1) + torch.cat([bs.double(), torch.zeros(1, dtype=torch.float64)])
+    b_bound = 17 * 2.0 ** -24 * (terms.abs().sum(1) + torch.cat([bs.double().abs(), torch.zeros(1, dtype=torch.float64)]))
+    assert bool(((bias2.cpu().double() - want_b).abs() <= b_bound).all()), (bias2, want_b)
 
     xa = ops.nchw_to_act(x.to(dev))
     dpq = torch.stack([dp, dq], dim=-1).contiguous().to(dev)
     # (1) G and the parameter gradients
     gbuf = torch.zeros(ops.side_folded_wgrad_floats(c), device=dev)
-    ops.side_folded_wgrad(xa, dpq, gbuf)
+    ops.side_folded_wgrad_multi([xa], [dpq], [gbuf])
     G = gbuf[:18 * c].view(9, 2, c).cpu().double()
     xpad = F.pad(x.double(), (1, 1, 1, 1))
     for t in range(9):
@@ -83,15 +88,16 @@ def test_folded_side_backward_kernels(dev, n, h, w, c):
     for pooled in (True, False):
         want = ((xr.grad if pooled else 0) + dx_ref) * (x > 0)
         colsum = torch.zeros(c, device=dev)
-        dz = ops.unpool_side_mask(ops.nchw_to_act(dpool.to(dev)) if pooled else None, xa, dpq, wfold, colsum=colsum)
+        dz = ops.unpool_mask(ops.nchw_to_act(dpool.to(dev)) if pooled else None, xa, dpq=dpq, wfold=wfold,
+                             colsum=colsum)
         got = ops.act_to_nchw(dz).cpu()
         assert maxrel(got, want) < 3e-5, (pooled, maxrel(got, want))
         assert maxrel(colsum.cpu(), want.sum((0, 2, 3))) < 3e-5
 
 
-def test_folded_wgrad_multi_scale_launch(dev):
+def test_folded_wgrad_scales_in_one_launch(dev):
     """osvos_side_folded_wgrad_multi: the four scales' G in one launch (block ranges per scale) equals one launch per scale
-    up to the order of the fp32 atomics."""
+    (the same entry point with one item) up to the order of the fp32 atomics."""
     from osvos_pytorch_b200 import ops
     g = torch.Generator().manual_seed(31)
     shapes = [(1, 30, 53, 128), (1, 15, 27, 256), (1, 8, 14, 512), (1, 4, 7, 512)]
@@ -103,7 +109,7 @@ def test_folded_wgrad_multi_scale_launch(dev):
         single = []
         for x, d in zip(xs, dpqs):
             gb = torch.zeros(ops.side_folded_wgrad_floats(x.shape[3]), device=dev)
-            ops.side_folded_wgrad(x, d, gb)
+            ops.side_folded_wgrad_multi([x], [d], [gb])
             single.append(gb)
         multi = [torch.zeros_like(s) for s in single]
         ops.side_folded_wgrad_multi(xs, dpqs, multi)

@@ -7,7 +7,7 @@ torch.profiler confirms which instantiation each launch ran and how many times.
   CTA's tile walk crosses from one scale (and chunk count) into the next.
 - side_folded_wgrad_kernel<DET>: {atomic, deterministic} x {exact, fast} x {one chunk per block, a ring that wraps with
   uneven chunk counts, a multi-scale launch with a scale clamped to one block per slab, rows narrower than a chunk}.
-- unpool_add_mask_kernel<POOL, SIDE, DET>: all eight through the four entry points, with the folded weights in global
+- unpool_add_mask_kernel<POOL, SIDE, DET>: all eight through osvos_unpool_mask, with the folded weights in global
   and in shared memory, at c = 64 .. 512, more tiles than CTAs, odd sizes, tied window maxima, +-0 and negative x.
 - tail_fwd_kernel<DET>: more rows than blocks, odd width, with and without a label, output and label planes 16-byte
   aligned and 4 bytes off.
@@ -144,7 +144,8 @@ class SideScale:
         self.proj_b = (torch.randn(1, generator=g) * 0.1).to(dev)
         self.a = ops.nchw_to_act(x.to(dev), fast)
         if nco == 2:
-            self.wp, self.bias = ops.fold_side_weights(side_w.to(dev), side_b.to(dev), self.proj, self.proj_b)
+            (self.wp, self.bias, _), = ops.fold_side_weights_multi(
+                [(side_w.to(dev), side_b.to(dev), self.proj, self.proj_b)], want_f32=False)
         else:
             self.wp, self.bias = ops.pack_conv3x3_weights(side_w.to(dev)), side_b.to(dev)
         torch.cuda.synchronize()
@@ -170,7 +171,7 @@ SIDE_TARGETS = [(nco, fast, regime) for nco in (2, 16) for fast in (False, True)
 
 @pytest.mark.parametrize("target", SIDE_TARGETS,
                          ids=[f"nco{c}-{'fast' if f else 'exact'}-{r}" for c, f, r in SIDE_TARGETS])
-def test_side_conv(dev, sms, target):
+def test_side_conv_schedule(dev, sms, target):
     from osvos_pytorch_b200 import ops
     nco, fast, regime = target
     n, h, w = sdr.find_side_shape(regime, sms)
@@ -196,7 +197,7 @@ SIDE_MULTI_TARGETS = [(count, fast) for count in (2, 3, 4) for fast in (False, T
 
 @pytest.mark.parametrize("target", SIDE_MULTI_TARGETS,
                          ids=[f"{c}scales-{'fast' if f else 'exact'}" for c, f in SIDE_MULTI_TARGETS])
-def test_side_conv_multi_scale(dev, sms, target):
+def test_side_conv_scales_in_one_launch(dev, sms, target):
     """The scales are passed shallowest first (the network's order); the launch runs them deepest first."""
     from osvos_pytorch_b200 import ops
     count, fast = target
@@ -361,7 +362,7 @@ def _bits(t):
 
 @pytest.mark.parametrize("fast", [False, True], ids=["exact", "fast"])
 @pytest.mark.parametrize("target,c", UNPOOL_TARGETS, ids=[_unpool_id(t, c) for t, c in UNPOOL_TARGETS])
-def test_unpool(dev, sms, target, c, fast):
+def test_unpool_mask(dev, sms, target, c, fast):
     from osvos_pytorch_b200 import ops
     pool, side, det, wf = target
     n, h, w = sdr.find_unpool_shape(pool, side, det, wf, c, sms)
@@ -378,29 +379,15 @@ def test_unpool(dev, sms, target, c, fast):
     if side:
         def launches():
             cs = zeros()
-            return [(ops.unpool_side_mask(dpool, p.x, p.dpq, p.wfold, colsum=cs, deterministic=det), cs)]
+            return [(ops.unpool_mask(dpool, p.x, dpq=p.dpq, wfold=p.wfold, colsum=cs, deterministic=det), cs)]
     else:
-        def launches():
+        def launches():                 # with and without the fp32 side map; without dpool the map is the only consumer
             runs = []
-            if det:
+            for ds in ((p.dside, None) if pool else (p.dside,)):
                 cs = zeros()
-                runs.append((ops.unpool_dside_mask(dpool, p.x, p.dside, colsum=cs, deterministic=True), cs, p.dside))
-                if pool:
-                    cs = zeros()
-                    runs.append((ops.unpool_add_mask(dpool, p.x, None, colsum=cs, deterministic=True), cs, None))
-            else:
-                cs = zeros()
-                runs.append((ops.unpool_dside_mask(dpool, p.x, p.dside, colsum=cs), cs, p.dside))
-                if pool:
-                    for ds in (p.dside, None):
-                        cs = zeros()
-                        runs.append((ops.unpool_add_mask(dpool, p.x, ds, colsum=cs), cs, ds))
+                runs.append((ops.unpool_mask(dpool, p.x, dside=ds, colsum=cs, deterministic=det), cs, ds))
             return runs
-    if side or not pool:
-        expected = 1
-    else:
-        expected = 2 if det else 3
-    runs = ran(launches, {inst: expected})
+    runs = ran(launches, {inst: 2 if pool and not side else 1})
     depth = p.colsum_depth(plan, det)
     for run in runs:
         dz, cs = run[0], run[1]

@@ -15,8 +15,8 @@ torch.profiler confirms which kernels each call ran and how many times.
   walk the row) and n h > 8 SMs (blocks stride rows), with and without a label; maps, the 13 sums and six losses.
 - cbce_fwd_kernel<DET> and cbce_bwd_kernel: numel 1 - 3 (no vector), one block, and a capped grid with three vectors
   per thread, each with numel % 4 = 1, 2, 3 and 0; all-positive, all-negative and exactly-0.5 labels.
-- sum_f32 (both forms), channel_sum at c = 64 .. 512 (npix not a multiple of the block's rows, lo planes absent, a
-  capped grid) and osvos_reduce_rows at nrows 1, 63, 64, 65 and 4100, ncols not a multiple of 32, with accumulate.
+- sum_f32 (both forms) and osvos_reduce_rows at nrows 1, 63, 64, 65 and 4100, ncols not a multiple of 32, with
+  accumulate.
 
 Bounds.  U = 2^-23 is the unit of one fp32 rounding.  An output the kernel forms by `steps` fp32 roundings of running
 sums of terms t_i is within steps * U * sum |t_i| of the exact sum of the terms it read, computed here in fp64 from the
@@ -39,8 +39,7 @@ absolute values of the operands, so the check also holds where the output cancel
   atomics, or the ordered sum: ceil(blocks / 256) + 256) + E, over |softplus(x)| + |x| per term; the loss adds 2 U.
   cbce backward: E + 6 roundings of |w g| (sigmoid + 1) per element.
 - sum_f32: the elements per thread + 5 shuffle levels + 1 (the fp32 result); deterministic: the elements per thread
-  + 256 threads + 256 blocks in order + 1.  channel_sum: the pixels per thread + the block's pixel rows + the grid's
-  atomics.  reduce_rows: side_dispatch_ref.reduce_rows_depth.
+  + 256 threads + 256 blocks in order + 1.  reduce_rows: side_dispatch_ref.reduce_rows_depth.
 At module end each family reports its largest share of the bound."""
 import math
 import os
@@ -462,7 +461,7 @@ def _cbce_id(regime, i, det, kind):
 
 
 @pytest.mark.parametrize("target", CBCE_TARGETS, ids=[_cbce_id(*t) for t in CBCE_TARGETS])
-def test_cbce(dev, sms, target):
+def test_cbce_fwd_bwd(dev, sms, target):
     """One numel of a regime (its remainder mod 4 does not depend on the SM count).  Labels: 0 / 0.5 / 1 at random,
     all positive or all negative.  With a single class (and so at numel = 1) the class weights make every gradient
     exactly 0, as in the reference loss."""
@@ -478,13 +477,14 @@ def test_cbce(dev, sms, target):
     sums = torch.zeros(tdr.cbce_det_sums(numel, sms) if det else 5, dtype=torch.float64, device=dev)
     loss = torch.empty(1, device=dev)
     divisor = 3.0
-    fwd = lib.osvos_cbce_fwd_deterministic if det else lib.osvos_cbce_fwd
-    ran(lambda: nat.check(fwd(d_x.data_ptr(), d_y.data_ptr(), numel, divisor, sums.data_ptr(), loss.data_ptr(),
-                              _stream()), "cbce fwd"), {("cbce_fwd_kernel", (det,)): 1})
+    flags = nat.FLAG_DETERMINISTIC if det else 0
+    ran(lambda: nat.check(lib.osvos_cbce_fwd(d_x.data_ptr(), d_y.data_ptr(), numel, divisor, sums.data_ptr(),
+                                             loss.data_ptr(), flags, _stream()), "cbce fwd"),
+        {("cbce_fwd_kernel", (det,)): 1})
     if det:
         s2, l2 = sums.clone(), loss.clone()
-        nat.check(fwd(d_x.data_ptr(), d_y.data_ptr(), numel, divisor, s2.data_ptr(), l2.data_ptr(), _stream()),
-                  "cbce fwd")
+        nat.check(lib.osvos_cbce_fwd(d_x.data_ptr(), d_y.data_ptr(), numel, divisor, s2.data_ptr(), l2.data_ptr(),
+                                     flags, _stream()), "cbce fwd")
         assert torch.equal(s2[:4], sums[:4]) and torch.equal(l2, loss), "deterministic cbce differs between runs"
     xd = x.double()
     pos = y >= 0.5
@@ -533,22 +533,6 @@ def test_sum_f32(dev, sms, det):
             depth = -(-numel // (tdr.sum_grid(numel, sms) * 256)) + 5 + 1
         check_bound(f"sum_f32 {'det' if det else 'atomic'}", got, x.double().sum().view(1),
                     (depth * U * x.double().abs().sum()).view(1), f"sum of {numel}")
-
-
-@pytest.mark.parametrize("c", [64, 128, 256, 512])
-def test_channel_sum(dev, sms, c):
-    from osvos_pytorch_b200 import ops
-    rows = 256 // (c // 8)
-    for (n, h, w), fast in (((2, 37, 53), False), ((2, 37, 53), True), ((2, 97, 131), False)):
-        npix = n * h * w
-        assert npix % rows != 0
-        a = ops.nchw_to_act(torch.randn(n, c, h, w, generator=_gen(c + h + fast)).to(dev), fast)
-        assert (a.lo is None) == fast
-        got = ran(lambda: ops.channel_sum(a), {("channel_sum_kernel", ()): 1})
-        v = a.hi.double() + (a.lo.double() if a.lo is not None else 0.0)
-        grid = tdr.channel_sum_grid(npix, c, sms)
-        depth = -(-npix // (grid * rows)) + rows + grid
-        check_bound("channel_sum", got, v.sum((0, 1, 2)), depth * U * v.abs().sum((0, 1, 2)), f"{(n, h, w, c)}")
 
 
 @pytest.mark.parametrize("nrows", [1, 63, 64, 65, 4100])

@@ -46,18 +46,20 @@ SW_SHAPES = [(n, h, w, c) for n in (1, 2, 12) for h, w in SIZES for c in (128, 2
 
 
 @pytest.mark.parametrize("count", [1, 2, 3, 4])
-def test_side_wgrad_workspace_matches(lib, count):
-    """osvos_side_folded_wgrad_deterministic_workspace_bytes is the restated partial rows plus the row reduction's
-    scratch, over 1 - 4 scales."""
+def test_side_wgrad_workspace_query_matches(lib, count):
+    """osvos_side_folded_wgrad_workspace_bytes of the deterministic form is the restated partial rows plus the row
+    reduction's scratch, over 1 - 4 scales; the default form needs none."""
+    from osvos_pytorch_b200._native import FLAG_DETERMINISTIC as DET
     for k in range(0, len(SW_SHAPES), 7):
         shapes = [SW_SHAPES[(k + 13 * j) % len(SW_SHAPES)] for j in range(count)]
         plan = ref.side_wgrad_plan(shapes, HOST_SMS)
-        got = lib.osvos_side_folded_wgrad_deterministic_workspace_bytes(_sw_items(shapes), count)
+        got = lib.osvos_side_folded_wgrad_workspace_bytes(_sw_items(shapes), count, DET)
         assert got == 4 * plan.workspace_floats, (shapes, got, plan)
+        assert lib.osvos_side_folded_wgrad_workspace_bytes(_sw_items(shapes), count, 0) == 0
         assert plan.total_blocks <= 2 * HOST_SMS + 4 * count * 4
         for sc in plan.scales:
             assert 1 <= sc.blocks_per_slab <= sc.chunks and sum(sc.chunks_per_block) == sc.chunks
-    assert lib.osvos_side_folded_wgrad_deterministic_workspace_bytes(_sw_items([(1, 8, 8, 64)]), 1) == 0
+    assert lib.osvos_side_folded_wgrad_workspace_bytes(_sw_items([(1, 8, 8, 64)]), 1, DET) == 0
 
 
 def test_tail_det_sums_match(lib):

@@ -25,13 +25,15 @@ SIZES = [(1, 1), (3, 5), (8, 8), (9, 17), (16, 24), (31, 45), (60, 107), (97, 13
          (7, 64), (5, 65), (3, 129), (2, 1000)]
 
 
-def test_first_bwd_workspaces_match(lib):
-    assert lib.osvos_conv_first_bwd_workspace_bytes() == ref.first_bwd_workspace_bytes() == (16 * 1728 + 4) * 4
+def test_first_bwd_workspace_query_matches(lib):
+    from osvos_pytorch_b200._native import FLAG_DETERMINISTIC as DET
+    assert lib.osvos_conv_first_bwd_workspace_bytes(1, 8, 8, 0) == ref.first_bwd_workspace_bytes() == (16 * 1728 + 4) * 4
     for n, (h, w) in itertools.product((1, 2, 3, 12), SIZES):
         p = ref.first_wgrad_plan(n, h, w, HOST_SMS)
-        assert lib.osvos_conv_first_bwd_deterministic_workspace_bytes(n, h, w) == 4 * p.det_workspace_floats, (n, h, w)
+        assert lib.osvos_conv_first_bwd_workspace_bytes(n, h, w, 0) == ref.first_bwd_workspace_bytes(), (n, h, w)
+        assert lib.osvos_conv_first_bwd_workspace_bytes(n, h, w, DET) == 4 * p.det_workspace_floats, (n, h, w)
         assert sum(len(t) for t in p.block_tiles) == p.tiles and 1 <= p.last_valid <= ref.FW_PIX
-    assert lib.osvos_conv_first_bwd_deterministic_workspace_bytes(0, 8, 8) == 0
+    assert lib.osvos_conv_first_bwd_workspace_bytes(0, 8, 8, DET) == 0
 
 
 def test_reduce_rows_scratch_matches(lib):
@@ -49,10 +51,12 @@ def test_general_tail_plans_match(lib):
     assert lib.osvos_tail_general_fwd_sums(1, 0, 4) == 0 and lib.osvos_tail_general_bwd_workspace_bytes(1, 4, 0) == 0
 
 
-def test_cbce_det_sums_match(lib):
+def test_cbce_sums_query_matches(lib):
+    from osvos_pytorch_b200._native import FLAG_DETERMINISTIC as DET
     for numel in (1, 2, 3, 4, 5, 1023, 1024, 1025, 4096, 4097, 270336, 1081344, 1081345, 5 * 10 ** 6, 854 * 480 * 12):
-        assert lib.osvos_cbce_fwd_deterministic_sums(numel) == ref.cbce_det_sums(numel, HOST_SMS), numel
-    assert lib.osvos_cbce_fwd_deterministic_sums(0) == 0
+        assert lib.osvos_cbce_fwd_sums(numel, DET) == ref.cbce_det_sums(numel, HOST_SMS), numel
+        assert lib.osvos_cbce_fwd_sums(numel, 0) == 5, numel
+    assert lib.osvos_cbce_fwd_sums(0, DET) == 0
 
 
 def test_tail_bwd_items_cover_the_plan():
@@ -149,12 +153,12 @@ def test_parse_train_kernel_names():
         assert parse(f"void osvos::{name}(int)") == (name, ())
     assert parse("void osvos::sum_f32_det_kernel(float const*)") == ("sum_f32_det_kernel", ())
     assert parse("void osvos::tail_fwd_kernel<true>(osvos::TailParams)") is None
-    assert parse("void osvos::my_channel_sum_kernel(int)") is None
+    assert parse("void osvos::my_sum_f32_kernel(int)") is None
     assert parse("void osvos::side_conv_kernel<2, 16>(x)") is None
     assert parse_kernel_name("void osvos::conv_first_tc_kernel<2, true>(x)") is None    # the default set is unchanged
 
 
-def test_compiled_instantiations(lib):
+def test_compiled_train_instantiations(lib):
     """conv_first_tc_kernel {1, 2} x {false, true}, conv_first_wgrad_kernel {false, true}, tail_bwd2_kernel
     {false, true}^2, tail_general_bwd_kernel {false, true} and cbce_fwd_kernel {false, true} - no more, no fewer; and
     each plain kernel named here exists."""

@@ -11,8 +11,7 @@ that reach each of their regimes at a given SM count.
   the segment's low-res columns, its source width, the padded width and the row groups of phase 1.
 - `gen_fwd_blocks` / `gen_fwd_sums` and `gen_bwd_plan` restate the general-weights tail's plans (csrc/tail_general.cu);
   `find_gen_fwd_shape` finds shapes for the forward's two regimes (one row per block, rows strided over blocks).
-- `loss_grid` and `cbce_det_sums` restate csrc/loss.cu; `sum_grid` and `channel_sum_grid` the `grid_cap(., 4)` grids
-  of osvos_sum_f32 and osvos_channel_sum.
+- `loss_grid` and `cbce_det_sums` restate csrc/loss.cu; `sum_grid` the `grid_cap(., 4)` grid of osvos_sum_f32.
 
 tests/test_train_dispatch.py checks the restatements against the library's own queries and the compiled kernel set, and
 tests/test_gpu_train_schedules.py runs the regimes found here against fp64 and checks which kernels actually ran."""
@@ -41,7 +40,7 @@ TRAIN_KERNELS = {"conv_first_tc_kernel": 1, "conv_first_wgrad_kernel": 0, "tail_
 # kernels that are not templates: matched by exact name
 PLAIN_KERNELS = ("conv_first_dgrad_kernel", "tail_general_fwd_kernel", "upsampling_fold_kernel",
                  "upsampling_grads_finish_kernel", "cbce_bwd_kernel", "reduce_rows_segments_kernel",
-                 "reduce_rows_final_kernel", "sum_f32_kernel", "sum_f32_det_kernel", "channel_sum_kernel")
+                 "reduce_rows_final_kernel", "sum_f32_kernel", "sum_f32_det_kernel")
 _PLAIN_RE = re.compile(r"\b(" + "|".join(PLAIN_KERNELS) + r")\(")
 
 # every instantiation the library compiles (and the entry points below can reach)
@@ -328,7 +327,7 @@ def loss_grid(numel, sms):
 
 
 def cbce_det_sums(numel, sms):
-    """Doubles of osvos_cbce_fwd_deterministic_sums: five leading values, then three per block."""
+    """Doubles of osvos_cbce_fwd_sums with OSVOS_FLAG_DETERMINISTIC: five leading values, then three per block."""
     return 5 + 3 * loss_grid(numel, sms) if numel > 0 else 0
 
 
@@ -342,10 +341,6 @@ def grid_cap4(blocks, sms):
 
 def sum_grid(numel, sms):
     return grid_cap4(_cdiv(numel, 256), sms)
-
-
-def channel_sum_grid(npix, c, sms):
-    return grid_cap4(_cdiv(npix, 256 // (c // 8)), sms)
 
 
 CBCE_REGIMES = ("tiny", "one_block", "capped")
