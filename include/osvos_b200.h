@@ -672,6 +672,21 @@ OSVOS_API int osvos_png_decode(const osvos_png_decode_args* args, osvos_stream_t
  *   osvos_jpeg_encode_workspace_bytes: host query; 0 for invalid arguments.                                          */
 OSVOS_API int osvos_overlay_mask(const uint8_t* frames, const float* logits, uint8_t* out, int n, int h, int w, int c0,
                                  int c1, int c2, osvos_stream_t stream);
+/*   osvos_overlay_labels: the overlay of a label map of K objects (replaces the reference's dataloaders/helpers.py
+ *                     overlay_mask, extended to K objects; DESIGN.md §25): frames [n][h][w][3] uint8 BGR and labels
+ *                     [n][h][w] uint8 object ids (both any alignment) -> out [n][h][w][3] uint8 (may be frames itself;
+ *                     must not overlap labels).  Per pixel of id k: k == 0 keeps v; k != 0 is (0, 0, 0) on its edge (a
+ *                     4-neighbour with another id or outside the frame: per object, the pixels
+ *                     cv2.drawContours(findContours(labels == k, RETR_TREE, CHAIN_APPROX_SIMPLE), -1, 0, 1) paints),
+ *                     else (v + c_k + 1) >> 1 per channel, c_k = colors->bgr[k] for k < n_colors and (0, 0, 0) past
+ *                     it.  `colors` is host memory, passed to the kernel by value; 0 <= n_colors <= 256.  With one id
+ *                     and bgr[1] = (0, 0, 255) the bytes are osvos_overlay_mask's.                                  */
+#define OSVOS_OVERLAY_MAX_COLORS 256
+typedef struct osvos_overlay_colors {
+  uint8_t bgr[OSVOS_OVERLAY_MAX_COLORS][3];
+} osvos_overlay_colors;
+OSVOS_API int osvos_overlay_labels(const uint8_t* frames, const uint8_t* labels, uint8_t* out, int n, int h, int w,
+                                   const osvos_overlay_colors* colors /* host */, int n_colors, osvos_stream_t stream);
 OSVOS_API size_t osvos_jpeg_max_bytes(int h, int w);
 OSVOS_API size_t osvos_jpeg_encode_workspace_bytes(int n, int h, int w);
 OSVOS_API int osvos_jpeg_encode(const uint8_t* src, uint8_t* out, int64_t* lengths, void* workspace, int n, int h, int w,

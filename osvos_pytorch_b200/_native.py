@@ -6,8 +6,8 @@ library cannot be loaded, or a call fails, an exception is raised.
 """
 import ctypes
 import os
-from ctypes import (POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32, c_size_t, c_uint32, c_uint64,
-                    c_void_p)
+from ctypes import (POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32, c_size_t, c_uint8, c_uint32,
+                    c_uint64, c_void_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libosvos_b200.so")
@@ -140,6 +140,14 @@ class UpsamplingGradsArgs(Structure):
                 ("d_score_b", c_void_p * 4), ("d_side_b", c_void_p * 4), ("accumulate", c_int)]
 
 
+OVERLAY_MAX_COLORS = 256
+
+
+class OverlayColors(Structure):
+    """osvos_overlay_colors (include/osvos_b200.h): BGR triples, entry k the colour of object id k."""
+    _fields_ = [("bgr", c_uint8 * (3 * OVERLAY_MAX_COLORS))]
+
+
 UPSAMPLING_TAPS = 1360
 U8_PROB, U8_BYTESCALE, U8_MASK = 0, 1, 2
 RESIZE_BILINEAR, RESIZE_NEAREST = 0, 1
@@ -232,6 +240,9 @@ SIGNATURES = {
                                              c_void_p]),
     # helpers.py:15-40 overlay_mask and the vis_res display of train_online.py:160-205, written as JPEG files
     "osvos_overlay_mask": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    # the same picture for a label map of K objects, each in its palette colour (DESIGN.md §25)
+    "osvos_overlay_labels": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(OverlayColors), c_int,
+                                     c_void_p]),
     "osvos_jpeg_max_bytes": (c_size_t, [c_int, c_int]),
     "osvos_jpeg_encode_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "osvos_jpeg_encode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),

@@ -15,7 +15,8 @@
 //   jpeg_ff_count_kernel one CTA per 4 KB chunk of scan bytes: its 0xFF bytes;
 //   jpeg_place_kernel    one CTA per frame: each chunk's output offset, the header, EOI and the file's length;
 //   jpeg_stuff_kernel    one CTA per chunk: the bytes copied to their place with 00 after every FF.
-// overlay_mask_kernel (end of file) draws the picture these files usually hold: the mask over the frame.
+// overlay_mask_kernel (end of file) draws the picture these files usually hold: the mask over the frame;
+// overlay_labels_kernel draws a label map of K objects the same way, each in its own colour (DESIGN.md §25).
 #include "common.cuh"
 
 namespace osvos {
@@ -652,6 +653,47 @@ __global__ void __launch_bounds__(256) overlay_mask_kernel(const uint8_t* __rest
   d[2] = v2;
 }
 
+__device__ __forceinline__ bool same_at(const uint8_t* l, int y, int x, int h, int w, uint8_t k) {
+  return y >= 0 && x >= 0 && y < h && x < w && l[static_cast<size_t>(y) * w + x] == k;
+}
+
+// One CTA per row of one frame, its threads striding along the row, one pixel each per step: 3 frame bytes in, 3 out,
+// the label and its four neighbours (the neighbours come from L1 / L2; DRAM sees each label byte about once).  A CTA
+// per row costs one 32-bit division per CTA where a flat pixel index costs 64-bit divisions per pixel, which bound
+// the flat layout's throughput.  Object k != 0: black where a 4-neighbour holds another id or lies outside the frame,
+// else (v + c_k + 1) >> 1 with c_k = colors.bgr[k] (black for k >= n_colors).  The table is a __grid_constant__ kernel
+// parameter, so the per-pixel lookup reads the constant bank.  Each thread reads only its own pixel's frame bytes, so
+// out may be frames itself.
+constexpr int kOverlayRowThreads = 128;
+
+__global__ void __launch_bounds__(kOverlayRowThreads) overlay_labels_kernel(
+    const uint8_t* frames, const uint8_t* __restrict__ labels, uint8_t* out, int h, int w,
+    const __grid_constant__ osvos_overlay_colors colors, int n_colors) {
+  const int row = blockIdx.x;                          // f * h + y
+  const int f = row / h, y = row - f * h;
+  const uint8_t* l = labels + static_cast<size_t>(f) * h * w;
+  const size_t base = static_cast<size_t>(row) * w;
+  for (int x = threadIdx.x; x < w; x += kOverlayRowThreads) {
+    const uint8_t k = __ldg(labels + base + x);
+    const uint8_t* s = frames + (base + x) * 3;
+    uint8_t* d = out + (base + x) * 3;
+    uint8_t v0 = s[0], v1 = s[1], v2 = s[2];
+    if (k != 0) {
+      const bool edge = !same_at(l, y - 1, x, h, w, k) || !same_at(l, y + 1, x, h, w, k) ||
+                        !same_at(l, y, x - 1, h, w, k) || !same_at(l, y, x + 1, h, w, k);
+      const bool known = k < n_colors;
+      const int c0 = known ? colors.bgr[k][0] : 0, c1 = known ? colors.bgr[k][1] : 0;
+      const int c2 = known ? colors.bgr[k][2] : 0;
+      v0 = edge ? 0 : static_cast<uint8_t>((v0 + c0 + 1) >> 1);
+      v1 = edge ? 0 : static_cast<uint8_t>((v1 + c1 + 1) >> 1);
+      v2 = edge ? 0 : static_cast<uint8_t>((v2 + c2 + 1) >> 1);
+    }
+    d[0] = v0;
+    d[1] = v1;
+    d[2] = v2;
+  }
+}
+
 }  // namespace osvos
 
 extern "C" int osvos_overlay_mask(const uint8_t* frames, const float* logits, uint8_t* out, int n, int h, int w, int c0,
@@ -663,6 +705,18 @@ extern "C" int osvos_overlay_mask(const uint8_t* frames, const float* logits, ui
   const long long total = static_cast<long long>(n) * h * w;
   overlay_mask_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream_)>>>(
       frames, logits, out, n, h, w, c0, c1, c2);
+  OSVOS_CHECK_CUDA(cudaGetLastError());
+  return OSVOS_OK;
+}
+
+extern "C" int osvos_overlay_labels(const uint8_t* frames, const uint8_t* labels, uint8_t* out, int n, int h, int w,
+                                    const osvos_overlay_colors* colors, int n_colors, osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(frames != nullptr && labels != nullptr && out != nullptr && colors != nullptr);
+  OSVOS_CHECK_ARG(n > 0 && h > 0 && w > 0 && static_cast<long long>(n) * h < (1ll << 31));
+  OSVOS_CHECK_ARG(static_cast<long long>(n) * h * w < (1ll << 40));
+  OSVOS_CHECK_ARG(n_colors >= 0 && n_colors <= OSVOS_OVERLAY_MAX_COLORS);
+  overlay_labels_kernel<<<static_cast<unsigned>(n * h), kOverlayRowThreads, 0, static_cast<cudaStream_t>(stream_)>>>(
+      frames, labels, out, h, w, *colors, n_colors);
   OSVOS_CHECK_CUDA(cudaGetLastError());
   return OSVOS_OK;
 }

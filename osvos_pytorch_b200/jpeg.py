@@ -365,3 +365,50 @@ def pack(parsed_list):
 def segment_count(blob):
     """The number of entropy-coded segments in a packed blob (its header's nseg)."""
     return int(HEADER.unpack_from(bytes(blob[:HEADER.size]))[2])
+
+
+def decode_host(data):
+    """One file's bytes -> uint8 [h, w, 3] BGR as cv2.imread(path) gives."""
+    import cv2
+    img = cv2.imdecode(np.frombuffer(bytes(data), np.uint8), cv2.IMREAD_COLOR)
+    if img is None:
+        raise ValueError("cv2 cannot decode this JPEG")
+    return img
+
+
+def decode_files(datas, device, parsed=None):
+    """A list of JPEG files' bytes, all of one size -> (uint8 [n,h,w,3] BGR on ``device``, fallback count, re-decoded
+    count), bit-identical to cv2.imread.
+
+    Files inside the subset are decoded on the device (ops.decode_jpeg); Fallback files, and after one read of the
+    status words the files the decoder flagged, are decoded by cv2 on the host.  ``parsed``: the files' ``parse``
+    results when the caller has them already (reader threads).  png.decode_files is the same for PNGs."""
+    import torch
+
+    from . import ops
+    if parsed is None:
+        parsed = [parse(d) for d in datas]
+    n = len(datas)
+    sub = [i for i, p in enumerate(parsed) if isinstance(p, Parsed)]
+    host = {i: decode_host(datas[i]) for i in range(n) if not isinstance(parsed[i], Parsed)}
+    fallback = len(host)
+    sizes = {(parsed[i].h, parsed[i].w) for i in sub} | {m.shape[:2] for m in host.values()}
+    if len(sizes) != 1:
+        raise ValueError("the files differ in size: " + ", ".join(f"{a}x{b}" for a, b in sorted(sizes)))
+    (h, w), = sizes
+    out = torch.empty((n, h, w, 3), dtype=torch.uint8, device=device)
+    if sub:
+        blob = pack([parsed[i] for i in sub])
+        dev_blob = torch.from_numpy(blob).to(device)
+        got, status = ops.decode_jpeg(dev_blob, len(sub), h, w, out=out if len(sub) == n else None,
+                                      nseg=segment_count(blob))
+        if len(sub) != n:
+            out[torch.tensor(sub, device=device)] = got
+        for j in torch.nonzero(status.cpu()).flatten().tolist():
+            host[sub[j]] = decode_host(datas[sub[j]])
+            if host[sub[j]].shape[:2] != (h, w):
+                raise ValueError("the files differ in size")
+    if host:
+        idx = sorted(host)
+        out[torch.tensor(idx, device=device)] = torch.from_numpy(np.stack([host[i] for i in idx])).to(device)
+    return out, fallback, len(host) - fallback

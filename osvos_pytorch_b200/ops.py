@@ -1000,6 +1000,40 @@ def overlay_mask(frames, logits, color=(0, 0, 255), out=None):
     return out
 
 
+def overlay_labels(frames, labels, palette=None, out=None):
+    """A label map drawn over the frame, each object in its palette colour (DESIGN.md §25): frames uint8 [N,H,W,3] BGR
+    and labels uint8 [N,H,W] or [N,1,H,W] of object ids -> uint8 [N,H,W,3].  Id 0 keeps the frame's bytes; a pixel of
+    id k != 0 with a 4-neighbour of another id or outside the frame (object k's contour as cv2.drawContours draws it)
+    is black, the rest of object k is (v + c_k + 1) >> 1 per channel.  ``palette``: the colours as RGB triples, the
+    PLTE chunk's bytes as png.palette_of returns them (1 .. 256 entries); ids past its end are drawn with (0, 0, 0).
+    None is the DAVIS palette (png.davis_palette).  With labels = logit > 0 and entry 1 = (255, 0, 0) RGB this is
+    overlay_mask.  ``out`` may be ``frames`` itself.  No host synchronisation."""
+    from .png import davis_palette
+    lib = nat.load()
+    x = _require_u8(frames, "frames", 4)
+    n, h, w, c = (int(v) for v in x.shape)
+    if c != 3:
+        raise ValueError("frames must be [N,H,W,3]")
+    _require_cuda(labels, "labels")
+    if (labels.dtype != torch.uint8 or labels.dim() not in (3, 4) or labels.numel() != n * h * w
+            or tuple(labels.shape[-2:]) != (h, w) or (labels.dim() == 4 and int(labels.shape[1]) != 1)):
+        raise ValueError(f"labels must be uint8 [N,H,W] or [N,1,H,W] matching frames {tuple(x.shape)}, got "
+                         f"{labels.dtype} {tuple(labels.shape)}")
+    pal = _palette_bytes(davis_palette() if palette is None else palette)
+    colors = nat.OverlayColors()
+    for k in range(len(pal) // 3):                           # RGB -> the frame's BGR order
+        colors.bgr[3 * k:3 * k + 3] = [pal[3 * k + 2], pal[3 * k + 1], pal[3 * k]]
+    lab = labels.contiguous()
+    if out is None:
+        out = torch.empty_like(x)
+    elif out.dtype != torch.uint8 or tuple(out.shape) != (n, h, w, 3) or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous uint8 tensor of shape {(n, h, w, 3)}")
+    _count()
+    nat.check(lib.osvos_overlay_labels(x.data_ptr(), lab.data_ptr(), out.data_ptr(), n, h, w, byref(colors),
+                                       len(pal) // 3, _stream()), "osvos_overlay_labels")
+    return out
+
+
 def jpeg_max_bytes(h, w):
     """Capacity of one encoded frame (osvos_jpeg_max_bytes): header and EOI plus twice the largest possible scan."""
     return int(nat.load().osvos_jpeg_max_bytes(int(h), int(w)))

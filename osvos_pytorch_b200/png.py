@@ -213,6 +213,22 @@ def palette_of(data):
     return None
 
 
+def davis_palette(n=256):
+    """The DAVIS palette's first ``n`` entries as PLTE bytes (RGB triples): the PASCAL VOC colour map, entry k's colour
+    built by spreading the bits of k over the three channels from the high bit down (1 -> (128, 0, 0), 2 -> (0, 128,
+    0), 3 -> (128, 128, 0), ...)."""
+    out = bytearray()
+    for k in range(int(n)):
+        rgb = [0, 0, 0]
+        c = k
+        for j in range(8):
+            for ch in range(3):
+                rgb[ch] |= ((c >> ch) & 1) << (7 - j)
+            c >>= 3
+        out += bytes(rgb)
+    return bytes(out)
+
+
 def decode_files(datas, device, parsed=None, palette=None):
     """A list of PNG files' bytes, all of one size -> (uint8 [n,h,w] on ``device``, fallback count, re-decoded count).
 

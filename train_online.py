@@ -78,7 +78,9 @@ def parse(argv=None):
     ap.add_argument("--overlay", action="store_true",
                     help="also write each frame with its mask drawn over it (the reference's vis_res picture: the "
                          "foreground blended 50/50 with red, its outline black) as Results/<seq>_overlay/<frame>.jpg, "
-                         "drawn and JPEG-encoded on the GPU (the bytes cv2.imwrite would write). Needs --loader native")
+                         "drawn and JPEG-encoded on the GPU (the bytes cv2.imwrite would write). Needs --loader native. "
+                         "With --davis 2017 each object is drawn in its palette colour with its own outline, from the "
+                         "written label files (visualize.render_results)")
     ap.add_argument("--overlay-quality", type=int, default=95, help="JPEG quality of --overlay (1..100)")
     ap.add_argument("--davis", default="2016", choices=["2016", "2017"],
                     help="2017: a DAVIS-2017 sequence (palette annotations of K objects). The parent is fine-tuned once "
@@ -105,8 +107,8 @@ def parse(argv=None):
         if a.synthetic or a.loader != "native":
             ap.error("--davis 2017 reads the sequence with --loader native; it cannot be combined with "
                      + ("--synthetic" if a.synthetic else "--loader reference"))
-        if a.input_res is not None or a.overlay:
-            ap.error("--davis 2017 writes label maps at the stored size: --input-res and --overlay do not apply")
+        if a.input_res is not None:
+            ap.error("--davis 2017 writes label maps at the stored size: --input-res does not apply")
     return a
 
 
@@ -373,6 +375,11 @@ def online_2017(a, parent, device, save_dir, iters, log_every):
                 im.save(path)
     if seg.jpeg_status is not None and int(seg.jpeg_status) != 0:
         print(f"WARNING: the device JPEG decoder flagged corrupt or cut-short frames (status sum {int(seg.jpeg_status)})")
+    if a.overlay:                                       # drawn from the label files just written, on the device
+        from osvos_pytorch_b200 import visualize
+        visualize.render_results(os.path.join(save_dir, "Results"), Path.db_root_dir(), sequences=[a.seq_name],
+                                 davis="2017", quality=a.overlay_quality, device=device, decode=a.decode,
+                                 palette=palette)
     if a.evaluate:
         scores = ObjectScores(k_objects)
         scores.add(seg.frame_counts())
