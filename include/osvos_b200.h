@@ -52,9 +52,12 @@ enum {
   OSVOS_FLAG_ACCUMULATE = 8, /* add into the existing output instead of overwriting it    */
   OSVOS_FLAG_DEFER_FINISH = 16, /* osvos_conv3x3_wgrad: accumulate into a caller-zeroed workspace only; the
                                   workspace -> OIHW step is done later by osvos_wgrad_finish for many layers */
-  OSVOS_FLAG_DETERMINISTIC = 32 /* reduce floats in an order that does not depend on scheduling: partial results go to
+  OSVOS_FLAG_DETERMINISTIC = 32, /* reduce floats in an order that does not depend on scheduling: partial results go to
                                    per-block / per-tile slots written with plain stores, which are added in a fixed order
                                    (see "Deterministic forms" below).  Without it the kernels add with atomics. */
+  OSVOS_FLAG_VOID_LABELS = 64   /* class-balanced BCE (osvos_cbce_fwd, osvos_tail_fwd, osvos_tail_loss_bwd): a label
+                                   y < 0 marks a void pixel, counted in neither class and given zero gradient; N is
+                                   then the number of pixels with y >= 0, and N == 0 gives loss 0 and gradient 0 */
 };
 
 typedef void* osvos_stream_t; /* cudaStream_t */
@@ -205,11 +208,16 @@ typedef struct {
   float loss_weights[5];   /* weights of the five losses in losses[5]                 */
   float divisor;           /* batch size (batch_average), numel (size_average) or 1   */
   int n, h, w;
-  int flags;               /* 0 or OSVOS_FLAG_DETERMINISTIC: then `sums` holds osvos_tail_fwd_deterministic_sums(n, h, w)
-                              doubles - the 15 above, then one row of block partials per block, added in a fixed order.
+  int flags;               /* OSVOS_FLAG_DETERMINISTIC: then `sums` holds osvos_tail_fwd_sums(n, h, w, flags) doubles -
+                              the 15 above, then one row of block partials per block, added in a fixed order.
+                              OSVOS_FLAG_VOID_LABELS (needs label): pixels with label < 0 enter no sum, sums[11] = N is
+                              the count of the others, and N == 0 gives losses of 0.
                               Added after the other members: zero-initialise the struct (other bits are refused). */
 } osvos_tail_fwd_args;
 OSVOS_API int osvos_tail_fwd(const osvos_tail_fwd_args* args /* host */, osvos_stream_t stream);
+/* doubles of osvos_tail_fwd's `sums` for these flags (OSVOS_TAIL_SUMS without OSVOS_FLAG_DETERMINISTIC), 0 for shapes
+ * or flags the call refuses; equal to osvos_tail_fwd_deterministic_sums(n, h, w) for OSVOS_FLAG_DETERMINISTIC alone. */
+OSVOS_API size_t osvos_tail_fwd_sums(int n, int h, int w, int flags);
 
 /* Standalone 1x1 projections of a side feature map (used when the features do
  * not come from osvos_conv3x3's fused epilogue): pq as above.                       */
@@ -220,12 +228,17 @@ OSVOS_API int osvos_side_project(const float* feat /* [n,h,w,16] */, const float
  * forward: sums[0..3] = {S_pos, S_neg, P, N} (osvos_cbce_fwd_sums(numel, flags) doubles; the call zeroes the first 5,
  * sums[4] is an arrival counter), loss[0] = (Nn/N*S_pos + P/N*S_neg)/divisor with divisor = numel (size_average), batch
  * (batch_average) or 1.  backward: grad_in = grad_out[0] * w * (sigmoid(x) - y) / divisor
- * (grad_out == NULL means 1).                                                        */
+ * (grad_out == NULL means 1).
+ * Void labels: osvos_cbce_fwd with OSVOS_FLAG_VOID_LABELS sums only pixels with y >= 0 and stores their count N in
+ * sums[3] (rows of four block sums under OSVOS_FLAG_DETERMINISTIC); osvos_cbce_bwd_void reads those sums and gives
+ * pixels with y < 0 zero gradient.  N == 0 gives loss 0 and gradient 0.              */
 OSVOS_API size_t osvos_cbce_fwd_sums(size_t numel, int flags);
 OSVOS_API int osvos_cbce_fwd(const float* output, const float* label, size_t numel, double divisor, double* sums,
                              float* loss, int flags, osvos_stream_t stream);
 OSVOS_API int osvos_cbce_bwd(const float* output, const float* label, const double* sums, const float* grad_out,
                              double divisor, size_t numel, float* grad_in, osvos_stream_t stream);
+OSVOS_API int osvos_cbce_bwd_void(const float* output, const float* label, const double* sums, const float* grad_out,
+                                  double divisor, size_t numel, float* grad_in, osvos_stream_t stream);
 
 /* ======================= backward (training) entry points ======================= */
 
@@ -294,7 +307,8 @@ typedef struct {
   float* dpq[4];            /* [n,h_k,w_k,2] */
   float* fuse_bias_grad;    /* [1] or NULL */
   int n, h, w;
-  int flags;                /* 0 or OSVOS_FLAG_DETERMINISTIC; zero-initialise the struct (other bits are refused) */
+  int flags;                /* OSVOS_FLAG_DETERMINISTIC | OSVOS_FLAG_VOID_LABELS (as passed to the forward call, whose
+                               sums[11] is then the non-void count); zero-initialise the struct (other bits are refused) */
 } osvos_tail_loss_bwd_args;
 OSVOS_API int osvos_tail_loss_bwd(const osvos_tail_loss_bwd_args* args /* host */, osvos_stream_t stream);
 
@@ -384,7 +398,7 @@ OSVOS_API int osvos_conv_first_bwd(const float* x_nchw, const void* dz_hi, const
  *                               block (osvos_cbce_bwd reads sums[0..4] either way).
  *   osvos_sum_f32:              a fixed grid of 256 contiguous ranges, their totals added in order by the last block.
  *   osvos_tail_fwd / osvos_tail_bwd / osvos_tail_loss_bwd: the `flags` member of their argument blocks (appended:
- *                               callers zero-initialise the blocks); tail_fwd's sums: osvos_tail_fwd_deterministic_sums.
+ *                               callers zero-initialise the blocks); tail_fwd's sums: osvos_tail_fwd_sums.
  * osvos_reduce_rows adds such partial rows: out[c] = (accumulate ? out[c] : 0) + sum_r rows[r][c], rows [nrows][ncols]
  * fp32, in a fixed order (up to 64 row segments, each summed by 8 interleaved row lanes); scratch:
  * osvos_reduce_rows_scratch_floats(nrows, ncols) floats.                                                            */
@@ -495,6 +509,21 @@ OSVOS_API int osvos_affine_warp_u8_indexed(const uint8_t* image_store, const uin
                                            const int* index_host, const double* inv_matrices_host,
                                            const int* flips_host, int n, int n_store, int h, int w, float mean_b,
                                            float mean_g, float mean_r, osvos_stream_t stream);
+
+/* ---- labels from object-id maps (DAVIS-2017 annotations: 0 background, 1..K objects, 255 void) ------------------
+ * The label of id v is -1 for v == 255 (void, for OSVOS_FLAG_VOID_LABELS), 1 for an object (1 <= v <= 254 when
+ * object == 0, v == object otherwise) and 0 else.
+ *   osvos_labels_from_ids: ids [n][h][w] uint8 -> dst [n][1][h][w] fp32.
+ *   osvos_affine_warp_ids: the mask half of osvos_affine_warp_u8 (index_host == NULL) or of osvos_affine_warp_u8_indexed
+ *                          for id maps: output sample i reads store frame index_host[i] (or i) of ids [n_store][h][w],
+ *                          always sampled nearest, out-of-frame samples 0.  Equal, bit for bit, to the label of the
+ *                          0/255 object mask warped by those calls, set to -1 where the warped 0/255 void mask is 1.
+ * object: 0 (every object) or 1..254.  Same size rules as the calls above.                                         */
+OSVOS_API int osvos_labels_from_ids(const uint8_t* ids, float* dst, int n, int h, int w, int object,
+                                    osvos_stream_t stream);
+OSVOS_API int osvos_affine_warp_ids(const uint8_t* ids_store, float* label_dst, const int* index_host,
+                                    const double* inv_matrices_host, const int* flips_host, int n, int n_store, int h,
+                                    int w, int object, osvos_stream_t stream);
 
 /* ---- resize of decoded frames (dataloaders/davis_2016.py:96-99 inputRes: scipy.misc.imresize, i.e. Pillow's 8-bit
  * Image.resize; DESIGN.md §17) ----------------------------------------------------------------------------------------

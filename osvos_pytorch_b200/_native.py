@@ -18,6 +18,7 @@ FLAG_RELU_MASK = 4
 FLAG_ACCUMULATE = 8
 FLAG_DEFER_FINISH = 16
 FLAG_DETERMINISTIC = 32
+FLAG_VOID_LABELS = 64
 WGRAD_FINISH_MAX = 24
 
 
@@ -174,6 +175,7 @@ SIGNATURES = {
     "osvos_cbce_fwd_sums": (c_size_t, [c_size_t, c_int]),
     "osvos_cbce_fwd": (c_int, [c_void_p, c_void_p, c_size_t, c_double, c_void_p, c_void_p, c_int, c_void_p]),
     "osvos_cbce_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_double, c_size_t, c_void_p, c_void_p]),
+    "osvos_cbce_bwd_void": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_double, c_size_t, c_void_p, c_void_p]),
     "osvos_wgrad_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "osvos_conv3x3_wgrad": (c_int, [POINTER(WgradArgs), c_void_p]),
     "osvos_wgrad_finish": (c_int, [POINTER(WgradFinishItem), POINTER(c_int), c_int, c_int, c_void_p]),
@@ -204,6 +206,9 @@ SIGNATURES = {
     "osvos_affine_warp_u8_indexed": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int),
                                              POINTER(c_double), POINTER(c_int), c_int, c_int, c_int, c_int, c_float,
                                              c_float, c_float, c_void_p]),
+    "osvos_labels_from_ids": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "osvos_affine_warp_ids": (c_int, [c_void_p, c_void_p, POINTER(c_int), POINTER(c_double), POINTER(c_int), c_int,
+                                      c_int, c_int, c_int, c_int, c_void_p]),
     "osvos_resize_u8_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
     "osvos_resize_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "osvos_resize_f32_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
@@ -216,6 +221,7 @@ SIGNATURES = {
     "osvos_wgrad_deterministic_splits": (c_int, [c_int, c_int, c_int, c_int, c_int]),
     "osvos_unpool_colsum_rows": (c_size_t, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "osvos_tail_fwd_deterministic_sums": (c_size_t, [c_int, c_int, c_int]),
+    "osvos_tail_fwd_sums": (c_size_t, [c_int, c_int, c_int, c_int]),
     "osvos_jpeg_decode_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_size_t, c_int]),
     "osvos_jpeg_decode": (c_int, [POINTER(JpegArgs), c_void_p]),
     "osvos_upsampling_fold": (c_int, [POINTER(UpsamplingFoldArgs), c_void_p]),

@@ -85,7 +85,7 @@ def augment_batch(sample, rots=(-30, 30), scales=(.75, 1.25), rng=random, params
     return {"image": affine_warp(sample["image"], params, "cubic"), "gt": affine_warp(sample["gt"], params, "nearest")}
 
 
-def affine_warp_u8(image_u8, gt_u8, params, stats=None, meanval=ops.MEANVAL, index=None):
+def affine_warp_u8(image_u8, gt_u8, params, stats=None, meanval=ops.MEANVAL, index=None, ids=False):
     """RandomHorizontalFlip + ScaleNRotate straight from decoded bytes: image_u8 uint8 [n,h,w,3] BGR and gt_u8 uint8
     [n,h,w] on the GPU -> {'image': f32 [n,3,h,w], 'gt': f32 [n,1,h,w]}, bit-identical to ingesting them
     (ops.image_from_bgr8 / ops.label_from_u8) and then warping with affine_warp.  The image is warped bicubic; each mask
@@ -95,8 +95,13 @@ def affine_warp_u8(image_u8, gt_u8, params, stats=None, meanval=ops.MEANVAL, ind
     ``index``: a sequence of frame indices.  Then image_u8, gt_u8 and stats are stores of any number of frames, and the
     output has len(index) samples, sample i warped from frame index[i] (repeats allowed): the same result as gathering
     those frames into a contiguous batch first, without the copy.  ``stats`` is required in this mode (computing it over
-    a whole store per batch would cost more than the warp); an index outside the store raises IndexError."""
+    a whole store per batch would cost more than the warp); an index outside the store raises IndexError.
+
+    ``ids``: False or None (gt_u8 holds masks) or "all" / k (1..254): gt_u8 holds DAVIS-2017 object-id maps, and the gt is their
+    label (ops.labels_from_ids with object None / k: 1 object, 0 background, -1 void), always sampled nearest
+    (osvos_affine_warp_ids); ``stats`` is then unused."""
     lib = nat.load()
+    obj = None if ids is None or ids is False else ops._id_object(ids)
     img = ops._require_u8(image_u8, "image_u8", 4)
     gt = ops._require_u8(gt_u8, "gt_u8", 3)
     n, h, w, c = (int(v) for v in img.shape)
@@ -104,12 +109,14 @@ def affine_warp_u8(image_u8, gt_u8, params, stats=None, meanval=ops.MEANVAL, ind
         raise ValueError("image_u8 must be [n,h,w,3] and gt_u8 [n,h,w]")
     m = n if index is None else len(index)
     mats, flips = _warp_tables(params, m, h, w)
+    if obj is not None:
+        stats = None
     if index is None:
-        stats = ops.label_stats_u8(gt) if stats is None else stats
+        stats = ops.label_stats_u8(gt) if stats is None and obj is None else stats
     else:
-        if stats is None:
+        if stats is None and obj is None:
             raise ValueError("affine_warp_u8(index=...) needs the store's label stats (ops.label_stats_u8)")
-        if tuple(stats.shape) != (n, 2):
+        if stats is not None and tuple(stats.shape) != (n, 2):
             raise ValueError(f"stats must be [{n},2] for a store of {n} frames, got {tuple(stats.shape)}")
         idx = [int(i) for i in index]
         bad = [i for i in idx if not 0 <= i < n]
@@ -120,7 +127,18 @@ def affine_warp_u8(image_u8, gt_u8, params, stats=None, meanval=ops.MEANVAL, ind
     out_g = torch.empty((m, 1, h, w), dtype=torch.float32, device=img.device)
     ops._count(2 * ((m + 31) // 32))
     with torch.cuda.device(img.device):
-        if index is None:
+        if obj is not None:
+            stream = torch.cuda.current_stream().cuda_stream
+            if index is None:
+                nat.check(lib.osvos_affine_warp_u8(img.data_ptr(), None, None, out_i.data_ptr(), None, mats, flips, n,
+                                                   h, w, *(float(v) for v in meanval), stream), "osvos_affine_warp_u8")
+            else:
+                nat.check(lib.osvos_affine_warp_u8_indexed(img.data_ptr(), None, None, out_i.data_ptr(), None, idx, mats,
+                                                           flips, m, n, h, w, *(float(v) for v in meanval), stream),
+                          "osvos_affine_warp_u8_indexed")
+            nat.check(lib.osvos_affine_warp_ids(gt.data_ptr(), out_g.data_ptr(), None if index is None else idx, mats,
+                                                flips, m, n, h, w, obj, stream), "osvos_affine_warp_ids")
+        elif index is None:
             nat.check(lib.osvos_affine_warp_u8(img.data_ptr(), gt.data_ptr(), stats.data_ptr(), out_i.data_ptr(),
                                                out_g.data_ptr(), mats, flips, n, h, w, *(float(v) for v in meanval),
                                                torch.cuda.current_stream().cuda_stream), "osvos_affine_warp_u8")

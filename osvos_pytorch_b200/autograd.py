@@ -35,7 +35,7 @@ class _OSVOSFunction(torch.autograd.Function):
 
     @staticmethod
     def _forward(ctx, engine, x, objective, *params):
-        """objective: None (plain forward: the five maps, each differentiable) or (label, loss_weights[5], divisor):
+        """objective: None (plain forward: the five maps, each differentiable) or (label, loss_weights[5], divisor, void):
         the package's own objective fused into the tail - outputs are then (5 maps, total, losses[5]) with only
         `total = sum_k w_k * class_balanced_cross_entropy_loss(map_k, label)` differentiable."""
         m = engine.m
@@ -95,7 +95,9 @@ class _OSVOSFunction(torch.autograd.Function):
             ctx.objective = None
             ctx.saved = (xin, acts, pooled)
             return tuple(out[k] for k in range(5))
-        label, weights, divisor = objective
+        label, weights, divisor, void = objective
+        if void and general:
+            raise ValueError("void labels are not supported by the general tail (learn_upsampling)")
         label = label.detach().to(xin.device).contiguous().float()
         if label.numel() != n * h * w:
             raise ValueError("objective label must be [N,1,H,W] like the output maps")
@@ -103,8 +105,9 @@ class _OSVOSFunction(torch.autograd.Function):
         if general:
             out, sums, losses = tail(label=label, loss_weights=weights, divisor=divisor)
         else:
-            out, sums, losses = tail(label=label, loss_weights=weights, divisor=divisor, deterministic=det)
+            out, sums, losses = tail(label=label, loss_weights=weights, divisor=divisor, deterministic=det, void=void)
         ctx.objective = (out, label, sums, weights, float(divisor))
+        ctx.void = void
         ctx.saved = (xin, acts, pooled)
         maps = tuple(out[k] for k in range(5))
         total = losses[5:6].reshape(())          # 0-dim view of the weighted total
@@ -221,7 +224,7 @@ class _OSVOSFunction(torch.autograd.Function):
             # the forward's sums
             out, label, sums, weights, divisor = obj
             dpq, fb = ops.tail_loss_bwd(out, label, sums, weights, divisor, g_total.detach().contiguous().float(),
-                                        n, h, w, want_fuse_bias=grads[4] is not None, deterministic=det)
+                                        n, h, w, want_fuse_bias=grads[4] is not None, deterministic=det, void=ctx.void)
             if fb is not None:
                 pg[m.fuse.bias] = fb.reshape(m.fuse.bias.shape)
         else:
@@ -361,9 +364,9 @@ def osvos_apply(engine, x):
     return list(outs)
 
 
-def osvos_apply_objective(engine, x, label, loss_weights, divisor):
-    """Forward + the weighted class-balanced BCE objective as one autograd node.
+def osvos_apply_objective(engine, x, label, loss_weights, divisor, void=False):
+    """Forward + the weighted class-balanced BCE objective as one autograd node (``void``: label < 0 is left out).
     -> (maps: list of 5 [N,1,H,W] logit tensors (detached), total: 0-dim differentiable loss, per_map: [5] losses)."""
     params = engine._param_list()
-    res = _OSVOSFunction.apply(engine, x, (label, loss_weights, divisor), *params)
+    res = _OSVOSFunction.apply(engine, x, (label, loss_weights, divisor, bool(void)), *params)
     return list(res[:5]), res[5], res[6]

@@ -118,6 +118,33 @@ label_from_u8_kernel(const uint8_t* __restrict__ src, const uint32_t* __restrict
   }
 }
 
+// uint8 id maps [n][hw] -> fp32 [n][hw] labels (label_of_id); four bytes -> one float4 per thread.
+__global__ void __launch_bounds__(kIngestThreads)
+labels_from_ids_kernel(const uint8_t* __restrict__ src, float* __restrict__ dst, int hw, uint32_t object) {
+  const int n = blockIdx.y;
+  const int p = blockIdx.x * kIngestPx + 4 * threadIdx.x;
+  if (p >= hw) return;
+  const int cnt = min(4, hw - p);
+  const uint8_t* s = src + static_cast<size_t>(n) * hw + p;
+  float* d = dst + static_cast<size_t>(n) * hw + p;
+  uint8_t b[4] = {0, 0, 0, 0};
+  if (cnt == 4 && (reinterpret_cast<uintptr_t>(s) & 3) == 0) {
+    const uint32_t word = __ldg(reinterpret_cast<const uint32_t*>(s));
+#pragma unroll
+    for (int j = 0; j < 4; ++j) b[j] = static_cast<uint8_t>(word >> (8 * j));
+  } else {
+    for (int j = 0; j < cnt; ++j) b[j] = __ldg(s + j);
+  }
+  float v[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) v[j] = label_of_id(b[j], object);
+  if (cnt == 4 && (reinterpret_cast<uintptr_t>(d) & 15) == 0) {
+    *reinterpret_cast<float4*>(d) = make_float4(v[0], v[1], v[2], v[3]);
+  } else {
+    for (int j = 0; j < cnt; ++j) d[j] = v[j];
+  }
+}
+
 }  // namespace osvos
 
 using namespace osvos;
@@ -207,4 +234,32 @@ extern "C" int osvos_affine_warp_u8_indexed(const uint8_t* image_store, const ui
                               n, 1, h, w, OSVOS_WARP_CUBIC, stream, index_host);
   }
   return OSVOS_OK;
+}
+
+extern "C" int osvos_labels_from_ids(const uint8_t* ids, float* dst, int n, int h, int w, int object,
+                                     osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(ids != nullptr && dst != nullptr && object >= 0 && object < 255);
+  OSVOS_CHECK_FRAME_DIMS(n, h, w);
+  const int hw = h * w;
+  labels_from_ids_kernel<<<dim3((hw + kIngestPx - 1) / kIngestPx, n), kIngestThreads, 0,
+                           static_cast<cudaStream_t>(stream_)>>>(ids, dst, hw, static_cast<uint32_t>(object));
+  OSVOS_CHECK_CUDA(cudaGetLastError());
+  return OSVOS_OK;
+}
+
+// The id mode of osvos_affine_warp_u8 (index_host == NULL) and osvos_affine_warp_u8_indexed: the same matrices, flips
+// and nearest fixed-point walk, with the label of each sampled id.
+extern "C" int osvos_affine_warp_ids(const uint8_t* ids_store, float* label_dst, const int* index_host,
+                                     const double* inv_matrices_host, const int* flips_host, int n, int n_store, int h,
+                                     int w, int object, osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(ids_store != nullptr && label_dst != nullptr && inv_matrices_host != nullptr);
+  OSVOS_CHECK_ARG(object >= 0 && object < 255);
+  OSVOS_CHECK_FRAME_DIMS(n, h, w);
+  if (index_host != nullptr) {
+    OSVOS_CHECK_ARG(n_store > 0);
+    for (int i = 0; i < n; ++i) OSVOS_CHECK_ARG(index_host[i] >= 0 && index_host[i] < n_store);
+  }
+  return launch_affine_warp(WarpSrcIds8{ids_store, h, w, static_cast<uint32_t>(object)}, label_dst, inv_matrices_host,
+                            flips_host, n, 1, h, w, OSVOS_WARP_NEAREST, static_cast<cudaStream_t>(stream_),
+                            index_host);
 }

@@ -42,6 +42,7 @@ constexpr int kTailThreads = 256;
 // fused map (sum_{y=1} (sigmoid(x) - 1), sum_{y=0} sigmoid(x): d fuse.bias without another pass), [14] = arrival counter
 constexpr int kTailSums = 15;
 constexpr int kTailVals = 13;   // block partials per block in the deterministic form: sums[0..10], [12], [13]
+constexpr int kTailVoidVals = 14;   // the void form (OSVOS_FLAG_VOID_LABELS) also counts N = #(y >= 0) into sums[11]
 
 static int tail_fwd_blocks(int n, int h) {
   size_t blocks = static_cast<size_t>(n) * h;                 // one output row per block iteration
@@ -57,8 +58,9 @@ __device__ __forceinline__ float softplus_f(float x) { return fmaxf(x, 0.f) + lo
 // whatever the row length) and blends HORIZONTALLY from shared memory: two LDS.64 and four FMAs per scale and pixel.
 // (The full 2 x 2 gather with its index arithmetic per pixel and scale costs ~850 instructions per pixel group.)
 // DET (OSVOS_FLAG_DETERMINISTIC): block partials go to rows behind the sums, added in a fixed order by the last block.
-template <bool DET = false>
-__global__ void __launch_bounds__(kTailThreads) tail_fwd_kernel(const TailParams p) {
+// VOID (OSVOS_FLAG_VOID_LABELS): pixels with y < 0 enter no sum; N is counted (sums[11]) and N == 0 gives losses of 0.
+template <bool DET, bool VOID>
+__device__ __forceinline__ void tail_fwd_body(const TailParams& p) {
   extern __shared__ float2 vbuf[];     // [scale 0 .. 3][wk_k] vertically blended (p, q)
   pdl_wait();               // side maps, biases and the accumulators all come from earlier kernels (ptx.cuh)
   pdl_launch_dependents();
@@ -70,7 +72,7 @@ __global__ void __launch_bounds__(kTailThreads) tail_fwd_kernel(const TailParams
   for (int k = 1; k < 4; ++k) voff[k] = voff[k - 1] + p.sc[k - 1].wk;
 
   float s_pos[5] = {0, 0, 0, 0, 0}, s_neg[5] = {0, 0, 0, 0, 0};
-  float cnt_pos = 0.f, a_pos = 0.f, a_neg = 0.f;
+  float cnt_pos = 0.f, a_pos = 0.f, a_neg = 0.f, cnt_all = 0.f;
 
   for (int row = blockIdx.x; row < p.n * p.h; row += gridDim.x) {
     const int img = row / p.h, y = row - img * p.h;
@@ -136,7 +138,8 @@ __global__ void __launch_bounds__(kTailThreads) tail_fwd_kernel(const TailParams
           fused += fmaf(w1, t1.y, w0 * t0.y);
         }
         o[4][j] = fused;
-        if (p.label && live) {
+        if (p.label && live && (!VOID || lab[j] >= 0.f)) {
+          if constexpr (VOID) cnt_all += 1.f;
           const bool pos = lab[j] >= 0.5f;
           cnt_pos += pos ? 1.f : 0.f;
 #pragma unroll
@@ -166,7 +169,7 @@ __global__ void __launch_bounds__(kTailThreads) tail_fwd_kernel(const TailParams
   }
 
   if (p.label && p.sums) {
-    constexpr int kVals = kTailVals;
+    constexpr int kVals = VOID ? kTailVoidVals : kTailVals;
     __shared__ float red[kTailThreads / 32][kVals];
     float vals[kVals];
 #pragma unroll
@@ -177,6 +180,7 @@ __global__ void __launch_bounds__(kTailThreads) tail_fwd_kernel(const TailParams
     vals[10] = cnt_pos;
     vals[11] = a_pos;
     vals[12] = a_neg;
+    if constexpr (VOID) vals[13] = cnt_all;
 #pragma unroll
     for (int i = 0; i < kVals; ++i) {
 #pragma unroll
@@ -188,7 +192,7 @@ __global__ void __launch_bounds__(kTailThreads) tail_fwd_kernel(const TailParams
       for (int i = 0; i < kVals; ++i) red[warp][i] = vals[i];
     }
     __syncthreads();
-    const int slot = threadIdx.x < 11 ? threadIdx.x : threadIdx.x + 1;
+    const int slot = threadIdx.x < 11 ? threadIdx.x : threadIdx.x < 13 ? threadIdx.x + 1 : 11;
     if (threadIdx.x < kVals) {
       double acc = 0.0;
       for (int wv = 0; wv < kTailThreads / 32; ++wv) acc += static_cast<double>(red[wv][threadIdx.x]);
@@ -201,7 +205,7 @@ __global__ void __launch_bounds__(kTailThreads) tail_fwd_kernel(const TailParams
         __shared__ double dred[kTailThreads];
         for (int i = 0; i < kVals; ++i) {
           const double t = block_ordered_sum(p.sums + kTailSums + i, static_cast<int>(gridDim.x), kVals, dred);
-          if (threadIdx.x == 0) p.sums[i < 11 ? i : i + 1] = t;
+          if (threadIdx.x == 0) p.sums[i < 11 ? i : i < 13 ? i + 1 : 11] = t;
         }
         __syncthreads();
       }
@@ -209,14 +213,15 @@ __global__ void __launch_bounds__(kTailThreads) tail_fwd_kernel(const TailParams
     // the last block to arrive turns the sums into the five losses and their weighted total:
     // L_k = (Nn/N * S_pos_k + P/N * S_neg_k) / divisor   (layers/osvos_layers.py:38-46)
     if (last && threadIdx.x == 0) {
-      const double tot = static_cast<double>(total);
+      const double tot = VOID ? __ldcg(p.sums + 11) : static_cast<double>(total);
       const double pcount = __ldcg(p.sums + 10), nn = tot - pcount;
-      p.sums[11] = tot;
+      if constexpr (!VOID) p.sums[11] = tot;
       if (p.losses) {
         double wsum = 0.0;
         for (int k = 0; k < 5; ++k) {
-          const double lk = (nn / tot * __ldcg(p.sums + 2 * k) + pcount / tot * __ldcg(p.sums + 2 * k + 1)) *
-                            static_cast<double>(p.inv_divisor);
+          double lk = (nn / tot * __ldcg(p.sums + 2 * k) + pcount / tot * __ldcg(p.sums + 2 * k + 1)) *
+                      static_cast<double>(p.inv_divisor);
+          if constexpr (VOID) lk = tot > 0.0 ? lk : 0.0;
           p.losses[k] = static_cast<float>(lk);
           wsum += static_cast<double>(p.loss_weights[k]) * lk;
         }
@@ -224,6 +229,16 @@ __global__ void __launch_bounds__(kTailThreads) tail_fwd_kernel(const TailParams
       }
     }
   }
+}
+
+template <bool DET = false>
+__global__ void __launch_bounds__(kTailThreads) tail_fwd_kernel(const TailParams p) {
+  tail_fwd_body<DET, false>(p);
+}
+
+template <bool DET>
+__global__ void __launch_bounds__(kTailThreads) tail_fwd_void_kernel(const TailParams p) {
+  tail_fwd_body<DET, true>(p);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -255,8 +270,9 @@ constexpr int kTailBwdCols = 512 + 32;
 
 // DET: with several row groups per column, their column sums are added into shared memory in row-group order instead of
 // with shared-memory atomics.
-template <bool LOSS, bool DET = false>
-__global__ void __launch_bounds__(256) tail_bwd2_kernel(const __grid_constant__ TailBwdParams p) {
+// VOID (LOSS only, OSVOS_FLAG_VOID_LABELS): pixels with y < 0 get weight 0, and N = sums[11] == 0 gives zero gradients.
+template <bool LOSS, bool DET, bool VOID>
+__device__ __forceinline__ void tail_bwd2_body(const TailBwdParams& p) {
   __shared__ float colp[kTailBwdCols], colq[kTailBwdCols];
   const int tid = threadIdx.x;
   int k = 3;
@@ -280,8 +296,15 @@ __global__ void __launch_bounds__(256) tail_bwd2_kernel(const __grid_constant__ 
     const float up = (p.upstream ? __ldg(p.upstream) : 1.f) * p.inv_divisor;
     cp = p.coeff[k] * up;
     cq = p.coeff[4] * up;
-    if (blockIdx.x == 0 && tid == 0 && p.fuse_bias_grad)   // d fuse.bias = sum_px g_4, from the forward's A sums
-      p.fuse_bias_grad[0] = cq * static_cast<float>((nt - pc) / nt * p.sums[12] + pc / nt * p.sums[13]);
+    if constexpr (VOID) {
+      if (!(nt > 0.0)) wpos = wneg = cp = cq = 0.f;
+    }
+    if (blockIdx.x == 0 && tid == 0 && p.fuse_bias_grad) {  // d fuse.bias = sum_px g_4, from the forward's A sums
+      if (VOID && !(nt > 0.0))
+        p.fuse_bias_grad[0] = 0.f;
+      else
+        p.fuse_bias_grad[0] = cq * static_cast<float>((nt - pc) / nt * p.sums[12] + pc / nt * p.sums[13]);
+    }
   }
   const bool use_p = LOSS ? (p.coeff[k] != 0.f) : (p.src[k] != nullptr);
   const bool use_q = LOSS ? (p.coeff[4] != 0.f) : (p.src[4] != nullptr);
@@ -319,7 +342,8 @@ __global__ void __launch_bounds__(256) tail_bwd2_kernel(const __grid_constant__ 
         for (int u = 0; u < 4; ++u) {
           if (LOSS) {
             const bool pos = lv[u] >= 0.5f;
-            const float wgt = (pos ? wpos : wneg) * fyv[u];
+            float wgt = (pos ? wpos : wneg) * fyv[u];
+            if constexpr (VOID) wgt = lv[u] < 0.f ? 0.f : wgt;
             const float yv = pos ? 1.f : 0.f;
             if (use_p) ap = fmaf(wgt, 1.f / (1.f + __expf(-pv[u])) - yv, ap);
             if (use_q) aq = fmaf(wgt, 1.f / (1.f + __expf(-qv[u])) - yv, aq);
@@ -373,6 +397,16 @@ __global__ void __launch_bounds__(256) tail_bwd2_kernel(const __grid_constant__ 
   }
 }
 
+template <bool LOSS, bool DET = false>
+__global__ void __launch_bounds__(256) tail_bwd2_kernel(const __grid_constant__ TailBwdParams p) {
+  tail_bwd2_body<LOSS, DET, false>(p);
+}
+
+template <bool DET>
+__global__ void __launch_bounds__(256) tail_bwd2_void_kernel(const __grid_constant__ TailBwdParams p) {
+  tail_bwd2_body<true, DET, true>(p);
+}
+
 }  // namespace osvos
 
 using namespace osvos;
@@ -396,8 +430,9 @@ static void fill_tail_scales(TailParams& p, const float* const* pq, int h, int w
 
 extern "C" int osvos_tail_fwd(const osvos_tail_fwd_args* a, osvos_stream_t stream_) {
   OSVOS_CHECK_ARG(a != nullptr && a->n > 0 && a->h > 0 && a->w > 0);
-  OSVOS_CHECK_ARG((a->flags & ~OSVOS_FLAG_DETERMINISTIC) == 0);
+  OSVOS_CHECK_ARG((a->flags & ~(OSVOS_FLAG_DETERMINISTIC | OSVOS_FLAG_VOID_LABELS)) == 0);
   OSVOS_CHECK_ARG(a->label == nullptr || a->sums != nullptr);
+  OSVOS_CHECK_ARG(!(a->flags & OSVOS_FLAG_VOID_LABELS) || a->label != nullptr);
   OSVOS_CHECK_ARG(a->losses == nullptr || (a->label != nullptr && a->divisor > 0.f));
   OSVOS_CHECK_ARG(static_cast<size_t>(a->n) * a->h * a->w < (1ull << 31));   // 32-bit element indices in the kernel
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -425,7 +460,12 @@ extern "C" int osvos_tail_fwd(const osvos_tail_fwd_args* a, osvos_stream_t strea
   const size_t smem = sizeof(float2) * (p.sc[0].wk + p.sc[1].wk + p.sc[2].wk + p.sc[3].wk);
   OSVOS_CHECK_ARG(smem <= 48 * 1024);                               // rows up to ~13,000 pixels
   // (with a loss, the memset above is this kernel's stream predecessor: plain launch)
-  if (a->sums && (a->flags & OSVOS_FLAG_DETERMINISTIC))
+  if (a->flags & OSVOS_FLAG_VOID_LABELS) {
+    if (a->flags & OSVOS_FLAG_DETERMINISTIC)
+      tail_fwd_void_kernel<true><<<static_cast<int>(blocks), kTailThreads, smem, stream>>>(p);
+    else
+      tail_fwd_void_kernel<false><<<static_cast<int>(blocks), kTailThreads, smem, stream>>>(p);
+  } else if (a->sums && (a->flags & OSVOS_FLAG_DETERMINISTIC))
     tail_fwd_kernel<true><<<static_cast<int>(blocks), kTailThreads, smem, stream>>>(p);
   else if (a->sums)
     tail_fwd_kernel<false><<<static_cast<int>(blocks), kTailThreads, smem, stream>>>(p);
@@ -480,7 +520,7 @@ extern "C" int osvos_tail_bwd(const osvos_tail_bwd_args* a, osvos_stream_t strea
 extern "C" int osvos_tail_loss_bwd(const osvos_tail_loss_bwd_args* a, osvos_stream_t stream_) {
   OSVOS_CHECK_ARG(a != nullptr && a->n > 0 && a->h > 0 && a->w > 0 && a->label != nullptr && a->sums != nullptr);
   OSVOS_CHECK_ARG(a->divisor > 0.f);
-  OSVOS_CHECK_ARG((a->flags & ~OSVOS_FLAG_DETERMINISTIC) == 0);
+  OSVOS_CHECK_ARG((a->flags & ~(OSVOS_FLAG_DETERMINISTIC | OSVOS_FLAG_VOID_LABELS)) == 0);
   for (int k = 0; k < 4; ++k) OSVOS_CHECK_ARG(a->dpq[k] != nullptr);
   for (int k = 0; k < 5; ++k) OSVOS_CHECK_ARG(a->logits[k] != nullptr || a->loss_weights[k] == 0.f);
   TailBwdParams p;
@@ -496,10 +536,18 @@ extern "C" int osvos_tail_loss_bwd(const osvos_tail_loss_bwd_args* a, osvos_stre
   p.inv_divisor = 1.f / a->divisor;
   p.fuse_bias_grad = a->fuse_bias_grad;
   p.n = a->n, p.h = a->h, p.w = a->w;
-  if (a->flags & OSVOS_FLAG_DETERMINISTIC)
-    tail_bwd2_kernel<true, true><<<items, 256, 0, static_cast<cudaStream_t>(stream_)>>>(p);
-  else
-    tail_bwd2_kernel<true><<<items, 256, 0, static_cast<cudaStream_t>(stream_)>>>(p);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const bool det = (a->flags & OSVOS_FLAG_DETERMINISTIC) != 0;
+  if (a->flags & OSVOS_FLAG_VOID_LABELS) {
+    if (det)
+      tail_bwd2_void_kernel<true><<<items, 256, 0, stream>>>(p);
+    else
+      tail_bwd2_void_kernel<false><<<items, 256, 0, stream>>>(p);
+  } else if (det) {
+    tail_bwd2_kernel<true, true><<<items, 256, 0, stream>>>(p);
+  } else {
+    tail_bwd2_kernel<true><<<items, 256, 0, stream>>>(p);
+  }
   OSVOS_CHECK_CUDA(cudaGetLastError());
   return OSVOS_OK;
 }
@@ -507,4 +555,11 @@ extern "C" int osvos_tail_loss_bwd(const osvos_tail_loss_bwd_args* a, osvos_stre
 extern "C" size_t osvos_tail_fwd_deterministic_sums(int n, int h, int w) {
   if (n <= 0 || h <= 0 || w <= 0) return 0;
   return kTailSums + static_cast<size_t>(tail_fwd_blocks(n, h)) * kTailVals;
+}
+
+extern "C" size_t osvos_tail_fwd_sums(int n, int h, int w, int flags) {
+  if (n <= 0 || h <= 0 || w <= 0 || (flags & ~(OSVOS_FLAG_DETERMINISTIC | OSVOS_FLAG_VOID_LABELS)) != 0) return 0;
+  if (!(flags & OSVOS_FLAG_DETERMINISTIC)) return kTailSums;
+  const int vals = (flags & OSVOS_FLAG_VOID_LABELS) ? kTailVoidVals : kTailVals;
+  return kTailSums + static_cast<size_t>(tail_fwd_blocks(n, h)) * vals;
 }

@@ -89,6 +89,29 @@ struct WarpSrcLabel8 {
   }
 };
 
+// The label of a DAVIS-2017 object-id byte: -1 for 255 (void), 1 for an object (1..254, or == object when object != 0),
+// 0 else (osvos_labels_from_ids).
+__device__ __forceinline__ float label_of_id(uint32_t v, uint32_t object) {
+  return v == 255u ? -1.f : (object != 0u ? v == object : v != 0u) ? 1.f : 0.f;
+}
+
+// uint8 id maps [n][h][w], always sampled nearest (out-of-frame samples are 0 like the mask's).
+struct WarpSrcIds8 {
+  const uint8_t* p;
+  int h, w;
+  uint32_t object;
+  struct Sample {
+    const uint8_t* base;
+    int w;
+    uint32_t object;
+    __device__ __forceinline__ float operator()(int, int y, int x) const {
+      return label_of_id(__ldg(base + static_cast<size_t>(y) * w + x), object);
+    }
+  };
+  __device__ __forceinline__ int mode(int, int) const { return OSVOS_WARP_NEAREST; }
+  __device__ __forceinline__ Sample sample(int s) const { return {p + static_cast<size_t>(s) * h * w, w, object}; }
+};
+
 template <class Src>
 __global__ void __launch_bounds__(256)
 affine_warp_kernel(const Src src, float* __restrict__ dst, const __grid_constant__ WarpTable t, int sample0, int c, int h,

@@ -330,20 +330,25 @@ def upload(batch, device, input_res=None, jpeg_status=None):
     return img, gt, ops.label_stats_u8(gt)
 
 
-def to_device(batch, device, augment=None, meanval=MEANVAL, input_res=None, jpeg_status=None):
+def to_device(batch, device, augment=None, meanval=MEANVAL, input_res=None, jpeg_status=None, ids=False):
     """Collated batch -> {'image': f32 [N,3,H,W], 'gt': f32 [N,1,H,W]} on ``device``.
 
     augment None: the reference's make_img_gt_pair + ToTensor, bit for bit (ops.image_from_bgr8, ops.label_from_u8).
     Otherwise RandomHorizontalFlip + ScaleNRotate as the reference composes them, fused with the ingest
     (augment.affine_warp_u8): ``augment`` is a list of per-sample (flip, rot, scale) triples, or a random generator
     from which augment.draw_params draws them in the reference's order.  ``input_res``: the reference's ``inputRes``,
-    applied on the device before all of that (upload, which also decodes a decode="device" batch's JPEGs)."""
+    applied on the device before all of that (upload, which also decodes a decode="device" batch's JPEGs).
+    ``ids``: False or None for DAVIS-2016 masks, or "all" / k for DAVIS2017Frames batches, whose masks are object-id maps: the
+    gt is then ops.labels_from_ids(ids, object) (1 object, 0 background, -1 void; "all": every object), warped in the
+    id mode of the fused warp (always nearest)."""
     with torch.cuda.device(device):
         img, gt, stats = upload(batch, device, input_res, jpeg_status)
         if augment is None:
-            return {"image": ops.image_from_bgr8(img, meanval), "gt": ops.label_from_u8(gt, stats)}
+            masks = ids is None or ids is False
+            label = ops.label_from_u8(gt, stats) if masks else ops.labels_from_ids(gt, ids)
+            return {"image": ops.image_from_bgr8(img, meanval), "gt": label}
         params = augment if isinstance(augment, (list, tuple)) else _augment.draw_params(int(img.shape[0]), rng=augment)
-        return _augment.affine_warp_u8(img, gt, params, stats, meanval)
+        return _augment.affine_warp_u8(img, gt, params, stats, meanval, ids=ids)
 
 
 _MAX_STATS_FRAMES = 65535                                # osvos_label_stats_u8 takes n < 65536
@@ -369,7 +374,7 @@ def shard_plan(sizes, world):
 
 
 class DeviceFrames:
-    """Every item of a DAVIS2016Frames, decoded once and kept on ``device`` as uint8 bytes.
+    """Every item of a DAVIS2016Frames or DAVIS2017Frames, decoded once and kept on ``device`` as uint8 bytes.
 
     Frames are grouped by size; group g holds ``img`` uint8 [n_g,H,W,3], ``gt`` uint8 [n_g,H,W] and ``stats``
     (ops.label_stats_u8 of gt).  ``where[i]`` is dataset index i's (group, slot); ``has_gt`` and ``fname`` are the
@@ -396,13 +401,18 @@ class DeviceFrames:
     A ``decode="device"`` dataset's frames are decoded on the device (device_views).  Before the store is shared, every
     frame whose decoder status is nonzero (a corrupt or cut-short stream) is decoded again with cv2.imread, so the store
     holds cv2's bytes whatever the files.  ``fallback_frames``: frames outside the device decoder's subset (decoded by
-    cv2.imread in the workers); ``redecoded_frames``: frames decoded again after a nonzero status."""
+    cv2.imread in the workers); ``redecoded_frames``: frames decoded again after a nonzero status.
 
-    def __init__(self, dataset, device, workers=0, group=None, input_res=None, keep_stored_gt=False):
+    Over a DAVIS2017Frames the store keeps the annotations' object ids, and ``ids`` ("all" unless given; False, "all"
+    or k as to_device's) selects the labels augmented() and ingest() make from them (ops.labels_from_ids and the id
+    mode of the fused warp)."""
+
+    def __init__(self, dataset, device, workers=0, group=None, input_res=None, keep_stored_gt=False, ids=None):
         import torch.distributed as dist
         from torch.utils.data import DataLoader, Subset
         t0 = time.perf_counter()
         self.device = torch.device(device)
+        self.ids = ("all" if isinstance(dataset, DAVIS2017Frames) else False) if ids is None else ids
         world = 1 if group is None else dist.get_world_size(group)
         rank = 0 if group is None else dist.get_rank(group)
         n = len(dataset)
@@ -513,7 +523,8 @@ class DeviceFrames:
             raise ValueError("all frames of a batch must share a size")
         grp = self.groups[g]
         with torch.cuda.device(self.device):
-            return _augment.affine_warp_u8(grp["img"], grp["gt"], params, grp["stats"], index=[s for _, s in where])
+            return _augment.affine_warp_u8(grp["img"], grp["gt"], params, grp["stats"], index=[s for _, s in where],
+                                           ids=self.ids)
 
     def batches(self, index_batches, rng=random):
         """Augmented batches for an iterable of index batches (e.g. a DataLoader over dataset indices), the (flip, rot,
@@ -531,8 +542,9 @@ class DeviceFrames:
         grp = self.groups[g]
         gt = grp["gt"][s:s + 1]
         with torch.cuda.device(self.device):
-            item = {"image": ops.image_from_bgr8(grp["img"][s:s + 1]), "gt": ops.label_from_u8(gt, grp["stats"][s:s + 1]),
-                    "gt_u8": gt, "fname": [self.fname[i]]}
+            label = (ops.label_from_u8(gt, grp["stats"][s:s + 1]) if self.ids is False
+                     else ops.labels_from_ids(gt, self.ids))
+            item = {"image": ops.image_from_bgr8(grp["img"][s:s + 1]), "gt": label, "gt_u8": gt, "fname": [self.fname[i]]}
         if self.stored_groups:
             g0, s0 = self.where_stored[i]
             item["gt_u8_stored"] = self.stored_groups[g0]["gt"][s0:s0 + 1]

@@ -215,7 +215,7 @@ class OSVOSEngine:
             return self._forward_graphed(x, fresh_outputs)
         return self.forward_inference(x)
 
-    def forward_objective(self, x, gts, loss_weights, size_average=False, batch_average=True):
+    def forward_objective(self, x, gts, loss_weights, size_average=False, batch_average=True, void=False):
         """See OSVOS.forward_objective."""
         if not isinstance(x, torch.Tensor) or x.dim() != 4 or x.size(1) != 3:
             raise ValueError("OSVOS.forward_objective expects a [N, 3, H, W] tensor")
@@ -223,6 +223,11 @@ class OSVOSEngine:
             raise RuntimeError("osvos_pytorch_b200.OSVOS runs on CUDA (sm_90a) only; there is no CPU fallback")
         if len(loss_weights) != 5:
             raise ValueError("loss_weights: one weight per output map (5)")
+        if void and size_average:
+            raise ValueError("void labels with size_average are not supported: the divisor would be the non-void count")
+        if void and self.uses_general_tail():
+            raise ValueError("void labels are not supported with learn_upsampling or non-bilinear deconvolution "
+                             "weights (the general tail)")
         if size_average:
             divisor = float(gts.numel())
         elif batch_average:
@@ -231,9 +236,9 @@ class OSVOSEngine:
             divisor = 1.0
         if x.device != torch.device("cuda", torch.cuda.current_device()):
             with torch.cuda.device(x.device):
-                return self.forward_objective(x, gts, loss_weights, size_average, batch_average)
+                return self.forward_objective(x, gts, loss_weights, size_average, batch_average, void)
         from .autograd import osvos_apply_objective
-        return osvos_apply_objective(self, x, gts, loss_weights, divisor)
+        return osvos_apply_objective(self, x, gts, loss_weights, divisor, void)
 
     def _forward_graphed(self, x, fresh_outputs=True):
         """Inference through a captured CUDA graph.  Two kinds of entry:

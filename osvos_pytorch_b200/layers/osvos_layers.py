@@ -62,7 +62,7 @@ def center_crop(x, height, width):
 
 class _ClassBalancedBCE(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, output, label, divisor):
+    def forward(ctx, output, label, divisor, void):
         if not output.is_cuda:
             raise RuntimeError("class_balanced_cross_entropy_loss: CUDA tensors required; the H100 package has no "
                                "CPU fallback (oracle/ holds the CPU restatement used by the tests)")
@@ -74,11 +74,14 @@ class _ClassBalancedBCE(torch.autograd.Function):
         stream = torch.cuda.current_stream().cuda_stream
         # deterministic: block sums added in a fixed order instead of with fp64 atomics (rows behind sums[0..4])
         flags = nat.FLAG_DETERMINISTIC if torch.are_deterministic_algorithms_enabled() else 0
+        if void:
+            flags |= nat.FLAG_VOID_LABELS     # label < 0: void, in neither class (sums[3] = the non-void count)
         sums = torch.empty(lib.osvos_cbce_fwd_sums(x.numel(), flags), dtype=torch.float64, device=x.device)
         nat.check(lib.osvos_cbce_fwd(x.data_ptr(), y.data_ptr(), x.numel(), float(divisor), sums.data_ptr(),
                                      loss.data_ptr(), flags, stream), "osvos_cbce_fwd")
         ctx.save_for_backward(x, y, sums)
         ctx.divisor = float(divisor)
+        ctx.void = void
         ctx.shape = output.shape
         return loss
 
@@ -89,18 +92,25 @@ class _ClassBalancedBCE(torch.autograd.Function):
         g = grad_out.detach().contiguous().float().reshape(1)
         dx = torch.empty_like(x)
         stream = torch.cuda.current_stream().cuda_stream
-        nat.check(lib.osvos_cbce_bwd(x.data_ptr(), y.data_ptr(), sums.data_ptr(), g.data_ptr(), ctx.divisor,
-                                     x.numel(), dx.data_ptr(), stream), "osvos_cbce_bwd")
-        return dx.reshape(ctx.shape), None, None
+        bwd = lib.osvos_cbce_bwd_void if ctx.void else lib.osvos_cbce_bwd
+        nat.check(bwd(x.data_ptr(), y.data_ptr(), sums.data_ptr(), g.data_ptr(), ctx.divisor, x.numel(), dx.data_ptr(),
+                      stream), "osvos_cbce_bwd")
+        return dx.reshape(ctx.shape), None, None, None
 
 
-def class_balanced_cross_entropy_loss(output, label, size_average=True, batch_average=True):
+def class_balanced_cross_entropy_loss(output, label, size_average=True, batch_average=True, void=False):
     """Class-balanced sigmoid BCE (reference :19-48): same arguments, returns a 0-dim tensor that
-    supports .item(), /=, .backward(), python sum() and scalar multiplication."""
+    supports .item(), /=, .backward(), python sum() and scalar multiplication.
+
+    ``void`` (extension): a label < 0 marks a void pixel (DAVIS-2017's 255), counted in neither class and given zero
+    gradient; the class weights then use the non-void count, and an all-void label gives 0.  Not with size_average,
+    whose divisor would be that count."""
+    if void and size_average:
+        raise ValueError("class_balanced_cross_entropy_loss: void=True needs size_average=False")
     if size_average:
         divisor = float(np.prod(label.size()))
     elif batch_average:
         divisor = float(label.size()[0])
     else:
         divisor = 1.0
-    return _ClassBalancedBCE.apply(output, label, divisor)
+    return _ClassBalancedBCE.apply(output, label, divisor, bool(void))

@@ -74,15 +74,18 @@ class OSVOS(nn.Module):
     def forward(self, x):
         return self._engine.forward(x)
 
-    def forward_objective(self, x, gts, loss_weights=(0.0, 0.0, 0.0, 0.0, 1.0), size_average=False, batch_average=True):
+    def forward_objective(self, x, gts, loss_weights=(0.0, 0.0, 0.0, 0.0, 1.0), size_average=False, batch_average=True,
+                          void=False):
         """Extension (not in the reference): forward + the weighted sum of the five class-balanced BCE losses as ONE
         autograd node whose tail (upsample + crop + fuse + loss) is a single kernel forward and a single kernel
         backward.  Equivalent to
             outs = net(x); total = sum(w_k * class_balanced_cross_entropy_loss(outs[k], gts, size_average, batch_average))
         with loss_weights = (0,0,0,0,1) for the online objective (train_online.py:127) and (s,s,s,s,1),
         s = 1 - epoch/nEpochs, for the parent objective (train_parent.py:143-147).
+        ``void``: gts < 0 marks void pixels, which the losses leave out (class_balanced_cross_entropy_loss(..., void=True);
+        not with size_average or learn_upsampling).
         -> (outs: list of 5 logit maps, detached; total: 0-dim loss to call .backward() on; per_map: [5] losses)."""
-        return self._engine.forward_objective(x, gts, loss_weights, size_average, batch_average)
+        return self._engine.forward_objective(x, gts, loss_weights, size_average, batch_average, void)
 
     # ------------------------------------------------------------- initialisation
     def _initialize_weights(self, pretrained, verbose=True):

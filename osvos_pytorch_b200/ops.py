@@ -257,20 +257,25 @@ def side_project(feat, proj_w, proj_b):
     return pq
 
 
-def tail_fwd(pqs, fuse_bias, n, h, w, label=None, out=None, loss_weights=None, divisor=None, deterministic=False):
+def tail_fwd(pqs, fuse_bias, n, h, w, label=None, out=None, loss_weights=None, divisor=None, deterministic=False,
+             void=False):
     """Upsample + crop + fuse (+ loss sums, + the five class-balanced BCE losses and their weighted total).
     Returns (out [5,n,1,h,w] fp32, sums [TAIL_SUMS] f64 | None) and, with `loss_weights` (5 floats) and `divisor`,
-    additionally losses [6] fp32 = the five per-map losses and sum_k loss_weights[k] * loss_k."""
+    additionally losses [6] fp32 = the five per-map losses and sum_k loss_weights[k] * loss_k.  ``void``: label < 0
+    marks void pixels, left out of the loss (OSVOS_FLAG_VOID_LABELS)."""
     lib = nat.load()
     dev = pqs[0].device
     if out is None:
         # each map starts on a 16-byte boundary so the kernel can use 128-bit stores
         per = (n * h * w + 3) // 4 * 4
         out = torch.empty((5, per), dtype=torch.float32, device=dev)[:, :n * h * w].view(5, n, 1, h, w)
-    nsums = lib.osvos_tail_fwd_deterministic_sums(n, h, w) if deterministic else nat.TAIL_SUMS
+    if void and label is None:
+        raise ValueError("tail_fwd: void needs a label")
+    flags = (nat.FLAG_DETERMINISTIC if deterministic else 0) | (nat.FLAG_VOID_LABELS if void else 0)
+    nsums = lib.osvos_tail_fwd_sums(n, h, w, flags)
     sums = torch.empty(nsums, dtype=torch.float64, device=dev) if label is not None else None
     a = nat.TailFwdArgs()
-    a.flags = nat.FLAG_DETERMINISTIC if deterministic else 0
+    a.flags = flags
     for k in range(4):
         a.pq[k] = pqs[k].data_ptr()
     for k in range(5):
@@ -295,13 +300,14 @@ def tail_fwd(pqs, fuse_bias, n, h, w, label=None, out=None, loss_weights=None, d
     return out, sums
 
 
-def tail_loss_bwd(out, label, sums, loss_weights, divisor, upstream, n, h, w, want_fuse_bias=True, deterministic=False):
+def tail_loss_bwd(out, label, sums, loss_weights, divisor, upstream, n, h, w, want_fuse_bias=True, deterministic=False,
+                  void=False):
     """Backward of tail + the weighted class-balanced BCE objective in one launch (see include/osvos_b200.h):
-    -> (list of 4 dpq tensors [n,hk,wk,2], fuse.bias gradient [1] | None)."""
+    -> (list of 4 dpq tensors [n,hk,wk,2], fuse.bias gradient [1] | None).  ``void`` as passed to tail_fwd."""
     lib = nat.load()
     dev = out.device
     a = nat.TailLossBwdArgs()
-    a.flags = nat.FLAG_DETERMINISTIC if deterministic else 0
+    a.flags = (nat.FLAG_DETERMINISTIC if deterministic else 0) | (nat.FLAG_VOID_LABELS if void else 0)
     for k in range(5):
         a.logits[k] = out[k].data_ptr()
         a.loss_weights[k] = float(loss_weights[k])
@@ -697,6 +703,30 @@ def label_from_u8(masks, stats=None, out=None):
     _count()
     nat.check(lib.osvos_label_from_u8(x.data_ptr(), stats.data_ptr(), out.data_ptr(), n, h, w, _stream()),
               "osvos_label_from_u8")
+    return out
+
+
+def _id_object(obj):
+    """The native `object` argument of the id-map ingest: 0 for every object (None / "all"), else k in 1..254."""
+    if obj is None or obj == "all":
+        return 0
+    if isinstance(obj, bool) or not isinstance(obj, int) or not 1 <= obj <= 254:
+        raise ValueError(f"object must be None, 'all' or an object id in 1..254, got {obj!r}")
+    return obj
+
+
+def labels_from_ids(ids, object=None, out=None):
+    """DAVIS-2017 object-id maps uint8 [N,H,W] (0 background, 1..K objects, 255 void) -> fp32 labels [N,1,H,W]:
+    -1 for void, 1 for an object (any of 1..254 with ``object`` None / "all", only id ``object`` otherwise), else 0
+    (osvos_labels_from_ids).  The labels of the class-balanced loss's void form (OSVOS_FLAG_VOID_LABELS)."""
+    lib = nat.load()
+    x = _require_u8(ids, "ids", 3)
+    k = _id_object(object)
+    n, h, w = (int(v) for v in x.shape)
+    if out is None:
+        out = torch.empty((n, 1, h, w), dtype=torch.float32, device=x.device)
+    _count()
+    nat.check(lib.osvos_labels_from_ids(x.data_ptr(), out.data_ptr(), n, h, w, k, _stream()), "osvos_labels_from_ids")
     return out
 
 

@@ -70,10 +70,15 @@ class GraphedTrainStep:
 
     The graph keeps the kernels of the mode ``torch.are_deterministic_algorithms_enabled()`` had at capture; a replay
     under the other mode raises instead of silently running those.
+
+    ``void``: gt < 0 marks void pixels, left out of the fused objective (``OSVOS.forward_objective(void=True)``); only
+    with loss weights as the objective.
     """
 
-    def __init__(self, net, objective, sample, grad_scale=1.0, external_pack=False):
-        self.net, self.objective, self.grad_scale = net, objective, float(grad_scale)
+    def __init__(self, net, objective, sample, grad_scale=1.0, external_pack=False, void=False):
+        if void and callable(objective):
+            raise ValueError("GraphedTrainStep(void=True) needs the fused objective (a tuple of five loss weights)")
+        self.net, self.objective, self.grad_scale, self.void = net, objective, float(grad_scale), bool(void)
         self.deterministic = torch.are_deterministic_algorithms_enabled()
         self.x = sample["image"].detach().clone()
         self.gt = sample["gt"].detach().clone()
@@ -111,7 +116,7 @@ class GraphedTrainStep:
             # loss weights of the package's fused objective (tail + five losses = one kernel each way); grad_scale is
             # folded into the weights, so no scaling kernel runs either
             w = [float(v) * self.grad_scale for v in self.objective]
-            _, total, per_map = self.net.forward_objective(self.x, self.gt, w)
+            _, total, per_map = self.net.forward_objective(self.x, self.gt, w, void=self.void)
             with self.net._engine.direct_grad_accumulation():
                 total.backward()
             self.per_map = per_map
@@ -145,13 +150,13 @@ class GraphedTrainStep:
 
 
 def online_finetune(net, sample_fn, iters, n_ave_grad=5, lr=1e-8, wd=0.0002, log_every=0, log=print, use_graph=True,
-                    fused_optimizer=True, upsampling_lr=0.0):
+                    fused_optimizer=True, upsampling_lr=0.0, void=False):
     """`iters` forward/backward passes on the annotated frame, SGD step every `n_ave_grad` (reference
     train_online.py:112-149).  Losses are kept on the device; one host read per `log_every` iterations
     instead of the reference's per-iteration .item() sync.  With `use_graph` the fwd+loss+bwd of a micro-batch
     is a replayed CUDA graph (shapes must not change between iterations); with `fused_optimizer` the SGD step,
-    the gradient zeroing and the repack of the conv weights are one kernel (optim.FusedSGD).  Returns the list of
-    logged losses."""
+    the gradient zeroing and the repack of the conv weights are one kernel (optim.FusedSGD).  ``void``: gt < 0 marks
+    void pixels, left out of the loss.  Returns the list of logged losses."""
     net.train()
     opt = make_optimizer(net, "online", lr, wd, fused=fused_optimizer, upsampling_lr=upsampling_lr)
     opt.zero_grad()
@@ -164,7 +169,7 @@ def online_finetune(net, sample_fn, iters, n_ave_grad=5, lr=1e-8, wd=0.0002, log
         if use_graph:
             if step is None:
                 step = GraphedTrainStep(net, ONLINE_WEIGHTS, sample, grad_scale=1.0 / n_ave_grad,
-                                        external_pack=fused_optimizer)
+                                        external_pack=fused_optimizer, void=void)
             loss_val = step(sample)
             running = loss_val.clone() if running is None else running + loss_val
             if (it + 1) % n_ave_grad == 0:
@@ -176,7 +181,7 @@ def online_finetune(net, sample_fn, iters, n_ave_grad=5, lr=1e-8, wd=0.0002, log
                     step.zero_grads()
         else:
             # fuse-map loss only (train_online.py:127), 1/nAveGrad folded into the weight (train_online.py:140)
-            _, loss, per_map = net.forward_objective(inputs, gts, [v / n_ave_grad for v in ONLINE_WEIGHTS])
+            _, loss, per_map = net.forward_objective(inputs, gts, [v / n_ave_grad for v in ONLINE_WEIGHTS], void=void)
             running = per_map[4].clone() if running is None else running + per_map[4]
             with net._engine.direct_grad_accumulation():
                 loss.backward()
@@ -194,7 +199,7 @@ def online_finetune(net, sample_fn, iters, n_ave_grad=5, lr=1e-8, wd=0.0002, log
     return history
 
 
-def parent_epoch(net, opt, bucket, batches, epoch, n_epochs, n_ave_grad=1, group=None, state=None):
+def parent_epoch(net, opt, bucket, batches, epoch, n_epochs, n_ave_grad=1, group=None, state=None, void=False):
     """One epoch of the parent objective on this rank's shard: deep-supervision loss
     (1 - epoch/nEpochs) * sum_{k<4} L_k + L_fuse (train_parent.py:143-147), gradient accumulation over
     `n_ave_grad` local micro-batches, then ONE allreduce(mean) and one SGD step.
@@ -203,7 +208,8 @@ def parent_epoch(net, opt, bucket, batches, epoch, n_epochs, n_ave_grad=1, group
     parallel, lets rank skew accumulate; here the host only waits when it logs).
     `state`: a dict the caller keeps across epochs; it carries the accumulation counter, which the reference does NOT
     reset at epoch boundaries (`aveGrad`, train_parent.py:125,165-172) - leftover micro-batches of an epoch whose length
-    is not a multiple of nAveGrad complete their group in the next epoch instead of inflating its first step."""
+    is not a multiple of nAveGrad complete their group in the next epoch instead of inflating its first step.
+    ``void``: gt < 0 marks void pixels (DAVIS-2017's 255), left out of the five losses."""
     net.train()
     if state is None:
         state = {}
@@ -215,7 +221,7 @@ def parent_epoch(net, opt, bucket, batches, epoch, n_epochs, n_ave_grad=1, group
         # (1 - epoch/nEpochs) * sum(side losses) + fuse loss, / nAveGrad (train_parent.py:143-147,163), as the fused
         # objective: tail + five losses are one kernel forward and one backward
         w = [side_w / n_ave_grad] * 4 + [1.0 / n_ave_grad]
-        _, loss, per_map = net.forward_objective(sample["image"], sample["gt"], w)
+        _, loss, per_map = net.forward_objective(sample["image"], sample["gt"], w, void=void)
         totals += per_map
         count += 1
         with net._engine.direct_grad_accumulation():

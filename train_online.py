@@ -88,7 +88,16 @@ def parse(argv=None):
                          "and each pixel takes the object of the largest positive fused logit; the results are palette "
                          "PNGs of object ids (the first annotation's palette) and --evaluate scores every object. "
                          "Needs --loader native; K fine-tunes take K times as long")
+    ap.add_argument("--ignore-void", action="store_true",
+                    help="with --davis 2017: leave the annotation's void pixels (255) out of each object's fine-tuning "
+                         "loss instead of counting them as background. Needs a parent whose deconvolution weights are "
+                         "the bilinear taps (not one trained with --upsampling-lr)")
     a = ap.parse_args(argv)
+    if a.ignore_void and a.davis != "2017":
+        ap.error("--ignore-void applies to --davis 2017 (DAVIS-2016 annotations have no void pixels)")
+    if a.ignore_void and a.upsampling_lr != 0.0:
+        ap.error("--ignore-void trains with void labels, which the learned-upsampling tail does not support; it cannot "
+                 "be combined with a nonzero --upsampling-lr")
     if a.evaluate and (a.synthetic or a.loader != "native"):
         ap.error("--evaluate scores against the DAVIS annotations read by --loader native; it cannot be combined with "
                  + ("--synthetic" if a.synthetic else "--loader reference"))
@@ -314,6 +323,12 @@ def online_2017(a, parent, device, save_dir, iters, log_every):
     if k_objects < 1:
         raise SystemExit(f"sequence {a.seq_name}: the first annotation has no object")
     img_u8, ids_u8, _ = davis.upload(davis.collate([first]), device)
+    if a.ignore_void:                                # refused before any fine-tune starts, not at its first step
+        probe = vo.OSVOS(pretrained=0, precision=a.precision, verbose=False)
+        probe.load_state_dict(parent)
+        if probe._engine.uses_general_tail():
+            raise SystemExit("--ignore-void: the parent's deconvolution weights are not the bilinear taps, and void "
+                             "labels are not supported by the general tail they need")
     print(f"Start of Online Training, sequence: {a.seq_name}, {k_objects} object(s)")
     nets, history = [], []
     t0 = timeit.default_timer()
@@ -321,14 +336,18 @@ def online_2017(a, parent, device, save_dir, iters, log_every):
         net = vo.OSVOS(pretrained=0, precision=a.precision, learn_upsampling=a.upsampling_lr != 0.0)
         net.load_state_dict(parent)
         net.to(device)
-        gt_k = torch.where(ids_u8 == k, 255, 0).to(torch.uint8)          # the object's binary mask as 0 / 255 bytes
-        stats_k = ops.label_stats_u8(gt_k)
         rng = random.Random(a.seed)
+        if a.ignore_void:                            # id == k -> 1, 255 -> void, else 0 (the warp's id mode)
+            def sample_fn(it, k=k, rng=rng):
+                return augment.affine_warp_u8(img_u8, ids_u8, augment.draw_params(1, rng=rng), ids=k)
+        else:
+            gt_k = torch.where(ids_u8 == k, 255, 0).to(torch.uint8)      # the object's binary mask as 0 / 255 bytes
+            stats_k = ops.label_stats_u8(gt_k)
 
-        def sample_fn(it, gt_k=gt_k, stats_k=stats_k, rng=rng):
-            return augment.affine_warp_u8(img_u8, gt_k, augment.draw_params(1, rng=rng), stats_k)
+            def sample_fn(it, gt_k=gt_k, stats_k=stats_k, rng=rng):
+                return augment.affine_warp_u8(img_u8, gt_k, augment.draw_params(1, rng=rng), stats_k)
         hist = training.online_finetune(net, sample_fn, iters, a.n_ave_grad, a.lr, a.wd, log_every,
-                                        upsampling_lr=a.upsampling_lr)
+                                        upsampling_lr=a.upsampling_lr, void=a.ignore_void)
         if hist and not all(v == v and abs(v) != float("inf") for v in hist):
             print(f"WARNING: object {k}: non-finite loss - lower --lr for this initialisation")
         history.append(hist)

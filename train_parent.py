@@ -81,7 +81,18 @@ def parse(argv=None):
                          "nearest-resized annotations (network), or upsample the fused logits to each frame's stored "
                          "size on the device, as scipy 1.0's imresize(mode='F') does, and score them against the "
                          "original annotations (stored). The validation loss stays at the network resolution")
+    ap.add_argument("--davis", default="2016", choices=["2016", "2017"],
+                    help="2017: train on ImageSets/2017/train.txt with every object as foreground and void (255) pixels "
+                         "left out of the loss, validate on val.txt (--val-measures: J and F of the union of the "
+                         "objects, void ignored); needs --loader native")
     a = ap.parse_args(argv)
+    if a.davis == "2017":
+        if a.synthetic or a.loader != "native":
+            ap.error("--davis 2017 reads DAVIS-2017 with --loader native; it cannot be combined with "
+                     + ("--synthetic" if a.synthetic else "--loader reference"))
+        if a.upsampling_lr != 0.0:
+            ap.error("--davis 2017 trains with void labels, which the learned-upsampling tail does not support; it "
+                     "cannot be combined with a nonzero --upsampling-lr")
     if a.val_measures and (a.synthetic or a.loader != "native"):
         ap.error("--val-measures scores against the DAVIS annotations read by --loader native; it cannot be combined "
                  "with " + ("--synthetic" if a.synthetic else "--loader reference"))
@@ -123,6 +134,17 @@ def main(argv=None):
     bucket = parallel.GradientBucket(parallel.trainable_parameters(net), device)
 
     stored = False                                   # J and F at the stored size (--input-res --output-res stored)
+    void = a.davis == "2017"                         # DAVIS-2017: labels from object ids, void left out of the loss
+
+    def gt_label(gt, stats):
+        return ops.labels_from_ids(gt, "all") if void else ops.label_from_u8(gt, stats)
+
+    def measures(logits, gt_u8):
+        if not void:
+            return ops.davis_measures(logits, gt_u8)
+        # the union of the objects: the fused map > 0 against every object id (void, 255, kept and ignored)
+        union = torch.where(gt_u8 == 255, gt_u8, (gt_u8 != 0).to(torch.uint8))
+        return ops.davis_measures_objects((logits > 0).to(torch.uint8), union, 1)
     jpeg_status = None                               # --decode device, streaming: the decoder's status words, summed
     if a.synthetic:
         def epoch_batches(epoch):
@@ -139,9 +161,14 @@ def main(argv=None):
         from torch.utils.data import DataLoader
         from torch.utils.data.distributed import DistributedSampler
         from osvos_pytorch_b200 import davis
-        db_train = davis.DAVIS2016Frames(train=True, db_root_dir=Path.db_root_dir(), decode=a.decode)
+        if void:                                     # object ids: labels 1 (any object), 0, -1 (void)
+            db_train = davis.DAVIS2017Frames("train", db_root_dir=Path.db_root_dir(), decode=a.decode)
+            db_test = davis.DAVIS2017Frames("val", db_root_dir=Path.db_root_dir(), decode=a.decode)
+        else:
+            db_train = davis.DAVIS2016Frames(train=True, db_root_dir=Path.db_root_dir(), decode=a.decode)
+            db_test = davis.DAVIS2016Frames(train=False, db_root_dir=Path.db_root_dir(), decode=a.decode)
+        ids = "all" if void else False
         sampler = DistributedSampler(db_train, world, rank, shuffle=True, drop_last=True) if world > 1 else None
-        db_test = davis.DAVIS2016Frames(train=False, db_root_dir=Path.db_root_dir(), decode=a.decode)
         res = None if a.input_res is None else tuple(a.input_res)
         stored = res is not None and a.val_measures and a.output_res == "stored"
         if res is not None and rank == 0:
@@ -186,24 +213,24 @@ def main(argv=None):
                     with torch.cuda.device(device):
                         if not stored:
                             img, gt, stats = davis.upload(b, device, input_res=res, jpeg_status=jpeg_status)
-                            return {"image": ops.image_from_bgr8(img), "gt": ops.label_from_u8(gt, stats), "gt_u8": gt,
+                            return {"image": ops.image_from_bgr8(img), "gt": gt_label(gt, stats), "gt_u8": gt,
                                     "fname": b["fname"]}
                         # davis.upload, keeping the collated mask's view at the stored size
                         img0, gt0, _ = davis.device_views(b, device, jpeg_status)
                         img, gt = davis.resize_pair(img0, gt0, res)
                         stats = ops.label_stats_u8(gt)
-                        return {"image": ops.image_from_bgr8(img), "gt": ops.label_from_u8(gt, stats), "gt_u8": gt,
+                        return {"image": ops.image_from_bgr8(img), "gt": gt_label(gt, stats), "gt_u8": gt,
                                 "gt_u8_stored": gt0, "fname": b["fname"]}
                 val_batches = _Mapped(val_loader, val_item)
             else:
                 val_batches = _Mapped(val_loader, lambda b: davis.to_device(b, device, input_res=res,
-                                                                            jpeg_status=jpeg_status))
+                                                                            jpeg_status=jpeg_status, ids=ids))
 
             def epoch_batches(epoch):
                 if sampler is not None:
                     sampler.set_epoch(epoch)
                 for b in loader:      # flip / rotation / scale drawn from Python's random, as the reference's transforms do
-                    yield davis.to_device(b, device, augment=random, input_res=res, jpeg_status=jpeg_status)
+                    yield davis.to_device(b, device, augment=random, input_res=res, jpeg_status=jpeg_status, ids=ids)
     else:
         from dataloaders import davis_2016 as db
         from dataloaders import custom_transforms as tr
@@ -231,7 +258,8 @@ def main(argv=None):
     loop_state = {}                                  # accumulation counter, carried across epochs as in the reference
     for epoch in range(a.resume_epoch, a.epochs):
         t0 = timeit.default_timer()
-        losses = training.parent_epoch(net, opt, bucket, epoch_batches(epoch), epoch, a.epochs, n_ave, state=loop_state)
+        losses = training.parent_epoch(net, opt, bucket, epoch_batches(epoch), epoch, a.epochs, n_ave, state=loop_state,
+                                       void=void)
         torch.cuda.synchronize()
         if jpeg_status is not None and int(jpeg_status) != 0:     # read after the epoch's synchronisation
             print(f"WARNING: rank {rank}: the device JPEG decoder flagged corrupt or cut-short frames in epoch {epoch} "
@@ -250,13 +278,14 @@ def main(argv=None):
                 for s in val_batches:
                     outs = net.forward(s["image"].to(device))
                     tot += torch.stack([training.class_balanced_cross_entropy_loss(o, s["gt"].to(device),
-                                                                                   size_average=False) for o in outs])
+                                                                                   size_average=False, void=void)
+                                        for o in outs])
                     if a.val_measures:
                         if stored:                   # the fused map at the annotation's own size (DESIGN.md §18)
                             g0 = s["gt_u8_stored"]
-                            counts = ops.davis_measures(ops.resize_f32(outs[-1], g0.shape[1:]), g0)
+                            counts = measures(ops.resize_f32(outs[-1], g0.shape[1:]), g0)
                         else:
-                            counts = ops.davis_measures(outs[-1], s["gt_u8"])
+                            counts = measures(outs[-1], s["gt_u8"])
                         for i, fname in enumerate(s["fname"]):
                             per_seq.setdefault(fname.split("/")[0], evaluation.SequenceScores()).add(counts[i:i + 1])
             print("***Testing *** " + " ".join(f"Loss {k}: {v:.4f}" for k, v in enumerate((tot / len(val_batches)).tolist())))
