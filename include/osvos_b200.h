@@ -595,6 +595,23 @@ OSVOS_API int osvos_davis_measures_objects(const uint8_t* labels, const uint8_t*
                                            int k, int h, int w, int r, osvos_stream_t stream);
 OSVOS_API int osvos_merge_objects(const float* const* maps, int k, uint8_t* out, size_t pixels, osvos_stream_t stream);
 
+/* ---- reduced-resolution DAVIS-2017: per-object upsample fused with the merge (DESIGN.md §27) ---------------------
+ *   osvos_upsample_merge_objects: `maps` (host array of k device pointers, each to fp32 [n][h][w], 4-byte aligned) ->
+ *                         out [n][out_h][out_w] uint8 (any alignment), bit-identical to osvos_merge_objects of the k maps
+ *                         each resized by osvos_resize_f32 to out_h x out_w, without the resized maps: two launches (the
+ *                         coefficient tables, then one tile kernel that stages each map's horizontal pass in shared memory
+ *                         and keeps the running argmax in registers), one when the sizes are equal (a plain merge).
+ *                         1 <= k <= OSVOS_MERGE_MAX_OBJECTS, n < 65536, h, w, out_h, out_w < 32768.  A vertical downscale
+ *                         too steep to stage one output row's source rows, 128 columns of doubles each, in 48 KiB of
+ *                         shared memory is refused (status 1): min(h, 2 * ceil(h / out_h) + 3) > 48, i.e. h / out_h > 22.
+ *                         `workspace`: osvos_upsample_merge_objects_workspace_bytes(...) bytes (the tables), 8-byte
+ *                         aligned, owned by the caller (may be NULL when that is 0); nothing is allocated and nothing
+ *                         waits for the host.
+ *   osvos_upsample_merge_objects_workspace_bytes: host query; 0 for equal sizes and for invalid or refused arguments. */
+OSVOS_API size_t osvos_upsample_merge_objects_workspace_bytes(int n, int k, int h, int w, int out_h, int out_w);
+OSVOS_API int osvos_upsample_merge_objects(const float* const* maps, int k, uint8_t* out, void* workspace, int n, int h,
+                                           int w, int out_h, int out_w, osvos_stream_t stream);
+
 /* ---- baseline JPEG decode, bit-identical to cv2.imread (libjpeg-turbo; DESIGN.md §19) ----------------------------
  *   osvos_jpeg_decode: a batch of n JPEGs of one size h x w, packed by osvos_pytorch_b200.jpeg.pack into `blob`
  *                      (blob_bytes bytes, 16-byte aligned; headers, tables and de-stuffed entropy-coded segments) ->

@@ -241,6 +241,9 @@ SIGNATURES = {
     "osvos_png_encode_palette": (c_int, [c_void_p, c_char_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                          c_void_p]),
     "osvos_merge_objects": (c_int, [POINTER(c_void_p), c_int, c_void_p, c_size_t, c_void_p]),
+    "osvos_upsample_merge_objects_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int, c_int]),
+    "osvos_upsample_merge_objects": (c_int, [POINTER(c_void_p), c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                             c_int, c_void_p]),
     "osvos_davis_measures_objects_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "osvos_davis_measures_objects": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                              c_void_p]),

@@ -10,6 +10,7 @@
 //                The loop runs from d = 0 outwards and stops once every boundary bit of the word is matched.
 // Counts are reduced per block (warp shuffles, then shared memory) and added with one atomicAdd per block and count.
 #include "common.cuh"
+#include "merge.cuh"
 
 namespace osvos {
 
@@ -275,10 +276,6 @@ extern "C" int osvos_davis_measures_objects(const uint8_t* labels, const uint8_t
 // ---- merge of per-object fused maps (DESIGN.md §24) ------------------------------------------------------------------
 
 namespace osvos {
-
-struct MergeMaps {
-  const float* map[OSVOS_MERGE_MAX_OBJECTS];
-};
 
 // label = 1 + the first k of the largest logit if that logit is > 0, else 0: `best` starts at +0 and only a strictly
 // larger value replaces it, so ±0 and NaN never win and ties go to the lowest k.  Four pixels per thread; float4 loads

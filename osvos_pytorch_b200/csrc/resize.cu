@@ -16,7 +16,10 @@
 // The fp32 resize (osvos_resize_f32, DESIGN.md §18) upsamples fused logit maps to the annotations' stored size: Pillow's
 // BILINEAR resize of an 'F' image (scipy 1.0's imresize(mode='F')), the same tables kept in double and accumulated in
 // double, with an fp32 intermediate between the passes.
+// osvos_upsample_merge_objects (DESIGN.md §27) is that fp32 resize of K maps followed by osvos_merge_objects, in one
+// tile kernel that keeps the intermediate in shared memory and the running argmax in registers.
 #include "common.cuh"
+#include "merge.cuh"
 
 namespace osvos {
 
@@ -346,6 +349,193 @@ int launch_resize_f32(const float* src, float* dst, uint8_t* ws, const ResizeF32
   return OSVOS_OK;
 }
 
+// ---- fp32 resize of K maps fused with their merge (DESIGN.md §27) ----------------------------------------------------
+// labels = osvos_merge_objects({osvos_resize_f32(map_k -> out_h x out_w)}_k), bit for bit, without the K resized maps.
+// A CTA owns kUmTileCols output columns x tile_h output rows of one frame.  For each k it stages, in shared memory, the
+// rows [r0, r1) of the horizontal pass's fp32 intermediate that the tile's vertical taps read (resize_f32_horizontal_
+// kernel's arithmetic for the tile's columns only; without a horizontal pass, the source values), each held as the
+// double of its fp32 value, which is what the vertical pass converts it to.  Each thread then forms its pixels'
+// vertical sums (resize_f32_vertical_kernel's; without a vertical pass, the staged value of its own row), rounds them
+// to fp32 and updates a running best / label in registers exactly as merge_objects_kernel does.  Labels are written
+// once.  The pass structure is the composition's (same passes, same tap order, same roundings), so no value, ±0 and
+// NaN included, differs from what the merge would read.
+constexpr int kUmThreads = 256;
+constexpr int kUmTileCols = 128;                                 // one column per thread, two row phases
+constexpr int kUmRowsPerThread = 8;
+constexpr int kUmMaxTileRows = kUmRowsPerThread * (kUmThreads / kUmTileCols);
+constexpr size_t kUmMaxStageBytes = 48 * 1024;                   // no opt-in needed on any device
+
+// T = 3: every axis has at most 3 taps (any upsample): the taps are unrolled, each thread keeps its column's horizontal
+// weights in registers, and the tile's vertical bounds and weights are read once into shared memory.  T = 0: any
+// count, read from the tables as they are used.
+template <bool H, bool V, int T>
+__global__ void __launch_bounds__(kUmThreads, 4)
+upsample_merge_objects_kernel(MergeMaps maps, int nobj, uint8_t* __restrict__ out, const int* __restrict__ hbounds,
+                              const double* __restrict__ hk, int kh, const int* __restrict__ vbounds,
+                              const double* __restrict__ vk, int kv, int h, int w, int out_h, int out_w, int tile_h) {
+  extern __shared__ double stage[];                              // [rows][kUmTileCols]
+  __shared__ double vw_s[T > 0 ? kUmMaxTileRows * T : 1];        // T > 0: the tile's vertical weights, 0 past count
+  __shared__ int vmin_s[T > 0 ? kUmMaxTileRows : 1], vcnt_s[T > 0 ? kUmMaxTileRows : 1];
+  const int f = blockIdx.z;
+  const int c = threadIdx.x % kUmTileCols;
+  const int phase = threadIdx.x / kUmTileCols;
+  const int xo = blockIdx.x * kUmTileCols + c;
+  const int y0 = blockIdx.y * tile_h;
+  const int y1 = min(y0 + tile_h, out_h);
+  // source rows of the tile: from the first output's xmin to the largest xmin + count (Pillow's ybox per tile)
+  int r0 = y0, r1 = y1;
+  if (V) {
+    r0 = __ldg(vbounds + 2 * y0);
+    r1 = r0;
+    for (int y = y0; y < y1; ++y) r1 = max(r1, __ldg(vbounds + 2 * y) + __ldg(vbounds + 2 * y + 1));
+    if (T > 0) {
+      for (int i = threadIdx.x; i < (y1 - y0) * T; i += kUmThreads) {
+        const int yo = y0 + i / T, t = i % T;
+        const int cnt = __ldg(vbounds + 2 * yo + 1);
+        vw_s[i] = t < cnt ? __ldg(vk + static_cast<size_t>(yo) * kv + t) : 0.0;
+        if (t == 0) {
+          vmin_s[i / T] = __ldg(vbounds + 2 * yo) - r0;
+          vcnt_s[i / T] = cnt;
+        }
+      }
+    }
+  }
+  const int rows = r1 - r0;
+  int hx = xo, hcnt = 1;
+  if (H && xo < out_w) {
+    hx = __ldg(hbounds + 2 * xo);
+    hcnt = __ldg(hbounds + 2 * xo + 1);
+  }
+  const double* hrow = hk + static_cast<size_t>(xo) * kh;
+  double hw[T > 0 ? T : 1];
+#pragma unroll
+  for (int t = 0; t < (T > 0 ? T : 1); ++t) hw[t] = (T > 0 && H && xo < out_w && t < hcnt) ? __ldg(hrow + t) : 0.0;
+  float best[kUmRowsPerThread];
+  uint32_t lab[kUmRowsPerThread];
+#pragma unroll
+  for (int j = 0; j < kUmRowsPerThread; ++j) {
+    best[j] = 0.f;
+    lab[j] = 0;
+  }
+  for (int k = 0; k < nobj; ++k) {
+    const float* src = maps.map[k] + (static_cast<size_t>(f) * h + r0) * w;
+    __syncthreads();                                             // the previous map's stage has been read
+    if (xo < out_w) {
+#pragma unroll 2
+      for (int r = phase; r < rows; r += kUmThreads / kUmTileCols) {
+        const float* s = src + static_cast<size_t>(r) * w + hx;
+        float v;
+        if (H) {
+          double ss = 0.0;
+          if (T > 0) {
+#pragma unroll
+            for (int t = 0; t < T; ++t)
+              if (t < hcnt) ss = __dadd_rn(ss, __dmul_rn(static_cast<double>(__ldg(s + t)), hw[t]));
+          } else {
+            for (int t = 0; t < hcnt; ++t)
+              ss = __dadd_rn(ss, __dmul_rn(static_cast<double>(__ldg(s + t)), __ldg(hrow + t)));
+          }
+          v = __double2float_rn(ss);
+        } else {
+          v = __ldg(s);
+        }
+        stage[r * kUmTileCols + c] = static_cast<double>(v);
+      }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int j = 0; j < kUmRowsPerThread; ++j) {
+      const int yo = y0 + phase + j * (kUmThreads / kUmTileCols);
+      if (yo < y1 && xo < out_w) {
+        float v;
+        if (V) {
+          double ss = 0.0;
+          if (T > 0) {
+            const int jj = yo - y0, ymin = vmin_s[jj], cnt = vcnt_s[jj];
+#pragma unroll
+            for (int t = 0; t < T; ++t)
+              if (t < cnt) ss = __dadd_rn(ss, __dmul_rn(stage[(ymin + t) * kUmTileCols + c], vw_s[jj * T + t]));
+          } else {
+            const int ymin = __ldg(vbounds + 2 * yo) - r0, cnt = __ldg(vbounds + 2 * yo + 1);
+            const double* kk = vk + static_cast<size_t>(yo) * kv;
+            for (int t = 0; t < cnt; ++t)
+              ss = __dadd_rn(ss, __dmul_rn(stage[(ymin + t) * kUmTileCols + c], __ldg(kk + t)));
+          }
+          v = __double2float_rn(ss);
+        } else {
+          v = static_cast<float>(stage[(yo - r0) * kUmTileCols + c]);    // exact: the staged fp32 value
+        }
+        if (v > best[j]) {                                       // ±0 and NaN never win, ties keep the lowest k
+          best[j] = v;
+          lab[j] = k + 1;
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < kUmRowsPerThread; ++j) {
+    const int yo = y0 + phase + j * (kUmThreads / kUmTileCols);
+    if (yo < y1 && xo < out_w) out[(static_cast<size_t>(f) * out_h + yo) * out_w + xo] = static_cast<uint8_t>(lab[j]);
+  }
+}
+
+// Source rows a tile of `tile_h` output rows can read along an axis of `in` -> `out` samples with ksize `k`: the
+// centers of its first and last outputs lie (tile_h - 1) * scale apart, and each output reads [xmin, xmin + count)
+// with xmin > center - support - 1/2 and xmin + count <= center + support + 1/2, support <= (k - 1) / 2.  One row more
+// covers the rounding of the centers.
+inline int upsample_merge_stage_rows(int in, int out, int k, int tile_h, bool need_v) {
+  if (!need_v) return tile_h;
+  const double scale = static_cast<double>(in) / out;
+  const double span = floor((tile_h - 1) * scale) + k + 2;
+  return static_cast<int>(span < in ? span : in);
+}
+
+struct UpsampleMergePlan {
+  ResizeF32Plan tables;    // the fp32 resize's tables; its intermediate is not used
+  int tile_h;              // 0: even a 1-row tile cannot be staged
+  size_t smem;
+};
+
+UpsampleMergePlan upsample_merge_plan(int n, int h, int w, int out_h, int out_w) {
+  UpsampleMergePlan p{};
+  p.tables = resize_f32_plan(n, h, w, out_h, out_w);
+  p.tables.bytes = p.tables.tmp_off;
+  for (int t = kUmMaxTileRows; t >= 1 && p.tile_h == 0; t /= 2) {
+    const size_t smem = sizeof(double) * kUmTileCols *
+                        static_cast<size_t>(upsample_merge_stage_rows(h, out_h, p.tables.kv, t, p.tables.need_v));
+    if (smem <= kUmMaxStageBytes) {
+      p.tile_h = t;
+      p.smem = smem;
+    }
+  }
+  return p;
+}
+
+template <bool H, bool V>
+int launch_upsample_merge(const MergeMaps& m, int nobj, uint8_t* out, uint8_t* ws, const UpsampleMergePlan& p, int n,
+                          int h, int w, int out_h, int out_w, cudaStream_t stream) {
+  const ResizeF32Plan& t = p.tables;
+  int* hbounds = reinterpret_cast<int*>(ws);
+  int* vbounds = reinterpret_cast<int*>(ws + t.vbounds_off);
+  double* hk = reinterpret_cast<double*>(ws + t.hk_off);
+  double* vk = reinterpret_cast<double*>(ws + t.vk_off);
+  const ResizeAxisF64 ax{hbounds, hk, w, H ? out_w : 0, t.kh};
+  const ResizeAxisF64 ay{vbounds, vk, h, V ? out_h : 0, t.kv};
+  resize_f32_tables_kernel<<<(ax.out + ay.out + 127) / 128, 128, 0, stream>>>(ax, ay);
+  OSVOS_CHECK_CUDA(cudaGetLastError());
+  const dim3 grid((out_w + kUmTileCols - 1) / kUmTileCols, (out_h + p.tile_h - 1) / p.tile_h, n);
+  if (t.kh <= 3 && t.kv <= 3)                                    // an upsample (or a kept size) along both axes
+    upsample_merge_objects_kernel<H, V, 3><<<grid, kUmThreads, p.smem, stream>>>(m, nobj, out, hbounds, hk, t.kh,
+                                                                                 vbounds, vk, t.kv, h, w, out_h, out_w,
+                                                                                 p.tile_h);
+  else
+    upsample_merge_objects_kernel<H, V, 0><<<grid, kUmThreads, p.smem, stream>>>(m, nobj, out, hbounds, hk, t.kh,
+                                                                                 vbounds, vk, t.kv, h, w, out_h, out_w,
+                                                                                 p.tile_h);
+  OSVOS_CHECK_CUDA(cudaGetLastError());
+  return OSVOS_OK;
+}
+
 }  // namespace osvos
 
 using namespace osvos;
@@ -393,4 +583,32 @@ extern "C" int osvos_resize_f32(const float* src, float* dst, void* workspace, i
     return OSVOS_OK;
   }
   return launch_resize_f32(src, dst, static_cast<uint8_t*>(workspace), p, n, h, w, out_h, out_w, stream);
+}
+
+extern "C" size_t osvos_upsample_merge_objects_workspace_bytes(int n, int k, int h, int w, int out_h, int out_w) {
+  if (!resize_dims_ok(n, h, w, 1, out_h, out_w, OSVOS_RESIZE_BILINEAR) || k < 1 || k > OSVOS_MERGE_MAX_OBJECTS) return 0;
+  const UpsampleMergePlan p = upsample_merge_plan(n, h, w, out_h, out_w);
+  return p.tile_h == 0 ? 0 : p.tables.bytes;
+}
+
+extern "C" int osvos_upsample_merge_objects(const float* const* maps, int k, uint8_t* out, void* workspace, int n, int h,
+                                            int w, int out_h, int out_w, osvos_stream_t stream_) {
+  OSVOS_CHECK_ARG(maps != nullptr && out != nullptr);
+  OSVOS_CHECK_ARG(k >= 1 && k <= OSVOS_MERGE_MAX_OBJECTS);
+  OSVOS_CHECK_ARG(resize_dims_ok(n, h, w, 1, out_h, out_w, OSVOS_RESIZE_BILINEAR));
+  MergeMaps m{};
+  for (int i = 0; i < k; ++i) {
+    OSVOS_CHECK_ARG(maps[i] != nullptr && (reinterpret_cast<uintptr_t>(maps[i]) & 3) == 0);
+    m.map[i] = maps[i];
+  }
+  const UpsampleMergePlan p = upsample_merge_plan(n, h, w, out_h, out_w);
+  OSVOS_CHECK_ARG(p.tile_h > 0);                        // a downscale too steep to stage one output row
+  const bool need_h = p.tables.need_h, need_v = p.tables.need_v;
+  if (!need_h && !need_v) return osvos_merge_objects(maps, k, out, static_cast<size_t>(n) * h * w, stream_);
+  OSVOS_CHECK_ARG(workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 7) == 0);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  if (need_h && need_v) return launch_upsample_merge<true, true>(m, k, out, ws, p, n, h, w, out_h, out_w, stream);
+  if (need_h) return launch_upsample_merge<true, false>(m, k, out, ws, p, n, h, w, out_h, out_w, stream);
+  return launch_upsample_merge<false, true>(m, k, out, ws, p, n, h, w, out_h, out_w, stream);
 }

@@ -64,8 +64,12 @@ class SequenceSegmenter:
     the slot's uint8 label map (1 + the object of the largest positive logit, 0 background), so each result is uint8
     [N,1,H,W] of object ids.  ``score=True`` scores it with ops.davis_measures_objects against the slot's annotation
     (object ids, 255 void) and ``frame_counts()`` returns [frames*N, K, 6].  ``encode="png"`` with ``palette`` (the
-    PLTE bytes, e.g. the first annotation's) writes palette files.  ``input_res``, ``output_res="stored"`` and
-    ``overlay`` are not available with labels."""
+    PLTE bytes, e.g. the first annotation's) writes palette files.  With ``input_res`` labels need
+    ``output_res="stored"`` (DESIGN.md §27): the K forwards run on the resized slot and ops.upsample_merge_objects
+    writes the stored-size label map straight from the K fused maps (each upsampled as ops.resize_f32 does, then
+    merged; an argmax cannot be upsampled after the merge), so results, scores against the original annotations and
+    palette files are at the stored size.  A label map at the network resolution is not what the DAVIS-2017 toolkit
+    scores, so labels with ``input_res`` and ``output_res="network"`` are refused, as is ``overlay`` with labels."""
 
     def __init__(self, net=None, output="logits", depth=3, frames="nchw_f32", meanval=ops.MEANVAL, score=False,
                  input_res=None, output_res="network", encode=None, overlay=None, overlay_quality=95, nets=None,
@@ -79,8 +83,9 @@ class SequenceSegmenter:
             raise ValueError("output must be one of logits / bytescale / prob / mask / labels")
         if len(nets) > 1 and output != "labels":
             raise ValueError("several nets are merged into a label map: they need output='labels'")
-        if output == "labels" and (input_res is not None or output_res != "network" or overlay is not None):
-            raise ValueError("output='labels' does not take input_res, output_res='stored' or overlay")
+        if output == "labels" and ((input_res is not None and output_res != "stored") or overlay is not None):
+            raise ValueError("output='labels' writes label maps at the stored size: with input_res it needs "
+                             "output_res='stored', and it does not take overlay")
         if palette is not None and (output != "labels" or encode != "png"):
             raise ValueError("palette writes label maps as palette PNGs: it needs output='labels' and encode='png'")
         if frames not in ("nchw_f32", "bgr8", "jpeg"):
@@ -143,7 +148,7 @@ class SequenceSegmenter:
             self._dev_jlen = [torch.empty(n, dtype=torch.int64, device=device) for _ in range(self.depth)]
             self._host_jpg = [torch.empty((n, ocap), dtype=torch.uint8).pin_memory() for _ in range(self.depth)]
             self._host_jlen = [torch.empty(n, dtype=torch.int64).pin_memory() for _ in range(self.depth)]
-        if self._upsample:
+        if self._upsample and self.output != "labels":     # labels are upsampled inside the merge
             self._dev_up = [torch.empty((n, 1, h0, w0), dtype=torch.float32, device=device) for _ in range(self.depth)]
         if self.score:
             self._dev_gt = [torch.empty((n, h0, w0), dtype=torch.uint8, device=device) for _ in range(self.depth)]
@@ -216,10 +221,13 @@ class SequenceSegmenter:
                 else:
                     fused_maps.append(net(self._dev_in[k])[-1])
             fused = fused_maps[0]
-            if self._upsample:                                  # back to the stored size, before anything reads it
+            if self._upsample and self.output != "labels":     # back to the stored size, before anything reads it
                 fused = ops.resize_f32(fused, self._dev_up[k].shape[2:4], out=self._dev_up[k])
             if self.output == "labels":
-                labels = ops.merge_objects(fused_maps, out=self._dev_out[k])
+                if self._upsample:                              # each object's map upsampled, then merged
+                    labels = ops.upsample_merge_objects(fused_maps, self._dev_out[k].shape[2:4], out=self._dev_out[k])
+                else:
+                    labels = ops.merge_objects(fused_maps, out=self._dev_out[k])
                 if self.score:
                     self._counts.append(ops.davis_measures_objects(labels, gt_dev, len(self.nets)))
             elif self.score:

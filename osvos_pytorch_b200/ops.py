@@ -867,16 +867,12 @@ def davis_measures(logits, gt_u8, r=None, out=None):
     return out
 
 
-def merge_objects(maps, out=None):
-    """Per-object fused logit maps -> uint8 label map [N,H,W] (csrc/measures.cu, DESIGN.md §24): label = 1 + argmax_k
-    logit_k where that maximum is > 0, else 0; ties go to the lowest k, NaN never wins and ±0 is background.  ``maps``:
-    a list of K fp32 tensors of one shape [N,1,H,W] or [N,H,W], or one fp32 tensor [K,N,1,H,W] / [K,N,H,W];
-    1 <= K <= 254.  ``out`` may be any contiguous uint8 [N,H,W] tensor (e.g. a view of a [N,1,H,W] buffer), at any
-    alignment.  No host synchronisation."""
-    lib = nat.load()
+def _object_maps(maps, name):
+    """The K contiguous fp32 maps of merge_objects / upsample_merge_objects: a list of K tensors of one shape
+    [N,1,H,W] or [N,H,W] on one CUDA device, or one tensor [K,N,1,H,W] / [K,N,H,W]; 1 <= K <= 254."""
     items = list(maps.unbind(0)) if torch.is_tensor(maps) else list(maps)
     if not 1 <= len(items) <= nat.DAVIS_MAX_OBJECTS:
-        raise ValueError(f"merge_objects takes 1 .. {nat.DAVIS_MAX_OBJECTS} maps, got {len(items)}")
+        raise ValueError(f"{name} takes 1 .. {nat.DAVIS_MAX_OBJECTS} maps, got {len(items)}")
     shape = tuple(items[0].shape)
     if len(shape) not in (3, 4) or (len(shape) == 4 and shape[1] != 1):
         raise ValueError(f"maps must be fp32 [N,1,H,W] or [N,H,W], got {shape}")
@@ -886,7 +882,18 @@ def merge_objects(maps, out=None):
         if t.dtype != torch.float32 or tuple(t.shape) != shape or t.device != items[0].device:
             raise ValueError(f"every map must be fp32 {shape} on one device, got {t.dtype} {tuple(t.shape)}")
         keep.append(t.detach().contiguous())
-    n, h, w = shape[0], shape[-2], shape[-1]
+    return keep
+
+
+def merge_objects(maps, out=None):
+    """Per-object fused logit maps -> uint8 label map [N,H,W] (csrc/measures.cu, DESIGN.md §24): label = 1 + argmax_k
+    logit_k where that maximum is > 0, else 0; ties go to the lowest k, NaN never wins and ±0 is background.  ``maps``:
+    a list of K fp32 tensors of one shape [N,1,H,W] or [N,H,W], or one fp32 tensor [K,N,1,H,W] / [K,N,H,W];
+    1 <= K <= 254.  ``out`` may be any contiguous uint8 [N,H,W] tensor (e.g. a view of a [N,1,H,W] buffer), at any
+    alignment.  No host synchronisation."""
+    lib = nat.load()
+    keep = _object_maps(maps, "merge_objects")
+    n, h, w = int(keep[0].shape[0]), int(keep[0].shape[-2]), int(keep[0].shape[-1])
     if out is None:
         out = torch.empty((n, h, w), dtype=torch.uint8, device=keep[0].device)
     elif out.dtype != torch.uint8 or out.numel() != n * h * w or not out.is_contiguous():
@@ -894,6 +901,34 @@ def merge_objects(maps, out=None):
     ptrs = (c_void_p * len(keep))(*(t.data_ptr() for t in keep))
     _count()
     nat.check(lib.osvos_merge_objects(ptrs, len(keep), out.data_ptr(), n * h * w, _stream()), "osvos_merge_objects")
+    return out
+
+
+def upsample_merge_objects(maps, size, out=None):
+    """Per-object fused logit maps at the network resolution -> uint8 label map [N, h', w'] at ``size`` = (h', w')
+    (csrc/resize.cu, DESIGN.md §27): bit-identical to merge_objects([resize_f32(m, size) for m in maps]), in two
+    launches whatever K (one for equal sizes) and without the K resized maps.  ``maps`` as merge_objects';
+    ``out`` may be any contiguous uint8 tensor of N * h' * w' elements, at any alignment.  A vertical downscale by more
+    than about 22 is refused.  No host synchronisation."""
+    lib = nat.load()
+    keep = _object_maps(maps, "upsample_merge_objects")
+    n, h, w = int(keep[0].shape[0]), int(keep[0].shape[-2]), int(keep[0].shape[-1])
+    oh, ow = (int(v) for v in size)
+    if not (0 < n < 65536 and all(0 < v < 32768 for v in (h, w, oh, ow))):
+        raise ValueError(f"cannot resize [{n},{h},{w}] to ({oh}, {ow}): sizes must lie in [1, 32767] and N < 65536")
+    nbytes = lib.osvos_upsample_merge_objects_workspace_bytes(n, len(keep), h, w, oh, ow)
+    if nbytes == 0 and (oh, ow) != (h, w):
+        raise ValueError(f"cannot resize [{n},{h},{w}] to ({oh}, {ow}) in upsample_merge_objects: a vertical downscale "
+                         "by more than about 22 is not supported")
+    if out is None:
+        out = torch.empty((n, oh, ow), dtype=torch.uint8, device=keep[0].device)
+    elif out.dtype != torch.uint8 or out.numel() != n * oh * ow or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous uint8 tensor of {n * oh * ow} elements, e.g. [{n},{oh},{ow}]")
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=keep[0].device) if nbytes else None
+    ptrs = (c_void_p * len(keep))(*(t.data_ptr() for t in keep))
+    _count(1 if (oh, ow) == (h, w) else 2)
+    nat.check(lib.osvos_upsample_merge_objects(ptrs, len(keep), out.data_ptr(), nat.ptr(ws), n, h, w, oh, ow, _stream()),
+              "osvos_upsample_merge_objects")
     return out
 
 

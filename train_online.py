@@ -6,6 +6,7 @@ first frame with SGD(lr 1e-8, momentum .9), save the weights, then segment the s
     SEQ_NAME=blackswan python train_online.py --loader native # DAVIS on disk (needs cv2 + the dataset)
     SEQ_NAME=blackswan python train_online.py --loader native --evaluate   # ... and score the masks (J and F)
     SEQ_NAME=dogs-jump python train_online.py --loader native --davis 2017 --evaluate   # DAVIS-2017, one net per object
+    SEQ_NAME=dogs-jump python train_online.py --loader native --davis 2017 --input-res 240 427 --output-res stored
     SEQ_NAME=blackswan python train_online.py                 # the same through the reference's dataloaders package
     python train_online.py --synthetic --iters 200            # synthetic 480x854 frame, no dataset
 
@@ -66,12 +67,15 @@ def parse(argv=None):
     ap.add_argument("--input-res", type=int, nargs=2, default=None, metavar=("H", "W"),
                     help="the reference's inputRes: resize every frame (bilinear) and annotation (nearest) to H x W on "
                          "the device before training, segmentation and scoring, as scipy 1.0's imresize does. Needs "
-                         "--loader native (--synthetic has --height / --width)")
+                         "--loader native (--synthetic has --height / --width); with --davis 2017 it needs "
+                         "--output-res stored")
     ap.add_argument("--output-res", default="network", choices=["network", "stored"],
                     help="with --input-res: write (and with --evaluate score) the masks at the network resolution H x W "
                          "(network), or at each frame's stored size (stored): the fused logits are upsampled on the "
                          "device as scipy 1.0's imresize(mode='F') does and scored against the original annotations, "
-                         "so the PNGs and J / F compare with the DAVIS-2016 benchmark's")
+                         "so the PNGs and J / F compare with the DAVIS-2016 benchmark's. With --davis 2017 each "
+                         "object's logits are upsampled and then merged into the stored-size label map in one kernel "
+                         "(ops.upsample_merge_objects). Without --input-res it changes nothing")
     ap.add_argument("--encode", default="host", choices=["host", "device"],
                     help="write the result PNGs with Pillow on the host (host), or encode them on the GPU "
                          "(device: SequenceSegmenter(encode='png'); the bytes are written as they come, no Pillow)")
@@ -87,7 +91,8 @@ def parse(argv=None):
                          "per object on the first frame with that object's mask, every frame goes through the K nets "
                          "and each pixel takes the object of the largest positive fused logit; the results are palette "
                          "PNGs of object ids (the first annotation's palette) and --evaluate scores every object. "
-                         "Needs --loader native; K fine-tunes take K times as long")
+                         "Needs --loader native; K fine-tunes take K times as long. --input-res H W --output-res stored "
+                         "fine-tunes and segments at H x W and writes and scores the label maps at the stored size")
     ap.add_argument("--ignore-void", action="store_true",
                     help="with --davis 2017: leave the annotation's void pixels (255) out of each object's fine-tuning "
                          "loss instead of counting them as background. Needs a parent whose deconvolution weights are "
@@ -116,8 +121,8 @@ def parse(argv=None):
         if a.synthetic or a.loader != "native":
             ap.error("--davis 2017 reads the sequence with --loader native; it cannot be combined with "
                      + ("--synthetic" if a.synthetic else "--loader reference"))
-        if a.input_res is not None:
-            ap.error("--davis 2017 writes label maps at the stored size: --input-res does not apply")
+        if a.input_res is not None and a.output_res != "stored":
+            ap.error("--davis 2017 writes label maps at the stored size: --input-res needs --output-res stored")
     return a
 
 
@@ -322,7 +327,9 @@ def online_2017(a, parent, device, save_dir, iters, log_every):
     k_objects, palette = first["n_objects"], first_ds.palettes[a.seq_name]
     if k_objects < 1:
         raise SystemExit(f"sequence {a.seq_name}: the first annotation has no object")
-    img_u8, ids_u8, _ = davis.upload(davis.collate([first]), device)
+    input_res = None if a.input_res is None else tuple(a.input_res)
+    # the image bilinear, the id map nearest (ids survive): every object fine-tunes at the network resolution
+    img_u8, ids_u8, _ = davis.upload(davis.collate([first]), device, input_res=input_res)
     if a.ignore_void:                                # refused before any fine-tune starts, not at its first step
         probe = vo.OSVOS(pretrained=0, precision=a.precision, verbose=False)
         probe.load_state_dict(parent)
@@ -367,17 +374,25 @@ def online_2017(a, parent, device, save_dir, iters, log_every):
     test_loader = DataLoader(db_test, batch_size=1, shuffle=False, num_workers=1, collate_fn=davis.collate)
     jpeg_frames = a.decode == "device"
     names = collections.deque()
+    stored_hw = []                                      # the sequence's stored size (one size per sequence)
 
     def frames():
         for b in test_loader:
             names.append([os.path.basename(f) for f in b["fname"]])
+            if not stored_hw:
+                stored_hw.extend(int(v) for v in b["size"][1:3])
             if jpeg_frames:
                 yield b
             else:
                 img, gt = davis.views(davis.pinned(b["data"]), *(int(v) for v in b["size"]))
                 yield (img, gt) if a.evaluate else img
     encode = a.encode == "device"
+    if input_res is not None:
+        print(f"Frames resized to {input_res[0]}x{input_res[1]} (inputRes); each object's fused logits are upsampled to "
+              "the stored size and merged there, label maps are written at that size"
+              + (", scored against the original annotations" if a.evaluate else ""))
     seg = SequenceSegmenter(nets=nets, output="labels", frames="jpeg" if jpeg_frames else "bgr8", score=a.evaluate,
+                            input_res=input_res, output_res=a.output_res,
                             encode="png" if encode else None, palette=palette if encode else None)
     for pred in seg(frames()):
         batch_names = names.popleft()
@@ -403,6 +418,8 @@ def online_2017(a, parent, device, save_dir, iters, log_every):
         scores = ObjectScores(k_objects)
         scores.add(seg.frame_counts())
         res = scores.result()
+        if input_res is not None:
+            res = dict(network_res=list(input_res), scored_res=stored_hw, **res)
         for k, ob in res["objects"].items():
             st = ob["statistics"]
             print(f"Scores of {a.seq_name} object {k} (frames 1 .. n-2): "
