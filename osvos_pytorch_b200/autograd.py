@@ -13,13 +13,8 @@ sums of the fused objective and every float reduction of the backward then take 
 (OSVOS_FLAG_DETERMINISTIC, DESIGN.md §16), so two runs on one device give bit-identical losses and gradients.
 """
 import torch
-import torch.nn as nn
 
 from . import ops
-
-
-def _trunk_convs(m):
-    return [[c for c in stage if isinstance(c, nn.Conv2d)] for stage in m.stages]
 
 
 class _OSVOSFunction(torch.autograd.Function):
@@ -47,40 +42,17 @@ class _OSVOSFunction(torch.autograd.Function):
         ctx.det = det
         xin = x.detach().contiguous().float()
         n, _, h, w = (int(v) for v in xin.shape)
-        convs = _trunk_convs(m)
-        acts = []      # acts[i][j] = output act of conv j of stage i
-        pooled = [None]
-        a = ops.conv_first(xin, convs[0][0].weight.detach(), convs[0][0].bias.detach(), relu=True, fast=fast)
-        stage_acts = [a]
-        full, a = ops.conv3x3(a, engine._packed(convs[0][1], "s0c1"), convs[0][1].bias.detach(), 64, relu=True,
-                              fast=fast, pool=True)               # 2x2 max pool fused into the epilogue
-        stage_acts.append(full)
-        acts.append(stage_acts)
-        for i in range(1, 5):
-            pooled.append(a)
-            stage_acts = []
-            for j, conv in enumerate(convs[i]):
-                if j == len(convs[i]) - 1 and i < 4:
-                    full, a = ops.conv3x3(a, engine._packed(conv, f"s{i}c{j}"), conv.bias.detach(), conv.out_channels,
-                                          relu=True, fast=fast, pool=True)
-                else:
-                    a, _, _ = ops.conv3x3(a, engine._packed(conv, f"s{i}c{j}"), conv.bias.detach(), conv.out_channels,
-                                          relu=True, fast=fast)
-                    full = a
-                stage_acts.append(full)
-            acts.append(stage_acts)
-        # side_prep has no ReLU: side_prep o (score_dsn, fuse slice) is ONE 3x3 conv C -> 2 (csrc/side_conv.cu), all four
-        # scales in one launch; its backward needs neither the 16 features nor their gradient (csrc/side_bwd_folded.cu)
-        # general deconvolution weights: the 16 side features themselves feed the tail (csrc/tail_general.cu)
+        acts, pooled = engine._trunk(xin, fast, keep=True)      # acts[i][j] = output act of conv j of stage i
+        # side_prep has no ReLU: folded, its backward needs neither the 16 features nor their gradient
+        # (csrc/side_bwd_folded.cu); with general deconvolution weights the features feed the tail (csrc/tail_general.cu)
+        feats, pqs = engine._side_outputs([s[-1] for s in acts[1:]], fast)
         if general:
-            feats, pqs = engine._side_features([acts[i][-1] for i in range(1, 5)], fast)
             table = engine._upsampling_table()
             ctx.general = (feats, pqs, table)
 
             def tail(**kw):
                 return ops.tail_general_fwd(feats, pqs, table, m.fuse.bias.detach(), n, h, w, **kw)
         else:
-            pqs = ops.side_folded_multi([acts[i][-1] for i in range(1, 5)], engine._folded_side_all(), fast=fast)
             ctx.general = None
 
             def tail(**kw):
@@ -123,7 +95,7 @@ class _OSVOSFunction(torch.autograd.Function):
         det = ctx.det
         xin, acts, pooled = ctx.saved
         n, h, w = ctx.dims
-        convs = _trunk_convs(m)
+        convs = m.trunk_convs()
         pg = {}                                   # parameter -> gradient tensor
         obj = ctx.objective
         if obj is not None:
@@ -144,21 +116,15 @@ class _OSVOSFunction(torch.autograd.Function):
                     and g.is_contiguous() and g.device == xin.device:
                 return g
             return None
-        wconvs = [c for stage in convs for c in stage][1:]
-        in_shape = {}                                  # conv -> (n, h, w) of its input
-        for i, stage in enumerate(convs):
-            hs, ws_ = h, w
-            for _ in range(i):
-                hs, ws_ = (hs + 1) // 2, (ws_ + 1) // 2
-            for c in stage:
-                in_shape[c] = (n, hs, ws_)
+        # the saved activation each tensor-core conv reads: the operand of its weight gradient
+        inputs = {c: acts[i][j - 1] if j else pooled[i]
+                  for i, stage in enumerate(convs) for j, c in enumerate(stage) if i or j}
         general = ctx.general
         if general is not None:                        # side_prep's weight gradient from the 64-channel dF operand
-            for i, sp in enumerate(m.side_prep):
-                in_shape[sp] = in_shape[convs[i + 1][-1]]
-            wconvs = wconvs + list(m.side_prep)
-        ws_sizes = [(ops.wgrad_workspace_floats(64 if c in m.side_prep else c.out_channels, c.in_channels, in_shape[c],
-                                                det) + 3) // 4 * 4
+            inputs.update((sp, acts[i + 1][-1]) for i, sp in enumerate(m.side_prep))
+        wconvs = list(inputs)
+        ws_sizes = [(ops.wgrad_workspace_floats(64 if c in m.side_prep else c.out_channels, c.in_channels,
+                                                inputs[c].shape[:3], det) + 3) // 4 * 4
                     for c in wconvs]
         # folded side branch: G [18 C + 2] per scale (rounded up to 16 bytes) behind the wgrad workspaces
         g_sizes = [] if general is not None else [(ops.side_folded_wgrad_floats(sp.in_channels) + 3) // 4 * 4
@@ -315,40 +281,34 @@ class _OSVOSFunction(torch.autograd.Function):
                 pg[m.fuse.weight] = fresh_small[136:200].view(m.fuse.weight.shape)
             ops.side_grads_finish(entries, accumulate=in_place)
         dpool = None
-        for i in range(4, 0, -1):
-            s_out = acts[i][-1]
-            last_bias = bias_slices[convs[i][-1]]
-            # ReLU'(x) * (unpool(dpool) + side gradient), the latter formed on the fly from dpq and the fp32 folded weights
-            # (18 FMAs per element); deepest stage: dpool None, the side branch is the only consumer
-            if general is not None:
+        for i in range(4, -1, -1):
+            # ReLU'(x) * (unpool(dpool) + side gradient); deepest stage: dpool None, the side branch is the only consumer;
+            # stage 0 has no side branch.  Folded, the side gradient is formed on the fly from dpq and the fp32 folded
+            # weights (18 FMAs per element)
+            dside = dpq_i = wfold = None
+            if i and general is not None:
                 sp = m.side_prep[i - 1]
-                _, dside, _ = ops.conv3x3(dfs[i - 1], engine._packed(sp, f"sp{i}", transpose_flip=True), None,
-                                          sp.in_channels, fast=fast, out_act=False, out_f32=True)
-                dz = ops.unpool_mask(dpool, s_out, dside=dside, colsum=last_bias, deterministic=det)
-            else:
-                dz = ops.unpool_mask(dpool, s_out, dpq=dpq[i - 1], wfold=fold[i - 1][2], colsum=last_bias,
-                                     deterministic=det)
+                _, dside, _ = ops.conv3x3(dfs[i - 1], engine._packed(sp, transpose_flip=True), None, sp.in_channels,
+                                          fast=fast, out_act=False, out_f32=True)
+            elif i:
+                dpq_i, wfold = dpq[i - 1], fold[i - 1][2]
+            dz = ops.unpool_mask(dpool, acts[i][-1], dside=dside, dpq=dpq_i, wfold=wfold,
+                                 colsum=bias_slices[convs[i][-1]], deterministic=det)
             for j in range(len(convs[i]) - 1, -1, -1):
                 conv = convs[i][j]
-                inp = acts[i][j - 1] if j > 0 else pooled[i]
-                wgrad(conv, inp, dz)
                 pg[conv.bias] = bias_grad(conv)
-                wt = engine._packed(conv, f"s{i}c{j}", transpose_flip=True)
+                if i == j == 0:                        # conv1_1: weight and input gradient from the fp32 frame
+                    pg[conv.weight], dx = ops.conv_first_bwd(xin, dz, conv.weight.detach(), ctx.needs_input_grad[1],
+                                                             deterministic=det)
+                    break
+                inp = inputs[conv]
+                wgrad(conv, inp, dz)
+                wt = engine._packed(conv, transpose_flip=True)
                 if j > 0:
                     dz, _, _ = ops.conv3x3(dz, wt, None, conv.in_channels, fast=fast, mask=inp.hi,
                                            colsum=bias_slices[convs[i][j - 1]], deterministic=det)
                 else:
                     dpool, _, _ = ops.conv3x3(dz, wt, None, conv.in_channels, fast=fast)
-        # stage 1 (no side branch)
-        c12, c11 = convs[0][1], convs[0][0]
-        dz = ops.unpool_mask(dpool, acts[0][1], colsum=bias_slices[c12], deterministic=det)
-        wgrad(c12, acts[0][0], dz)
-        pg[c12.bias] = bias_grad(c12)
-        dz, _, _ = ops.conv3x3(dz, engine._packed(c12, "s0c1", transpose_flip=True), None, 64, fast=fast,
-                               mask=acts[0][0].hi, colsum=bias_slices[c11], deterministic=det)
-        dw0, dx = ops.conv_first_bwd(xin, dz, c11.weight.detach(), ctx.needs_input_grad[1], deterministic=det)
-        pg[c11.weight] = dw0
-        pg[c11.bias] = bias_grad(c11)
         ops.wgrad_finish(finish_items)
         ctx.saved = None
         ctx.objective = None

@@ -11,7 +11,6 @@ import gc
 import os
 
 import torch
-import torch.nn as nn
 
 from . import ops
 from .layers.osvos_layers import bilinear_deconv_weight
@@ -37,7 +36,8 @@ class OSVOSEngine:
     def __init__(self, module):
         # no reference cycle through nn.Module registration: keep a plain attribute
         object.__setattr__(self, "m", module)
-        self._pack_cache = {}
+        self._packed_layouts = {}        # (conv, transpose_flip) -> (weight version, packed layout)
+        self._derived = {}               # folded side weights, projections, upsampling table
         self._deconv_checked = {}
         # CUDA-graph cache for the inference path: (shape, device, precision, parameter versions) -> captured step.
         # One frame is ~22 kernel launches; replaying a graph removes the Python / launch overhead (OSVOS_CUDA_GRAPH=0
@@ -68,61 +68,53 @@ class OSVOSEngine:
         return _Ctx()
 
     # ------------------------------------------------------------ weight caches
-    def _cached(self, key, params, make):
+    def _cached(self, key, params, make, cache=None):
+        """make(), cached in `cache` (default: the derived-tensor cache) on the address and version of every tensor in
+        `params`."""
+        cache = self._derived if cache is None else cache
         ver = tuple((p.data_ptr(), p._version) for p in params)
-        hit = self._pack_cache.get(key)
+        hit = cache.get(key)
         if hit is not None and hit[0] == ver:
             return hit[1]
         val = make()
-        self._pack_cache[key] = (ver, val)
+        cache[key] = (ver, val)
         return val
 
-    def _packed(self, conv, key, transpose_flip=False, col_pad=64):
-        return self._cached((key, transpose_flip, col_pad), [conv.weight],
-                            lambda: ops.pack_conv3x3_weights(conv.weight, transpose_flip, col_pad))
+    def _packed(self, conv, transpose_flip=False):
+        """conv's packed tensor-core layout (transposed and flipped for the data gradient)."""
+        return self._cached((conv, transpose_flip), [conv.weight],
+                            lambda: ops.pack_conv3x3_weights(conv.weight, transpose_flip), self._packed_layouts)
 
     def _tensor_core_convs(self):
-        """(conv module, cache key) of every 3x3 conv that runs on the packed tensor-core path: the trunk convs (conv1_1
-        takes its OIHW weights directly) and, when the general tail runs (uses_general_tail), the four side_prep convs,
-        whose forward and data-gradient convolutions then read packed layouts too.  On the folded path side_prep is
-        folded with its 1x1 projections instead (engine._folded_side_all) and has no packed layout."""
-        m = self.m
-        out = []
-        for i in range(5):
-            convs = [c for c in m.stages[i] if isinstance(c, nn.Conv2d)]
-            for j, conv in enumerate(convs):
-                if i == 0 and j == 0:
-                    continue
-                out.append((conv, f"s{i}c{j}"))
-        if self.uses_general_tail():
-            out += [(sp, f"sp{i + 1}") for i, sp in enumerate(m.side_prep)]
-        return out
+        """Every 3x3 conv that runs on the packed tensor-core path: the trunk convs (conv1_1 takes its OIHW weights
+        directly) and, when the general tail runs (uses_general_tail), the four side_prep convs, whose forward and
+        data-gradient convolutions then read packed layouts too.  On the folded path side_prep is folded with its 1x1
+        projections instead (engine._folded_side_all) and has no packed layout."""
+        convs = [c for stage in self.m.trunk_convs() for c in stage][1:]
+        return convs + list(self.m.side_prep) if self.uses_general_tail() else convs
 
     def packed_weight_table(self):
         """[(weight Parameter, forward layout, transposed+flipped layout)] of the tensor-core convs, packed now if
         stale.  optim.FusedSGD rewrites these buffers in place from the updated weights."""
-        return [(conv.weight, self._packed(conv, key), self._packed(conv, key, transpose_flip=True))
-                for conv, key in self._tensor_core_convs()]
+        return [(conv.weight, self._packed(conv), self._packed(conv, transpose_flip=True))
+                for conv in self._tensor_core_convs()]
 
     def restamp_packed(self):
-        """Declare the cached layouts current for the present parameter versions (called by optim.FusedSGD after it
-        has updated the weights AND their packed layouts in one kernel)."""
-        for conv, key in self._tensor_core_convs():
-            ver = ((conv.weight.data_ptr(), conv.weight._version),)
+        """Declare the cached layouts of the tensor-core convs current for the present parameter versions (called by
+        optim.FusedSGD after it has updated the weights AND those layouts in one kernel).  Other cached layouts, such
+        as side_prep's on the folded path, were not rewritten and keep their stamps."""
+        for conv in self._tensor_core_convs():
             for flip in (False, True):
-                hit = self._pack_cache.get((key, flip, 64))
+                hit = self._packed_layouts.get((conv, flip))
                 if hit is not None:
-                    self._pack_cache[(key, flip, 64)] = (ver, hit[1])
+                    self._packed_layouts[(conv, flip)] = (((conv.weight.data_ptr(), conv.weight._version),), hit[1])
 
     def drop_derived_caches(self, keep_packed=False):
         """Forget cached derived tensors; with keep_packed the packed conv layouts (static buffers a captured graph
         may point at) are kept."""
+        self._derived.clear()
         if not keep_packed:
-            self._pack_cache.clear()
-            return
-        for k in [k for k in self._pack_cache if not (isinstance(k, tuple) and len(k) == 3 and k[2] == 64
-                                                      and isinstance(k[1], bool))]:
-            del self._pack_cache[k]
+            self._packed_layouts.clear()
 
     def _param_list(self):
         """Parameters the native path differentiates: everything, the eight deconvolution weights only when the module
@@ -184,18 +176,70 @@ class OSVOSEngine:
         return self._cached(("upsampling",), deps, lambda: ops.upsampling_fold(
             [l.weight for l in m.upscale], [l.weight for l in m.upscale_], m.fuse.weight))
 
-    def _side_features(self, stage_outs, fast):
-        """(feats, pqs) of the four scales for the general tail: side_prep's 16 fp32 features and their projections."""
+    def _side_features(self, stage_outs, fast, simt=False):
+        """(feats, pqs) of the four scales: side_prep's 16 fp32 features and their projections (simt: the SIMT conv and
+        a separate projection)."""
         m = self.m
         feats, pqs = [], []
         for i, full in enumerate(stage_outs):
             sp = m.side_prep[i]
-            _, feat, pq = ops.conv3x3(full, self._packed(sp, f"sp{i + 1}"), sp.bias.detach(), 16, relu=False, fast=fast,
-                                      out_act=False, out_f32=True, proj_w=self._proj(i),
-                                      proj_b=m.score_dsn[i].bias.detach())
+            if simt:
+                _, feat, _ = ops.conv3x3(full, self._packed(sp), sp.bias.detach(), 16, relu=False, fast=fast,
+                                         out_act=False, out_f32=True, simt=True)
+                pq = ops.side_project(feat, self._proj(i), m.score_dsn[i].bias.detach())
+            else:
+                _, feat, pq = ops.conv3x3(full, self._packed(sp), sp.bias.detach(), 16, relu=False, fast=fast,
+                                          out_act=False, out_f32=True, proj_w=self._proj(i),
+                                          proj_b=m.score_dsn[i].bias.detach())
             feats.append(feat)
             pqs.append(pq)
         return feats, pqs
+
+    def _side_outputs(self, stage_outs, fast, want_feats=False, simt=False):
+        """(feats | None, pqs) of the four side scales from the stage outputs of stages 1-4.  When the folded tail runs
+        and no side features are wanted, side_prep o (score_dsn, fuse slice) is folded into one 3x3 conv C -> 2
+        (include/osvos_b200.h) and the four scales run in ONE launch; the features themselves are then never formed."""
+        if want_feats or simt or self.uses_general_tail():
+            return self._side_features(stage_outs, fast, simt)
+        return None, ops.side_folded_multi(stage_outs, self._folded_side_all(), fast=fast)
+
+    def _trunk(self, x, fast, keep, simt=False, fuse_stage1=False):
+        """The 13 trunk convs over the fp32 NCHW frame x -> (acts, pooled).  With `keep`, acts[i] lists the outputs of
+        stage i's convs and pooled[i] is stage i's input (the backward reads them all); without it acts[i] holds only
+        the stage's output and pooled stays [None], so each inner activation is freed once the next conv has read it.
+        The last conv of stages 0-3 has the 2x2 max pool fused into its epilogue (simt: SIMT convs and a separate pool
+        after stages 1-3); conv1_2's full-resolution output is only written when kept.  fuse_stage1: conv1_1 and
+        conv1_2 in one kernel (exact-mode inference)."""
+        convs = self.m.trunk_convs()
+        c11, c12 = convs[0]
+        acts, pooled = [[]], [None]
+        if fuse_stage1:
+            full, a = ops.stage1_fused(x, c11.weight.detach().contiguous().float(), c11.bias.detach(),
+                                       self._packed(c12), c12.bias.detach(), pool=True, out_act=keep)
+        else:
+            a = ops.conv_first(x, c11.weight.detach(), c11.bias.detach(), relu=True, fast=fast)
+            if keep:
+                acts[0].append(a)
+            full, a = ops.conv3x3(a, self._packed(c12), c12.bias.detach(), c12.out_channels, relu=True, fast=fast,
+                                  pool=True, out_act=keep)
+        acts[0].append(full)
+        for i in range(1, 5):
+            if keep:
+                pooled.append(a)
+            acts.append([])
+            for j, conv in enumerate(convs[i]):
+                if j == len(convs[i]) - 1 and i < 4 and not simt:
+                    full, a = ops.conv3x3(a, self._packed(conv), conv.bias.detach(), conv.out_channels, relu=True,
+                                          fast=fast, pool=True)
+                else:
+                    a, _, _ = ops.conv3x3(a, self._packed(conv), conv.bias.detach(), conv.out_channels, relu=True,
+                                          fast=fast, simt=simt)
+                    full = a
+                if keep or j == len(convs[i]) - 1:
+                    acts[i].append(full)
+            if simt and i < 4:
+                a = ops.maxpool2x2(full)
+        return acts, pooled
 
     # ----------------------------------------------------------------- forward
     def forward(self, x, fresh_outputs=True):
@@ -319,65 +363,20 @@ class OSVOSEngine:
         general = self.uses_general_tail()
         x = x.detach().contiguous().float()
         n, _, h, w = (int(v) for v in x.shape)
-        inter = {}
-        convs0 = [c for c in m.stages[0] if isinstance(c, nn.Conv2d)]
-        if not fast and not simt and os.environ.get("OSVOS_FUSE_STAGE1", "0") == "1":
-            # stage 1 as one kernel (opt-in): conv1_1 is computed inside conv1_2's kernel on its halo patch (no 105 MB round
-            # trip).  Its fp32 conv1_1 builder warps take about as long as the tile's tensor work, and on an H100 it measured
-            # slower than the two kernels below (553 vs 584 frames/s at 480x854, 700 W card), so it is not the default.
-            full, a = ops.stage1_fused(x, convs0[0].weight.detach().contiguous().float(), convs0[0].bias.detach(),
-                                       self._packed(convs0[1], "s0c1"), convs0[1].bias.detach(), pool=True,
-                                       out_act=return_intermediates)
-        else:
-            a = ops.conv_first(x, convs0[0].weight.detach(), convs0[0].bias.detach(), relu=True, fast=fast)
-            # conv1_2 with the 2x2 max pool fused into its epilogue; the full-resolution map is only kept on request
-            full, a = ops.conv3x3(a, self._packed(convs0[1], "s0c1"), convs0[1].bias.detach(), convs0[1].out_channels,
-                                  relu=True, fast=fast, simt=False, pool=True, out_act=return_intermediates)
-        if return_intermediates:
-            inter["stage0"] = full
-        pqs = []
-        # side_prep o (score_dsn, fuse slice) folded into one 3x3 conv C -> 2 (include/osvos_b200.h), the four scales in
-        # ONE launch after the last trunk conv; the side features themselves are only computed on request
-        fold = not simt and not return_intermediates and not general
-        stage_outs, feats = [], []
-        for i in range(1, 5):
-            convs = [c for c in m.stages[i] if isinstance(c, nn.Conv2d)]
-            for j, conv in enumerate(convs):
-                if j == len(convs) - 1 and i < 4 and not simt:
-                    full, a = ops.conv3x3(a, self._packed(conv, f"s{i}c{j}"), conv.bias.detach(), conv.out_channels,
-                                          relu=True, fast=fast, pool=True)
-                else:
-                    a, _, _ = ops.conv3x3(a, self._packed(conv, f"s{i}c{j}"), conv.bias.detach(), conv.out_channels,
-                                          relu=True, fast=fast, simt=simt)
-                    full = a
-            if simt and i < 4:
-                a = ops.maxpool2x2(full)
-            if return_intermediates:
-                inter[f"stage{i}"] = full
-            sp = m.side_prep[i - 1]
-            if simt:
-                _, feat, _ = ops.conv3x3(full, self._packed(sp, f"sp{i}"), sp.bias.detach(), 16, relu=False, fast=fast,
-                                         out_act=False, out_f32=True, simt=True)
-                pq = ops.side_project(feat, self._proj(i - 1), m.score_dsn[i - 1].bias.detach())
-            elif fold:
-                stage_outs.append(full)
-                continue
-            else:
-                _, feat, pq = ops.conv3x3(full, self._packed(sp, f"sp{i}"), sp.bias.detach(), 16, relu=False, fast=fast,
-                                          out_act=False, out_f32=return_intermediates or general,
-                                          proj_w=self._proj(i - 1), proj_b=m.score_dsn[i - 1].bias.detach())
-            feats.append(feat)
-            if return_intermediates:
-                inter[f"side{i}"] = feat
-                inter[f"pq{i}"] = pq
-            pqs.append(pq)
-        if fold:
-            pqs = ops.side_folded_multi(stage_outs, self._folded_side_all(), fast=fast)
+        # stage 1 as one kernel (opt-in): conv1_1 is computed inside conv1_2's kernel on its halo patch (no 105 MB round
+        # trip).  Its fp32 conv1_1 builder warps take about as long as the tile's tensor work, and on an H100 it measured
+        # slower than the two kernels (553 vs 584 frames/s at 480x854, 700 W card), so it is not the default.
+        fuse_stage1 = not fast and not simt and os.environ.get("OSVOS_FUSE_STAGE1", "0") == "1"
+        acts, _ = self._trunk(x, fast, keep=return_intermediates, simt=simt, fuse_stage1=fuse_stage1)
+        feats, pqs = self._side_outputs([s[-1] for s in acts[1:]], fast, want_feats=return_intermediates, simt=simt)
         if general:
             out, _ = ops.tail_general_fwd(feats, pqs, self._upsampling_table(), m.fuse.bias.detach(), n, h, w)
         else:
             out, _ = ops.tail_fwd(pqs, m.fuse.bias.detach(), n, h, w)
         outs = [out[k] for k in range(5)]
-        if return_intermediates:
-            return outs, inter
-        return outs
+        if not return_intermediates:
+            return outs
+        inter = {f"stage{i}": s[-1] for i, s in enumerate(acts)}
+        for i in range(4):
+            inter[f"side{i + 1}"], inter[f"pq{i + 1}"] = feats[i], pqs[i]
+        return outs, inter

@@ -104,8 +104,9 @@ class OSVOS(nn.Module):
         elif pretrained == 2:
             self._load_caffe_vgg(verbose)
 
-    def _trunk_convs(self):
-        return [m for stage in self.stages for m in stage if isinstance(m, nn.Conv2d)]
+    def trunk_convs(self):
+        """The 13 trunk convs grouped by stage (2, 2, 3, 3, 3), in VGG-16 order."""
+        return [[m for m in stage if isinstance(m, nn.Conv2d)] for stage in self.stages]
 
     def _load_torchvision_vgg(self, verbose):
         from mypath import Path  # same config hook as the reference (:13,99)
@@ -113,7 +114,7 @@ class OSVOS(nn.Module):
             print("Loading weights from PyTorch VGG")
         sd = torch.load(os.path.join(Path.models_dir(), "vgg_pytorch.pth"), map_location="cpu")
         feats = sorted({int(k.split(".")[1]) for k in sd if k.startswith("features.") and k.endswith(".weight")})
-        convs = self._trunk_convs()
+        convs = [c for stage in self.trunk_convs() for c in stage]
         assert len(feats) >= len(convs)
         with torch.no_grad():
             for conv, idx in zip(convs, feats):
@@ -127,7 +128,7 @@ class OSVOS(nn.Module):
             print("Loading weights from Caffe VGG")
         mat = scipy.io.loadmat(os.path.join(Path.models_dir(), "vgg_caffe.mat"))
         with torch.no_grad():
-            for k, conv in enumerate(self._trunk_convs()):
+            for k, conv in enumerate(c for stage in self.trunk_convs() for c in stage):
                 w = torch.from_numpy(np.ascontiguousarray(mat["weights"][0][k].transpose()))
                 b = torch.from_numpy(np.ascontiguousarray(mat["biases"][0][k][:, 0]))
                 assert conv.weight.shape == w.shape and conv.bias.shape == b.shape  # reference :119,123

@@ -119,22 +119,27 @@ def test_launch_count():
 
 def test_launches_seen_by_the_profiler():
     """The two launches are the tables kernel and the tile kernel.  Late in a long process torch.profiler can record no
-    device activity at all (tests/test_gpu_side_schedules.py's ``ran``); such a window is retried, and skipped if it
-    stays blind - a window that records kernels must record exactly these two."""
+    device activity at all (tests/test_gpu_side_schedules.py's ``ran``), or lose a kernel record from a window
+    (tests/test_gpu_conv_schedules.py's ``profiled``; here it was the window's first, the tables kernel).  So each
+    window opens with a torch kernel of its own, and a window that records fewer than the two launches is retried, at
+    most twice; one that stays blind is skipped.  The package's kernels in a window must be exactly these two."""
     from osvos_pytorch_b200 import ops
     maps = [torch.ones(2, 1, 12, 20, device="cuda")] * 4
     out = torch.empty(2, 24, 40, dtype=torch.uint8, device="cuda")
+    first = torch.zeros(1, device="cuda")
     for _ in range(3):
         torch.cuda.synchronize()
         with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+            first.add_(1)
             ops.upsample_merge_objects(maps, (24, 40), out=out)
             torch.cuda.synchronize()
-        kernels = [(ev.key, ev.count) for ev in prof.key_averages() if ev.device_type.name == "CUDA"]
-        if kernels:
+        records = [(ev.key, ev.count) for ev in prof.key_averages() if ev.device_type.name == "CUDA"]
+        kernels = [(key, c) for key, c in records if "osvos::" in key]
+        if sum(c for _, c in kernels) >= 2:
             break
-    if not kernels:
+    if not records:
         pytest.skip("torch.profiler recorded no device activity in this process")
-    assert sum(c for _, c in kernels) == 2, kernels
+    assert sum(c for _, c in kernels) == 2, records
     assert any("upsample_merge_objects_kernel" in key for key, _ in kernels), kernels
     assert any("resize_f32_tables_kernel" in key for key, _ in kernels), kernels
 

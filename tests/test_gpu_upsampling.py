@@ -289,7 +289,7 @@ def test_online_finetune_graphed_fused_equals_eager():
     net = nets[True]
     for i, sp in enumerate(net.side_prep):
         for flip in (False, True):
-            cached = net._engine._pack_cache[(f"sp{i + 1}", flip, 64)][1]
+            cached = net._engine._packed_layouts[(sp, flip)][1]
             assert torch.equal(cached, ops.pack_conv3x3_weights(sp.weight, flip, 64)), (i, flip)
     for a, b in zip(hist[False], hist[True]):
         assert abs(a - b) <= 3e-4 * abs(a), (hist[False], hist[True])
