@@ -1,110 +1,45 @@
-// class_balanced_cross_entropy_loss (layers/osvos_layers.py:19-48 of the
-// reference) as two bandwidth-bound kernels with 128-bit loads, warp-shuffle
+// class_balanced_cross_entropy_loss (objective.cuh) as two bandwidth-bound kernels with 128-bit loads, warp-shuffle
 // reductions and one fp64 atomic per block and quantity:
-//   forward : sums = {S_pos = sum_{y=1} (softplus(x) - x), S_neg = sum_{y=0} softplus(x), P, N}
-//             loss = (Nn/N * S_pos + P/N * S_neg) / divisor,  Nn = N - P      (:38-46)
-//   backward: dx = g * w * (sigmoid(x) - y) / divisor, w = y*Nn/N + (1-y)*P/N
+//   forward : sums = {S_pos, S_neg, P, N}, loss[0] = (Nn/N * S_pos + P/N * S_neg) / divisor
+//   backward: dx = g * w * (sigmoid(x) - y) / divisor
 // The void forms (OSVOS_FLAG_VOID_LABELS, osvos_cbce_bwd_void) leave pixels with y < 0 out of every sum and count, and
 // give them zero gradient.
-#include "common.cuh"
+#include "objective.cuh"
 
 namespace osvos {
 
 constexpr int kLossThreads = 256;
 
-__device__ __forceinline__ float softplus_l(float x) { return fmaxf(x, 0.f) + log1pf(__expf(-fabsf(x))); }
-
 // DET: each block stores its sums in its own row behind sums[5] (plain stores), and the last block adds the rows in
 // block order instead of the fp64 atomics.
-// VOID (OSVOS_FLAG_VOID_LABELS): a label y < 0 is a void pixel, counted in neither class; N = #(y >= 0) is a fourth
-// block sum (sums[3]) instead of the element count, and N == 0 gives loss 0.
+// VOID (OSVOS_FLAG_VOID_LABELS): N = #(y >= 0) is a fourth block sum (sums[3]) instead of the element count, and
+// N == 0 gives loss 0.
 template <bool DET, bool VOID>
 __device__ __forceinline__ void cbce_fwd_body(const float* __restrict__ x, const float* __restrict__ label, size_t total,
                                               double* __restrict__ sums, double divisor, float* __restrict__ loss) {
-  constexpr int kVals = VOID ? 4 : 3;
-  float s_pos = 0.f, s_neg = 0.f, cnt = 0.f, cnt_all = 0.f;
+  CbceSums<1, false, VOID> acc;
   const size_t nvec = total / 4;
   for (size_t v = blockIdx.x * static_cast<size_t>(kLossThreads) + threadIdx.x; v < nvec;
        v += static_cast<size_t>(gridDim.x) * kLossThreads) {
     const float4 xv = __ldg(reinterpret_cast<const float4*>(x) + v);
     const float4 lv = __ldg(reinterpret_cast<const float4*>(label) + v);
-    const float xs[4] = {xv.x, xv.y, xv.z, xv.w};
-    const float ls[4] = {lv.x, lv.y, lv.z, lv.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      if constexpr (VOID) {
-        if (ls[j] < 0.f) continue;
-        cnt_all += 1.f;
-      }
-      const float sp = softplus_l(xs[j]);
-      if (ls[j] >= 0.5f) {
-        s_pos += sp - xs[j];
-        cnt += 1.f;
-      } else {
-        s_neg += sp;
-      }
-    }
+    acc.add({xv.x}, lv.x);
+    acc.add({xv.y}, lv.y);
+    acc.add({xv.z}, lv.z);
+    acc.add({xv.w}, lv.w);
   }
   if (blockIdx.x == 0 && threadIdx.x < (total & 3)) {
     const size_t e = nvec * 4 + threadIdx.x;
-    const float xe = x[e];
-    const float le = label[e];
-    if (!VOID || le >= 0.f) {
-      if constexpr (VOID) cnt_all += 1.f;
-      const float sp = softplus_l(xe);
-      if (le >= 0.5f) {
-        s_pos += sp - xe;
-        cnt += 1.f;
-      } else {
-        s_neg += sp;
-      }
-    }
+    acc.add({x[e]}, label[e]);
   }
-  float vals[kVals];
-  vals[0] = s_pos, vals[1] = s_neg, vals[2] = cnt;
-  if constexpr (VOID) vals[3] = cnt_all;
-  __shared__ float red[kLossThreads / 32][kVals];
-#pragma unroll
-  for (int i = 0; i < kVals; ++i)
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) vals[i] += __shfl_xor_sync(0xffffffffu, vals[i], off);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) {
-#pragma unroll
-    for (int i = 0; i < kVals; ++i) red[warp][i] = vals[i];
-  }
-  __syncthreads();
-  if (threadIdx.x < kVals) {
-    double acc = 0.0;
-    for (int w = 0; w < kLossThreads / 32; ++w) acc += static_cast<double>(red[w][threadIdx.x]);
-    if constexpr (DET)
-      sums[5 + kVals * static_cast<size_t>(blockIdx.x) + threadIdx.x] = acc;
-    else
-      atomicAdd(sums + threadIdx.x, acc);
-  }
-  // last block to arrive (counter in sums[4]): loss[0] = (Nn/N * S_pos + P/N * S_neg) / divisor ; sums[3] = N
-  const bool last = last_block_arrives(reinterpret_cast<unsigned int*>(sums + 4));
-  if constexpr (DET) {
-    if (last) {
-      __shared__ double dred[kLossThreads];
-      for (int i = 0; i < kVals; ++i) {
-        const double t = block_ordered_sum(sums + 5 + i, static_cast<int>(gridDim.x), kVals, dred);
-        if (threadIdx.x == 0) sums[i] = t;
-      }
-    }
-  }
+  // the last block to arrive (counter in sums[4]): loss[0] = numerator / divisor ; sums[3] = N
+  const bool last = commit_block_sums<kLossThreads, 5, DET>(acc.v, sums, IdentitySlot());
   if (last && threadIdx.x == 0) {
-    if constexpr (VOID) {
-      const double tot = __ldcg(sums + 3);
-      const double p = __ldcg(sums + 2), nn = tot - p;
-      loss[0] = tot > 0.0 ? static_cast<float>((nn / tot * __ldcg(sums + 0) + p / tot * __ldcg(sums + 1)) / divisor)
-                          : 0.f;
-    } else {
-      const double tot = static_cast<double>(total);
-      const double p = __ldcg(sums + 2), nn = tot - p;
-      sums[3] = tot;
-      loss[0] = static_cast<float>((nn / tot * __ldcg(sums + 0) + p / tot * __ldcg(sums + 1)) / divisor);
-    }
+    const double tot = VOID ? __ldcg(sums + 3) : static_cast<double>(total);
+    if constexpr (!VOID) sums[3] = tot;
+    loss[0] = !VOID || tot > 0.0
+                  ? static_cast<float>(cbce_numerator(__ldcg(sums + 0), __ldcg(sums + 1), __ldcg(sums + 2), tot) / divisor)
+                  : 0.f;
   }
 }
 
@@ -133,8 +68,8 @@ __device__ __forceinline__ void cbce_bwd_body(const float* __restrict__ x, const
   if (VOID && !(n > 0.0)) {
     w_pos = w_neg = 0.f;
   } else {
-    w_pos = static_cast<float>((n - p) / n) * g;
-    w_neg = static_cast<float>(p / n) * g;
+    w_pos = cbce_pos_weight(p, n) * g;
+    w_neg = cbce_neg_weight(p, n) * g;
   }
   const size_t nvec = total / 4;
   for (size_t v = blockIdx.x * static_cast<size_t>(kLossThreads) + threadIdx.x; v < nvec;
@@ -146,7 +81,7 @@ __device__ __forceinline__ void cbce_bwd_body(const float* __restrict__ x, const
     float o[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      const float sg = 1.f / (1.f + __expf(-xs[j]));
+      const float sg = sigmoid(xs[j]);
       o[j] = ls[j] >= 0.5f ? w_pos * (sg - 1.f) : w_neg * sg;
       if constexpr (VOID) o[j] = ls[j] < 0.f ? 0.f : o[j];
     }
@@ -154,7 +89,7 @@ __device__ __forceinline__ void cbce_bwd_body(const float* __restrict__ x, const
   }
   if (blockIdx.x == 0 && threadIdx.x < (total & 3)) {
     const size_t e = nvec * 4 + threadIdx.x;
-    const float sg = 1.f / (1.f + __expf(-x[e]));
+    const float sg = sigmoid(x[e]);
     const float le = label[e];
     float o = le >= 0.5f ? w_pos * (sg - 1.f) : w_neg * sg;
     if constexpr (VOID) o = le < 0.f ? 0.f : o;

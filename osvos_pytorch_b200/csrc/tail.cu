@@ -14,8 +14,9 @@
 // output pixel: with o = y + crop_top, a = o / s, r = o % s the rows are
 // a (weight (r + .5)/s, if a < h_k) and a - 1 (weight 1 - (r + .5)/s, if a >= 1);
 // rows outside the source contribute zero (zero padding => attenuated border).
-#include "common.cuh"
+#include "objective.cuh"
 #include "ptx.cuh"
+#include "tail_scales.cuh"
 
 namespace osvos {
 
@@ -38,19 +39,6 @@ struct TailParams {
 };
 
 constexpr int kTailThreads = 256;
-// sums layout (doubles): [2k] / [2k+1] = S_pos / S_neg of map k, [10] = P, [11] = N, [12] / [13] = A_pos / A_neg of the
-// fused map (sum_{y=1} (sigmoid(x) - 1), sum_{y=0} sigmoid(x): d fuse.bias without another pass), [14] = arrival counter
-constexpr int kTailSums = 15;
-constexpr int kTailVals = 13;   // block partials per block in the deterministic form: sums[0..10], [12], [13]
-constexpr int kTailVoidVals = 14;   // the void form (OSVOS_FLAG_VOID_LABELS) also counts N = #(y >= 0) into sums[11]
-
-static int tail_fwd_blocks(int n, int h) {
-  size_t blocks = static_cast<size_t>(n) * h;                 // one output row per block iteration
-  const size_t cap = static_cast<size_t>(device_sm_count()) * 8;
-  return static_cast<int>(blocks > cap ? cap : blocks);
-}
-
-__device__ __forceinline__ float softplus_f(float x) { return fmaxf(x, 0.f) + log1pf(__expf(-fabsf(x))); }
 
 // One block = one output row.  Phase 1 interpolates VERTICALLY once per row: for each scale the (at most two) source rows
 // are blended into shared memory, v_k[c] = wy0 * pq_k[ay - 1][c] + wy1 * pq_k[ay][c] (806 float2 for a 854-pixel row).
@@ -71,8 +59,7 @@ __device__ __forceinline__ void tail_fwd_body(const TailParams& p) {
 #pragma unroll
   for (int k = 1; k < 4; ++k) voff[k] = voff[k - 1] + p.sc[k - 1].wk;
 
-  float s_pos[5] = {0, 0, 0, 0, 0}, s_neg[5] = {0, 0, 0, 0, 0};
-  float cnt_pos = 0.f, a_pos = 0.f, a_neg = 0.f, cnt_all = 0.f;
+  CbceSums<5, true, VOID> acc;   // the maps' loss sums (objective.cuh)
 
   for (int row = blockIdx.x; row < p.n * p.h; row += gridDim.x) {
     const int img = row / p.h, y = row - img * p.h;
@@ -107,7 +94,7 @@ __device__ __forceinline__ void tail_fwd_body(const TailParams& p) {
     for (int g = threadIdx.x; g * 4 - shift < p.w; g += kTailThreads) {
       const int x_first = g * 4 - shift;
       const uint32_t e0 = row_base + x_first;          // multiple of 4 (may start before the row: those lanes are skipped)
-      float o[5][4];
+      float o[4][5];   // [pixel][map]
       float lab[4] = {0, 0, 0, 0};
       const bool full = x_first >= 0 && x_first + 3 < p.w;
       if (p.label) {
@@ -134,100 +121,30 @@ __device__ __forceinline__ void tail_fwd_body(const TailParams& p) {
           const float w0 = ax >= 1 ? 1.f - fx1 : 0.f, w1 = ax < sc.wk ? fx1 : 0.f;
           const float2 t0 = vbuf[voff[k] + (ax >= 1 ? ax - 1 : 0)];
           const float2 t1 = vbuf[voff[k] + (ax < sc.wk ? ax : sc.wk - 1)];
-          o[k][j] = fmaf(w1, t1.x, w0 * t0.x);
+          o[j][k] = fmaf(w1, t1.x, w0 * t0.x);
           fused += fmaf(w1, t1.y, w0 * t0.y);
         }
-        o[4][j] = fused;
-        if (p.label && live && (!VOID || lab[j] >= 0.f)) {
-          if constexpr (VOID) cnt_all += 1.f;
-          const bool pos = lab[j] >= 0.5f;
-          cnt_pos += pos ? 1.f : 0.f;
-#pragma unroll
-          for (int k = 0; k < 5; ++k) {
-            const float xk = o[k][j];
-            const float sp = softplus_f(xk);
-            if (pos) s_pos[k] += sp - xk;
-            else s_neg[k] += sp;
-          }
-          const float sg = 1.f / (1.f + __expf(-fused));
-          if (pos) a_pos += sg - 1.f;
-          else a_neg += sg;
-        }
+        o[j][4] = fused;
+        if (p.label && live) acc.add(o[j], lab[j]);
       }
 #pragma unroll
       for (int k = 0; k < 5; ++k) {
         if (!p.out[k]) continue;
         if (full && (p.vec_mask & (1 << k))) {
-          *reinterpret_cast<float4*>(p.out[k] + e0) = make_float4(o[k][0], o[k][1], o[k][2], o[k][3]);
+          *reinterpret_cast<float4*>(p.out[k] + e0) = make_float4(o[0][k], o[1][k], o[2][k], o[3][k]);
         } else {
 #pragma unroll
           for (int j = 0; j < 4; ++j)
-            if (x_first + j >= 0 && x_first + j < p.w) p.out[k][e0 + j] = o[k][j];
+            if (x_first + j >= 0 && x_first + j < p.w) p.out[k][e0 + j] = o[j][k];
         }
       }
     }
   }
 
   if (p.label && p.sums) {
-    constexpr int kVals = VOID ? kTailVoidVals : kTailVals;
-    __shared__ float red[kTailThreads / 32][kVals];
-    float vals[kVals];
-#pragma unroll
-    for (int k = 0; k < 5; ++k) {
-      vals[2 * k] = s_pos[k];
-      vals[2 * k + 1] = s_neg[k];
-    }
-    vals[10] = cnt_pos;
-    vals[11] = a_pos;
-    vals[12] = a_neg;
-    if constexpr (VOID) vals[13] = cnt_all;
-#pragma unroll
-    for (int i = 0; i < kVals; ++i) {
-#pragma unroll
-      for (int off = 16; off > 0; off >>= 1) vals[i] += __shfl_xor_sync(0xffffffffu, vals[i], off);
-    }
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (lane == 0) {
-#pragma unroll
-      for (int i = 0; i < kVals; ++i) red[warp][i] = vals[i];
-    }
-    __syncthreads();
-    const int slot = threadIdx.x < 11 ? threadIdx.x : threadIdx.x < 13 ? threadIdx.x + 1 : 11;
-    if (threadIdx.x < kVals) {
-      double acc = 0.0;
-      for (int wv = 0; wv < kTailThreads / 32; ++wv) acc += static_cast<double>(red[wv][threadIdx.x]);
-      if constexpr (DET) p.sums[kTailSums + static_cast<size_t>(blockIdx.x) * kVals + threadIdx.x] = acc;
-      else atomicAdd(p.sums + slot, acc);
-    }
-    const bool last = last_block_arrives(reinterpret_cast<unsigned int*>(p.sums + 14));
-    if constexpr (DET) {
-      if (last) {   // the block rows in a fixed order (block_ordered_sum), one value at a time
-        __shared__ double dred[kTailThreads];
-        for (int i = 0; i < kVals; ++i) {
-          const double t = block_ordered_sum(p.sums + kTailSums + i, static_cast<int>(gridDim.x), kVals, dred);
-          if (threadIdx.x == 0) p.sums[i < 11 ? i : i < 13 ? i + 1 : 11] = t;
-        }
-        __syncthreads();
-      }
-    }
-    // the last block to arrive turns the sums into the five losses and their weighted total:
-    // L_k = (Nn/N * S_pos_k + P/N * S_neg_k) / divisor   (layers/osvos_layers.py:38-46)
-    if (last && threadIdx.x == 0) {
-      const double tot = VOID ? __ldcg(p.sums + 11) : static_cast<double>(total);
-      const double pcount = __ldcg(p.sums + 10), nn = tot - pcount;
-      if constexpr (!VOID) p.sums[11] = tot;
-      if (p.losses) {
-        double wsum = 0.0;
-        for (int k = 0; k < 5; ++k) {
-          double lk = (nn / tot * __ldcg(p.sums + 2 * k) + pcount / tot * __ldcg(p.sums + 2 * k + 1)) *
-                      static_cast<double>(p.inv_divisor);
-          if constexpr (VOID) lk = tot > 0.0 ? lk : 0.0;
-          p.losses[k] = static_cast<float>(lk);
-          wsum += static_cast<double>(p.loss_weights[k]) * lk;
-        }
-        p.losses[5] = static_cast<float>(wsum);
-      }
-    }
+    // the last block to arrive turns the sums into the five losses and their weighted total
+    if (commit_block_sums<kTailThreads, kTailSums, DET>(acc.v, p.sums, TailSlot()) && threadIdx.x == 0)
+      tail_losses<VOID>(p.sums, total, p.losses, p.loss_weights, p.inv_divisor);
   }
 }
 
@@ -289,23 +206,7 @@ __device__ __forceinline__ void tail_bwd2_body(const TailBwdParams& p) {
   const float inv_s = 1.f / static_cast<float>(s);
 
   float wpos = 0.f, wneg = 0.f, cp = 1.f, cq = 1.f;
-  if (LOSS) {
-    const double pc = p.sums[10], nt = p.sums[11];
-    wpos = static_cast<float>((nt - pc) / nt);
-    wneg = static_cast<float>(pc / nt);
-    const float up = (p.upstream ? __ldg(p.upstream) : 1.f) * p.inv_divisor;
-    cp = p.coeff[k] * up;
-    cq = p.coeff[4] * up;
-    if constexpr (VOID) {
-      if (!(nt > 0.0)) wpos = wneg = cp = cq = 0.f;
-    }
-    if (blockIdx.x == 0 && tid == 0 && p.fuse_bias_grad) {  // d fuse.bias = sum_px g_4, from the forward's A sums
-      if (VOID && !(nt > 0.0))
-        p.fuse_bias_grad[0] = 0.f;
-      else
-        p.fuse_bias_grad[0] = cq * static_cast<float>((nt - pc) / nt * p.sums[12] + pc / nt * p.sums[13]);
-    }
-  }
+  if (LOSS) tail_loss_coeffs<VOID>(p, k, wpos, wneg, cp, cq);
   const bool use_p = LOSS ? (p.coeff[k] != 0.f) : (p.src[k] != nullptr);
   const bool use_q = LOSS ? (p.coeff[4] != 0.f) : (p.src[4] != nullptr);
 
@@ -345,8 +246,8 @@ __device__ __forceinline__ void tail_bwd2_body(const TailBwdParams& p) {
             float wgt = (pos ? wpos : wneg) * fyv[u];
             if constexpr (VOID) wgt = lv[u] < 0.f ? 0.f : wgt;
             const float yv = pos ? 1.f : 0.f;
-            if (use_p) ap = fmaf(wgt, 1.f / (1.f + __expf(-pv[u])) - yv, ap);
-            if (use_q) aq = fmaf(wgt, 1.f / (1.f + __expf(-qv[u])) - yv, aq);
+            if (use_p) ap = fmaf(wgt, sigmoid(pv[u]) - yv, ap);
+            if (use_q) aq = fmaf(wgt, sigmoid(qv[u]) - yv, aq);
           } else {
             ap = fmaf(fyv[u], pv[u], ap);
             aq = fmaf(fyv[u], qv[u], aq);
@@ -412,19 +313,17 @@ __global__ void __launch_bounds__(256) tail_bwd2_void_kernel(const __grid_consta
 using namespace osvos;
 
 static void fill_tail_scales(TailParams& p, const float* const* pq, int h, int w) {
-  int hk = h, wk = w;
   for (int k = 0; k < 4; ++k) {
-    hk = (hk + 1) / 2;
-    wk = (wk + 1) / 2;
-    const int s = 2 << k;
-    p.sc[k].pq = pq[k];
-    p.sc[k].hk = hk;
-    p.sc[k].wk = wk;
-    p.sc[k].s = s;
-    p.sc[k].log2s = k + 1;
-    p.sc[k].inv_s = 1.f / static_cast<float>(s);
-    p.sc[k].top = ((hk + 1) * s - h) / 2;   // layers/osvos_layers.py:52-56: floor(d/2) rows cropped on top
-    p.sc[k].left = ((wk + 1) * s - w) / 2;
+    const TailGeometry g = tail_geometry(k, h, w);
+    TailScale& sc = p.sc[k];
+    sc.pq = pq[k];
+    sc.hk = g.hk;
+    sc.wk = g.wk;
+    sc.s = g.s;
+    sc.log2s = k + 1;
+    sc.inv_s = 1.f / static_cast<float>(g.s);
+    sc.top = g.top;
+    sc.left = g.left;
   }
 }
 
@@ -479,22 +378,20 @@ extern "C" int osvos_tail_fwd(const osvos_tail_fwd_args* a, osvos_stream_t strea
 // segment sizes (low-res columns per work item) per scale: 2s rows x (seg_lo + 1) s columns = 2-4 k source pixels
 static int fill_tail_bwd_scales(TailBwdParams& p, float* const* dpq, int n, int h, int w) {
   static const int kSegLo[4] = {255, 63, 15, 7};
-  int hk = h, wk = w, items = 0;
+  int items = 0;
   for (int k = 0; k < 4; ++k) {
-    hk = (hk + 1) / 2;
-    wk = (wk + 1) / 2;
-    const int s = 2 << k;
+    const TailGeometry g = tail_geometry(k, h, w);
     TailBwdScale& sc = p.sc[k];
     sc.dpq = dpq[k];
-    sc.hk = hk;
-    sc.wk = wk;
-    sc.s = s;
-    sc.top = ((hk + 1) * s - h) / 2;
-    sc.left = ((wk + 1) * s - w) / 2;
+    sc.hk = g.hk;
+    sc.wk = g.wk;
+    sc.s = g.s;
+    sc.top = g.top;
+    sc.left = g.left;
     sc.seg_lo = kSegLo[k];
-    sc.segs = (wk + sc.seg_lo - 1) / sc.seg_lo;
+    sc.segs = (g.wk + sc.seg_lo - 1) / sc.seg_lo;
     sc.first_item = items;
-    items += n * hk * sc.segs;
+    items += n * g.hk * sc.segs;
   }
   p.total_items = items;
   return items;

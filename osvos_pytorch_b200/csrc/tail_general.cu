@@ -14,8 +14,9 @@
 // and every parameter gradient of the tail is algebra on H, gA and three sums over the source pixels
 // (upsampling_grads_finish_kernel).  Every reduction here is fixed-order by construction (per-block partial rows added
 // by osvos_reduce_rows), so OSVOS_FLAG_DETERMINISTIC changes nothing in this file.
-#include "common.cuh"
+#include "objective.cuh"
 #include "ptx.cuh"
+#include "tail_scales.cuh"
 
 namespace osvos {
 
@@ -24,20 +25,8 @@ static_assert(kGenTaps == 16 + 64 + 256 + 1024, "tap table layout");
 __host__ __device__ __forceinline__ int gen_tap_offset(int k) { return k == 0 ? 0 : k == 1 ? 16 : k == 2 ? 80 : 336; }
 __host__ __device__ __forceinline__ int gen_row_len(int taps) { return 17 * taps + 33; }   // H, gA, sum dp F, sum dp, sum dF
 
-// the loss sums of osvos_tail_fwd (tail.cu): same layout, so the objective's readers need not know which tail ran
-constexpr int kTailSums = OSVOS_TAIL_SUMS;
-constexpr int kTailVals = 13;
-
 int reduce_rows_launch(const float* rows, int nrows, int ncols, int ld, float* scratch, float* out, int accumulate,
                        cudaStream_t stream);   // bwd_kernels.cu
-
-static int gen_fwd_blocks(int n, int h) {
-  size_t blocks = static_cast<size_t>(n) * h;
-  const size_t cap = static_cast<size_t>(device_sm_count()) * 8;
-  return static_cast<int>(blocks > cap ? cap : blocks);
-}
-
-__device__ __forceinline__ float gen_softplus(float x) { return fmaxf(x, 0.f) + log1pf(__expf(-fabsf(x))); }
 
 struct GenScale {
   const float* feat;   // [n, hk, wk, 16]
@@ -46,19 +35,16 @@ struct GenScale {
 };
 
 static void fill_gen_scales(GenScale* sc, const float* const* feat, const float* const* pq, int h, int w) {
-  int hk = h, wk = w;
   for (int k = 0; k < 4; ++k) {
-    hk = (hk + 1) / 2;
-    wk = (wk + 1) / 2;
-    const int s = 2 << k;
+    const TailGeometry g = tail_geometry(k, h, w);
     sc[k].feat = feat[k];
     sc[k].pq = pq[k];
-    sc[k].hk = hk;
-    sc[k].wk = wk;
-    sc[k].s = s;
+    sc[k].hk = g.hk;
+    sc[k].wk = g.wk;
+    sc[k].s = g.s;
     sc[k].log2s = k + 1;
-    sc[k].top = ((hk + 1) * s - h) / 2;    // layers/osvos_layers.py:52-56, as in tail.cu
-    sc[k].left = ((wk + 1) * s - w) / 2;
+    sc[k].top = g.top;
+    sc[k].left = g.left;
   }
 }
 
@@ -117,8 +103,7 @@ __global__ void __launch_bounds__(kGenThreads) tail_general_fwd_kernel(const __g
   __syncthreads();
   const uint32_t total = static_cast<uint32_t>(p.n) * p.h * p.w;
   const float fb = p.fuse_bias ? __ldg(p.fuse_bias) : 0.f;
-  float s_pos[5] = {0, 0, 0, 0, 0}, s_neg[5] = {0, 0, 0, 0, 0};
-  float cnt_pos = 0.f, a_pos = 0.f, a_neg = 0.f;
+  CbceSums<5, true, false> acc;   // the maps' loss sums (objective.cuh)
   for (int row = blockIdx.x; row < p.n * p.h; row += gridDim.x) {
     const int img = row / p.h, y = row - img * p.h;
     for (int x = threadIdx.x; x < p.w; x += kGenThreads) {
@@ -164,71 +149,14 @@ __global__ void __launch_bounds__(kGenThreads) tail_general_fwd_kernel(const __g
 #pragma unroll
       for (int k = 0; k < 5; ++k)
         if (p.out[k]) p.out[k][e] = o[k];
-      if (p.label) {
-        const bool pos = __ldg(p.label + e) >= 0.5f;
-        cnt_pos += pos ? 1.f : 0.f;
-#pragma unroll
-        for (int k = 0; k < 5; ++k) {
-          const float sp = gen_softplus(o[k]);
-          if (pos) s_pos[k] += sp - o[k];
-          else s_neg[k] += sp;
-        }
-        const float sg = 1.f / (1.f + __expf(-fused));
-        if (pos) a_pos += sg - 1.f;
-        else a_neg += sg;
-      }
+      if (p.label) acc.add(o, __ldg(p.label + e));
     }
   }
   if (!p.label) return;
   // block partials to this block's row, then the last block adds the rows in block order (tail.cu's deterministic form)
-  __shared__ float red[kGenThreads / 32][kTailVals];
-  float vals[kTailVals];
-#pragma unroll
-  for (int k = 0; k < 5; ++k) {
-    vals[2 * k] = s_pos[k];
-    vals[2 * k + 1] = s_neg[k];
-  }
-  vals[10] = cnt_pos;
-  vals[11] = a_pos;
-  vals[12] = a_neg;
-#pragma unroll
-  for (int i = 0; i < kTailVals; ++i) {
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) vals[i] += __shfl_xor_sync(0xffffffffu, vals[i], off);
-  }
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) {
-#pragma unroll
-    for (int i = 0; i < kTailVals; ++i) red[warp][i] = vals[i];
-  }
-  __syncthreads();
-  if (threadIdx.x < kTailVals) {
-    double acc = 0.0;
-    for (int wv = 0; wv < kGenThreads / 32; ++wv) acc += static_cast<double>(red[wv][threadIdx.x]);
-    p.sums[kTailSums + static_cast<size_t>(blockIdx.x) * kTailVals + threadIdx.x] = acc;
-  }
-  const bool last = last_block_arrives(reinterpret_cast<unsigned int*>(p.sums + 14));
-  if (!last) return;
-  __shared__ double dred[kGenThreads];
-  for (int i = 0; i < kTailVals; ++i) {
-    const double t = block_ordered_sum(p.sums + kTailSums + i, static_cast<int>(gridDim.x), kTailVals, dred);
-    if (threadIdx.x == 0) p.sums[i < 11 ? i : i + 1] = t;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {   // L_k = (Nn/N * S_pos_k + P/N * S_neg_k) / divisor  (layers/osvos_layers.py:38-46)
-    const double tot = static_cast<double>(total);
-    const double pcount = p.sums[10], nn = tot - pcount;
-    p.sums[11] = tot;
-    if (p.losses) {
-      double wsum = 0.0;
-      for (int k = 0; k < 5; ++k) {
-        const double lk = (nn / tot * p.sums[2 * k] + pcount / tot * p.sums[2 * k + 1]) * static_cast<double>(p.inv_divisor);
-        p.losses[k] = static_cast<float>(lk);
-        wsum += static_cast<double>(p.loss_weights[k]) * lk;
-      }
-      p.losses[5] = static_cast<float>(wsum);
-    }
-  }
+  // and turns the sums into the losses
+  if (commit_block_sums<kGenThreads, kTailSums, true>(acc.v, p.sums, TailSlot()) && threadIdx.x == 0)
+    tail_losses<false>(p.sums, total, p.losses, p.loss_weights, p.inv_divisor);
 }
 
 // -------------------------------------------------------------------------------------------------------- backward
@@ -292,16 +220,7 @@ __global__ void __launch_bounds__(256) tail_general_bwd_kernel(const __grid_cons
   const float* A = p.atab + gen_tap_offset(k);
 
   float wpos = 0.f, wneg = 0.f, cp = 1.f, cq = 1.f;
-  if (LOSS) {
-    const double pc = p.sums[10], nt = p.sums[11];
-    wpos = static_cast<float>((nt - pc) / nt);
-    wneg = static_cast<float>(pc / nt);
-    const float up = (p.upstream ? __ldg(p.upstream) : 1.f) * p.inv_divisor;
-    cp = p.coeff[k] * up;
-    cq = p.coeff[4] * up;
-    if (blockIdx.x == 0 && tid == 0 && p.fuse_bias_grad)   // d fuse.bias = sum_px g_4, from the forward's sums
-      p.fuse_bias_grad[0] = cq * static_cast<float>((nt - pc) / nt * p.sums[12] + pc / nt * p.sums[13]);
-  }
+  if (LOSS) tail_loss_coeffs<false>(p, k, wpos, wneg, cp, cq);
   const bool use_p = LOSS ? (p.coeff[k] != 0.f) : (p.src[k] != nullptr);
   const bool use_q = LOSS ? (p.coeff[4] != 0.f) : (p.src[4] != nullptr);
   for (int i = tid; i < fs * rw; i += 256) {
@@ -313,8 +232,8 @@ __global__ void __launch_bounds__(256) tail_general_bwd_kernel(const __grid_cons
       if (LOSS) {
         const bool pos = __ldg(p.label + o) >= 0.5f;
         const float wgt = pos ? wpos : wneg, yv = pos ? 1.f : 0.f;
-        if (use_p) a = cp * wgt * (1.f / (1.f + __expf(-__ldg(p.src[k] + o))) - yv);
-        if (use_q) b = cq * wgt * (1.f / (1.f + __expf(-__ldg(p.src[4] + o))) - yv);
+        if (use_p) a = cp * wgt * (sigmoid(__ldg(p.src[k] + o)) - yv);
+        if (use_q) b = cq * wgt * (sigmoid(__ldg(p.src[4] + o)) - yv);
       } else {
         if (use_p) a = __ldg(p.src[k] + o);
         if (use_q) b = __ldg(p.src[4] + o);
@@ -446,26 +365,24 @@ __global__ void __launch_bounds__(256) upsampling_grads_finish_kernel(const __gr
 
 // work items of the backward per scale, and the floats of its partial rows
 static int gen_bwd_plan(GenBwdParams* p, int n, int h, int w, size_t* row_floats) {
-  int hk = h, wk = w, items = 0;
+  int items = 0;
   size_t rows = 0;
   for (int k = 0; k < 4; ++k) {
-    hk = (hk + 1) / 2;
-    wk = (wk + 1) / 2;
-    const int s = 2 << k;
-    const int segs = (wk + kGenSeg - 1) / kGenSeg;
+    const TailGeometry g = tail_geometry(k, h, w);
+    const int segs = (g.wk + kGenSeg - 1) / kGenSeg;
     if (p) {
       GenBwdScale& sc = p->sc[k];
-      sc.hk = hk;
-      sc.wk = wk;
-      sc.s = s;
-      sc.top = ((hk + 1) * s - h) / 2;
-      sc.left = ((wk + 1) * s - w) / 2;
+      sc.hk = g.hk;
+      sc.wk = g.wk;
+      sc.s = g.s;
+      sc.top = g.top;
+      sc.left = g.left;
       sc.segs = segs;
       sc.first_item = items;
     }
-    const int nk = n * hk * segs;
+    const int nk = n * g.hk * segs;
     if (row_floats) row_floats[k] = rows;
-    rows += static_cast<size_t>(nk) * gen_row_len(4 * s * s);
+    rows += static_cast<size_t>(nk) * gen_row_len(4 * g.s * g.s);
     items += nk;
   }
   if (row_floats) row_floats[4] = rows;
@@ -494,7 +411,7 @@ extern "C" int osvos_upsampling_fold(const osvos_upsampling_fold_args* a, osvos_
 
 extern "C" size_t osvos_tail_general_fwd_sums(int n, int h, int w) {
   if (n <= 0 || h <= 0 || w <= 0) return 0;
-  return kTailSums + static_cast<size_t>(gen_fwd_blocks(n, h)) * kTailVals;
+  return kTailSums + static_cast<size_t>(tail_fwd_blocks(n, h)) * kTailVals;
 }
 
 extern "C" int osvos_tail_general_fwd(const osvos_tail_general_fwd_args* a, osvos_stream_t stream_) {
@@ -530,7 +447,7 @@ extern "C" int osvos_tail_general_fwd(const osvos_tail_general_fwd_args* a, osvo
   const int smem = kGenTabFloats * static_cast<int>(sizeof(float));
   static uint64_t attr_done = 0;
   OSVOS_CHECK_CUDA(ensure_dynamic_smem(tail_general_fwd_kernel, smem, &attr_done));
-  tail_general_fwd_kernel<<<gen_fwd_blocks(a->n, a->h), kGenThreads, smem, stream>>>(p);
+  tail_general_fwd_kernel<<<tail_fwd_blocks(a->n, a->h), kGenThreads, smem, stream>>>(p);
   OSVOS_CHECK_CUDA(cudaGetLastError());
   return OSVOS_OK;
 }

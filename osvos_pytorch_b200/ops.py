@@ -257,6 +257,39 @@ def side_project(feat, proj_w, proj_b):
     return pq
 
 
+def _tail_maps(n, h, w, dev):
+    """The five output maps of a tail forward, [5,n,1,h,w] fp32, each starting on a 16-byte boundary so that the kernel
+    can use 128-bit stores."""
+    per = (n * h * w + 3) // 4 * 4
+    return torch.empty((5, per), dtype=torch.float32, device=dev)[:, :n * h * w].view(5, n, 1, h, w)
+
+
+def _tail_losses(a, name, label, loss_weights, divisor, dev):
+    """With `loss_weights`, points the forward args `a` at a new losses [6] tensor and sets the weights and divisor;
+    returns that tensor, or None without `loss_weights`."""
+    if loss_weights is None:
+        return None
+    if label is None or divisor is None:
+        raise ValueError(f"{name}: loss_weights needs label and divisor")
+    losses = torch.empty(6, dtype=torch.float32, device=dev)
+    a.losses = losses.data_ptr()
+    for k in range(5):
+        a.loss_weights[k] = float(loss_weights[k])
+    a.divisor = float(divisor)
+    return losses
+
+
+def _tail_dpq(a, n, h, w, dev):
+    """The four side-map gradients [n,hk,wk,2] of a tail backward, pointed to by the args `a`."""
+    dpq, hk, wk = [], h, w
+    for k in range(4):
+        hk, wk = (hk + 1) // 2, (wk + 1) // 2
+        t = torch.empty((n, hk, wk, 2), dtype=torch.float32, device=dev)
+        dpq.append(t)
+        a.dpq[k] = t.data_ptr()
+    return dpq
+
+
 def tail_fwd(pqs, fuse_bias, n, h, w, label=None, out=None, loss_weights=None, divisor=None, deterministic=False,
              void=False):
     """Upsample + crop + fuse (+ loss sums, + the five class-balanced BCE losses and their weighted total).
@@ -266,9 +299,7 @@ def tail_fwd(pqs, fuse_bias, n, h, w, label=None, out=None, loss_weights=None, d
     lib = nat.load()
     dev = pqs[0].device
     if out is None:
-        # each map starts on a 16-byte boundary so the kernel can use 128-bit stores
-        per = (n * h * w + 3) // 4 * 4
-        out = torch.empty((5, per), dtype=torch.float32, device=dev)[:, :n * h * w].view(5, n, 1, h, w)
+        out = _tail_maps(n, h, w, dev)
     if void and label is None:
         raise ValueError("tail_fwd: void needs a label")
     flags = (nat.FLAG_DETERMINISTIC if deterministic else 0) | (nat.FLAG_VOID_LABELS if void else 0)
@@ -283,15 +314,7 @@ def tail_fwd(pqs, fuse_bias, n, h, w, label=None, out=None, loss_weights=None, d
     a.fuse_bias = nat.ptr(fuse_bias)
     a.label = nat.ptr(label)
     a.sums = nat.ptr(sums)
-    losses = None
-    if loss_weights is not None:
-        if label is None or divisor is None:
-            raise ValueError("tail_fwd: loss_weights needs label and divisor")
-        losses = torch.empty(6, dtype=torch.float32, device=dev)
-        a.losses = losses.data_ptr()
-        for k in range(5):
-            a.loss_weights[k] = float(loss_weights[k])
-        a.divisor = float(divisor)
+    losses = _tail_losses(a, "tail_fwd", label, loss_weights, divisor, dev)
     a.n, a.h, a.w = n, h, w
     _count()
     nat.check(lib.osvos_tail_fwd(byref(a), _stream()), "osvos_tail_fwd")
@@ -313,12 +336,7 @@ def tail_loss_bwd(out, label, sums, loss_weights, divisor, upstream, n, h, w, wa
         a.loss_weights[k] = float(loss_weights[k])
     a.label, a.sums, a.upstream = label.data_ptr(), sums.data_ptr(), nat.ptr(upstream)
     a.divisor = float(divisor)
-    dpq, hk, wk = [], h, w
-    for k in range(4):
-        hk, wk = (hk + 1) // 2, (wk + 1) // 2
-        t = torch.empty((n, hk, wk, 2), dtype=torch.float32, device=dev)
-        dpq.append(t)
-        a.dpq[k] = t.data_ptr()
+    dpq = _tail_dpq(a, n, h, w, dev)
     fb = torch.empty(1, dtype=torch.float32, device=dev) if want_fuse_bias else None
     a.fuse_bias_grad = nat.ptr(fb)
     a.n, a.h, a.w = n, h, w
@@ -353,8 +371,7 @@ def tail_general_fwd(feats, pqs, table, fuse_bias, n, h, w, label=None, loss_wei
     the upsampling_fold table -> (out [5,n,1,h,w], sums | None[, losses [6]]) with tail_fwd's contract."""
     lib = nat.load()
     dev = feats[0].device
-    per = (n * h * w + 3) // 4 * 4
-    out = torch.empty((5, per), dtype=torch.float32, device=dev)[:, :n * h * w].view(5, n, 1, h, w)
+    out = _tail_maps(n, h, w, dev)
     sums = torch.empty(lib.osvos_tail_general_fwd_sums(n, h, w), dtype=torch.float64, device=dev) \
         if label is not None else None
     a = nat.TailGeneralFwdArgs()
@@ -365,15 +382,7 @@ def tail_general_fwd(feats, pqs, table, fuse_bias, n, h, w, label=None, loss_wei
     taps = nat.UPSAMPLING_TAPS
     a.vtab, a.atab = table.data_ptr(), table[16 * taps:].data_ptr()
     a.fuse_bias, a.label, a.sums = nat.ptr(fuse_bias), nat.ptr(label), nat.ptr(sums)
-    losses = None
-    if loss_weights is not None:
-        if label is None or divisor is None:
-            raise ValueError("tail_general_fwd: loss_weights needs label and divisor")
-        losses = torch.empty(6, dtype=torch.float32, device=dev)
-        a.losses = losses.data_ptr()
-        for k in range(5):
-            a.loss_weights[k] = float(loss_weights[k])
-        a.divisor = float(divisor)
+    losses = _tail_losses(a, "tail_general_fwd", label, loss_weights, divisor, dev)
     a.n, a.h, a.w = n, h, w
     _count(2 if label is not None else 1)
     nat.check(lib.osvos_tail_general_fwd(byref(a), _stream()), "osvos_tail_general_fwd")
@@ -547,12 +556,7 @@ def tail_bwd(grads, n, h, w, deterministic=False):
             g = g.contiguous().float()
             keep.append(g)
         a.grad_out[k] = nat.ptr(g)
-    dpq, hk, wk = [], h, w
-    for k in range(4):
-        hk, wk = (hk + 1) // 2, (wk + 1) // 2
-        t = torch.empty((n, hk, wk, 2), dtype=torch.float32, device=dev)
-        dpq.append(t)
-        a.dpq[k] = t.data_ptr()
+    dpq = _tail_dpq(a, n, h, w, dev)
     a.n, a.h, a.w = n, h, w
     _count(1)
     nat.check(lib.osvos_tail_bwd(byref(a), _stream()), "osvos_tail_bwd")
