@@ -830,6 +830,24 @@ typedef struct {
 } osvos_upsampling_grads_args;
 OSVOS_API int osvos_upsampling_grads_finish(const osvos_upsampling_grads_args* args /* host */, osvos_stream_t stream);
 
+/* ---- online adaptation targets (DESIGN.md §28) ------------------------------------------------------------------
+ *   osvos_adaptation_labels: fused logits [n][h][w] fp32 (4-byte aligned) and the last masks last_mask [n][h][w] uint8
+ *                         (any alignment) -> labels [n][h][w] fp32 (4-byte aligned) and counts [n][3] int32 (4-byte
+ *                         aligned).  Per frame, M = last_mask != 0; E = the pixels p of M with |p - q|² > e² for every
+ *                         background pixel q inside the frame (pixels outside the frame are not background; E = M when
+ *                         M fills the frame or e = 0); D(p) = min over q in E of |p - q|², exact.  Negative: E non-empty
+ *                         and D > d²; positive: not negative and logit > logit_threshold; labels 0 for a negative pixel,
+ *                         1 for a positive one, -1 (void) otherwise.  counts = {|E|, #positive, #negative}.  e, d >= 0,
+ *                         n < 65536, h, w < 32768.  Four launches (an exact separable squared distance transform, column
+ *                         then row pass, for E and again for D), all integer: the result does not depend on the launch
+ *                         configuration.  `workspace`: osvos_adaptation_workspace_bytes(n, h, w) bytes, 4-byte aligned,
+ *                         owned by the caller; nothing is allocated.  Zeroes counts itself.
+ *   osvos_adaptation_workspace_bytes: host query; 0 for a non-positive dimension.                                    */
+OSVOS_API size_t osvos_adaptation_workspace_bytes(int n, int h, int w);
+OSVOS_API int osvos_adaptation_labels(const float* logits, const uint8_t* last_mask, float* labels, int* counts,
+                                      void* workspace, int n, int h, int w, float logit_threshold, int erosion_r,
+                                      int distance_r, osvos_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

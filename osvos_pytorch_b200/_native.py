@@ -255,6 +255,10 @@ SIGNATURES = {
     "osvos_jpeg_max_bytes": (c_size_t, [c_int, c_int]),
     "osvos_jpeg_encode_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "osvos_jpeg_encode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    # online adaptation targets from the last mask (DESIGN.md §28)
+    "osvos_adaptation_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "osvos_adaptation_labels": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
+                                        c_int, c_int, c_void_p]),
 }
 
 DAVIS_MAX_RADIUS = 31

@@ -69,13 +69,28 @@ class SequenceSegmenter:
     writes the stored-size label map straight from the K fused maps (each upsampled as ops.resize_f32 does, then
     merged; an argmax cannot be upsampled after the merge), so results, scores against the original annotations and
     palette files are at the stored size.  A label map at the network resolution is not what the DAVIS-2017 toolkit
-    scores, so labels with ``input_res`` and ``output_res="network"`` are refused, as is ``overlay`` with labels."""
+    scores, so labels with ``input_res`` and ``output_res="network"`` are refused, as is ``overlay`` with labels.
+
+    ``adapt`` (a training.OnlineAdaptation of ``net``; DESIGN.md §28): online adaptation between frames.  Frame 0 (the
+    annotated frame) is segmented as without it; before each later frame, ``adapt.adapt`` trains the net on the fp32
+    slot at the network resolution, and the frame's fused map at that resolution, before any upsampling, becomes the
+    next frame's last mask.  The forwards then run eagerly (engine.forward_inference): the weights change every frame,
+    and a captured inference graph would be dropped and captured again each time.  Everything downstream of the forward
+    is unchanged.  Needs one net (not labels), frames="bgr8" or "jpeg" and batches of one frame."""
 
     def __init__(self, net=None, output="logits", depth=3, frames="nchw_f32", meanval=ops.MEANVAL, score=False,
                  input_res=None, output_res="network", encode=None, overlay=None, overlay_quality=95, nets=None,
-                 palette=None):
+                 palette=None, adapt=None):
         if (net is None) == (nets is None):
             raise ValueError("pass either net or nets")
+        if adapt is not None:
+            if nets is not None or adapt.net is not net:
+                raise ValueError("adapt adapts one network: pass net (the one adapt was built for), not nets")
+            if output == "labels":
+                raise ValueError("adapt segments one object: it does not take output='labels'")
+            if frames == "nchw_f32":
+                raise ValueError("adapt needs frames='bgr8' or 'jpeg'")
+        self.adapt = adapt
         nets = [net] if nets is None else list(nets)
         if not 1 <= len(nets) <= 254 or len({id(m) for m in nets}) != len(nets):
             raise ValueError("nets must be 1 .. 254 distinct networks")
@@ -129,6 +144,9 @@ class SequenceSegmenter:
             from .davis import imresize_size
             h, w = imresize_size(self.input_res, h0, w0)
             self._dev_rs = [torch.empty((n, h, w, 3), dtype=torch.uint8, device=device) for _ in range(self.depth)]
+        if self.adapt is not None and (n, h, w) != tuple(self.adapt.last_mask.shape):
+            raise ValueError(f"adapt takes batches of one frame at the network resolution of its first mask "
+                             f"{tuple(self.adapt.last_mask.shape)}, got {(n, h, w)}")
         out_dtype = torch.float32 if self.output == "logits" else torch.uint8
         rh, rw = (h0, w0) if self._upsample else (h, w)                  # the results' size
         self._dev_in = [torch.empty((n, 3, h, w), dtype=torch.float32, device=device) for _ in range(self.depth)]
@@ -212,7 +230,11 @@ class SequenceSegmenter:
             fused_maps = []
             for net in self.nets:
                 eng = getattr(net, "_engine", None)
-                if eng is not None:
+                if self.adapt is not None:
+                    if i > 0:
+                        self.adapt.adapt(self._dev_in[k])
+                    fused_maps.append(eng.forward_inference(self._dev_in[k])[-1])
+                elif eng is not None:
                     # the ring slot is a buffer that comes back: from its second frame on the engine replays a graph
                     # captured on the slot itself (no input copy), and the fused map is read out of the graph's static
                     # output right here on the same stream (no copy of the five maps into fresh tensors); each net has
@@ -221,6 +243,8 @@ class SequenceSegmenter:
                 else:
                     fused_maps.append(net(self._dev_in[k])[-1])
             fused = fused_maps[0]
+            if self.adapt is not None and i > 0:               # frame 0's last mask is the annotation
+                self.adapt.segmented(fused)
             if self._upsample and self.output != "labels":     # back to the stored size, before anything reads it
                 fused = ops.resize_f32(fused, self._dev_up[k].shape[2:4], out=self._dev_up[k])
             if self.output == "labels":

@@ -963,6 +963,64 @@ def davis_measures_objects(labels, gt, n_objects, r=None, out=None):
     return out
 
 
+def _non_negative_int(v, name):
+    if isinstance(v, bool) or not isinstance(v, int) or v < 0:
+        raise ValueError(f"{name} must be a non-negative integer, got {v!r}")
+    return v
+
+
+def adaptation_threshold(alpha):
+    """The logit threshold of the positives for a probability ``alpha`` (0 < alpha < 1): float32(ln(alpha / (1 - alpha))),
+    computed in float64."""
+    import math
+    if isinstance(alpha, bool) or not isinstance(alpha, (int, float)) or not 0.0 < float(alpha) < 1.0:
+        raise ValueError(f"alpha must lie strictly between 0 and 1, got {alpha!r}")
+    a = float(alpha)
+    return float(torch.tensor(math.log(a / (1.0 - a)), dtype=torch.float64).float())
+
+
+def adaptation_labels(logits, last_mask, alpha, erosion, distance, out=None):
+    """Online adaptation targets (csrc/adapt.cu, DESIGN.md §28): fused logits fp32 [N,1,H,W] and the last masks uint8
+    [N,H,W] (any alignment) -> (labels fp32 [N,1,H,W], counts int32 [N,3]).  Per frame, M = last_mask != 0, E = M eroded
+    by the disk of radius ``erosion`` (pixels outside the frame are not background), D = the exact squared distance to
+    E.  A pixel is negative (0) when E is non-empty and D > distance², positive (1) when it is not negative and its logit
+    exceeds adaptation_threshold(alpha), and void (-1) otherwise; counts = {|E|, #positive, #negative}.  ``out``: a
+    contiguous fp32 [N,1,H,W] tensor to write the labels into (e.g. a graphed training step's static label buffer).
+    Everything is checked before the launch.  No host synchronisation."""
+    lib = nat.load()
+    _require_cuda(logits, "logits")
+    _require_cuda(last_mask, "last_mask")
+    if last_mask.dtype != torch.uint8 or last_mask.dim() != 3:
+        raise ValueError(f"last_mask must be uint8 [N,H,W], got {last_mask.dtype} {tuple(last_mask.shape)}")
+    n, h, w = (int(v) for v in last_mask.shape)
+    if logits.dtype != torch.float32 or tuple(logits.shape) != (n, 1, h, w):
+        raise ValueError(f"logits must be fp32 [N,1,H,W] = {(n, 1, h, w)} matching last_mask, got {logits.dtype} "
+                         f"{tuple(logits.shape)}")
+    if logits.device != last_mask.device:
+        raise ValueError("logits and last_mask must be on one device")
+    if not (0 < n < 65536 and 0 < h < 32768 and 0 < w < 32768):
+        raise ValueError(f"cannot label [{n},{h},{w}]: sizes must lie in [1, 32767] and 0 < N < 65536")
+    threshold = adaptation_threshold(alpha)
+    e = _non_negative_int(erosion, "erosion")
+    d = _non_negative_int(distance, "distance")
+    if out is None:
+        out = torch.empty((n, 1, h, w), dtype=torch.float32, device=logits.device)
+    elif (out.dtype != torch.float32 or tuple(out.shape) != (n, 1, h, w) or not out.is_contiguous()
+          or out.device != logits.device):
+        raise ValueError(f"out must be a contiguous fp32 tensor of shape {(n, 1, h, w)} on the logits' device")
+    x = logits.detach().contiguous()
+    m = last_mask.contiguous()
+    counts = torch.empty((n, 3), dtype=torch.int32, device=logits.device)
+    ws = torch.empty(lib.osvos_adaptation_workspace_bytes(n, h, w), dtype=torch.uint8, device=logits.device)
+    _count(4)
+    # distances beyond the frame's diagonal all mean "no negative"; clamp so the radius fits the C int
+    cap = 1 << 16
+    nat.check(lib.osvos_adaptation_labels(x.data_ptr(), m.data_ptr(), out.data_ptr(), counts.data_ptr(), ws.data_ptr(),
+                                          n, h, w, threshold, min(e, cap), min(d, cap), _stream()),
+              "osvos_adaptation_labels")
+    return out, counts
+
+
 def decode_jpeg(blob, n, h, w, out=None, status=None, nseg=None, chunk_bits=0):
     """A batch of n JPEGs of size h x w packed by jpeg.pack (``blob``: uint8 device tensor) -> (out uint8 [n,h,w,3] BGR,
     bit-identical to cv2.imread; status int32 [n]: 1 bad Huffman code, 2 zig-zag index past 63, 4 data ended before the

@@ -199,6 +199,103 @@ def online_finetune(net, sample_fn, iters, n_ave_grad=5, lr=1e-8, wd=0.0002, log
     return history
 
 
+class OnlineAdaptation:
+    """Online adaptation of a fine-tuned network while a DAVIS-2016 sequence is segmented (OnAVOS, Voigtlaender & Leibe,
+    BMVC 2017; DESIGN.md §28), for ``inference.SequenceSegmenter(adapt=...)``.  Before frame t >= 1 is segmented:
+    one forward with the current weights, ops.adaptation_labels of its fused map against the last mask (the annotation
+    ``first_mask`` for frame 1, then each segmented frame's mask) -> the frame's labels; then, unless the eroded last mask
+    is empty (the object is lost: the frame is skipped), ``steps`` SGD steps of one micro-batch each.  Step s trains on
+    the current frame when s = floor(i * steps / current_steps) for some i < current_steps, with loss weights
+    (0, 0, 0, 0, ``weight``) on its labels (void pixels left out), and on a fresh sample of ``sample_fn`` (the
+    fine-tuning's augmented first-frame sampler, called with a running count) with ONLINE_WEIGHTS otherwise.
+
+    ``first_mask``: the annotation, uint8 [1,H,W] on the device at the network resolution.  ``alpha``, ``distance`` and
+    ``erosion``: the targets' parameters (ops.adaptation_labels).  The optimizer is make_optimizer(net, "online", lr, wd,
+    fused=True), with fresh momentum; the two micro-batches are GraphedTrainSteps over the packed layouts FusedSGD
+    rewrites, each captured when it first runs, so a run that takes no step of a kind captures no graph for it.
+    ``counts`` lists each adapted frame's int32 [3] counts {|E|, #positive, #negative}; ``skipped`` the
+    number of frames with |E| = 0."""
+
+    def __init__(self, net, sample_fn, first_mask, lr, wd, steps=15, current_steps=3, weight=0.05, alpha=0.97,
+                 distance=220, erosion=15):
+        from . import ops
+        if isinstance(steps, bool) or not isinstance(steps, int) or steps < 0:
+            raise ValueError(f"steps must be a non-negative integer, got {steps!r}")
+        if isinstance(current_steps, bool) or not isinstance(current_steps, int) or not 0 <= current_steps <= steps:
+            raise ValueError(f"current_steps must be an integer in 0 .. steps ({steps}), got {current_steps!r}")
+        ops.adaptation_threshold(alpha)                     # the checks of ops.adaptation_labels, before anything runs
+        ops._non_negative_int(distance, "distance")
+        ops._non_negative_int(erosion, "erosion")
+        if not torch.is_tensor(first_mask) or first_mask.dtype != torch.uint8 or first_mask.dim() != 3 \
+                or int(first_mask.shape[0]) != 1 or not first_mask.is_cuda:
+            raise ValueError("first_mask must be a uint8 CUDA tensor [1,H,W] at the network resolution")
+        if net._engine.uses_general_tail():
+            raise ValueError("online adaptation trains with void labels, which the general tail (learn_upsampling or "
+                             "non-bilinear deconvolution weights) does not support")
+        self.net, self.sample_fn = net, sample_fn
+        self.steps, self.current_steps = steps, current_steps
+        self.weight, self.alpha, self.distance, self.erosion = float(weight), float(alpha), distance, erosion
+        self.current_at = {i * steps // current_steps for i in range(current_steps)}
+        self.last_mask = first_mask.detach().clone()
+        self.opt = make_optimizer(net, "online", lr, wd, fused=True)
+        self.opt.zero_grad()
+        in_opt = {id(p) for g in self.opt.param_groups for p in g["params"]}
+        from .parallel import trainable_parameters
+        self._not_in_opt = [p for p in trainable_parameters(net) if id(p) not in in_opt]
+        self._first = self._current = None
+        self.samples = 0
+        self.counts = []
+        self.skipped = 0
+        self._events = []
+
+    @torch.enable_grad()
+    def adapt(self, x):
+        """The adaptation before the frame in ``x`` (fp32 [1,3,H,W] at the network resolution) is segmented.  Reads the
+        frame's counts back (one host synchronisation).  Runs with autograd enabled, also inside torch.no_grad() (the
+        segmenter's forwards): a training step captured here at its first use records its backward."""
+        from . import ops
+        t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        t0.record()
+        fused = self.net._engine.forward_inference(x)[-1]
+        cur = self._current                                # once captured, its static buffers take the frame directly
+        labels, counts = ops.adaptation_labels(fused, self.last_mask, self.alpha, self.erosion, self.distance,
+                                               out=None if cur is None else cur.gt)
+        if cur is not None:
+            cur.x.copy_(x)
+        counts = counts[0].cpu()
+        self.counts.append(counts)
+        if int(counts[0]) == 0:                            # the object is lost: no step
+            self.skipped += 1
+        else:
+            for s in range(self.steps):
+                if s in self.current_at:
+                    if self._current is None:              # captured on this frame's image and labels
+                        self._current = GraphedTrainStep(self.net, (0.0, 0.0, 0.0, 0.0, self.weight),
+                                                         {"image": x, "gt": labels}, external_pack=True, void=True)
+                    self._current()
+                else:
+                    sample = self.sample_fn(self.samples)
+                    self.samples += 1
+                    if self._first is None:
+                        self._first = GraphedTrainStep(self.net, ONLINE_WEIGHTS, sample, external_pack=True)
+                    self._first(sample)
+                self.opt.step(zero_grad=True)
+                for p in self._not_in_opt:                 # score_dsn: gradients written, not trained online
+                    p.grad.zero_()
+        t1.record()
+        self._events.append((t0, t1))
+
+    def segmented(self, fused):
+        """Record the frame's fused map (fp32 [1,1,H,W] at the network resolution) as the next frame's last mask."""
+        from . import ops
+        ops.logits_to_u8(fused, "mask", out=self.last_mask.view(fused.shape))
+
+    def seconds(self):
+        """Device time spent in adapt() so far (one synchronisation)."""
+        torch.cuda.synchronize()
+        return sum(a.elapsed_time(b) for a, b in self._events) / 1000.0
+
+
 def parent_epoch(net, opt, bucket, batches, epoch, n_epochs, n_ave_grad=1, group=None, state=None, void=False):
     """One epoch of the parent objective on this rank's shard: deep-supervision loss
     (1 - epoch/nEpochs) * sum_{k<4} L_k + L_fuse (train_parent.py:143-147), gradient accumulation over

@@ -5,6 +5,7 @@ first frame with SGD(lr 1e-8, momentum .9), save the weights, then segment the s
 
     SEQ_NAME=blackswan python train_online.py --loader native # DAVIS on disk (needs cv2 + the dataset)
     SEQ_NAME=blackswan python train_online.py --loader native --evaluate   # ... and score the masks (J and F)
+    SEQ_NAME=blackswan python train_online.py --loader native --adapt      # ... adapting the net online (OnAVOS)
     SEQ_NAME=dogs-jump python train_online.py --loader native --davis 2017 --evaluate   # DAVIS-2017, one net per object
     SEQ_NAME=dogs-jump python train_online.py --loader native --davis 2017 --input-res 240 427 --output-res stored
     SEQ_NAME=blackswan python train_online.py                 # the same through the reference's dataloaders package
@@ -97,7 +98,45 @@ def parse(argv=None):
                     help="with --davis 2017: leave the annotation's void pixels (255) out of each object's fine-tuning "
                          "loss instead of counting them as background. Needs a parent whose deconvolution weights are "
                          "the bilinear taps (not one trained with --upsampling-lr)")
+    ap.add_argument("--adapt", action="store_true",
+                    help="online adaptation while segmenting (OnAVOS; DESIGN.md §28): before each frame after the first, "
+                         "targets from the network's confident pixels and the previous frame's mask (built on the GPU), "
+                         "and --adapt-steps SGD steps interleaving that frame with augmented samples of the annotated "
+                         "one. Needs --loader native and DAVIS-2016")
+    ap.add_argument("--adapt-steps", type=int, default=None, help="--adapt: SGD steps per frame (default 15)")
+    ap.add_argument("--adapt-current-steps", type=int, default=None,
+                    help="--adapt: how many of them train on the current frame (default 3)")
+    ap.add_argument("--adapt-weight", type=float, default=None,
+                    help="--adapt: loss weight of the current frame's fused map (default 0.05)")
+    ap.add_argument("--adapt-alpha", type=float, default=None,
+                    help="--adapt: a pixel is positive when its probability exceeds this (default 0.97)")
+    ap.add_argument("--adapt-distance", type=int, default=None,
+                    help="--adapt: pixels farther than this from the eroded last mask are negative (default 220)")
+    ap.add_argument("--adapt-erosion", type=int, default=None,
+                    help="--adapt: radius of the disk the last mask is eroded by (default 15)")
     a = ap.parse_args(argv)
+    adapt_opts = {"adapt_steps": 15, "adapt_current_steps": 3, "adapt_weight": 0.05, "adapt_alpha": 0.97,
+                  "adapt_distance": 220, "adapt_erosion": 15}
+    for k, default in adapt_opts.items():
+        if getattr(a, k) is None:
+            setattr(a, k, default)
+        elif not a.adapt:
+            ap.error(f"--{k.replace('_', '-')} needs --adapt")
+    if a.adapt:
+        if a.synthetic or a.loader != "native":
+            ap.error("--adapt segments a sequence read by --loader native; it cannot be combined with "
+                     + ("--synthetic" if a.synthetic else "--loader reference"))
+        if a.davis == "2017":
+            ap.error("--adapt supports DAVIS-2016 (one object); --davis 2017 is not supported")
+        if a.upsampling_lr != 0.0:
+            ap.error("--adapt trains with void labels, which the learned-upsampling tail does not support; it cannot be "
+                     "combined with a nonzero --upsampling-lr")
+        if not 0.0 < a.adapt_alpha < 1.0:
+            ap.error("--adapt-alpha must lie strictly between 0 and 1")
+        if a.adapt_distance < 0 or a.adapt_erosion < 0:
+            ap.error("--adapt-distance and --adapt-erosion must be non-negative")
+        if not 0 <= a.adapt_current_steps <= a.adapt_steps:
+            ap.error("--adapt-steps must be non-negative and --adapt-current-steps lie in 0 .. --adapt-steps")
     if a.ignore_void and a.davis != "2017":
         ap.error("--ignore-void applies to --davis 2017 (DAVIS-2016 annotations have no void pixels)")
     if a.ignore_void and a.upsampling_lr != 0.0:
@@ -267,11 +306,18 @@ def main(argv=None):
     elif input_res is not None:
         print(f"Frames resized to {input_res[0]}x{input_res[1]} (inputRes); results are written at that size"
               + (", scored against the nearest-resized annotations" if a.evaluate else ""))
+    adapt = None
+    if a.adapt:
+        # the fine-tuning's sampler goes on drawing from its generator; the annotation at the network resolution is
+        # frame 1's last mask
+        adapt = training.OnlineAdaptation(net, sample_fn, gt_u8, a.lr, a.wd, steps=a.adapt_steps,
+                                          current_steps=a.adapt_current_steps, weight=a.adapt_weight,
+                                          alpha=a.adapt_alpha, distance=a.adapt_distance, erosion=a.adapt_erosion)
     seg = SequenceSegmenter(net, output="bytescale", frames=("jpeg" if jpeg_frames else "bgr8") if native else "nchw_f32",
                             score=a.evaluate,
                             input_res=input_res, output_res=a.output_res,
                             encode="png" if a.encode == "device" else None,
-                            overlay="jpeg" if a.overlay else None, overlay_quality=a.overlay_quality)
+                            overlay="jpeg" if a.overlay else None, overlay_quality=a.overlay_quality, adapt=adapt)
     if a.overlay:
         overlay_dir = os.path.join(save_dir, "Results", a.seq_name + "_overlay")
         os.makedirs(overlay_dir, exist_ok=True)
@@ -297,6 +343,9 @@ def main(argv=None):
     if seg.jpeg_status is not None and int(seg.jpeg_status) != 0:     # the segmenter's last wait covered the decodes
         print(f"WARNING: the device JPEG decoder flagged corrupt or cut-short frames (status sum {int(seg.jpeg_status)}); "
               "their bytes may differ from cv2.imread's")
+    if adapt is not None:
+        print(f"Online adaptation time: {adapt.seconds():.2f} s over {len(adapt.counts)} frame(s), "
+              f"{adapt.skipped} skipped (eroded last mask empty)")
     if a.evaluate:
         import json
         from osvos_pytorch_b200.evaluation import SequenceScores
@@ -308,6 +357,10 @@ def main(argv=None):
               + "  ".join(f"{m} M/O/D: {st[m]['M']:.4f} / {st[m]['O']:.4f} / {st[m]['D']:.4f}" for m in ("J", "F")))
         if upsample:
             res = dict(network_res=list(input_res), scored_res=stored_hw, **res)
+        if adapt is not None:                           # counts of frames 1 .. n-1: {|E|, #positive, #negative}
+            res = dict(adaptation=dict(steps=a.adapt_steps, current_steps=a.adapt_current_steps, weight=a.adapt_weight,
+                                       alpha=a.adapt_alpha, distance=a.adapt_distance, erosion=a.adapt_erosion,
+                                       skipped=adapt.skipped, counts=[c.tolist() for c in adapt.counts]), **res)
         with open(os.path.join(save_dir, "Results", a.seq_name + "_scores.json"), "w") as f:
             json.dump(dict(sequence=a.seq_name, **res), f, indent=1)
     return history
