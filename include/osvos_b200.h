@@ -848,6 +848,27 @@ OSVOS_API int osvos_adaptation_labels(const float* logits, const uint8_t* last_m
                                       void* workspace, int n, int h, int w, float logit_threshold, int erosion_r,
                                       int distance_r, osvos_stream_t stream);
 
+/* ---- dense CRF refinement (DESIGN.md §29) -------------------------------------------------------------------------
+ *   osvos_dense_crf:     frames [n][h][w][3] uint8 BGR (any alignment) and `maps` (host array of k device pointers, each
+ *                         to fp32 [n][h][w], 4-byte aligned, as osvos_merge_objects) -> out [k][n][h][w] fp32 (4-byte
+ *                         aligned): the refined maps r_k = a_k - a_0 of a Potts mean-field with labels 0 (background)
+ *                         and 1..k, unary a⁰ = (0, z_1..z_k), `iterations` updates a = a⁰ + w_a·B + w_g·S, Q = softmax(a).
+ *                         B: the permutohedral-lattice bilateral filter on (x/theta_a, y/theta_a, R/theta_b, G/theta_b,
+ *                         B/theta_b), normalised by its filter of 1; S: the exact 2-D Gaussian of sigma theta_g
+ *                         truncated at ceil(3·theta_g), normalised over the pixels inside the frame.  iterations == 0
+ *                         copies the maps.  Each frame has its own lattice; lattice vertices are sorted, not hashed, and
+ *                         every sum runs in a fixed order: the result does not depend on the launch configuration.  No
+ *                         host synchronisation.  1 <= k <= OSVOS_MERGE_MAX_OBJECTS, 1 <= n <= 2048, h, w < 32768,
+ *                         6·n·h·w < 2^31, weights finite and >= 0, thetas finite and > 0; a frame size and thetas whose
+ *                         lattice coordinates would not fit the packed 64-bit keys are refused before any launch.
+ *                         `workspace`: osvos_dense_crf_workspace_bytes(n, k, h, w) bytes, 256-byte aligned, owned by the
+ *                         caller; it starts with the n per-frame lattice vertex counts (int32) and their total.
+ *   osvos_dense_crf_workspace_bytes: host query; 0 for invalid sizes.                                               */
+OSVOS_API size_t osvos_dense_crf_workspace_bytes(int n, int k, int h, int w);
+OSVOS_API int osvos_dense_crf(const uint8_t* frames, const float* const* maps, float* out, void* workspace, int n, int k,
+                              int h, int w, int iterations, float w_a, double theta_a, double theta_b, float w_g,
+                              double theta_g, osvos_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -259,6 +259,10 @@ SIGNATURES = {
     "osvos_adaptation_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "osvos_adaptation_labels": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
                                         c_int, c_int, c_void_p]),
+    # fully connected CRF refinement of K fused maps (DESIGN.md §29)
+    "osvos_dense_crf_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "osvos_dense_crf": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                c_float, c_double, c_double, c_float, c_double, c_void_p]),
 }
 
 DAVIS_MAX_RADIUS = 31

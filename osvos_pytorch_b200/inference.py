@@ -76,11 +76,17 @@ class SequenceSegmenter:
     slot at the network resolution, and the frame's fused map at that resolution, before any upsampling, becomes the
     next frame's last mask.  The forwards then run eagerly (engine.forward_inference): the weights change every frame,
     and a captured inference graph would be dropped and captured again each time.  Everything downstream of the forward
-    is unchanged.  Needs one net (not labels), frames="bgr8" or "jpeg" and batches of one frame."""
+    is unchanged.  Needs one net (not labels), frames="bgr8" or "jpeg" and batches of one frame.
+
+    ``crf`` (an ops.CRF; DESIGN.md §29; frames="bgr8" or "jpeg"): right after the forward(s), on the compute stream,
+    ops.dense_crf refines the K fused maps against the slot's bytes at the network resolution (the resized slot under
+    ``input_res``), and the refined maps replace the fused maps for everything downstream: upsampling, merging,
+    scoring, the 8-bit maps, PNGs, overlays and ``output="logits"``.  With ``adapt`` the adaptation still reads the
+    unrefined fused map, so the adapted weights do not depend on ``crf``."""
 
     def __init__(self, net=None, output="logits", depth=3, frames="nchw_f32", meanval=ops.MEANVAL, score=False,
                  input_res=None, output_res="network", encode=None, overlay=None, overlay_quality=95, nets=None,
-                 palette=None, adapt=None):
+                 palette=None, adapt=None, crf=None):
         if (net is None) == (nets is None):
             raise ValueError("pass either net or nets")
         if adapt is not None:
@@ -90,7 +96,12 @@ class SequenceSegmenter:
                 raise ValueError("adapt segments one object: it does not take output='labels'")
             if frames == "nchw_f32":
                 raise ValueError("adapt needs frames='bgr8' or 'jpeg'")
-        self.adapt = adapt
+        if crf is not None:
+            if not isinstance(crf, ops.CRF):
+                raise ValueError(f"crf must be an ops.CRF, got {type(crf).__name__}")
+            if frames == "nchw_f32":
+                raise ValueError("crf reads the frames' bytes: it needs frames='bgr8' or 'jpeg'")
+        self.adapt, self.crf = adapt, crf
         nets = [net] if nets is None else list(nets)
         if not 1 <= len(nets) <= 254 or len({id(m) for m in nets}) != len(nets):
             raise ValueError("nets must be 1 .. 254 distinct networks")
@@ -166,6 +177,8 @@ class SequenceSegmenter:
             self._dev_jlen = [torch.empty(n, dtype=torch.int64, device=device) for _ in range(self.depth)]
             self._host_jpg = [torch.empty((n, ocap), dtype=torch.uint8).pin_memory() for _ in range(self.depth)]
             self._host_jlen = [torch.empty(n, dtype=torch.int64).pin_memory() for _ in range(self.depth)]
+        if self.crf is not None:                            # compute stream only: read before the next frame's CRF
+            self._dev_crf = torch.empty((len(self.nets), n, 1, h, w), dtype=torch.float32, device=device)
         if self._upsample and self.output != "labels":     # labels are upsampled inside the merge
             self._dev_up = [torch.empty((n, 1, h0, w0), dtype=torch.float32, device=device) for _ in range(self.depth)]
         if self.score:
@@ -245,6 +258,9 @@ class SequenceSegmenter:
             fused = fused_maps[0]
             if self.adapt is not None and i > 0:               # frame 0's last mask is the annotation
                 self.adapt.segmented(fused)
+            if self.crf is not None:                           # the bytes the network saw, before any upsampling
+                fused_maps = list(ops.dense_crf(raw, fused_maps, self.crf, out=self._dev_crf).unbind(0))
+                fused = fused_maps[0]
             if self._upsample and self.output != "labels":     # back to the stored size, before anything reads it
                 fused = ops.resize_f32(fused, self._dev_up[k].shape[2:4], out=self._dev_up[k])
             if self.output == "labels":

@@ -1,6 +1,7 @@
 """Tensor-level wrappers over the C ABI: they allocate outputs with torch (device
 memory + stream plumbing only) and enqueue the native kernels on the current
 torch stream.  No arithmetic happens in Python / PyTorch here."""
+import dataclasses
 from ctypes import byref, c_void_p
 
 import torch
@@ -1019,6 +1020,81 @@ def adaptation_labels(logits, last_mask, alpha, erosion, distance, out=None):
                                           n, h, w, threshold, min(e, cap), min(d, cap), _stream()),
               "osvos_adaptation_labels")
     return out, counts
+
+
+@dataclasses.dataclass(frozen=True)
+class CRF:
+    """Parameters of dense_crf (DESIGN.md §29): ``iterations`` mean-field updates, the bilateral message's weight and
+    its position / colour scales in pixels and intensity levels, and the Gaussian message's weight and scale.  The
+    defaults are pydensecrf's example values; nobody has tuned them for OSVOS, and their effect on J and F is not
+    measured."""
+    iterations: int = 5
+    bilateral_weight: float = 10.0
+    bilateral_xy: float = 80.0
+    bilateral_rgb: float = 13.0
+    gaussian_weight: float = 3.0
+    gaussian_xy: float = 3.0
+
+    def __post_init__(self):
+        import math
+        if isinstance(self.iterations, bool) or not isinstance(self.iterations, int) or self.iterations < 0:
+            raise ValueError(f"iterations must be a non-negative integer, got {self.iterations!r}")
+        for name in ("bilateral_weight", "gaussian_weight", "bilateral_xy", "bilateral_rgb", "gaussian_xy"):
+            v = getattr(self, name)
+            if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v):
+                raise ValueError(f"{name} must be a finite number, got {v!r}")
+            if v < 0 or (name.endswith(("_xy", "_rgb")) and v == 0):
+                raise ValueError(f"{name} must be {'> 0' if name.endswith(('_xy', '_rgb')) else '>= 0'}, got {v!r}")
+
+
+def dense_crf(frames, maps, crf=CRF(), out=None, vertices=None):
+    """Refine K fused logit maps with a fully connected CRF (csrc/crf.cu, DESIGN.md §29): ``frames`` the bytes the
+    network saw, uint8 [N,H,W,3] BGR at any alignment; ``maps`` the forms merge_objects takes (K maps of [N,1,H,W] or
+    [N,H,W], 1 <= K <= 254) -> fp32 [K,N,1,H,W], map k the refined logit a_k - a_0 of labels 0 (background) and 1..K
+    after ``crf.iterations`` Potts mean-field updates, which merge_objects / upsample_merge_objects take as they are.
+    ``out``: a contiguous fp32 tensor of K*N*H*W elements.  ``vertices``: an int32 [N] tensor that receives each
+    frame's lattice vertex count (with iterations > 0).  Everything is checked before the launch.  No host
+    synchronisation."""
+    lib = nat.load()
+    if not isinstance(crf, CRF):
+        raise ValueError(f"crf must be an ops.CRF, got {type(crf).__name__}")
+    x = _require_u8(frames, "frames", 4)
+    n, h, w, c = (int(v) for v in x.shape)
+    if c != 3:
+        raise ValueError("frames must be [N,H,W,3]")
+    keep = _object_maps(maps, "dense_crf")
+    k = len(keep)
+    if int(keep[0].shape[0]) != n or tuple(keep[0].shape[-2:]) != (h, w) or keep[0].device != x.device:
+        raise ValueError(f"maps must be [N,1,H,W] or [N,H,W] matching frames {tuple(x.shape)} on their device, got "
+                         f"{tuple(keep[0].shape)}")
+    nbytes = lib.osvos_dense_crf_workspace_bytes(n, k, h, w)
+    if nbytes == 0:
+        raise ValueError(f"cannot refine [{n},{h},{w}] with {k} maps: sizes must lie in [1, 32767], N in [1, 2048] and "
+                         "6*N*H*W below 2^31")
+    if out is None:
+        out = torch.empty((k, n, 1, h, w), dtype=torch.float32, device=x.device)
+    elif (out.dtype != torch.float32 or out.numel() != k * n * h * w or not out.is_contiguous()
+          or out.device != x.device or out.data_ptr() % 4):
+        raise ValueError(f"out must be a contiguous fp32 tensor of {k * n * h * w} elements on the frames' device")
+    if vertices is not None and (vertices.dtype != torch.int32 or vertices.numel() != n or vertices.device != x.device):
+        raise ValueError(f"vertices must be an int32 tensor of {n} elements on the frames' device")
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    ptrs = (c_void_p * k)(*(t.data_ptr() for t in keep))
+    # the library refuses, before any launch, frame sizes and scales whose lattice coordinates overflow the packed keys
+    nat.check(lib.osvos_dense_crf(x.data_ptr(), ptrs, out.data_ptr(), ws.data_ptr(), n, k, h, w, crf.iterations,
+                                  crf.bilateral_weight, crf.bilateral_xy, crf.bilateral_rgb, crf.gaussian_weight,
+                                  crf.gaussian_xy, _stream()), "osvos_dense_crf")
+    _count(CRF_LAUNCHES_BUILD + CRF_LAUNCHES_PER_ITERATION * crf.iterations if crf.iterations else 0)
+    if vertices is not None and crf.iterations:
+        vertices.copy_(ws[:4 * n].view(torch.int32).view(vertices.shape))
+    return out
+
+
+# launches of one dense_crf call: elevate, sort (counted once), mark, scan (once), compact, neighbours, the F(1)
+# filter (splat, 6 blurs, slice), taps, the initial softmax; then per iteration the filter, the Gaussian rows, the update.
+# With 0 iterations the maps are only copied.
+CRF_LAUNCHES_BUILD = 16
+CRF_LAUNCHES_PER_ITERATION = 10
 
 
 def decode_jpeg(blob, n, h, w, out=None, status=None, nseg=None, chunk_bits=0):

@@ -6,6 +6,7 @@ first frame with SGD(lr 1e-8, momentum .9), save the weights, then segment the s
     SEQ_NAME=blackswan python train_online.py --loader native # DAVIS on disk (needs cv2 + the dataset)
     SEQ_NAME=blackswan python train_online.py --loader native --evaluate   # ... and score the masks (J and F)
     SEQ_NAME=blackswan python train_online.py --loader native --adapt      # ... adapting the net online (OnAVOS)
+    SEQ_NAME=blackswan python train_online.py --loader native --crf        # ... refining each mask with a dense CRF
     SEQ_NAME=dogs-jump python train_online.py --loader native --davis 2017 --evaluate   # DAVIS-2017, one net per object
     SEQ_NAME=dogs-jump python train_online.py --loader native --davis 2017 --input-res 240 427 --output-res stored
     SEQ_NAME=blackswan python train_online.py                 # the same through the reference's dataloaders package
@@ -13,6 +14,7 @@ first frame with SGD(lr 1e-8, momentum .9), save the weights, then segment the s
 
 Single GPU by design (BASELINE.json: online fine-tune stays single-GPU; run one sequence per GPU)."""
 import argparse
+import dataclasses
 import os
 import timeit
 
@@ -114,7 +116,34 @@ def parse(argv=None):
                     help="--adapt: pixels farther than this from the eroded last mask are negative (default 220)")
     ap.add_argument("--adapt-erosion", type=int, default=None,
                     help="--adapt: radius of the disk the last mask is eroded by (default 15)")
+    ap.add_argument("--crf", action="store_true",
+                    help="refine every frame's fused map(s) with a fully connected CRF on the GPU (DESIGN.md §29): "
+                         "permutohedral-lattice mean-field over the frame's bytes at the network resolution, before "
+                         "anything is upsampled, merged, scored or written. Needs --loader native. The default "
+                         "parameters are pydensecrf's example values; their effect on J and F is not measured")
+    ap.add_argument("--crf-iterations", type=int, default=None, metavar="T", help="--crf: mean-field updates (default 5)")
+    ap.add_argument("--crf-bilateral", type=float, nargs=3, default=None, metavar=("W", "XY", "RGB"),
+                    help="--crf: weight, position and colour scales of the bilateral message (default 10 80 13)")
+    ap.add_argument("--crf-gaussian", type=float, nargs=2, default=None, metavar=("W", "XY"),
+                    help="--crf: weight and position scale of the Gaussian message (default 3 3)")
     a = ap.parse_args(argv)
+    crf_opts = {"crf_iterations": 5, "crf_bilateral": [10.0, 80.0, 13.0], "crf_gaussian": [3.0, 3.0]}
+    for k, default in crf_opts.items():
+        if getattr(a, k) is None:
+            setattr(a, k, default)
+        elif not a.crf:
+            ap.error(f"--{k.replace('_', '-')} needs --crf")
+    a.crf_params = None
+    if a.crf:
+        if a.synthetic or a.loader != "native":
+            ap.error("--crf reads the bytes of the frames read by --loader native; it cannot be combined with "
+                     + ("--synthetic" if a.synthetic else "--loader reference"))
+        try:
+            a.crf_params = ops.CRF(iterations=a.crf_iterations, bilateral_weight=a.crf_bilateral[0],
+                                   bilateral_xy=a.crf_bilateral[1], bilateral_rgb=a.crf_bilateral[2],
+                                   gaussian_weight=a.crf_gaussian[0], gaussian_xy=a.crf_gaussian[1])
+        except ValueError as e:
+            ap.error(f"--crf: {e}")
     adapt_opts = {"adapt_steps": 15, "adapt_current_steps": 3, "adapt_weight": 0.05, "adapt_alpha": 0.97,
                   "adapt_distance": 220, "adapt_erosion": 15}
     for k, default in adapt_opts.items():
@@ -317,7 +346,8 @@ def main(argv=None):
                             score=a.evaluate,
                             input_res=input_res, output_res=a.output_res,
                             encode="png" if a.encode == "device" else None,
-                            overlay="jpeg" if a.overlay else None, overlay_quality=a.overlay_quality, adapt=adapt)
+                            overlay="jpeg" if a.overlay else None, overlay_quality=a.overlay_quality, adapt=adapt,
+                            crf=a.crf_params)
     if a.overlay:
         overlay_dir = os.path.join(save_dir, "Results", a.seq_name + "_overlay")
         os.makedirs(overlay_dir, exist_ok=True)
@@ -357,6 +387,8 @@ def main(argv=None):
               + "  ".join(f"{m} M/O/D: {st[m]['M']:.4f} / {st[m]['O']:.4f} / {st[m]['D']:.4f}" for m in ("J", "F")))
         if upsample:
             res = dict(network_res=list(input_res), scored_res=stored_hw, **res)
+        if a.crf_params is not None:
+            res = dict(crf=dataclasses.asdict(a.crf_params), **res)
         if adapt is not None:                           # counts of frames 1 .. n-1: {|E|, #positive, #negative}
             res = dict(adaptation=dict(steps=a.adapt_steps, current_steps=a.adapt_current_steps, weight=a.adapt_weight,
                                        alpha=a.adapt_alpha, distance=a.adapt_distance, erosion=a.adapt_erosion,
@@ -446,7 +478,7 @@ def online_2017(a, parent, device, save_dir, iters, log_every):
               + (", scored against the original annotations" if a.evaluate else ""))
     seg = SequenceSegmenter(nets=nets, output="labels", frames="jpeg" if jpeg_frames else "bgr8", score=a.evaluate,
                             input_res=input_res, output_res=a.output_res,
-                            encode="png" if encode else None, palette=palette if encode else None)
+                            encode="png" if encode else None, palette=palette if encode else None, crf=a.crf_params)
     for pred in seg(frames()):
         batch_names = names.popleft()
         for jj, name in enumerate(batch_names):
@@ -473,6 +505,8 @@ def online_2017(a, parent, device, save_dir, iters, log_every):
         res = scores.result()
         if input_res is not None:
             res = dict(network_res=list(input_res), scored_res=stored_hw, **res)
+        if a.crf_params is not None:
+            res = dict(crf=dataclasses.asdict(a.crf_params), **res)
         for k, ob in res["objects"].items():
             st = ob["statistics"]
             print(f"Scores of {a.seq_name} object {k} (frames 1 .. n-2): "
