@@ -176,6 +176,14 @@ def softmax(a):
     return e / e.sum(0, keepdims=True)
 
 
+def mean_field_step(lat, a0, q, norm, w_a, w_g, theta_g):
+    """One mean-field update: a = a⁰ + w_α B + w_γ S from the label probabilities q [K+1,N,H,W], with B = F(q) / F(1)
+    (``norm`` = F(1) per pixel) and S the Gaussian message."""
+    b = (lat.filter(q.reshape(q.shape[0], -1).T) / norm[:, None]).T.reshape(q.shape)
+    s = smoothness(q, theta_g)
+    return a0 + w_a * b + w_g * s
+
+
 def dense_crf(frames, maps, iterations=5, w_a=10.0, theta_a=80.0, theta_b=13.0, w_g=3.0, theta_g=3.0, lattice=None,
               weights_f32=True):
     """frames uint8 [N,H,W,3], maps [K,N,H,W] -> refined maps float64 [K,N,H,W] (r_k = a_k - a_0 of the last
@@ -191,8 +199,6 @@ def dense_crf(frames, maps, iterations=5, w_a=10.0, theta_a=80.0, theta_b=13.0, 
     q = softmax(a0)
     norm = lat.filter(np.ones((lat.pixels, 1)))[:, 0]
     for _ in range(iterations):
-        b = (lat.filter(q.reshape(k + 1, -1).T) / norm[:, None]).T.reshape(q.shape)
-        s = smoothness(q, theta_g)
-        a = a0 + w_a * b + w_g * s
+        a = mean_field_step(lat, a0, q, norm, w_a, w_g, theta_g)
         q = softmax(a)
     return a[1:] - a[0]

@@ -98,6 +98,41 @@ def test_constant_image_averages_over_the_frame():
     assert np.allclose(b, q.mean(0, keepdims=True), rtol=1e-12)
 
 
+def _structured_frame(h, w):
+    """A colour ramp in x, y and x + y with a flat blob: edges in colour as well as in position."""
+    yy, xx = np.mgrid[0:h, 0:w]
+    f = np.stack([xx * 255 // (w - 1), yy * 255 // (h - 1), (3 * xx + 5 * yy) % 256], -1)
+    f[(xx - w / 3) ** 2 + (yy - h / 2) ** 2 < (h / 3) ** 2] = (200, 60, 90)
+    return f.astype(np.uint8)[None]
+
+
+@pytest.mark.parametrize("thetas", [(3.0, 13.0), (5.0, 20.0), (8.0, 30.0)])
+def test_lattice_filter_has_the_width_the_parameters_name(thetas):
+    """The normalised lattice filter F(Q)/F(1) approximates the dense Gaussian exp(-|Δf|² / 2) of
+    f = (x/θα, y/θα, R/θβ, G/θβ, B/θβ) (DESIGN §29), and that Gaussian better than the same one at scale 0.7 or 1.4:
+    the lattice's scale factors give the filter the width θα, θβ name, not one that is off by a constant factor.
+    The approximation itself (one simplex per pixel, a 3-tap blur per direction) errs by a few hundredths here."""
+    h, w = 24, 32
+    frames = _structured_frame(h, w)
+    u = np.random.default_rng(15).random(h * w)
+    q = np.stack([u, 1 - u], 1)
+    lat = ref.Lattice(frames, *thetas)
+    b = lat.filter(q) / lat.filter(np.ones((lat.pixels, 1)))
+    yy, xx = np.mgrid[0:h, 0:w]
+    px = frames[0].reshape(-1, 3).astype(np.float64)
+    ta, tb = thetas
+    feat = np.stack([xx.ravel() / ta, yy.ravel() / ta, px[:, 2] / tb, px[:, 1] / tb, px[:, 0] / tb], 1)
+    d2 = ((feat[:, None] - feat[None]) ** 2).sum(-1)
+    err = {}
+    for s in (0.7, 1.0, 1.4):
+        k = np.exp(-d2 / (2 * s * s))
+        diff = b - k @ q / k.sum(1, keepdims=True)
+        err[s] = (float(np.abs(diff).max()), float(np.sqrt((diff ** 2).mean())))
+    assert err[1.0][0] < 0.08 and err[1.0][1] < 0.015, err
+    for s in (0.7, 1.4):
+        assert err[1.0][0] < err[s][0] and 2 * err[1.0][1] < err[s][1], err
+
+
 @pytest.mark.parametrize("theta,shape", [(3.0, (2, 20, 31)), (0.4, (1, 5, 6)), (1.7, (1, 3, 40)), (5.0, (1, 8, 8))])
 def test_gaussian_message_is_the_truncated_correlation_renormalised(theta, shape):
     rng = np.random.default_rng(9)
