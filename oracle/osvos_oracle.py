@@ -162,7 +162,7 @@ def upsample_zero_padded(x: torch.Tensor, stride: int) -> torch.Tensor:
         m = np.zeros((n_out, n_in), dtype=np.float64)
         for i in range(n_in):
             m[i * stride:i * stride + 2 * stride, i] = f
-        return torch.from_numpy(m).to(x.dtype)
+        return torch.from_numpy(m).to(x.device, x.dtype)
 
     my, mx = matrix(h), matrix(w)
     return torch.einsum("oy,ncyx,px->ncop", my, x, mx)
