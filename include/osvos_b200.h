@@ -869,6 +869,40 @@ OSVOS_API int osvos_dense_crf(const uint8_t* frames, const float* const* maps, f
                               int h, int w, int iterations, float w_a, double theta_a, double theta_b, float w_g,
                               double theta_g, osvos_stream_t stream);
 
+/* ---- connected components and the component filter (DESIGN.md §30) ----------------------------------------------
+ *   osvos_connected_components: masks [n][h][w] uint8 (any alignment; nonzero = foreground) -> labels [n][h][w] int32
+ *                         and counts [n] int32 (4-byte aligned): per frame, scipy.ndimage.label of the foreground with
+ *                         the cross structure (connectivity 4) or the 3x3 square (8): 0 background, components numbered
+ *                         1..counts[f] in the raster order of their first pixels.  Union-find in 32x16 tiles, then
+ *                         across tile borders, every link by atomicMin to the smaller root; the roots' ranks come from a
+ *                         CUB scan.  The result does not depend on the launch configuration.  h, w < 32768,
+ *                         n·h·w < 2^31.  `workspace`: osvos_connected_components_workspace_bytes(n, h, w) bytes,
+ *                         256-byte aligned, owned by the caller.
+ *   osvos_filter_components: `maps` (host array of k device pointers, each to fp32 [n][h][w], 4-byte aligned, as
+ *                         osvos_merge_objects), prior [k][h][w] uint8 (any alignment, nonzero = object) or NULL -> out
+ *                         [k][n][h][w] fp32 (4-byte aligned), kept [k][n][h][w] uint8 (0/1) and stats [k][n][4] int32
+ *                         (4-byte aligned).  Per object and frame, F = z > 0 (NaN, ±0 are not) and its components C_i at
+ *                         `connectivity`; C* the largest (ties: the smallest label).  OSVOS_COMPONENTS_LARGEST keeps
+ *                         C*.  OSVOS_COMPONENTS_NEAR keeps every C_i whose exact minimum squared distance to the prior
+ *                         mask P is <= radius², or C* when P is empty or none is; P is `prior` for frame 0 (empty when
+ *                         NULL) and the kept mask of frame f - 1 after that, so frames are taken in order.  out = z where
+ *                         F is false or the component is kept, -z on the pixels of dropped components; kept = the kept
+ *                         mask; stats = {components, components kept, |F|, pixels removed}.  Integer after the z > 0
+ *                         test: the result does not depend on the launch configuration.  No host synchronisation.
+ *                         1 <= k <= OSVOS_MERGE_MAX_OBJECTS, h, w < 32768, n·k·h·w < 2^31, radius >= 0.
+ *                         `workspace`: osvos_filter_components_workspace_bytes(n, k, h, w, mode) bytes, 256-byte aligned,
+ *                         owned by the caller.
+ *   *_workspace_bytes:   host queries; 0 for invalid sizes or mode.                                                */
+#define OSVOS_COMPONENTS_LARGEST 0
+#define OSVOS_COMPONENTS_NEAR 1
+OSVOS_API size_t osvos_connected_components_workspace_bytes(int n, int h, int w);
+OSVOS_API int osvos_connected_components(const uint8_t* masks, int* labels, int* counts, void* workspace, int n, int h,
+                                         int w, int connectivity, osvos_stream_t stream);
+OSVOS_API size_t osvos_filter_components_workspace_bytes(int n, int k, int h, int w, int mode);
+OSVOS_API int osvos_filter_components(const float* const* maps, const uint8_t* prior, float* out, uint8_t* kept,
+                                      int* stats, void* workspace, int n, int k, int h, int w, int mode, int radius,
+                                      int connectivity, osvos_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

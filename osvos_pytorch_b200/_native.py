@@ -152,6 +152,7 @@ class OverlayColors(Structure):
 UPSAMPLING_TAPS = 1360
 U8_PROB, U8_BYTESCALE, U8_MASK = 0, 1, 2
 RESIZE_BILINEAR, RESIZE_NEAREST = 0, 1
+COMPONENTS_LARGEST, COMPONENTS_NEAR = 0, 1
 SGD_MAX_SEGMENTS = 64
 
 # name -> (restype, argtypes); mirrors include/osvos_b200.h one to one (tests/test_abi.py checks it)
@@ -263,6 +264,13 @@ SIGNATURES = {
     "osvos_dense_crf_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "osvos_dense_crf": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                 c_float, c_double, c_double, c_float, c_double, c_void_p]),
+    # connected components of masks and the component filter of K fused maps (DESIGN.md §30)
+    "osvos_connected_components_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "osvos_connected_components": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                           c_void_p]),
+    "osvos_filter_components_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
+    "osvos_filter_components": (c_int, [POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                        c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
 }
 
 DAVIS_MAX_RADIUS = 31

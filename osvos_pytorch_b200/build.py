@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libosvos_b200.so")
-SOURCES = ["runtime.cu", "layout_kernels.cu", "conv3x3_halo.cu", "conv_stage1_fused.cu", "conv_first_tc.cu", "side_conv.cu", "tail.cu", "tail_general.cu", "loss.cu", "wgrad_tc.cu", "bwd_kernels.cu", "side_bwd_folded.cu", "output_kernels.cu", "augment.cu", "frames.cu", "measures.cu", "resize.cu", "jpeg.cu", "png.cu", "png_decode.cu", "jpeg_encode.cu", "adapt.cu", "crf.cu"]
+SOURCES = ["runtime.cu", "layout_kernels.cu", "conv3x3_halo.cu", "conv_stage1_fused.cu", "conv_first_tc.cu", "side_conv.cu", "tail.cu", "tail_general.cu", "loss.cu", "wgrad_tc.cu", "bwd_kernels.cu", "side_bwd_folded.cu", "output_kernels.cu", "augment.cu", "frames.cu", "measures.cu", "resize.cu", "jpeg.cu", "png.cu", "png_decode.cu", "jpeg_encode.cu", "adapt.cu", "crf.cu", "components.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 

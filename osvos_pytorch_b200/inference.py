@@ -82,11 +82,19 @@ class SequenceSegmenter:
     ops.dense_crf refines the K fused maps against the slot's bytes at the network resolution (the resized slot under
     ``input_res``), and the refined maps replace the fused maps for everything downstream: upsampling, merging,
     scoring, the 8-bit maps, PNGs, overlays and ``output="logits"``.  With ``adapt`` the adaptation still reads the
-    unrefined fused map, so the adapted weights do not depend on ``crf``."""
+    unrefined fused map, so the adapted weights do not depend on ``crf``.
+
+    ``components`` (an ops.Components; DESIGN.md §30): right after the forward(s) and the CRF, on the compute stream,
+    ops.filter_components drops each object's stray connected components at the network resolution, and the filtered
+    maps replace the fused maps for everything downstream, as the CRF's do.  "near" measures each frame against the
+    previous frame's kept mask, kept per object across frames and batches; ``components_prior`` (uint8 [K,H,W] at the
+    network resolution, nonzero = object) seeds it for the first frame, without it the first frame keeps its largest
+    component.  With ``adapt`` the adaptation still reads the unfiltered fused map.  ``component_stats()`` returns each
+    frame's statistics."""
 
     def __init__(self, net=None, output="logits", depth=3, frames="nchw_f32", meanval=ops.MEANVAL, score=False,
                  input_res=None, output_res="network", encode=None, overlay=None, overlay_quality=95, nets=None,
-                 palette=None, adapt=None, crf=None):
+                 palette=None, adapt=None, crf=None, components=None, components_prior=None):
         if (net is None) == (nets is None):
             raise ValueError("pass either net or nets")
         if adapt is not None:
@@ -101,7 +109,16 @@ class SequenceSegmenter:
                 raise ValueError(f"crf must be an ops.CRF, got {type(crf).__name__}")
             if frames == "nchw_f32":
                 raise ValueError("crf reads the frames' bytes: it needs frames='bgr8' or 'jpeg'")
+        if components is not None and not isinstance(components, ops.Components):
+            raise ValueError(f"components must be an ops.Components, got {type(components).__name__}")
+        if components_prior is not None:
+            if components is None:
+                raise ValueError("components_prior seeds the component filter: it needs components")
+            if not torch.is_tensor(components_prior) or components_prior.dtype != torch.uint8 or components_prior.dim() != 3:
+                raise ValueError("components_prior must be a uint8 tensor [K,H,W]")
         self.adapt, self.crf = adapt, crf
+        self.components, self.components_prior = components, components_prior
+        self._component_stats = []
         nets = [net] if nets is None else list(nets)
         if not 1 <= len(nets) <= 254 or len({id(m) for m in nets}) != len(nets):
             raise ValueError("nets must be 1 .. 254 distinct networks")
@@ -179,6 +196,15 @@ class SequenceSegmenter:
             self._host_jlen = [torch.empty(n, dtype=torch.int64).pin_memory() for _ in range(self.depth)]
         if self.crf is not None:                            # compute stream only: read before the next frame's CRF
             self._dev_crf = torch.empty((len(self.nets), n, 1, h, w), dtype=torch.float32, device=device)
+        if self.components is not None:                     # compute stream only, as the CRF's maps
+            self._dev_comp = torch.empty((len(self.nets), n, 1, h, w), dtype=torch.float32, device=device)
+            self._dev_prior = torch.empty((len(self.nets), h, w), dtype=torch.uint8, device=device)
+            self._seed_prior = None
+            if self.components_prior is not None:
+                if tuple(self.components_prior.shape) != (len(self.nets), h, w):
+                    raise ValueError(f"components_prior must be uint8 [K,H,W] = {(len(self.nets), h, w)} at the network "
+                                     f"resolution, got {tuple(self.components_prior.shape)}")
+                self._seed_prior = self.components_prior.to(device).contiguous()
         if self._upsample and self.output != "labels":     # labels are upsampled inside the merge
             self._dev_up = [torch.empty((n, 1, h0, w0), dtype=torch.float32, device=device) for _ in range(self.depth)]
         if self.score:
@@ -261,6 +287,17 @@ class SequenceSegmenter:
             if self.crf is not None:                           # the bytes the network saw, before any upsampling
                 fused_maps = list(ops.dense_crf(raw, fused_maps, self.crf, out=self._dev_crf).unbind(0))
                 fused = fused_maps[0]
+            if self.components is not None:                    # at the network resolution, before any upsampling
+                prior = None
+                if self.components.mode == "near":
+                    prior = self._dev_prior if i > 0 else self._seed_prior
+                filtered, kept, stats = ops.filter_components(fused_maps, self.components, prior=prior,
+                                                              out=self._dev_comp)
+                if self.components.mode == "near":             # the next batch's prior: this batch's last kept mask
+                    self._dev_prior.copy_(kept[:, -1])
+                self._component_stats.append(stats.permute(1, 0, 2))
+                fused_maps = list(filtered.unbind(0))
+                fused = fused_maps[0]
             if self._upsample and self.output != "labels":     # back to the stored size, before anything reads it
                 fused = ops.resize_f32(fused, self._dev_up[k].shape[2:4], out=self._dev_up[k])
             if self.output == "labels":
@@ -314,6 +351,7 @@ class SequenceSegmenter:
             raise RuntimeError("SequenceSegmenter runs on CUDA only; there is no CPU fallback for the OSVOS hot path")
         submitted = 0
         self._counts = []
+        self._component_stats = []
         with torch.cuda.device(device):
             if self.frames == "jpeg":
                 self.jpeg_status = torch.zeros(1, dtype=torch.int32, device=device)
@@ -365,6 +403,15 @@ class SequenceSegmenter:
         if not self._counts:
             return torch.zeros((0, len(self.nets), 6) if self.output == "labels" else (0, 6), dtype=torch.int32)
         return torch.cat(self._counts).cpu()
+
+    def component_stats(self):
+        """int32 [frames*N, K, 4] host tensor of the last run's ops.filter_components statistics, frame order
+        ({components, components kept, |F|, pixels removed} per object; ``components``).  One synchronisation."""
+        if self.components is None:
+            raise RuntimeError("component_stats() needs SequenceSegmenter(..., components=ops.Components(...))")
+        if not self._component_stats:
+            return torch.zeros((0, len(self.nets), 4), dtype=torch.int32)
+        return torch.cat(self._component_stats).cpu()
 
     def join_current_stream(self):
         """Make the current stream wait for every copy issued so far (lets CUDA events on the current stream bracket

@@ -1097,6 +1097,114 @@ CRF_LAUNCHES_BUILD = 16
 CRF_LAUNCHES_PER_ITERATION = 10
 
 
+def _connectivity(c):
+    if isinstance(c, bool) or c not in (4, 8):
+        raise ValueError(f"connectivity must be 4 or 8, got {c!r}")
+    return c
+
+
+def _component_sizes_ok(n, k, h, w):
+    if not (0 < h < 32768 and 0 < w < 32768) or n * k * h * w >= 1 << 31:
+        raise ValueError(f"cannot label {k} x [{n},{h},{w}]: H and W must lie in [1, 32767] and N*K*H*W below 2^31")
+
+
+def connected_components(masks, connectivity=8):
+    """Connected components of uint8 masks [N,H,W] (nonzero = foreground, any alignment; csrc/components.cu, DESIGN.md
+    §30) -> (labels int32 [N,H,W], counts int32 [N]): per frame scipy.ndimage.label(mask != 0, structure), the cross
+    structure for ``connectivity`` 4 and the 3x3 square for 8: 0 background, components 1..counts[f] numbered in the
+    raster order of their first pixels.  Frames are independent.  Checked before the launch; no host synchronisation."""
+    lib = nat.load()
+    x = _require_u8(masks, "masks", 3)
+    c = _connectivity(connectivity)
+    n, h, w = (int(v) for v in x.shape)
+    if n == 0:
+        raise ValueError("masks must hold at least one frame")
+    _component_sizes_ok(n, 1, h, w)
+    labels = torch.empty((n, h, w), dtype=torch.int32, device=x.device)
+    counts = torch.empty(n, dtype=torch.int32, device=x.device)
+    ws = torch.empty(lib.osvos_connected_components_workspace_bytes(n, h, w), dtype=torch.uint8, device=x.device)
+    _count(5)                                       # local, border, compress, scan (counted once), numbering
+    nat.check(lib.osvos_connected_components(x.data_ptr(), labels.data_ptr(), counts.data_ptr(), ws.data_ptr(), n, h, w,
+                                             c, _stream()), "osvos_connected_components")
+    return labels, counts
+
+
+@dataclasses.dataclass(frozen=True)
+class Components:
+    """Parameters of filter_components (DESIGN.md §30): ``mode`` "largest" keeps each object's largest connected
+    component; "near" keeps every component within ``radius`` pixels (exact Euclidean distance) of the prior mask, or
+    the largest when the prior is empty or none is that near.  ``connectivity`` 4 or 8.  The defaults are this project's
+    choices, not tuned; their effect on J and F is not measured."""
+    mode: str
+    radius: int = 32
+    connectivity: int = 8
+
+    def __post_init__(self):
+        if self.mode not in ("largest", "near"):
+            raise ValueError(f"mode must be 'largest' or 'near', got {self.mode!r}")
+        if isinstance(self.radius, bool) or not isinstance(self.radius, int) or self.radius < 0:
+            raise ValueError(f"radius must be a non-negative integer, got {self.radius!r}")
+        _connectivity(self.connectivity)
+
+
+_COMPONENT_MODES = {"largest": nat.COMPONENTS_LARGEST, "near": nat.COMPONENTS_NEAR}
+
+
+def filter_components(maps, params, prior=None, out=None):
+    """Drop stray components from K fused logit maps (csrc/components.cu, DESIGN.md §30).  ``maps``: the forms
+    merge_objects takes (K maps of [N,1,H,W] or [N,H,W], 1 <= K <= 254); ``params`` an ops.Components; ``prior``: uint8
+    [K,H,W] (nonzero = object), the mask "near" measures frame 0 against, or None (frame 0 keeps its largest component).
+    Frame j > 0 is measured against frame j - 1's kept mask.  Per object and frame, F = z > 0 (NaN and ±0 are not
+    foreground); the pixels of dropped components get -z, every other pixel keeps z, so every later stage sees them as
+    background.  Returns (out fp32 [K,N,1,H,W], kept uint8 [K,N,H,W] 0/1, stats int32 [K,N,4] = {components, components
+    kept, |F|, pixels removed}).  ``out``: a contiguous fp32 tensor of K*N*H*W elements.  Everything is checked before
+    the launch.  No host synchronisation."""
+    lib = nat.load()
+    if not isinstance(params, Components):
+        raise ValueError(f"params must be an ops.Components, got {type(params).__name__}")
+    keep = _object_maps(maps, "filter_components")
+    k = len(keep)
+    n, h, w = int(keep[0].shape[0]), int(keep[0].shape[-2]), int(keep[0].shape[-1])
+    dev = keep[0].device
+    if n == 0:
+        raise ValueError("maps must hold at least one frame")
+    _component_sizes_ok(n, k, h, w)
+    if prior is not None:
+        _require_cuda(prior, "prior")
+        if prior.dtype != torch.uint8 or tuple(prior.shape) != (k, h, w) or prior.device != dev:
+            raise ValueError(f"prior must be uint8 [K,H,W] = {(k, h, w)} on the maps' device, got {prior.dtype} "
+                             f"{tuple(prior.shape)}")
+        prior = prior.contiguous()
+    if out is None:
+        out = torch.empty((k, n, 1, h, w), dtype=torch.float32, device=dev)
+    elif (out.dtype != torch.float32 or out.numel() != k * n * h * w or not out.is_contiguous() or out.device != dev
+          or out.data_ptr() % 4):
+        raise ValueError(f"out must be a contiguous fp32 tensor of {k * n * h * w} elements on the maps' device")
+    mode = _COMPONENT_MODES[params.mode]
+    kept = torch.empty((k, n, h, w), dtype=torch.uint8, device=dev)
+    stats = torch.empty((k, n, 4), dtype=torch.int32, device=dev)
+    ws = torch.empty(lib.osvos_filter_components_workspace_bytes(n, k, h, w, mode), dtype=torch.uint8, device=dev)
+    ptrs = (c_void_p * k)(*(t.data_ptr() for t in keep))
+    radius = min(params.radius, 1 << 16)            # past the frame's diagonal every radius means the same
+    if params.mode == "largest":
+        _count(COMPONENTS_LAUNCHES_LABEL + COMPONENTS_LAUNCHES_PER_DECISION)
+    else:
+        _count(COMPONENTS_LAUNCHES_LABEL + COMPONENTS_LAUNCHES_PER_DECISION * n
+               + COMPONENTS_LAUNCHES_PER_DISTANCE * (n - 1 + (prior is not None)))
+    nat.check(lib.osvos_filter_components(ptrs, nat.ptr(prior), out.data_ptr(), kept.data_ptr(), stats.data_ptr(),
+                                          ws.data_ptr(), n, k, h, w, mode, radius, params.connectivity, _stream()),
+              "osvos_filter_components")
+    return out.view(k, n, 1, h, w), kept, stats
+
+
+# launches of one filter_components call: the labelling of every plane (local, border, compress); per decision (all
+# frames at once for "largest", each frame for "near") the decision and the write; per distance transform ("near", each
+# frame with a prior) the column and row passes.
+COMPONENTS_LAUNCHES_LABEL = 3
+COMPONENTS_LAUNCHES_PER_DECISION = 2
+COMPONENTS_LAUNCHES_PER_DISTANCE = 2
+
+
 def decode_jpeg(blob, n, h, w, out=None, status=None, nseg=None, chunk_bits=0):
     """A batch of n JPEGs of size h x w packed by jpeg.pack (``blob``: uint8 device tensor) -> (out uint8 [n,h,w,3] BGR,
     bit-identical to cv2.imread; status int32 [n]: 1 bad Huffman code, 2 zig-zag index past 63, 4 data ended before the

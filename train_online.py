@@ -7,6 +7,7 @@ first frame with SGD(lr 1e-8, momentum .9), save the weights, then segment the s
     SEQ_NAME=blackswan python train_online.py --loader native --evaluate   # ... and score the masks (J and F)
     SEQ_NAME=blackswan python train_online.py --loader native --adapt      # ... adapting the net online (OnAVOS)
     SEQ_NAME=blackswan python train_online.py --loader native --crf        # ... refining each mask with a dense CRF
+    SEQ_NAME=blackswan python train_online.py --loader native --components near   # ... dropping stray blobs
     SEQ_NAME=dogs-jump python train_online.py --loader native --davis 2017 --evaluate   # DAVIS-2017, one net per object
     SEQ_NAME=dogs-jump python train_online.py --loader native --davis 2017 --input-res 240 427 --output-res stored
     SEQ_NAME=blackswan python train_online.py                 # the same through the reference's dataloaders package
@@ -126,7 +127,33 @@ def parse(argv=None):
                     help="--crf: weight, position and colour scales of the bilateral message (default 10 80 13)")
     ap.add_argument("--crf-gaussian", type=float, nargs=2, default=None, metavar=("W", "XY"),
                     help="--crf: weight and position scale of the Gaussian message (default 3 3)")
+    ap.add_argument("--components", default=None, choices=["largest", "near"],
+                    help="drop stray blobs from every frame's fused map(s) on the GPU (DESIGN.md §30): keep each "
+                         "object's largest connected component (largest), or the components within --components-radius "
+                         "pixels of the previous frame's kept mask (near; the first annotation is frame 0's with "
+                         "--loader native, otherwise frame 0 keeps its largest). Runs at the network resolution after "
+                         "--crf, before anything is upsampled, merged, scored or written. The defaults are not tuned; "
+                         "their effect on J and F is not measured")
+    ap.add_argument("--components-radius", type=int, default=None, metavar="R",
+                    help="--components near: keep the components within R pixels of the prior mask (default 32)")
+    ap.add_argument("--components-connectivity", type=int, default=None, choices=[4, 8],
+                    help="--components: 4- or 8-connected components (default 8)")
     a = ap.parse_args(argv)
+    if a.components_radius is not None and a.components is not None and a.components != "near":
+        ap.error("--components-radius applies to --components near")
+    comp_opts = {"components_radius": 32, "components_connectivity": 8}
+    for k, default in comp_opts.items():
+        if getattr(a, k) is None:
+            setattr(a, k, default)
+        elif a.components is None:
+            ap.error(f"--{k.replace('_', '-')} needs --components")
+    a.components_params = None
+    if a.components is not None:
+        try:
+            a.components_params = ops.Components(a.components, radius=a.components_radius,
+                                                 connectivity=a.components_connectivity)
+        except ValueError as e:
+            ap.error(f"--components: {e}")
     crf_opts = {"crf_iterations": 5, "crf_bilateral": [10.0, 80.0, 13.0], "crf_gaussian": [3.0, 3.0]}
     for k, default in crf_opts.items():
         if getattr(a, k) is None:
@@ -342,12 +369,14 @@ def main(argv=None):
         adapt = training.OnlineAdaptation(net, sample_fn, gt_u8, a.lr, a.wd, steps=a.adapt_steps,
                                           current_steps=a.adapt_current_steps, weight=a.adapt_weight,
                                           alpha=a.adapt_alpha, distance=a.adapt_distance, erosion=a.adapt_erosion)
+    # the annotation at the network resolution is frame 0's prior of --components near
+    prior = (gt_u8 != 0).to(torch.uint8) if native and a.components_params is not None else None
     seg = SequenceSegmenter(net, output="bytescale", frames=("jpeg" if jpeg_frames else "bgr8") if native else "nchw_f32",
                             score=a.evaluate,
                             input_res=input_res, output_res=a.output_res,
                             encode="png" if a.encode == "device" else None,
                             overlay="jpeg" if a.overlay else None, overlay_quality=a.overlay_quality, adapt=adapt,
-                            crf=a.crf_params)
+                            crf=a.crf_params, components=a.components_params, components_prior=prior)
     if a.overlay:
         overlay_dir = os.path.join(save_dir, "Results", a.seq_name + "_overlay")
         os.makedirs(overlay_dir, exist_ok=True)
@@ -373,6 +402,7 @@ def main(argv=None):
     if seg.jpeg_status is not None and int(seg.jpeg_status) != 0:     # the segmenter's last wait covered the decodes
         print(f"WARNING: the device JPEG decoder flagged corrupt or cut-short frames (status sum {int(seg.jpeg_status)}); "
               "their bytes may differ from cv2.imread's")
+    comp_stats = _report_components(a, seg)
     if adapt is not None:
         print(f"Online adaptation time: {adapt.seconds():.2f} s over {len(adapt.counts)} frame(s), "
               f"{adapt.skipped} skipped (eroded last mask empty)")
@@ -389,6 +419,8 @@ def main(argv=None):
             res = dict(network_res=list(input_res), scored_res=stored_hw, **res)
         if a.crf_params is not None:
             res = dict(crf=dataclasses.asdict(a.crf_params), **res)
+        if comp_stats is not None:
+            res = dict(components=comp_stats, **res)
         if adapt is not None:                           # counts of frames 1 .. n-1: {|E|, #positive, #negative}
             res = dict(adaptation=dict(steps=a.adapt_steps, current_steps=a.adapt_current_steps, weight=a.adapt_weight,
                                        alpha=a.adapt_alpha, distance=a.adapt_distance, erosion=a.adapt_erosion,
@@ -478,7 +510,10 @@ def online_2017(a, parent, device, save_dir, iters, log_every):
               + (", scored against the original annotations" if a.evaluate else ""))
     seg = SequenceSegmenter(nets=nets, output="labels", frames="jpeg" if jpeg_frames else "bgr8", score=a.evaluate,
                             input_res=input_res, output_res=a.output_res,
-                            encode="png" if encode else None, palette=palette if encode else None, crf=a.crf_params)
+                            encode="png" if encode else None, palette=palette if encode else None, crf=a.crf_params,
+                            components=a.components_params,
+                            components_prior=None if a.components_params is None else
+                            torch.stack([ids_u8[0] == k for k in range(1, k_objects + 1)]).to(torch.uint8))
     for pred in seg(frames()):
         batch_names = names.popleft()
         for jj, name in enumerate(batch_names):
@@ -494,6 +529,7 @@ def online_2017(a, parent, device, save_dir, iters, log_every):
                 im.save(path)
     if seg.jpeg_status is not None and int(seg.jpeg_status) != 0:
         print(f"WARNING: the device JPEG decoder flagged corrupt or cut-short frames (status sum {int(seg.jpeg_status)})")
+    comp_stats = _report_components(a, seg)
     if a.overlay:                                       # drawn from the label files just written, on the device
         from osvos_pytorch_b200 import visualize
         visualize.render_results(os.path.join(save_dir, "Results"), Path.db_root_dir(), sequences=[a.seq_name],
@@ -507,6 +543,8 @@ def online_2017(a, parent, device, save_dir, iters, log_every):
             res = dict(network_res=list(input_res), scored_res=stored_hw, **res)
         if a.crf_params is not None:
             res = dict(crf=dataclasses.asdict(a.crf_params), **res)
+        if comp_stats is not None:
+            res = dict(components=comp_stats, **res)
         for k, ob in res["objects"].items():
             st = ob["statistics"]
             print(f"Scores of {a.seq_name} object {k} (frames 1 .. n-2): "
@@ -514,6 +552,18 @@ def online_2017(a, parent, device, save_dir, iters, log_every):
         with open(os.path.join(save_dir, "Results", a.seq_name + "_scores.json"), "w") as f:
             json.dump(dict(sequence=a.seq_name, davis="2017", n_objects=k_objects, **res), f, indent=1)
     return history
+
+
+def _report_components(a, seg):
+    """--components: print the components removed and the pixels they covered; return the scores file's entry (the
+    parameters and each frame's per-object {components, components kept, |F|, pixels removed}), or None."""
+    if a.components_params is None:
+        return None
+    stats = seg.component_stats()
+    removed = int((stats[..., 0] - stats[..., 1]).sum())
+    print(f"Components ({a.components}): removed {removed} component(s) covering {int(stats[..., 3].sum())} pixel(s) "
+          f"over {stats.shape[0]} frame(s)")
+    return dict(dataclasses.asdict(a.components_params), stats=stats.tolist())
 
 
 if __name__ == "__main__":
